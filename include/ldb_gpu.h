@@ -362,8 +362,14 @@ enum LdbOp {
    LDB_OP_STRLIKE = 21,/* dst = columns[a] LIKE strings[arg]; b = 0 'x%', 1 '%x', 2 '%x%' */
    LDB_OP_YEAR = 22,   /* dst = extract(year from date32 a) */
    LDB_OP_PROBE = 23,  /* dst = payload of int32 key a in tables[arg]; NULL when absent */
-   LDB_OP_STRKEY8 = 24 /* dst = first 8 bytes of columns[a], zero padded, big-endian (an order-preserving int64 group / sort key for short
+   LDB_OP_STRKEY8 = 24,/* dst = first 8 bytes of columns[a], zero padded, big-endian (an order-preserving int64 group / sort key for short
                           strings: char(n<=8), flags, codes; longer strings need a dictionary and are not keys here) */
+   LDB_OP_ROWID = 25,  /* dst = global row number of the scanned row in its table (a row-id build payload for side-column reads) */
+   LDB_OP_PROBE_EACH = 26 /* dst = payload of EACH match of int32 key a in tables[arg] (plain single-key or direct-address tables); the
+                             instructions after it, the filter and the sink run once per match.  b = 0 inner join (no match: no tuple),
+                             b = 1 left outer join (no match: one tuple with dst NULL).  A NULL key never matches.  At most one per
+                             program; later instructions may not overwrite registers written at or before it.  A probe run longer
+                             than the interpreter's bound fails the call (LDB_ERR_CAPACITY) rather than dropping matches. */
 };
 enum LdbAggKind { LDB_AGG_SUM = 1, LDB_AGG_SUM_F64 = 2, LDB_AGG_COUNT = 3, LDB_AGG_COUNT_STAR = 4, LDB_AGG_MIN = 5, LDB_AGG_MAX = 6 /* 64-bit signed */,
                   LDB_AGG_MIN_F64 = 7, LDB_AGG_MAX_F64 = 8, LDB_AGG_ANY = 9 };
@@ -387,7 +393,7 @@ typedef struct LdbProgramDesc {
    const LdbI128* consts;
    int32_t n_strings;            /* <= 12, each <= 32 bytes */
    const char* const* strings;
-   int32_t n_tables;             /* <= 4 join tables (single int32 key or direct-address) for LDB_OP_PROBE */
+   int32_t n_tables;             /* <= 4 join tables (single int32 key or direct-address) for LDB_OP_PROBE / LDB_OP_PROBE_EACH */
    LdbState* const* tables;
    int32_t filter_reg;           /* the row is kept when this register is TRUE (NULL is not true); -1 = keep all */
    int32_t sink_kind;            /* LdbProgramSink */
@@ -398,12 +404,33 @@ typedef struct LdbProgramDesc {
    LdbProgAgg aggs[LDB_MAX_AGGS];
    int32_t build_key_reg, build_payload_reg; /* JOIN_BUILD: payload_reg -1 = 0 */
    /* MATERIALIZE: out_regs → a new DEVICE table (columns "c0".."cN": decimal128(38,0) cells = the raw i128 / double bits in the
-    * low 8 bytes, each with a validity byte); capacity = source rows */
+    * low 8 bytes, each with a validity byte); capacity = source rows, regrown to the produced row count (one more run of the
+    * program) when a PROBE_EACH yields more tuples than that */
    int32_t n_out;
    int32_t out_regs[LDB_MAX_AGGS];
    LdbTable** out_table;
 } LdbProgramDesc;
 int ldb_gpu_run_program(LdbContext* ctx, const LdbProgramDesc* desc, LdbError* err);
+/* Side columns: columns of OTHER tables ("side tables", same context, any number of batches), read at the row number a register
+ * holds — typically a ROWID payload returned by PROBE / PROBE_EACH, so a join can read any number of build-side attributes,
+ * decimals and strings included.  A NULL row register (or one outside the side table) reads NULL: outer-join semantics.
+ * Side column k takes program column index desc->n_columns + k; source and side columns share the 12-column budget.  LOAD, STRCMP,
+ * STRLIKE and STRKEY8 read them like source columns (validity bitmaps and bytes honoured); utf8 side columns are operands of the
+ * string ops only.  The row register must be written before the first instruction that reads the column. */
+typedef struct LdbSideColumn {
+   int32_t table;      /* index into LdbProgramJoins.side_tables */
+   const char* column;
+   int32_t row_reg;    /* register holding the side table's row number */
+} LdbSideColumn;
+typedef struct LdbProgramJoins {
+   int32_t n_side_tables;
+   LdbTable* const* side_tables;
+   int32_t n_side_columns;
+   const LdbSideColumn* side_columns;
+} LdbProgramJoins;
+/* ldb_gpu_run_program with side columns (joins may be NULL).  A JOIN_BUILD program that uses ROWID is rejected when its source
+ * has 2^31 rows or more (join payloads are int32). */
+int ldb_gpu_run_program_ex(LdbContext* ctx, const LdbProgramDesc* desc, const LdbProgramJoins* joins, LdbError* err);
 /* hash aggregation state sized for `expected_groups` (the directory holds 2x that; LDB_ERR_CAPACITY when it overflows) */
 int ldb_gpu_hashagg_create(LdbContext* ctx, int32_t n_keys, int32_t n_aggs, const LdbProgAgg* aggs, int64_t expected_groups, LdbState** out, LdbError* err);
 int ldb_gpu_hashagg_count(LdbState* s, int64_t* n_groups, LdbError* err);

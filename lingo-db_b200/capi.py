@@ -119,6 +119,14 @@ class ProgramDesc(C.Structure):
                 ("out_table", C.POINTER(C.c_void_p))]
 
 
+class SideColumn(C.Structure):
+    _fields_ = [("table", C.c_int32), ("column", C.c_char_p), ("row_reg", C.c_int32)]
+
+
+class ProgramJoins(C.Structure):
+    _fields_ = [("n_side_tables", C.c_int32), ("side_tables", C.POINTER(C.c_void_p)), ("n_side_columns", C.c_int32), ("side_columns", C.POINTER(SideColumn))]
+
+
 class HashAggRow(C.Structure):
     _fields_ = [("keys", C.c_int64 * 4), ("key_null_mask", C.c_uint32), ("agg_valid_mask", C.c_uint32), ("aggs", I128 * MAX_AGGS)]
 
@@ -183,6 +191,7 @@ SIGNATURES = {
     "ldb_gpu_register_state": (C.c_int, [_P, C.c_char_p, _P, _E]),
     "ldb_gpu_find_state": (C.c_void_p, [_P, C.c_char_p]),
     "ldb_gpu_run_program": (C.c_int, [_P, C.POINTER(ProgramDesc), _E]),
+    "ldb_gpu_run_program_ex": (C.c_int, [_P, C.POINTER(ProgramDesc), C.POINTER(ProgramJoins), _E]),
     "ldb_gpu_hashagg_create": (C.c_int, [_P, C.c_int32, C.c_int32, C.POINTER(ProgAgg), C.c_int64, C.POINTER(_P), _E]),
     "ldb_gpu_hashagg_count": (C.c_int, [_P, C.POINTER(C.c_int64), _E]),
     "ldb_gpu_hashagg_read": (C.c_int, [_P, C.POINTER(HashAggRow), C.c_int64, C.POINTER(C.c_int64), _E]),

@@ -67,7 +67,8 @@ struct JoinTableDev {
    uint32_t bloomMask;        // words - 1
    unsigned long long* count; // inserted entries
    int32_t* error;            // 1 = table full, 2 = duplicate key in a unique table, 3 = unstorable pair, 4 = negative payload in a wide table,
-                              // 5 = key outside the declared range of a direct-address table
+                              // 5 = key outside the declared range of a direct-address table, 6 = a program's PROBE_EACH met a
+                              // probe run longer than its bound
    int32_t unique;
    int32_t direct;            // stride 4: direct-address table
    int32_t keyMin;

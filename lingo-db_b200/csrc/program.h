@@ -21,6 +21,17 @@ constexpr int kProgMaxTables = 4;
 constexpr int kProgMaxKeys = 4;
 constexpr int kProgMaxAggs = 8;
 
+// one batch of a side table (the device-resident batch directory of a side column over a multi-batch table)
+struct ProgSideBatch {
+   const uint8_t* data;
+   const uint8_t* bytes;
+   const uint8_t* validity;
+   const uint8_t* validBytes;
+   int64_t bitOffset;
+   int64_t firstRow; // global row number of the batch's row 0
+   int32_t elemBytes;
+   int32_t pad;
+};
 struct ProgCol {
    const uint8_t* data;     // values, or utf8 offsets (int32)
    const uint8_t* bytes;    // utf8 data
@@ -29,6 +40,12 @@ struct ProgCol {
    int64_t bitOffset;       // bit index of row 0 inside `validity`
    int32_t type;            // LdbPhysType
    int32_t elemBytes;       // as staged (decimal128: 16, or 8 when the HOST batch was narrowed)
+   // side column: read at the row register rowReg holds instead of the scanned row (-1 = a column of the scanned table).  A
+   // single-batch side table uses the fields above; a multi-batch one the directory `dir` of nBatches batches, sorted by firstRow.
+   int32_t rowReg;
+   int32_t nBatches;
+   int64_t sideRows;        // rows of the side table: a NULL row register or one outside 0..sideRows-1 reads NULL
+   const ProgSideBatch* dir;
 };
 struct ProgInstr {
    uint8_t op, dst, a, b;
@@ -49,9 +66,13 @@ struct HashAggDev {
    unsigned long long* count; // groups
    int32_t* error;            // 1 = table full
 };
+// The kernel takes ProgramParams by value (__grid_constant__): 3 176 bytes with the limits above, within the classic 4 096-byte
+// kernel-parameter limit (program_rt.cpp checks it at compile time).
 struct ProgramParams {
    int64_t nRows;
+   int64_t firstRow; // global row number of this batch's row 0 (LDB_OP_ROWID)
    int32_t nCols, nInstr, nTables;
+   int32_t eachPc;   // index of the LDB_OP_PROBE_EACH instruction, -1 = none: from there on the program runs once per match
    ProgCol cols[kProgMaxCols];
    ProgInstr instr[kProgMaxInstr];
    unsigned long long constLo[kProgMaxConsts];

@@ -236,182 +236,304 @@ int ldb_gpu_hashagg_to_table(LdbState* s, const char* name, LdbTable** out, LdbE
    });
 }
 
-int ldb_gpu_run_program(LdbContext* ctx, const LdbProgramDesc* d, LdbError* err) {
-   return guardedP(err, [&] {
-      if (!ctx || !d || !d->source) failP(LDB_ERR_INVALID, "null argument");
-      LdbTable* t = d->source;
-      if (t->ctx != ctx) failP(LDB_ERR_INVALID, "table belongs to another context");
-      if (d->n_columns < 0 || d->n_columns > kProgMaxCols || d->n_instr < 0 || d->n_instr > kProgMaxInstr || d->n_consts < 0 || d->n_consts > kProgMaxConsts ||
-          d->n_strings < 0 || d->n_strings > kProgMaxStrings || d->n_tables < 0 || d->n_tables > kProgMaxTables)
-         failP(LDB_ERR_UNSUPPORTED, "program exceeds the interpreter's limits (12 columns, 96 instructions, 24 constants, 12 strings, 4 tables)");
-      LDB_CUDA(cudaSetDevice(ctx->device));
-      ProgramParams base{};
-      base.nCols = d->n_columns;
-      base.nInstr = d->n_instr;
-      base.nTables = d->n_tables;
-      std::vector<int> colIdx((size_t) d->n_columns);
-      for (int c = 0; c < d->n_columns; c++) {
-         colIdx[c] = t->colIndex(d->columns[c]);
-         if (colIdx[c] < 0) failP(LDB_ERR_INVALID, std::string("unknown column ") + (d->columns[c] ? d->columns[c] : "(null)"));
+static_assert(sizeof(ProgramParams) <= 4096, "ProgramParams exceeds the 4 KB kernel-parameter limit");
+
+// the pointers of column `ci` of batch `b` (validity bitmap or validity bytes included)
+static void bindColumn(ProgCol& pc, const LdbBatch& b, int ci) {
+   pc.data = (const uint8_t*) b.data[ci];
+   pc.bytes = (const uint8_t*) b.bytes[ci];
+   pc.elemBytes = b.elemBytes[ci];
+   pc.validity = ci < (int) b.validity.size() ? (const uint8_t*) b.validity[ci] : nullptr;
+   pc.bitOffset = ci < (int) b.validityBitOffset.size() ? b.validityBitOffset[ci] : 0;
+   pc.validBytes = ci < (int) b.validBytes.size() ? b.validBytes[ci] : nullptr;
+}
+
+static void runProgram(LdbContext* ctx, const LdbProgramDesc* d, const LdbProgramJoins* j) {
+   if (!ctx || !d || !d->source) failP(LDB_ERR_INVALID, "null argument");
+   LdbTable* t = d->source;
+   if (t->ctx != ctx) failP(LDB_ERR_INVALID, "table belongs to another context");
+   if (j && (j->n_side_tables < 0 || j->n_side_columns < 0 || (j->n_side_tables > 0 && !j->side_tables) || (j->n_side_columns > 0 && !j->side_columns)))
+      failP(LDB_ERR_INVALID, "malformed side-table list");
+   const int nSide = j ? j->n_side_columns : 0;
+   if (d->n_columns < 0 || d->n_columns + nSide > kProgMaxCols || d->n_instr < 0 || d->n_instr > kProgMaxInstr || d->n_consts < 0 || d->n_consts > kProgMaxConsts ||
+       d->n_strings < 0 || d->n_strings > kProgMaxStrings || d->n_tables < 0 || d->n_tables > kProgMaxTables)
+      failP(LDB_ERR_UNSUPPORTED, "program exceeds the interpreter's limits (12 source + side columns, 96 instructions, 24 constants, 12 strings, 4 tables)");
+   LDB_CUDA(cudaSetDevice(ctx->device));
+   const int nCols = d->n_columns + nSide;
+   ProgramParams base{};
+   base.nCols = nCols;
+   base.nInstr = d->n_instr;
+   base.nTables = d->n_tables;
+   base.eachPc = -1;
+   std::vector<int> colIdx((size_t) nCols), rowReg((size_t) nCols, -1);
+   std::vector<LdbTable*> colTable((size_t) nCols, t);
+   for (int c = 0; c < d->n_columns; c++) {
+      colIdx[c] = t->colIndex(d->columns[c]);
+      if (colIdx[c] < 0) failP(LDB_ERR_INVALID, std::string("unknown column ") + (d->columns[c] ? d->columns[c] : "(null)"));
+   }
+   for (int k = 0; k < nSide; k++) {
+      const LdbSideColumn& sc = j->side_columns[k];
+      const int c = d->n_columns + k;
+      if (sc.table < 0 || sc.table >= j->n_side_tables || !j->side_tables[sc.table]) failP(LDB_ERR_INVALID, "side column: side table index out of range");
+      LdbTable* st = j->side_tables[sc.table];
+      if (st->ctx != ctx) failP(LDB_ERR_INVALID, "side table belongs to another context");
+      colIdx[c] = st->colIndex(sc.column);
+      if (colIdx[c] < 0) failP(LDB_ERR_INVALID, std::string("unknown side column ") + (sc.column ? sc.column : "(null)"));
+      if (sc.row_reg < 0 || sc.row_reg >= kProgMaxRegs) failP(LDB_ERR_INVALID, "side column: row register out of range");
+      colTable[c] = st;
+      rowReg[c] = sc.row_reg;
+   }
+   auto colType = [&](int c) { return colTable[c]->columns[colIdx[c]].type; };
+   // static validation: every register read was written before, every index is in range, types fit the opcode
+   bool written[kProgMaxRegs] = {}, beforeEach[kProgMaxRegs] = {};
+   auto wantReg = [&](int r, const char* what) {
+      if (r < 0 || r >= kProgMaxRegs || !written[r]) failP(LDB_ERR_INVALID, std::string("program reads an unwritten or out-of-range register (") + what + ")");
+   };
+   auto wantCol = [&](int c, const char* what) {
+      if (c < 0 || c >= nCols) failP(LDB_ERR_INVALID, std::string(what) + ": column index out of range");
+      if (rowReg[c] >= 0) wantReg(rowReg[c], "row register of a side column");
+   };
+   bool usesRowid = false;
+   int eachTable = -1;
+   for (int i = 0; i < d->n_instr; i++) {
+      const LdbInstr& in = d->instr[i];
+      if (in.dst >= kProgMaxRegs) failP(LDB_ERR_INVALID, "destination register out of range");
+      switch (in.op) {
+         case LDB_OP_LOAD:
+            wantCol(in.arg, "LOAD");
+            if (colType(in.arg) == LDB_UTF8) failP(LDB_ERR_UNSUPPORTED, "LOAD of a string column (strings are operands of STRCMP / STRLIKE / STRKEY8 only)");
+            break;
+         case LDB_OP_CONST:
+            if (in.arg < 0 || in.arg >= d->n_consts) failP(LDB_ERR_INVALID, "CONST: constant index out of range");
+            break;
+         case LDB_OP_ADD: case LDB_OP_SUB: case LDB_OP_MUL: case LDB_OP_DIV: case LDB_OP_AND: case LDB_OP_OR:
+         case LDB_OP_FADD: case LDB_OP_FSUB: case LDB_OP_FMUL: case LDB_OP_FDIV:
+            wantReg(in.a, "a");
+            wantReg(in.b, "b");
+            break;
+         case LDB_OP_CMP: case LDB_OP_FCMP:
+            wantReg(in.a, "a");
+            wantReg(in.b, "b");
+            if (in.arg < LDB_EQ || in.arg > LDB_GTE) failP(LDB_ERR_INVALID, "CMP: unknown comparison");
+            break;
+         case LDB_OP_NEG: case LDB_OP_NOT: case LDB_OP_ISNULL: case LDB_OP_I2F: case LDB_OP_YEAR: wantReg(in.a, "a"); break;
+         case LDB_OP_SELECT:
+            wantReg(in.a, "a");
+            wantReg(in.b, "b");
+            wantReg(in.arg, "condition");
+            break;
+         case LDB_OP_STRKEY8:
+            if (in.a >= nCols || colType(in.a) != LDB_UTF8) failP(LDB_ERR_INVALID, "STRKEY8 needs a utf8 column");
+            wantCol(in.a, "STRKEY8");
+            break;
+         case LDB_OP_STRCMP: case LDB_OP_STRLIKE:
+            if (in.a >= nCols || colType(in.a) != LDB_UTF8) failP(LDB_ERR_INVALID, "string op needs a utf8 column");
+            wantCol(in.a, "string op");
+            if (in.arg < 0 || in.arg >= d->n_strings) failP(LDB_ERR_INVALID, "string constant index out of range");
+            if (in.op == LDB_OP_STRCMP ? in.b > LDB_GTE : in.b > 2) failP(LDB_ERR_INVALID, "string op: unknown comparison / pattern kind");
+            break;
+         case LDB_OP_PROBE:
+            wantReg(in.a, "key");
+            if (in.arg < 0 || in.arg >= d->n_tables) failP(LDB_ERR_INVALID, "PROBE: table index out of range");
+            break;
+         case LDB_OP_ROWID: usesRowid = true; break;
+         case LDB_OP_PROBE_EACH:
+            wantReg(in.a, "key");
+            if (in.arg < 0 || in.arg >= d->n_tables) failP(LDB_ERR_INVALID, "PROBE_EACH: table index out of range");
+            if (in.b > 1) failP(LDB_ERR_INVALID, "PROBE_EACH: b is 0 (inner) or 1 (left outer)");
+            if (base.eachPc >= 0) failP(LDB_ERR_UNSUPPORTED, "at most one PROBE_EACH per program");
+            base.eachPc = i;
+            eachTable = in.arg;
+            break;
+         default: failP(LDB_ERR_UNSUPPORTED, "unknown opcode " + std::to_string(in.op));
       }
-      // static validation: every register read was written before, every index is in range, types fit the opcode
-      bool written[kProgMaxRegs] = {};
-      auto wantReg = [&](int r, const char* what) {
-         if (r < 0 || r >= kProgMaxRegs || !written[r]) failP(LDB_ERR_INVALID, std::string("program reads an unwritten or out-of-range register (") + what + ")");
-      };
-      for (int i = 0; i < d->n_instr; i++) {
-         const LdbInstr& in = d->instr[i];
-         if (in.dst >= kProgMaxRegs) failP(LDB_ERR_INVALID, "destination register out of range");
-         switch (in.op) {
-            case LDB_OP_LOAD:
-               if (in.arg < 0 || in.arg >= d->n_columns) failP(LDB_ERR_INVALID, "LOAD: column index out of range");
-               if (t->columns[colIdx[in.arg]].type == LDB_UTF8) failP(LDB_ERR_UNSUPPORTED, "LOAD of a string column (strings are operands of STRCMP / STRLIKE only)");
-               break;
-            case LDB_OP_CONST:
-               if (in.arg < 0 || in.arg >= d->n_consts) failP(LDB_ERR_INVALID, "CONST: constant index out of range");
-               break;
-            case LDB_OP_ADD: case LDB_OP_SUB: case LDB_OP_MUL: case LDB_OP_DIV: case LDB_OP_AND: case LDB_OP_OR:
-            case LDB_OP_FADD: case LDB_OP_FSUB: case LDB_OP_FMUL: case LDB_OP_FDIV:
-               wantReg(in.a, "a");
-               wantReg(in.b, "b");
-               break;
-            case LDB_OP_CMP: case LDB_OP_FCMP:
-               wantReg(in.a, "a");
-               wantReg(in.b, "b");
-               if (in.arg < LDB_EQ || in.arg > LDB_GTE) failP(LDB_ERR_INVALID, "CMP: unknown comparison");
-               break;
-            case LDB_OP_NEG: case LDB_OP_NOT: case LDB_OP_ISNULL: case LDB_OP_I2F: case LDB_OP_YEAR: wantReg(in.a, "a"); break;
-            case LDB_OP_SELECT:
-               wantReg(in.a, "a");
-               wantReg(in.b, "b");
-               wantReg(in.arg, "condition");
-               break;
-            case LDB_OP_STRKEY8:
-               if (in.a >= d->n_columns || t->columns[colIdx[in.a]].type != LDB_UTF8) failP(LDB_ERR_INVALID, "STRKEY8 needs a utf8 column");
-               break;
-            case LDB_OP_STRCMP: case LDB_OP_STRLIKE:
-               if (in.a >= d->n_columns || t->columns[colIdx[in.a]].type != LDB_UTF8) failP(LDB_ERR_INVALID, "string op needs a utf8 column");
-               if (in.arg < 0 || in.arg >= d->n_strings) failP(LDB_ERR_INVALID, "string constant index out of range");
-               if (in.op == LDB_OP_STRCMP ? in.b > LDB_GTE : in.b > 2) failP(LDB_ERR_INVALID, "string op: unknown comparison / pattern kind");
-               break;
-            case LDB_OP_PROBE:
-               wantReg(in.a, "key");
-               if (in.arg < 0 || in.arg >= d->n_tables) failP(LDB_ERR_INVALID, "PROBE: table index out of range");
-               break;
-            default: failP(LDB_ERR_UNSUPPORTED, "unknown opcode " + std::to_string(in.op));
+      // the instructions after PROBE_EACH run once per match: they may not overwrite what the first pass left for the next one
+      if (base.eachPc >= 0 && i > base.eachPc && beforeEach[in.dst]) failP(LDB_ERR_INVALID, "an instruction after PROBE_EACH overwrites a register written at or before it");
+      written[in.dst] = true;
+      if (base.eachPc == i) std::copy(written, written + kProgMaxRegs, beforeEach);
+      base.instr[i] = ProgInstr{in.op, in.dst, in.a, in.b, in.arg};
+   }
+   for (int c = 0; c < d->n_consts; c++) {
+      base.constLo[c] = d->consts[c].lo;
+      base.constHi[c] = d->consts[c].hi;
+   }
+   for (int c = 0; c < d->n_strings; c++) {
+      const size_t n = d->strings[c] ? strlen(d->strings[c]) : 0;
+      if (n > (size_t) kProgStringBytes) failP(LDB_ERR_UNSUPPORTED, "string constant longer than 32 bytes");
+      memcpy(base.strings[c], d->strings[c], n);
+      base.stringLen[c] = (int32_t) n;
+   }
+   for (int k = 0; k < d->n_tables; k++) {
+      LdbState* js = d->tables[k];
+      if (k == eachTable && js && js->kind == LDB_STATE_JOIN_TABLE && !(js->join.stride == 8 || js->join.direct))
+         failP(LDB_ERR_UNSUPPORTED, "PROBE_EACH takes a plain single-key or direct-address join table (not a pair table or a group-join map)");
+      if (!js || js->kind != LDB_STATE_JOIN_TABLE || js->join.stride == 16) failP(LDB_ERR_INVALID, "PROBE tables are single-key join tables");
+      base.tables[k] = js->join;
+   }
+   base.filterReg = d->filter_reg;
+   if (d->filter_reg >= 0) wantReg(d->filter_reg, "filter");
+   base.sinkKind = d->sink_kind;
+   LdbState* sink = d->sink;
+   std::vector<void*> outOwned;
+   std::vector<uint8_t*> outVals, outValid;
+   unsigned long long* outCount = nullptr;
+   // materialize output buffers for `rows` rows (+ the row counter)
+   auto allocOut = [&](size_t rows) {
+      for (void* q : outOwned) ctx->stagingRelease(q);
+      outOwned.clear();
+      outVals.clear();
+      outValid.clear();
+      for (int c = 0; c < d->n_out; c++) {
+         outVals.push_back((uint8_t*) ctx->stagingAlloc(rows * 16));
+         outValid.push_back((uint8_t*) ctx->stagingAlloc(rows));
+         outOwned.push_back(outVals.back());
+         outOwned.push_back(outValid.back());
+         base.outValues[c] = outVals.back();
+         base.outValid[c] = outValid.back();
+      }
+      outCount = (unsigned long long*) ctx->stagingAlloc(8);
+      outOwned.push_back(outCount);
+      LDB_CUDA(cudaMemsetAsync(outCount, 0, 8, ctx->compute));
+      base.outCapacity = (int64_t) rows;
+      base.outCount = outCount;
+   };
+   if (d->sink_kind == LDB_SINK_HASHAGG) {
+      checkHashAgg(sink);
+      if (sink->ctx != ctx || d->n_keys != sink->hashagg.nKeys || d->n_aggs != sink->hashagg.nAggs) failP(LDB_ERR_INVALID, "key / aggregate count differs from the state's");
+      base.nKeys = d->n_keys;
+      base.nAggs = d->n_aggs;
+      for (int k = 0; k < d->n_keys; k++) {
+         wantReg(d->key_regs[k], "group key");
+         base.keyReg[k] = d->key_regs[k];
+      }
+      for (int a = 0; a < d->n_aggs; a++) {
+         if (d->aggs[a].kind != sink->aggKinds[a]) failP(LDB_ERR_INVALID, "aggregate kind differs from the state's");
+         if (d->aggs[a].kind != LDB_AGG_COUNT_STAR) wantReg(d->aggs[a].reg, "aggregate input");
+         base.aggs[a] = ProgAgg{d->aggs[a].kind, d->aggs[a].reg};
+      }
+      base.agg = sink->hashagg;
+   } else if (d->sink_kind == LDB_SINK_JOIN_BUILD) {
+      if (!sink || sink->kind != LDB_STATE_JOIN_TABLE || sink->join.stride != 8 || sink->join.direct) failP(LDB_ERR_INVALID, "build sink must be a plain single-key join table");
+      if (usesRowid && t->numRows > (int64_t) INT32_MAX) failP(LDB_ERR_UNSUPPORTED, "ROWID build payloads are int32: the source has 2^31 rows or more");
+      wantReg(d->build_key_reg, "build key");
+      if (d->build_payload_reg >= 0) wantReg(d->build_payload_reg, "build payload");
+      base.buildKeyReg = d->build_key_reg;
+      base.buildPayloadReg = d->build_payload_reg;
+      base.build = sink->join;
+   } else if (d->sink_kind == LDB_SINK_MATERIALIZE) {
+      if (d->n_out < 1 || d->n_out > kProgMaxAggs || !d->out_table) failP(LDB_ERR_INVALID, "materialize needs 1..8 output registers and out_table");
+      base.nOut = d->n_out;
+      for (int c = 0; c < d->n_out; c++) {
+         wantReg(d->out_regs[c], "output");
+         base.outReg[c] = d->out_regs[c];
+      }
+      allocOut((size_t) std::max<int64_t>(t->numRows, 1));
+   } else {
+      failP(LDB_ERR_INVALID, "unknown sink kind");
+   }
+   // side columns: bound once for all batches of the source; a multi-batch side table through a device-resident batch directory
+   std::vector<void*> dirs;
+   for (int c = d->n_columns; c < nCols; c++) {
+      LdbTable* st = colTable[c];
+      ProgCol& pc = base.cols[c];
+      pc.type = colType(c);
+      pc.rowReg = rowReg[c];
+      std::vector<ProgSideBatch> dir;
+      int64_t first = 0;
+      const LdbBatch* only = nullptr;
+      for (auto& b : st->batches) {
+         ldb_gpu_wait_batch_internal(ctx, &b);
+         if (b.nRows > 0) {
+            ProgCol one{};
+            bindColumn(one, b, colIdx[c]);
+            dir.push_back(ProgSideBatch{one.data, one.bytes, one.validity, one.validBytes, one.bitOffset, first, one.elemBytes, 0});
+            only = &b;
          }
-         written[in.dst] = true;
-         base.instr[i] = ProgInstr{in.op, in.dst, in.a, in.b, in.arg};
+         first += b.nRows;
       }
-      for (int c = 0; c < d->n_consts; c++) {
-         base.constLo[c] = d->consts[c].lo;
-         base.constHi[c] = d->consts[c].hi;
+      pc.sideRows = first;
+      pc.nBatches = (int32_t) dir.size();
+      if (dir.size() == 1) {
+         bindColumn(pc, *only, colIdx[c]);
+      } else if (dir.size() > 1) {
+         void* dd = ctx->stagingAlloc(dir.size() * sizeof(ProgSideBatch));
+         dirs.push_back(dd);
+         LDB_CUDA(cudaMemcpyAsync(dd, dir.data(), dir.size() * sizeof(ProgSideBatch), cudaMemcpyHostToDevice, ctx->compute));
+         pc.dir = (const ProgSideBatch*) dd;
       }
-      for (int c = 0; c < d->n_strings; c++) {
-         const size_t n = d->strings[c] ? strlen(d->strings[c]) : 0;
-         if (n > (size_t) kProgStringBytes) failP(LDB_ERR_UNSUPPORTED, "string constant longer than 32 bytes");
-         memcpy(base.strings[c], d->strings[c], n);
-         base.stringLen[c] = (int32_t) n;
-      }
-      for (int k = 0; k < d->n_tables; k++) {
-         LdbState* js = d->tables[k];
-         if (!js || js->kind != LDB_STATE_JOIN_TABLE || js->join.stride == 16) failP(LDB_ERR_INVALID, "PROBE tables are single-key join tables");
-         base.tables[k] = js->join;
-      }
-      base.filterReg = d->filter_reg;
-      if (d->filter_reg >= 0) wantReg(d->filter_reg, "filter");
-      base.sinkKind = d->sink_kind;
-      LdbState* sink = d->sink;
-      std::vector<void*> outOwned;
-      std::vector<uint8_t*> outVals, outValid;
-      unsigned long long* outCount = nullptr;
-      if (d->sink_kind == LDB_SINK_HASHAGG) {
-         checkHashAgg(sink);
-         if (sink->ctx != ctx || d->n_keys != sink->hashagg.nKeys || d->n_aggs != sink->hashagg.nAggs) failP(LDB_ERR_INVALID, "key / aggregate count differs from the state's");
-         base.nKeys = d->n_keys;
-         base.nAggs = d->n_aggs;
-         for (int k = 0; k < d->n_keys; k++) {
-            wantReg(d->key_regs[k], "group key");
-            base.keyReg[k] = d->key_regs[k];
-         }
-         for (int a = 0; a < d->n_aggs; a++) {
-            if (d->aggs[a].kind != sink->aggKinds[a]) failP(LDB_ERR_INVALID, "aggregate kind differs from the state's");
-            if (d->aggs[a].kind != LDB_AGG_COUNT_STAR) wantReg(d->aggs[a].reg, "aggregate input");
-            base.aggs[a] = ProgAgg{d->aggs[a].kind, d->aggs[a].reg};
-         }
-         base.agg = sink->hashagg;
-      } else if (d->sink_kind == LDB_SINK_JOIN_BUILD) {
-         if (!sink || sink->kind != LDB_STATE_JOIN_TABLE || sink->join.stride != 8 || sink->join.direct) failP(LDB_ERR_INVALID, "build sink must be a plain single-key join table");
-         wantReg(d->build_key_reg, "build key");
-         if (d->build_payload_reg >= 0) wantReg(d->build_payload_reg, "build payload");
-         base.buildKeyReg = d->build_key_reg;
-         base.buildPayloadReg = d->build_payload_reg;
-         base.build = sink->join;
-      } else if (d->sink_kind == LDB_SINK_MATERIALIZE) {
-         if (d->n_out < 1 || d->n_out > kProgMaxAggs || !d->out_table) failP(LDB_ERR_INVALID, "materialize needs 1..8 output registers and out_table");
-         const size_t rows = (size_t) std::max<int64_t>(t->numRows, 1);
-         base.nOut = d->n_out;
-         for (int c = 0; c < d->n_out; c++) {
-            wantReg(d->out_regs[c], "output");
-            base.outReg[c] = d->out_regs[c];
-            outVals.push_back((uint8_t*) ctx->stagingAlloc(rows * 16));
-            outValid.push_back((uint8_t*) ctx->stagingAlloc(rows));
-            outOwned.push_back(outVals.back());
-            outOwned.push_back(outValid.back());
-            base.outValues[c] = outVals.back();
-            base.outValid[c] = outValid.back();
-         }
-         outCount = (unsigned long long*) ctx->stagingAlloc(8);
-         outOwned.push_back(outCount);
-         LDB_CUDA(cudaMemsetAsync(outCount, 0, 8, ctx->compute));
-         base.outCapacity = (int64_t) rows;
-         base.outCount = outCount;
-      } else {
-         failP(LDB_ERR_INVALID, "unknown sink kind");
-      }
+   }
+   for (int c = 0; c < d->n_columns; c++) base.cols[c].rowReg = -1;
+   auto runBatches = [&] {
+      int64_t first = 0;
       for (auto& b : t->batches) {
+         const int64_t firstRow = first;
+         first += b.nRows;
          if (b.nRows == 0) continue;
          ProgramParams p = base;
          p.nRows = b.nRows;
+         p.firstRow = firstRow;
          for (int c = 0; c < d->n_columns; c++) {
             const int ci = colIdx[c];
-            ProgCol& pc = p.cols[c];
-            pc.data = (const uint8_t*) b.data[ci];
-            pc.bytes = (const uint8_t*) b.bytes[ci];
-            pc.type = t->columns[ci].type;
-            pc.elemBytes = b.elemBytes[ci];
-            pc.validity = ci < (int) b.validity.size() ? (const uint8_t*) b.validity[ci] : nullptr;
-            pc.bitOffset = ci < (int) b.validityBitOffset.size() ? b.validityBitOffset[ci] : 0;
-            pc.validBytes = ci < (int) b.validBytes.size() ? b.validBytes[ci] : nullptr;
+            p.cols[c].type = t->columns[ci].type;
+            bindColumn(p.cols[c], b, ci);
          }
          ldb_gpu_wait_batch_internal(ctx, &b);
          ctx->launch("program", [&] { launchProgram(p, ctx->smCount, ctx->compute); });
       }
-      if (d->sink_kind == LDB_SINK_MATERIALIZE) {
-         unsigned long long n = 0;
+   };
+   runBatches();
+   if (eachTable >= 0) { // a probe run longer than the bound: fail rather than return a truncated match list
+      int32_t e = 0;
+      LDB_CUDA(cudaMemcpyAsync(&e, base.tables[eachTable].error, 4, cudaMemcpyDeviceToHost, ctx->compute));
+      ctx->syncStream(ctx->compute);
+      if (e == 6) {
+         for (void* q : outOwned) ctx->stagingRelease(q);
+         for (void* q : dirs) ctx->stagingRelease(q);
+         failP(LDB_ERR_CAPACITY, "PROBE_EACH: a probe run is longer than the interpreter's bound of 16384 slots (an overfull join table)");
+      }
+   }
+   if (d->sink_kind == LDB_SINK_MATERIALIZE) {
+      unsigned long long n = 0;
+      LDB_CUDA(cudaMemcpyAsync(&n, outCount, 8, cudaMemcpyDeviceToHost, ctx->compute));
+      ctx->syncStream(ctx->compute);
+      if (n > (unsigned long long) base.outCapacity) { // PROBE_EACH produced more rows than the source has: regrow and run once more
+         allocOut((size_t) n);
+         runBatches();
          LDB_CUDA(cudaMemcpyAsync(&n, outCount, 8, cudaMemcpyDeviceToHost, ctx->compute));
          ctx->syncStream(ctx->compute);
-         auto* ot = new LdbTable;
-         ot->ctx = ctx;
-         ot->name = t->name + "_out";
-         LdbBatch ob;
-         ob.nRows = (int64_t) n;
-         for (int c = 0; c < d->n_out; c++) {
-            ot->columns.push_back({"c" + std::to_string(c), LDB_DECIMAL128, 38, 0});
-            ob.data.push_back(outVals[c]);
-            ob.bytes.push_back(nullptr);
-            ob.elemBytes.push_back(16);
-            ob.validBytes.push_back(outValid[c]);
-         }
-         ob.validity.assign(ob.data.size(), nullptr);
-         ob.validityBitOffset.assign(ob.data.size(), 0);
-         ob.owned = outOwned;
-         ot->numRows = (int64_t) n;
-         ot->batches.push_back(std::move(ob));
-         ctx->tables.push_back(ot);
-         *d->out_table = ot;
+         if (n > (unsigned long long) base.outCapacity) failP(LDB_ERR_INVALID, "materialize: the rerun produced more rows than the first run");
       }
-   });
+      auto* ot = new LdbTable;
+      ot->ctx = ctx;
+      ot->name = t->name + "_out";
+      LdbBatch ob;
+      ob.nRows = (int64_t) n;
+      for (int c = 0; c < d->n_out; c++) {
+         ot->columns.push_back({"c" + std::to_string(c), LDB_DECIMAL128, 38, 0});
+         ob.data.push_back(outVals[c]);
+         ob.bytes.push_back(nullptr);
+         ob.elemBytes.push_back(16);
+         ob.validBytes.push_back(outValid[c]);
+      }
+      ob.validity.assign(ob.data.size(), nullptr);
+      ob.validityBitOffset.assign(ob.data.size(), 0);
+      ob.owned = outOwned;
+      ot->numRows = (int64_t) n;
+      ot->batches.push_back(std::move(ob));
+      ctx->tables.push_back(ot);
+      *d->out_table = ot;
+   }
+   if (!dirs.empty()) {
+      ctx->syncStream(ctx->compute); // the batch directories are read until the last launch ends
+      for (void* q : dirs) ctx->stagingRelease(q);
+   }
+}
+
+int ldb_gpu_run_program(LdbContext* ctx, const LdbProgramDesc* d, LdbError* err) {
+   return guardedP(err, [&] { runProgram(ctx, d, nullptr); });
+}
+int ldb_gpu_run_program_ex(LdbContext* ctx, const LdbProgramDesc* d, const LdbProgramJoins* joins, LdbError* err) {
+   return guardedP(err, [&] { runProgram(ctx, d, joins); });
 }
 
 // ---------------------------------------------------------------- ORDER BY … LIMIT and result gather

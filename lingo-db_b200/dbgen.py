@@ -115,9 +115,11 @@ def _categorical_utf8(idx: np.ndarray, names):
     return offs, np.frombuffer(b"".join(enc[i] for i in idx.tolist()), dtype=np.uint8).copy()
 
 
-def tpch(sf: float = 1.0, chunk_rows: int = 1 << 20, extended: bool = False) -> Dict[str, TableData]:
+def tpch(sf: float = 1.0, chunk_rows: int = 1 << 20, extended: bool = False, attributes: bool = False) -> Dict[str, TableData]:
     """extended=True adds orders.o_orderpriority, orders.o_totalprice, lineitem.l_shipmode and customer.c_name — the columns the
-    Q4 / Q12 / Q18 twins of the oracle read."""
+    Q4 / Q12 / Q18 twins of the oracle read.  attributes=True adds part.p_mfgr / p_brand / p_type / p_container (utf8) and p_size,
+    partsupp.ps_availqty, supplier.s_acctbal (decimal(12,2)) and lineitem.l_shipinstruct (utf8), from part_attributes,
+    balances_and_quantities and extra_columns — the columns Q2, Q8, Q11, Q14, Q17, Q19 and Q20 read."""
     n_o, n_c, n_s, n_p = int(1500000 * sf), int(150000 * sf), int(10000 * sf), int(200000 * sf)
     # ---- orders
     idx = np.arange(1, n_o + 1, dtype=np.int64)
@@ -182,6 +184,7 @@ def tpch(sf: float = 1.0, chunk_rows: int = 1 << 20, extended: bool = False) -> 
     partsupp = {"ps_partkey": pp.astype(np.int32), "ps_suppkey": part_supplier(pp, jj, n_s).astype(np.int32),
                 "ps_supplycost": _dec128(unif(stream(SEED["ps_supplycost"], 4 * n_p), 100, 100000))}
     li_schema, od_schema, cu_schema = list(LINEITEM_SCHEMA), list(ORDERS_SCHEMA), list(CUSTOMER_SCHEMA)
+    su_schema, pa_schema, ps_schema = list(SUPPLIER_SCHEMA), list(PART_SCHEMA), list(PARTSUPP_SCHEMA)
     if extended:
         from .datagen import ColumnSpec
         x = extra_columns(sf, lcnt)
@@ -198,9 +201,24 @@ def tpch(sf: float = 1.0, chunk_rows: int = 1 << 20, extended: bool = False) -> 
         od_schema.append(ColumnSpec("o_totalprice", "decimal128", 12, 2))
         customer["c_name"] = _utf8(["Customer#%09d" % k for k in range(1, n_c + 1)])
         cu_schema.append(ColumnSpec("c_name", "utf8"))
+    if attributes:
+        from .datagen import ColumnSpec
+        pa, bq = part_attributes(sf), balances_and_quantities(sf)
+        part["p_mfgr"] = _utf8(["Manufacturer#%d" % (b // 10) for b in pa["p_brand"].tolist()])
+        part["p_brand"] = _utf8(["Brand#%d" % b for b in pa["p_brand"].tolist()])
+        part["p_type"] = _categorical_utf8(pa["p_type"], [type_name(i) for i in range(150)])
+        part["p_size"] = pa["p_size"]
+        part["p_container"] = _categorical_utf8(pa["p_container"], [f"{a} {b}" for a in CONTAINER_SYLLABLES[0] for b in CONTAINER_SYLLABLES[1]])
+        pa_schema += [ColumnSpec("p_mfgr", "utf8"), ColumnSpec("p_brand", "utf8"), ColumnSpec("p_type", "utf8"), ColumnSpec("p_size", "int32"), ColumnSpec("p_container", "utf8")]
+        partsupp["ps_availqty"] = bq["ps_availqty"].astype(np.int32)
+        ps_schema.append(ColumnSpec("ps_availqty", "int32"))
+        supplier["s_acctbal"] = _dec128(bq["s_acctbal"])
+        su_schema.append(ColumnSpec("s_acctbal", "decimal128", 12, 2))
+        lineitem["l_shipinstruct"] = _categorical_utf8(extra_columns(sf, lcnt)["l_shipinstruct"], SHIP_INSTRUCTIONS)
+        li_schema.append(ColumnSpec("l_shipinstruct", "utf8"))
     return {"lineitem": _chunked("lineitem", li_schema, lineitem, n_l, chunk_rows), "orders": _chunked("orders", od_schema, orders, n_o, chunk_rows),
-            "customer": _chunked("customer", cu_schema, customer, n_c, chunk_rows), "supplier": _chunked("supplier", SUPPLIER_SCHEMA, supplier, n_s, chunk_rows),
-            "part": _chunked("part", PART_SCHEMA, part, n_p, chunk_rows), "partsupp": _chunked("partsupp", PARTSUPP_SCHEMA, partsupp, 4 * n_p, chunk_rows),
+            "customer": _chunked("customer", cu_schema, customer, n_c, chunk_rows), "supplier": _chunked("supplier", su_schema, supplier, n_s, chunk_rows),
+            "part": _chunked("part", pa_schema, part, n_p, chunk_rows), "partsupp": _chunked("partsupp", ps_schema, partsupp, 4 * n_p, chunk_rows),
             "nation": nation(), "region": region()}
 
 

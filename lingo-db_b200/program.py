@@ -10,6 +10,12 @@ An expression is a nested tuple:
   ("strcmp", op, column, "constant") ("like", "prefix"|"suffix"|"contains", column, "text") ("strkey8", column)
   ("year", a)                                                extract(year from date32)
   ("probe", join_table_state, key)                           payload, or NULL when the key is absent (semi / anti / mark / outer joins)
+  ("probe_each", join_table_state, key[, "outer"])           payload of EACH match: what follows runs once per match (inner join; "outer":
+                                                             a row without a match yields one tuple with a NULL payload).  At most one
+                                                             per program; emitted once, never re-evaluated.
+  ("rowid",)                                                 the scanned row's number in its table (a build payload for "fetch")
+  ("fetch", side_table, row, "column")                       `column` of another table at the row `row` evaluates to (NULL row → NULL);
+                                                             accepted wherever a column name is, also as the column of strcmp / like / strkey8
 This is test/bench plumbing over the C-ABI, like runtime.py; in a LingoDB build the sub-operator lowering would emit LdbInstr lists."""
 import ctypes as C
 import struct
@@ -19,7 +25,7 @@ from . import capi
 from .capi import Error, check
 
 OPS = dict(load=1, const=2, add=3, sub=4, mul=5, div=6, neg=7, cmp=8, **{"and": 9, "or": 10, "not": 11}, isnull=12, select=13, i2f=14, fadd=15, fsub=16, fmul=17,
-           fdiv=18, fcmp=19, strcmp=20, strlike=21, year=22, probe=23, strkey8=24)
+           fdiv=18, fcmp=19, strcmp=20, strlike=21, year=22, probe=23, strkey8=24, rowid=25, probe_each=26)
 CMP = {"=": 0, "!=": 1, "<": 2, "<=": 3, ">": 4, ">=": 5}
 AGG = dict(sum=1, sum_f64=2, count=3, count_star=4, min=5, max=6, min_f64=7, max_f64=8, any=9)
 LIKE = dict(prefix=0, suffix=1, contains=2)
@@ -29,7 +35,8 @@ SINK_HASHAGG, SINK_JOIN_BUILD, SINK_MATERIALIZE = 1, 2, 3
 class Builder:
     def __init__(self):
         self.instr, self.columns, self.consts, self.strings, self.tables = [], [], [], [], []
-        self._cache, self._next = {}, 0
+        self.side_tables, self.side_columns = [], []  # side tables (handles); side columns as (side table index, column, row register)
+        self._cache, self._rows, self._next, self._each = {}, {}, 0, None
 
     def _reg(self):
         r = self._next
@@ -39,9 +46,37 @@ class Builder:
         return r
 
     def _col(self, name):
+        """Column operand: a source column name, or a ("fetch", side_table, row, "column") side column.  Side columns come after
+        the source columns, whose number is only known at the end: until instructions() they are numbered -1, -2, …"""
+        if isinstance(name, tuple):
+            if name[0] != "fetch":
+                raise ValueError(f"not a column: {name[0]}")
+            h = _handle(name[1])
+            if h not in self.side_tables:
+                self.side_tables.append(h)
+            rk = repr(name[2])  # columns fetched through the same row expression share its register (and its probe)
+            if rk not in self._rows:
+                self._rows[rk] = self.expr(name[2])
+            sc = (self.side_tables.index(h), name[3], self._rows[rk])
+            if sc not in self.side_columns:
+                self.side_columns.append(sc)
+            return -1 - self.side_columns.index(sc)
         if name not in self.columns:
             self.columns.append(name)
         return self.columns.index(name)
+
+    def instructions(self):
+        """The LdbInstr tuples with side columns numbered after the source columns."""
+        n = len(self.columns)
+        fix = lambda c: n - 1 - c if c < 0 else c
+        out = []
+        for op, dst, a, b, arg in self.instr:
+            if op == OPS["load"]:
+                arg = fix(arg)
+            elif op in (OPS["strcmp"], OPS["strlike"], OPS["strkey8"]):
+                a = fix(a)
+            out.append((op, dst, a, b, arg))
+        return out
 
     def _emit(self, op, a=0, b=0, arg=0):
         r = self._reg()
@@ -66,6 +101,18 @@ class Builder:
         k = e[0]
         if k == "col":
             r = self._emit("load", arg=self._col(e[1]))
+        elif k == "fetch":
+            r = self._emit("load", arg=self._col(e))
+        elif k == "rowid":
+            r = self._emit("rowid")
+        elif k == "probe_each":
+            if self._each is not None:
+                raise ValueError("at most one probe_each per program")
+            if e[1] not in self.tables:
+                self.tables.append(e[1])
+            outer = len(e) > 3 and e[3] == "outer"
+            r = self._emit("probe_each", self.expr(e[2]), int(outer), self.tables.index(e[1]))
+            self._each = r
         elif k == "const":
             r = self._emit("const", arg=self._const(int(e[1])))
         elif k == "f64":
@@ -107,7 +154,7 @@ def _desc(ctx, table, b: Builder, filter_reg: int):
     cols = [c.encode() for c in b.columns]
     arr = (C.c_char_p * max(1, len(cols)))(*cols)
     d.n_columns, d.columns = len(cols), arr
-    ins = (capi.Instr * max(1, len(b.instr)))(*[capi.Instr(*i) for i in b.instr])
+    ins = (capi.Instr * max(1, len(b.instr)))(*[capi.Instr(*i) for i in b.instructions()])
     d.n_instr, d.instr = len(b.instr), ins
     cs = (capi.I128 * max(1, len(b.consts)))(*[capi.I128(v & 0xFFFFFFFFFFFFFFFF, (v >> 64) - (1 << 64 if v >> 127 else 0)) for v in b.consts])
     d.n_consts, d.consts = len(b.consts), cs
@@ -119,6 +166,26 @@ def _desc(ctx, table, b: Builder, filter_reg: int):
     d.filter_reg = filter_reg
     keep += [cols, arr, ins, cs, ss, sarr, tarr]
     return d, keep
+
+
+def _handle(t):
+    h = getattr(t, "h", t)
+    return h.value if isinstance(h, C.c_void_p) else h
+
+
+def _run(ctx, d, b: Builder):
+    """ldb_gpu_run_program, or ldb_gpu_run_program_ex when the program reads side columns."""
+    e = Error()
+    if not b.side_columns:
+        check(ctx.L.ldb_gpu_run_program(ctx.h, C.byref(d), C.byref(e)), e)
+        return
+    names = [c.encode() for _, c, _ in b.side_columns]
+    j = capi.ProgramJoins()
+    tarr = (C.c_void_p * len(b.side_tables))(*b.side_tables)
+    sarr = (capi.SideColumn * len(b.side_columns))(*[capi.SideColumn(t, n, r) for (t, _, r), n in zip(b.side_columns, names)])
+    j.n_side_tables, j.side_tables = len(b.side_tables), tarr
+    j.n_side_columns, j.side_columns = len(b.side_columns), sarr
+    check(ctx.L.ldb_gpu_run_program_ex(ctx.h, C.byref(d), C.byref(j), C.byref(e)), e)
 
 
 def hashagg_state(ctx, n_keys: int, agg_kinds: List[str], expected_groups: int) -> C.c_void_p:
@@ -143,8 +210,7 @@ def group_by(ctx, table, keys: list, aggs: list, where=None, expected_groups: in
     d.n_aggs = len(aggs)
     for i, ((kind, _), r) in enumerate(zip(aggs, aregs)):
         d.aggs[i] = capi.ProgAgg(AGG[kind], r)
-    e = Error()
-    check(ctx.L.ldb_gpu_run_program(ctx.h, C.byref(d), C.byref(e)), e)
+    _run(ctx, d, b)
     return st
 
 
@@ -186,8 +252,7 @@ def build_join(ctx, table, join_state, key, payload=None, where=None):
     d, keep = _desc(ctx, table, b, f)
     d.sink_kind, d.sink = SINK_JOIN_BUILD, join_state
     d.build_key_reg, d.build_payload_reg = kr, pr
-    e = Error()
-    check(ctx.L.ldb_gpu_run_program(ctx.h, C.byref(d), C.byref(e)), e)
+    _run(ctx, d, b)
 
 
 def materialize(ctx, table, outs: list, where=None) -> C.c_void_p:
@@ -202,8 +267,7 @@ def materialize(ctx, table, outs: list, where=None) -> C.c_void_p:
         d.out_regs[i] = r
     out = C.c_void_p()
     d.out_table = C.pointer(out)
-    e = Error()
-    check(ctx.L.ldb_gpu_run_program(ctx.h, C.byref(d), C.byref(e)), e)
+    _run(ctx, d, b)
     return out
 
 
