@@ -362,8 +362,10 @@ enum LdbOp {
    LDB_OP_STRLIKE = 21,/* dst = columns[a] LIKE strings[arg]; b = 0 'x%', 1 '%x', 2 '%x%' */
    LDB_OP_YEAR = 22,   /* dst = extract(year from date32 a) */
    LDB_OP_PROBE = 23,  /* dst = payload of int32 key a in tables[arg]; NULL when absent */
-   LDB_OP_STRKEY8 = 24,/* dst = first 8 bytes of columns[a], zero padded, big-endian (an order-preserving int64 group / sort key for short
-                          strings: char(n<=8), flags, codes; longer strings need a dictionary and are not keys here) */
+   LDB_OP_STRKEY8 = 24,/* dst = first 8 bytes of columns[a], zero padded, big-endian, as a signed int64 (a group / sort key for short
+                          strings: char(n<=8), flags, codes; longer strings need a dictionary and are not keys here).  It preserves the
+                          bytewise string order only while the first byte is below 0x80 (7-bit text): a first byte >= 0x80 makes the
+                          key negative, so such strings order before ASCII ones. */
    LDB_OP_ROWID = 25,  /* dst = global row number of the scanned row in its table (a row-id build payload for side-column reads) */
    LDB_OP_PROBE_EACH = 26 /* dst = payload of EACH match of int32 key a in tables[arg] (plain single-key or direct-address tables); the
                              instructions after it, the filter and the sink run once per match.  b = 0 inner join (no match: no tuple),
@@ -371,7 +373,8 @@ enum LdbOp {
                              program; later instructions may not overwrite registers written at or before it.  A probe run longer
                              than the interpreter's bound fails the call (LDB_ERR_CAPACITY) rather than dropping matches. */
 };
-enum LdbAggKind { LDB_AGG_SUM = 1, LDB_AGG_SUM_F64 = 2, LDB_AGG_COUNT = 3, LDB_AGG_COUNT_STAR = 4, LDB_AGG_MIN = 5, LDB_AGG_MAX = 6 /* 64-bit signed */,
+/* SUM wraps at 128 bits; MIN / MAX compare signed 128-bit values; the _F64 kinds work on doubles */
+enum LdbAggKind { LDB_AGG_SUM = 1, LDB_AGG_SUM_F64 = 2, LDB_AGG_COUNT = 3, LDB_AGG_COUNT_STAR = 4, LDB_AGG_MIN = 5, LDB_AGG_MAX = 6,
                   LDB_AGG_MIN_F64 = 7, LDB_AGG_MAX_F64 = 8, LDB_AGG_ANY = 9 };
 typedef struct LdbInstr {
    uint8_t op, dst, a, b;
@@ -402,7 +405,10 @@ typedef struct LdbProgramDesc {
    int32_t key_regs[LDB_PROG_MAX_KEYS];
    int32_t n_aggs;
    LdbProgAgg aggs[LDB_MAX_AGGS];
-   int32_t build_key_reg, build_payload_reg; /* JOIN_BUILD: payload_reg -1 = 0 */
+   /* JOIN_BUILD: payload_reg -1 = 0.  Rows with a NULL key are not inserted; a NULL payload is stored as 0.  The call fails when a
+    * row could not be stored: a non-NULL key or payload outside int32 (LDB_ERR_UNSUPPORTED), a table smaller than the build side
+    * (LDB_ERR_CAPACITY), the reserved pair key -1 / payload -1 (LDB_ERR_UNSUPPORTED). */
+   int32_t build_key_reg, build_payload_reg;
    /* MATERIALIZE: out_regs → a new DEVICE table (columns "c0".."cN": decimal128(38,0) cells = the raw i128 / double bits in the
     * low 8 bytes, each with a validity byte); capacity = source rows, regrown to the produced row count (one more run of the
     * program) when a PROBE_EACH yields more tuples than that */

@@ -222,3 +222,7 @@ struct LdbState {
    uint32_t is64Mask = 0; // aggregates that are 64-bit sums (COL / ONE): normalised to a sign-extended i64 on read
    std::vector<void*> allocations;
 };
+
+// reads a join table's error word (synchronises the compute stream) and throws ApiError with the status and message of a
+// non-zero code (runtime.cpp); every caller that reports a join table's failure goes through it
+void ldb_gpu_check_join_error_internal(LdbState* s);

@@ -44,6 +44,17 @@ struct Val {
 __device__ __forceinline__ double asF64(const Val& x) { return __longlong_as_double((long long) (uint64_t) x.v); }
 __device__ __forceinline__ Val fromF64(double d, bool null) { return Val{(s128) (uint64_t) __double_as_longlong(d), null}; }
 
+// yearOfDays for EVERY date32 value: the same civil-from-days steps in 64-bit arithmetic (days + 719468 leaves int32 for dates past
+// the year 5 879 609; the specialised kernels only see TPC-H dates and keep the 32-bit form)
+__device__ __forceinline__ int64_t yearOfDaysWide(int32_t days) {
+   const int64_t z = (int64_t) days + 719468;
+   const int64_t era = (z >= 0 ? z : z - 146096) / 146097;
+   const int64_t doe = z - era * 146097;
+   const int64_t yoe = (doe - doe / 1460 + doe / 36524 - doe / 146096) / 365;
+   const int64_t doy = doe - (365 * yoe + yoe / 4 - yoe / 100);
+   const int64_t mp = (5 * doy + 2) / 153;
+   return yoe + era * 400 + (mp >= 10 ? 1 : 0);
+}
 __device__ __forceinline__ bool colIsNull(const ProgCol& c, int64_t row) {
    if (c.validBytes) return c.validBytes[row] == 0;
    if (!c.validity) return false;
@@ -61,8 +72,9 @@ __device__ __forceinline__ Val loadCol(const ProgCol& c, int64_t row) {
       case LDB_INT64: r.v = (s128) ((const int64_t*) c.data)[row]; break;
       case LDB_INT8: r.v = (s128) ((const int8_t*) c.data)[row]; break;
       case LDB_INT16: r.v = (s128) ((const int16_t*) c.data)[row]; break;
-      case LDB_FLOAT32: return fromF64((double) ((const float*) c.data)[row], r.null);
-      case LDB_FLOAT64: return fromF64(((const double*) c.data)[row], r.null);
+      // at the column's cell width: exported float aggregates keep 16-byte cells (the double's bits in the low 8 bytes)
+      case LDB_FLOAT32: return fromF64((double) *(const float*) (c.data + (size_t) row * c.elemBytes), r.null);
+      case LDB_FLOAT64: return fromF64(*(const double*) (c.data + (size_t) row * c.elemBytes), r.null);
       case LDB_DECIMAL128:
          if (c.elemBytes == 16) {
             const ulonglong2 cell = ((const ulonglong2*) c.data)[row];
@@ -209,8 +221,11 @@ __device__ uint8_t* hashAggFind(const ProgramParams& p, const int64_t* keys, uin
             for (int a = 0; a < t.nAggs; a++) {
                unsigned long long lo = 0, hi = 0;
                switch (p.aggs[a].kind) {
-                  case LDB_AGG_MIN: lo = (unsigned long long) INT64_MAX; break;
-                  case LDB_AGG_MAX: lo = (unsigned long long) INT64_MIN; break;
+                  case LDB_AGG_MIN: // INT128_MAX
+                     lo = ~0ull;
+                     hi = ~0ull >> 1;
+                     break;
+                  case LDB_AGG_MAX: hi = 1ull << 63; break; // INT128_MIN
                   case LDB_AGG_MIN_F64: lo = (unsigned long long) __double_as_longlong(INFINITY); break;
                   case LDB_AGG_MAX_F64: lo = (unsigned long long) __double_as_longlong(-INFINITY); break;
                   default: break;
@@ -236,6 +251,21 @@ __device__ uint8_t* hashAggFind(const ProgramParams& p, const int64_t* keys, uin
    atomicExch(t.error, 1);
    return nullptr;
 }
+// exact MIN / MAX of a 16-byte aggregate cell: a 16-byte compare-and-swap loop (one atomic per update when uncontended, like the
+// 8-byte atomicMin it replaces).  The plain read is only the first guess of the CAS: its two 8-byte halves may come from different
+// updates, so a "not better" decision taken on it alone could drop a value.  The loop ends on a CAS that either installs x or
+// confirms (by rewriting the same value) that the cell already holds one at least as good.
+__device__ __forceinline__ void atomicMinMax128(unsigned long long* cell, s128 x, bool isMax) {
+   unsigned __int128* p = (unsigned __int128*) cell; // 16-byte aligned: entries are 48 + 16 nAggs bytes from an aligned base
+   const volatile unsigned long long* vc = cell;
+   unsigned __int128 cur = ((unsigned __int128) vc[1] << 64) | vc[0];
+   while (true) {
+      const bool better = isMax ? x > (s128) cur : x < (s128) cur;
+      const unsigned __int128 prev = atomicCAS(p, cur, better ? (unsigned __int128) x : cur);
+      if (prev == cur) return;
+      cur = prev;
+   }
+}
 // in-place aggregate update (subop.reduce lowering + combine functions, SubOpToControlFlow.cpp:3540-3769, RelAlgToSubOp.cpp:1809-2025):
 // NULL inputs are skipped, an aggregate that never saw a value stays NULL (its "seen" bit)
 __device__ void hashAggUpdate(const ProgramParams& p, uint8_t* e, const Val* regs) {
@@ -255,8 +285,8 @@ __device__ void hashAggUpdate(const ProgramParams& p, uint8_t* e, const Val* reg
          case LDB_AGG_SUM: atomicAdd128(lo, lo + 1, i128{(uint64_t) x.v, (int64_t) (x.v >> 64)}); break;
          case LDB_AGG_SUM_F64: atomicAdd((double*) lo, asF64(x)); break;
          case LDB_AGG_COUNT: atomicAdd(lo, 1ull); break;
-         case LDB_AGG_MIN: atomicMin((long long*) lo, (long long) x.v); break;
-         case LDB_AGG_MAX: atomicMax((long long*) lo, (long long) x.v); break;
+         case LDB_AGG_MIN:
+         case LDB_AGG_MAX: atomicMinMax128(lo, x.v, kind == LDB_AGG_MAX); break;
          case LDB_AGG_MIN_F64:
          case LDB_AGG_MAX_F64: {
             const double d = asF64(x);
@@ -375,7 +405,7 @@ __global__ void __launch_bounds__(256) programKernel(const __grid_constant__ Pro
                      if (!r.null) r.v = strLike(*c, at, p.strings[in.arg], p.stringLen[in.arg], in.b);
                      break;
                   }
-                  case LDB_OP_YEAR: r.v = (s128) yearOfDays((int32_t) a.v); r.null = a.null; break;
+                  case LDB_OP_YEAR: r.v = (s128) yearOfDaysWide((int32_t) a.v); r.null = a.null; break;
                   case LDB_OP_STRKEY8: {
                      ProgCol tmp;
                      int64_t at;
@@ -479,9 +509,10 @@ __global__ void __launch_bounds__(256) programKernel(const __grid_constant__ Pro
          } else if (p.sinkKind == 2) {
             if (pass) {
                const Val k = regs[p.buildKeyReg];
-               if (!k.null) { // NULL keys never match (SQL join semantics)
-                  const int32_t pay = p.buildPayloadReg >= 0 && !regs[p.buildPayloadReg].null ? (int32_t) regs[p.buildPayloadReg].v : 0;
-                  if (joinInsertProg(p.build, (int32_t) k.v, pay)) inserted++;
+               if (!k.null) { // NULL keys never match (SQL join semantics); a NULL payload is stored as 0
+                  const s128 pay = p.buildPayloadReg >= 0 && !regs[p.buildPayloadReg].null ? regs[p.buildPayloadReg].v : 0;
+                  if (k.v != (s128) (int32_t) k.v || pay != (s128) (int32_t) pay) atomicExch(p.build.error, 7); // keys and payloads are int32
+                  else if (joinInsertProg(p.build, (int32_t) k.v, (int32_t) pay)) inserted++;
                }
             }
          } else if (p.sinkKind == 3) { // warp-aggregated append of the selected registers

@@ -93,8 +93,11 @@ int ldb_gpu_hashagg_create(LdbContext* ctx, int32_t n_keys, int32_t n_aggs, cons
          for (int a = 0; a < n_aggs; a++) {
             double inf = 1.0 / 0.0, ninf = -inf;
             switch (aggs[a].kind) {
-               case LDB_AGG_MIN: ea[2 * a] = (unsigned long long) INT64_MAX; break;
-               case LDB_AGG_MAX: ea[2 * a] = (unsigned long long) INT64_MIN; break;
+               case LDB_AGG_MIN: // INT128_MAX
+                  ea[2 * a] = ~0ull;
+                  ea[2 * a + 1] = ~0ull >> 1;
+                  break;
+               case LDB_AGG_MAX: ea[2 * a + 1] = 1ull << 63; break; // INT128_MIN
                case LDB_AGG_MIN_F64: memcpy(&ea[2 * a], &inf, 8); break;
                case LDB_AGG_MAX_F64: memcpy(&ea[2 * a], &ninf, 8); break;
                default: break;
@@ -482,14 +485,17 @@ static void runProgram(LdbContext* ctx, const LdbProgramDesc* d, const LdbProgra
       }
    };
    runBatches();
-   if (eachTable >= 0) { // a probe run longer than the bound: fail rather than return a truncated match list
-      int32_t e = 0;
-      LDB_CUDA(cudaMemcpyAsync(&e, base.tables[eachTable].error, 4, cudaMemcpyDeviceToHost, ctx->compute));
-      ctx->syncStream(ctx->compute);
-      if (e == 6) {
+   // a probe run longer than the bound (PROBE_EACH), or a build that could not store a row (table full, the reserved pair, a key or
+   // payload outside int32): fail rather than return a truncated match list or a table with rows missing
+   for (LdbState* js : {eachTable >= 0 ? d->tables[eachTable] : nullptr, d->sink_kind == LDB_SINK_JOIN_BUILD ? sink : nullptr}) {
+      if (!js) continue;
+      try {
+         ldb_gpu_check_join_error_internal(js);
+      } catch (...) {
+         ctx->syncStream(ctx->compute);
          for (void* q : outOwned) ctx->stagingRelease(q);
          for (void* q : dirs) ctx->stagingRelease(q);
-         failP(LDB_ERR_CAPACITY, "PROBE_EACH: a probe run is longer than the interpreter's bound of 16384 slots (an overfull join table)");
+         throw;
       }
    }
    if (d->sink_kind == LDB_SINK_MATERIALIZE) {
@@ -585,12 +591,16 @@ int ldb_gpu_table_gather(LdbTable* t, const char* column, const int64_t* row_ids
       LDB_CUDA(cudaSetDevice(ctx->device));
       ldb_gpu_wait_batch_internal(ctx, &b);
       const size_t w = (size_t) b.elemBytes[c];
-      for (int64_t i = 0; i < n; i++) {
+      for (int64_t i = 0; i < n; i++)
          if (row_ids[i] < 0 || row_ids[i] >= b.nRows) failP(LDB_ERR_INVALID, "row id out of range");
-         LDB_CUDA(cudaMemcpyAsync((uint8_t*) host_dst + (size_t) i * w, (const uint8_t*) b.data[c] + (size_t) row_ids[i] * w, w, cudaMemcpyDeviceToHost, ctx->compute));
+      // one copy per run of consecutive row ids (a whole column read back in order is one copy)
+      for (int64_t i = 0, j; i < n; i = j) {
+         for (j = i + 1; j < n && row_ids[j] == row_ids[j - 1] + 1;) j++;
+         const size_t m = (size_t) (j - i);
+         LDB_CUDA(cudaMemcpyAsync((uint8_t*) host_dst + (size_t) i * w, (const uint8_t*) b.data[c] + (size_t) row_ids[i] * w, m * w, cudaMemcpyDeviceToHost, ctx->compute));
          if (host_valid) {
-            if (c < (int) b.validBytes.size() && b.validBytes[c]) LDB_CUDA(cudaMemcpyAsync(host_valid + i, b.validBytes[c] + row_ids[i], 1, cudaMemcpyDeviceToHost, ctx->compute));
-            else host_valid[i] = 1;
+            if (c < (int) b.validBytes.size() && b.validBytes[c]) LDB_CUDA(cudaMemcpyAsync(host_valid + i, b.validBytes[c] + row_ids[i], m, cudaMemcpyDeviceToHost, ctx->compute));
+            else memset(host_valid + i, 1, m);
          }
       }
       ctx->syncStream(ctx->compute);

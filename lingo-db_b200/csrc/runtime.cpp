@@ -944,7 +944,13 @@ static void checkJoinError(LdbState* s) {
    if (e == 3) fail(LDB_ERR_UNSUPPORTED, "the pair (key=-1, payload=-1) cannot be stored in a join table");
    if (e == 4) fail(LDB_ERR_UNSUPPORTED, "join tables with side/aggregate lanes need non-negative inline payloads");
    if (e == 5) fail(LDB_ERR_INVALID, "key outside the declared range of a direct-address table");
+   if (e == 6) fail(LDB_ERR_CAPACITY, "PROBE_EACH: a probe run is longer than the interpreter's bound of 16384 slots (an overfull join table)");
+   if (e == 7) fail(LDB_ERR_UNSUPPORTED, "a program join build met a key or payload outside int32 (join tables store int32 keys and payloads)");
+   if (e != 0) fail(LDB_ERR_INVALID, "join table error word " + std::to_string(e));
 }
+} // extern "C"
+void ldb_gpu_check_join_error_internal(LdbState* s) { checkJoinError(s); }
+extern "C" {
 int ldb_gpu_join_table_count(LdbState* s, int64_t* n_entries, LdbError* err) {
    return guarded(err, [&] {
       if (!s || s->kind != LDB_STATE_JOIN_TABLE) fail(LDB_ERR_INVALID, "not a join table");

@@ -128,8 +128,10 @@ class Table:
         self._keep = []
         ctx._tables.append(self)
 
-    def _append(self, n_rows: int, bufs: Dict[str, object], location: int, utf8_sizes: Dict[str, int], valids: Optional[Dict[str, int]] = None):
-        """bufs: column → address (int) or (offsets_addr, bytes_addr) for utf8; valids: column → address of an Arrow validity bitmap."""
+    def _append(self, n_rows: int, bufs: Dict[str, object], location: int, utf8_sizes: Dict[str, int], valids: Optional[Dict[str, int]] = None,
+                offset: int = 0):
+        """bufs: column → address (int) or (offsets_addr, bytes_addr) for utf8; valids: column → address of an Arrow validity bitmap.
+        offset: the batch's first row is row `offset` of every buffer (Arrow's ArrayView.offset, bitmaps included)."""
         nc = len(self.columns)
         views = (capi.ArrayView * nc)()
         sizes = (C.c_int64 * nc)()
@@ -147,14 +149,15 @@ class Table:
                 arr[0] = valids[c.name]
                 nulls = -1  # "unknown, look at the bitmap" (Arrow's convention)
             keep.append(arr)
-            views[i] = capi.ArrayView(n_rows, nulls, 0, 3 if c.phys == "utf8" else 2, 0, C.cast(arr, C.POINTER(C.c_void_p)), None)
+            views[i] = capi.ArrayView(n_rows, nulls, offset, 3 if c.phys == "utf8" else 2, 0, C.cast(arr, C.POINTER(C.c_void_p)), None)
         e = Error()
         check(self.ctx.L.ldb_gpu_table_append_batch(self.h, n_rows, views, sizes, location, C.byref(e)), e)
         self._keep.append((keep, views))
 
-    def append_host(self, chunk: Dict[str, object], n_rows: int):
+    def append_host(self, chunk: Dict[str, object], n_rows: int, offset: int = 0):
         """chunk: column → numpy buffer ((offsets, bytes) for utf8); an optional entry "<column>$valid" holds the column's Arrow
-        validity bitmap (numpy uint8, LSB first, bit i = row i is NOT NULL)."""
+        validity bitmap (numpy uint8, LSB first, bit i = row i is NOT NULL).  With `offset`, the batch is rows offset .. offset +
+        n_rows - 1 of every buffer and bitmap (an Arrow slice)."""
         bufs, sizes, valids = {}, {}, {}
         for c in self.columns:
             v = chunk[c.name]
@@ -163,24 +166,27 @@ class Table:
             if c.phys == "utf8":
                 offs, data = v
                 bufs[c.name] = (offs.ctypes.data, data.ctypes.data)
-                sizes[c.name] = int(offs[n_rows])
+                sizes[c.name] = int(offs[offset + n_rows])
             else:
                 bufs[c.name] = v.ctypes.data
         self._keep.append(chunk)
-        self._append(n_rows, bufs, capi.MEM_HOST, sizes, valids)
+        self._append(n_rows, bufs, capi.MEM_HOST, sizes, valids, offset)
 
     def append_device(self, tensors: Dict[str, object], n_rows: int):
-        """tensors: column → torch CUDA tensor (or (offsets, bytes) pair for utf8); borrowed."""
-        bufs, sizes = {}, {}
+        """tensors: column → torch CUDA tensor (or (offsets, bytes) pair for utf8), and optionally "<column>$valid" → the column's
+        Arrow validity bitmap as a uint8 CUDA tensor; borrowed."""
+        bufs, sizes, valids = {}, {}, {}
         for c in self.columns:
             v = tensors[c.name]
+            if c.name + "$valid" in tensors:
+                valids[c.name] = tensors[c.name + "$valid"].data_ptr()
             if c.phys == "utf8":
                 bufs[c.name] = (v[0].data_ptr(), v[1].data_ptr())
                 sizes[c.name] = int(v[1].numel())
             else:
                 bufs[c.name] = v.data_ptr()
         self._keep.append(tensors)
-        self._append(n_rows, bufs, capi.MEM_DEVICE, sizes)
+        self._append(n_rows, bufs, capi.MEM_DEVICE, sizes, valids)
 
     def clear(self):
         e = Error()
