@@ -196,7 +196,7 @@ typedef struct LdbTopKRow {
  * logical build side OR their filters together (NCCL all_reduce BOR) so every rank can pre-filter its probe side. */
 int ldb_gpu_join_table_bloom(LdbState* s, void** dev_ptr, int64_t* bytes, LdbError* err);
 /* scan of the group-join map + Heap (include/lingodb/runtime/Heap.h): marked groups ordered by
- * (agg0 desc, side0 asc, key asc), first k */
+ * (agg0 desc, side0 asc, key asc), first k; agg0 compares as a signed 128-bit value (a 64-bit SUM sign-extended) */
 int ldb_gpu_join_table_topk(LdbState* s, int32_t k, LdbTopKRow* rows, int32_t* n_rows, LdbError* err);
 
 /* ------------------------------------------------------------------------------------ pipelines
@@ -234,7 +234,10 @@ enum LdbExprKind {
    LDB_EXPR_MUL_1MINUS_MINUS_PAYMUL = 5 /* a * (1 - b) - $payload0 * c   decimal(34,4) i128; K9 only ($payload0 = probe 0's int64 payload) */
 };
 typedef struct LdbAggDesc {
-   int32_t expr;            /* LdbExprKind; every aggregate is SUM (count = SUM of ONE); i64 sums wrap at 64 bits */
+   int32_t expr;            /* LdbExprKind; every aggregate is SUM (count = SUM of ONE); i64 sums (COL, ONE) wrap at 64 bits and
+                               are read back sign-extended (LdbI128.hi = lo >> 63) by every sink, the group-join map's top-k included;
+                               i128 sums wrap at 128 bits.  An aggregate of a state keeps the width of the first pipeline that
+                               summed into it: a later pipeline of the other width fails with LDB_ERR_UNSUPPORTED */
    const char* columns[3];  /* a, b, c */
 } LdbAggDesc;
 

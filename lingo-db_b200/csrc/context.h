@@ -219,7 +219,8 @@ struct LdbState {
    int32_t aggKinds[ldb::kProgMaxAggs] = {};
    int32_t nSide = 0, nAggs = 0;
    bool selfTimed = false; // created inside a captured query: its scan kernel's self-measured time is harvested at read
-   uint32_t is64Mask = 0; // aggregates that are 64-bit sums (COL / ONE): normalised to a sign-extended i64 on read
+   uint32_t is64Mask = 0;   // aggregates that are 64-bit sums (COL / ONE): normalised to a sign-extended i64 on read
+   uint32_t laneBound = 0;  // aggregates whose width (64 / 128 bits) a pipeline fixed already: a later one must agree
    std::vector<void*> allocations;
 };
 

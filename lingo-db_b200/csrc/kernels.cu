@@ -1412,11 +1412,13 @@ __global__ void __launch_bounds__(kThreads, FS == FS_GENERIC ? 4 : 5) scanProbe2
          if (!bpB[j].mayContain()) continue;
          joinProbeSlots(p.tableA, key[j], bp[j].h, [&](int64_t, int32_t payA) {
             joinProbeSlots(p.tableB, keyB[j], bpB[j].h, [&](int64_t, int32_t payB) {
-               if (((payA ^ payB) & (p.tableA.stride == 32 || p.tableB.stride == 32 ? 0x7fffffff : -1)) != 0) return;
+               // bit 31 of a wide entry is the group-join marker, not payload: each side drops its own marker before the compare
+               const int32_t a = p.tableA.stride == 32 ? (payA & 0x7fffffff) : payA, b = p.tableB.stride == 32 ? (payB & 0x7fffffff) : payB;
+               if (a != b) return;
                int64_t vals[NV];
 #pragma unroll
                for (int c = 0; c < NV; c++) vals[c] = lazyLo64(p.values, c, rowBase + lrs[j]);
-               int32_t kk[2] = {p.tableB.stride == 32 ? (payB & 0x7fffffff) : payB, 0}; // bit 31 of a wide entry is the group-join marker, not payload
+               int32_t kk[2] = {b, 0};
                int slot = groupLookupOrInsert(p.groups, kk);
                if (slot >= 0) groupAtomicAdd(p.groups, slot, 0, evalAggDyn(p.agg, vals, one), p.agg.expr == LDB_EXPR_COL || p.agg.expr == LDB_EXPR_ONE);
             });
@@ -1537,14 +1539,14 @@ __global__ void __launch_bounds__(kBlock, 4) scanStarProbeGroupByKernel(const __
    __syncthreads();
    groups.flush(p.groups, false);
 }
-void launchScanStarProbeGroupBy(const StarProbeParams& p, int smCount, cudaStream_t s) {
+bool launchScanStarProbeGroupBy(const StarProbeParams& p, int smCount, cudaStream_t s, const char** why) {
    size_t dyn;
    const int ns = tuning().stagesStar, rpt = tuning().rptStar;
 #define LDB_STAR_CASE(DBV, RPTV, NSV)                                                                                          \
    if (p.src.cols.decBytes == DBV && rpt == RPTV && ns == NSV) {                                                               \
       int grid = persistentGrid(scanStarProbeGroupByKernel<DBV, RPTV, NSV>, p.src.cols, p.src.nRows, smCount, &dyn, kBlock, NSV); \
       scanStarProbeGroupByKernel<DBV, RPTV, NSV><<<grid, kBlock, dyn, s>>>(p);                                                 \
-      return;                                                                                                                  \
+      return true;                                                                                                             \
    }
    // filter-shape instantiations: tuned tile shape (2 rows per thread, 2 stages) only
    const int fs = rpt == 2 && ns == 2 ? filterShape(p.src.filters) : FS_GENERIC;
@@ -1552,14 +1554,18 @@ void launchScanStarProbeGroupBy(const StarProbeParams& p, int smCount, cudaStrea
    if (p.src.cols.decBytes == DBV && fs == FSV) {                                                                                    \
       int grid = persistentGrid(scanStarProbeGroupByKernel<DBV, 2, 2, FSV>, p.src.cols, p.src.nRows, smCount, &dyn, kBlock, 2);      \
       scanStarProbeGroupByKernel<DBV, 2, 2, FSV><<<grid, kBlock, dyn, s>>>(p);                                                       \
-      return;                                                                                                                        \
+      return true;                                                                                                                   \
    }
    LDB_STAR_FS(16, FS_NONE) LDB_STAR_FS(16, FS_I32_ONE) LDB_STAR_FS(16, FS_I32_RANGE) LDB_STAR_FS(8, FS_NONE) LDB_STAR_FS(8, FS_I32_ONE) LDB_STAR_FS(8, FS_I32_RANGE)
 #undef LDB_STAR_FS
    // the staged columns of a star probe are int32 keys only (the operands are late-materialised): decBytes stays at its default
    LDB_STAR_CASE(16, 1, 2) LDB_STAR_CASE(16, 2, 2) LDB_STAR_CASE(16, 4, 2) LDB_STAR_CASE(16, 1, 3) LDB_STAR_CASE(16, 2, 3) LDB_STAR_CASE(16, 4, 3)
+   LDB_STAR_CASE(16, 1, 4) LDB_STAR_CASE(16, 2, 4) LDB_STAR_CASE(16, 4, 4)
    LDB_STAR_CASE(8, 1, 2) LDB_STAR_CASE(8, 2, 2) LDB_STAR_CASE(8, 4, 2) LDB_STAR_CASE(8, 1, 3) LDB_STAR_CASE(8, 2, 3) LDB_STAR_CASE(8, 4, 3)
+   LDB_STAR_CASE(8, 1, 4) LDB_STAR_CASE(8, 2, 4) LDB_STAR_CASE(8, 4, 4)
 #undef LDB_STAR_CASE
+   *why = "no star-probe instantiation for this tile shape"; // a missing instantiation must not leave the group-by silently empty
+   return false;
 }
 
 // =================================================================================== top-k over the group-join map
@@ -1572,7 +1578,9 @@ __device__ __forceinline__ bool topkBefore(const TopKRowDev& a, const TopKRowDev
    return a.key < b.key;
 }
 constexpr int kTopKMax = 64;
-__global__ void __launch_bounds__(kBlock) joinTopKKernel(JoinTableDev t, int k, TopKRowDev* out) {
+// agg64: the aggregate lane holds a 64-bit SUM (LdbExprKind COL / ONE): its value is the low word, sign-extended — the high word only
+// collected the carries of the two-word atomics.  It is normalised here, before the ranking and the threshold see it.
+__global__ void __launch_bounds__(kBlock) joinTopKKernel(JoinTableDev t, int k, bool agg64, TopKRowDev* out) {
    __shared__ TopKRowDev best[kTopKMax];
    // Lock-free reject: once the CTA holds k rows, sThreshold is the k-th row's aggregate when that fits 64 unsigned bits (0 otherwise).
    // The k-th only ever improves, so a stale value is merely a weaker filter, and a single 64-bit shared word cannot be read torn: a
@@ -1637,7 +1645,7 @@ __global__ void __launch_bounds__(kBlock) joinTopKKernel(JoinTableDev t, int k, 
          c.side1 = (int32_t) lo[u].w;
          c.valid = 1;
          c.aggLo = ((unsigned long long) hi[u].y << 32) | hi[u].x;
-         c.aggHi = (long long) (((unsigned long long) hi[u].w << 32) | hi[u].z);
+         c.aggHi = agg64 ? (long long) c.aggLo >> 63 : (long long) (((unsigned long long) hi[u].w << 32) | hi[u].z);
          consider(c);
       }
    }
@@ -1648,10 +1656,10 @@ __global__ void __launch_bounds__(kBlock) joinTopKKernel(JoinTableDev t, int k, 
       out[(size_t) blockIdx.x * k + i] = r;
    }
 }
-void launchJoinTopK(const JoinTableDev& t, int k, TopKRowDev* out, int* outBlocks, int smCount, cudaStream_t s) {
+void launchJoinTopK(const JoinTableDev& t, int k, bool agg64, TopKRowDev* out, int* outBlocks, int smCount, cudaStream_t s) {
    int grid = smCount * 2;
    *outBlocks = grid;
-   joinTopKKernel<<<grid, kBlock, 0, s>>>(t, k, out);
+   joinTopKKernel<<<grid, kBlock, 0, s>>>(t, k, agg64, out);
 }
 
 // 32-byte entries start as {empty marker, zero side lanes, zero aggregate}

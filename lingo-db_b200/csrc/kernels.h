@@ -252,10 +252,10 @@ bool launchScanGroupBy(const GroupByParams& p, int smCount, cudaStream_t s, cons
 void launchScanBuild(const BuildParams& p, int smCount, cudaStream_t s);
 bool launchScanProbeAgg(const ProbeAggParams& p, int smCount, cudaStream_t s, const char** why);
 bool launchScanProbe2GroupBy(const Probe2GroupByParams& p, int smCount, cudaStream_t s, const char** why);
-void launchScanStarProbeGroupBy(const StarProbeParams& p, int smCount, cudaStream_t s);
+bool launchScanStarProbeGroupBy(const StarProbeParams& p, int smCount, cudaStream_t s, const char** why);
 void launchScanMaterialize(const MaterializeParams& p, int smCount, cudaStream_t s);
 void launchInitWideTable(uint8_t* base, uint64_t capacity, int smCount, cudaStream_t s);
-void launchJoinTopK(const JoinTableDev& t, int k, TopKRowDev* out, int* outBlocks, int smCount, cudaStream_t s);
+void launchJoinTopK(const JoinTableDev& t, int k, bool agg64, TopKRowDev* out, int* outBlocks, int smCount, cudaStream_t s);
 void launchFill64(unsigned long long* p, unsigned long long v, int64_t n, int smCount, cudaStream_t s);
 void launchInsertTuples(const JoinTableDev& t, const int32_t* keys, const int32_t* payloads, const int32_t* side0, const int32_t* side1, int64_t n, int smCount, cudaStream_t s);
 void launchColumnRange(const int32_t* col, int64_t n, int32_t* minMax /* device: {min, max} */, int smCount, cudaStream_t s);

@@ -44,17 +44,6 @@ struct Val {
 __device__ __forceinline__ double asF64(const Val& x) { return __longlong_as_double((long long) (uint64_t) x.v); }
 __device__ __forceinline__ Val fromF64(double d, bool null) { return Val{(s128) (uint64_t) __double_as_longlong(d), null}; }
 
-// yearOfDays for EVERY date32 value: the same civil-from-days steps in 64-bit arithmetic (days + 719468 leaves int32 for dates past
-// the year 5 879 609; the specialised kernels only see TPC-H dates and keep the 32-bit form)
-__device__ __forceinline__ int64_t yearOfDaysWide(int32_t days) {
-   const int64_t z = (int64_t) days + 719468;
-   const int64_t era = (z >= 0 ? z : z - 146096) / 146097;
-   const int64_t doe = z - era * 146097;
-   const int64_t yoe = (doe - doe / 1460 + doe / 36524 - doe / 146096) / 365;
-   const int64_t doy = doe - (365 * yoe + yoe / 4 - yoe / 100);
-   const int64_t mp = (5 * doy + 2) / 153;
-   return yoe + era * 400 + (mp >= 10 ? 1 : 0);
-}
 __device__ __forceinline__ bool colIsNull(const ProgCol& c, int64_t row) {
    if (c.validBytes) return c.validBytes[row] == 0;
    if (!c.validity) return false;
@@ -405,7 +394,7 @@ __global__ void __launch_bounds__(256) programKernel(const __grid_constant__ Pro
                      if (!r.null) r.v = strLike(*c, at, p.strings[in.arg], p.stringLen[in.arg], in.b);
                      break;
                   }
-                  case LDB_OP_YEAR: r.v = (s128) yearOfDaysWide((int32_t) a.v); r.null = a.null; break;
+                  case LDB_OP_YEAR: r.v = (s128) yearOfDays((int32_t) a.v); r.null = a.null; break;
                   case LDB_OP_STRKEY8: {
                      ProgCol tmp;
                      int64_t at;

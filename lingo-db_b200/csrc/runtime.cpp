@@ -977,7 +977,7 @@ int ldb_gpu_join_table_topk(LdbState* s, int32_t k, LdbTopKRow* rows, int32_t* n
       int blocks = ctx->smCount * 2;
       size_t bytes = sizeof(TopKRowDev) * (size_t) blocks * k;
       void* d = ctx->stagingAlloc(bytes);
-      ctx->launch("join_topk", [&] { launchJoinTopK(s->join, k, (TopKRowDev*) d, &blocks, ctx->smCount, ctx->compute); });
+      ctx->launch("join_topk", [&] { launchJoinTopK(s->join, k, (s->is64Mask & 1u) != 0, (TopKRowDev*) d, &blocks, ctx->smCount, ctx->compute); });
       std::vector<TopKRowDev> h((size_t) blocks * k);
       LDB_CUDA(cudaMemcpyAsync(h.data(), d, bytes, cudaMemcpyDeviceToHost, ctx->compute));
       ctx->syncStream(ctx->compute);
@@ -1076,9 +1076,12 @@ static int64_t filterConstant(const LdbColumn& col, bool isInt, const char* str,
       case LDB_DECIMAL128: {
          if (col.precision >= 19) fail(LDB_ERR_UNSUPPORTED, "decimal precision >= 19 is not supported on the GPU path yet");
          if (!isInt) return parseDecimal(str, col.scale);
-         int64_t v = ival;
-         for (int s = 0; s < col.scale; s++) v *= 10;
-         return v;
+         __int128 v = ival;
+         for (int s = 0; s < col.scale; s++) {
+            v *= 10;
+            if (v > (__int128) INT64_MAX || v < (__int128) INT64_MIN) fail(LDB_ERR_UNSUPPORTED, "decimal constant beyond 64 bits");
+         }
+         return (int64_t) v;
       }
       default: fail(LDB_ERR_UNSUPPORTED, "unsupported type in filter");
    }
@@ -1198,6 +1201,17 @@ void bindLazy(LdbTable* t, const LdbBatch& b, const int* cols, int n, LazyCols& 
       out.elemBytes[i] = b.elemBytes[cols[i]];
    }
 }
+// An aggregate lane of a state keeps one width for its whole life: a 64-bit SUM (COL / ONE; wraps at 64 bits, read back
+// sign-extended) or a 128-bit one.  A pipeline that would add the other kind into the same lane is rejected: the read could not
+// tell the two apart.
+void bindLaneWidth(LdbState* s, int lane, int expr) {
+   const uint32_t bit = 1u << lane;
+   const bool is64 = expr == LDB_EXPR_COL || expr == LDB_EXPR_ONE;
+   if ((s->laneBound & bit) && ((s->is64Mask & bit) != 0) != is64)
+      fail(LDB_ERR_UNSUPPORTED, "aggregate " + std::to_string(lane) + " of this state was summed at another width: 64-bit (COL, ONE) and 128-bit expressions cannot share a lane");
+   s->laneBound |= bit;
+   if (is64) s->is64Mask |= bit;
+}
 LdbState* wantState(LdbState* s, int kind, const char* role) {
    if (!s || s->kind != kind) fail(LDB_ERR_INVALID, std::string("wrong or missing state for ") + role);
    return s;
@@ -1227,8 +1241,7 @@ int ldb_gpu_run_pipeline(LdbContext* ctx, const LdbPipelineDesc* d, LdbError* er
             LdbState* sink = wantState(d->sink, keyless ? LDB_STATE_SIMPLE : LDB_STATE_GROUPBY, "sink");
             AggPlan ap = planAggs(R, d->aggs, d->n_aggs);
             if (ap.nAggs != sink->group.nAggs) fail(LDB_ERR_INVALID, "aggregate count differs from the state's");
-            for (int a = 0; a < ap.nAggs; a++)
-               if (ap.aggs[a].expr == LDB_EXPR_COL || ap.aggs[a].expr == LDB_EXPR_ONE) sink->is64Mask |= 1u << a;
+            for (int a = 0; a < ap.nAggs; a++) bindLaneWidth(sink, a, ap.aggs[a].expr);
             int nKeys = keyless ? 0 : d->n_keys;
             if (nKeys != sink->group.nKeys) fail(LDB_ERR_INVALID, "key count differs from the state's");
             int keyCol[kMaxKeys] = {0, 0};
@@ -1322,6 +1335,7 @@ int ldb_gpu_run_pipeline(LdbContext* ctx, const LdbPipelineDesc* d, LdbError* er
             if (!table->nAggs) fail(LDB_ERR_INVALID, "join table was created without aggregate lanes");
             if (d->n_probes != 1 || d->probe_states[0] != table) fail(LDB_ERR_INVALID, "probe-aggregate pipelines probe their own sink");
             AggPlan ap = planAggs(R, d->aggs, 1);
+            bindLaneWidth(table, 0, ap.aggs[0].expr); // the top-k ranks a 64-bit lane by its sign-extended value
             int probeCol = R.col(d->probe_key_columns[0], {LDB_INT32, LDB_DATE32, LDB_FSB4}, "probe key");
             int probeStage = sp.add(t, probeCol);
             for (auto& b : t->batches) {
@@ -1351,6 +1365,7 @@ int ldb_gpu_run_pipeline(LdbContext* ctx, const LdbPipelineDesc* d, LdbError* er
             int ca = R.col(d->probe_key_columns[0], {LDB_INT32, LDB_DATE32, LDB_FSB4}, "probe key A");
             int cb = R.col(d->probe_key_columns[1], {LDB_INT32, LDB_DATE32, LDB_FSB4}, "probe key B");
             int stageA = sp.add(t, ca), stageB = sp.add(t, cb);
+            bindLaneWidth(sink, 0, ap.aggs[0].expr);
             for (auto& b : t->batches) {
                if (b.nRows == 0) continue;
                Probe2GroupByParams p{};
@@ -1364,7 +1379,6 @@ int ldb_gpu_run_pipeline(LdbContext* ctx, const LdbPipelineDesc* d, LdbError* er
                p.agg = ap.aggs[0];
                bindLazy(t, b, ap.valueCol, ap.nValueCols, p.values);
                p.groups = sink->group;
-               if (p.agg.expr == LDB_EXPR_COL || p.agg.expr == LDB_EXPR_ONE) sink->is64Mask |= 1u;
                waitBatch(ctx, b);
                bool ok = true;
                ctx->launch("join_probe2_groupby", [&] { ok = launchScanProbe2GroupBy(p, ctx->smCount, ctx->compute, &why); });
@@ -1448,7 +1462,9 @@ int ldb_gpu_run_pipeline(LdbContext* ctx, const LdbPipelineDesc* d, LdbError* er
                p.tableO = to->join;
                p.groups = sink->group;
                waitBatch(ctx, b);
-               ctx->launch("join_star_probe_groupby", [&] { launchScanStarProbeGroupBy(p, ctx->smCount, ctx->compute); });
+               bool ok = true;
+               ctx->launch("join_star_probe_groupby", [&] { ok = launchScanStarProbeGroupBy(p, ctx->smCount, ctx->compute, &why); });
+               if (!ok) fail(LDB_ERR_UNSUPPORTED, why);
             }
             break;
          }
