@@ -158,7 +158,10 @@ typedef struct LdbGroupRow {
 } LdbGroupRow;
 /* rt::PreAggregationHashtable::createIterator + BufferIterator::iterate, for a tiny result */
 int ldb_gpu_groupby_read(LdbState* s, LdbGroupRow* rows, int32_t max_rows, int32_t* n_rows, LdbError* err);
-/* fold another GPU's partial groups into this state (K7 merge; rt::PreAggregationHashtable::merge) */
+/* fold another GPU's partial groups into this state (K7 merge; rt::PreAggregationHashtable::merge).  Every merge (_merge_rows,
+ * _merge_exported, ldb_gpu_groupby_allmerge) adds the 128-bit cells per key and carries no width: a merged lane is read at the width
+ * of its TARGET (a 64-bit lane as the sign-extended low word).  So the target's lanes must have been bound by a pipeline (LdbAggDesc);
+ * a merge into a state with an unbound aggregate lane fails with LDB_ERR_UNSUPPORTED. */
 int ldb_gpu_groupby_merge_rows(LdbState* s, const LdbGroupRow* rows, int32_t n_rows, LdbError* err);
 
 /* Multi-GPU merge without a host round trip: copy the table image {state[cap], keys[cap][2], acc[cap][8][2]}
@@ -237,7 +240,9 @@ typedef struct LdbAggDesc {
    int32_t expr;            /* LdbExprKind; every aggregate is SUM (count = SUM of ONE); i64 sums (COL, ONE) wrap at 64 bits and
                                are read back sign-extended (LdbI128.hi = lo >> 63) by every sink, the group-join map's top-k included;
                                i128 sums wrap at 128 bits.  An aggregate of a state keeps the width of the first pipeline that
-                               summed into it: a later pipeline of the other width fails with LDB_ERR_UNSUPPORTED */
+                               summed into it: a later pipeline of the other width fails with LDB_ERR_UNSUPPORTED.  Every group
+                               sink binds its lanes: K1/K2 and K4 by their aggregates, K5 lane 0 of the group-join map, and K9,
+                               ldb_gpu_probe_received_groupby and _groupby2 lane 0 as 128-bit */
    const char* columns[3];  /* a, b, c */
 } LdbAggDesc;
 
@@ -266,7 +271,10 @@ enum LdbPipelineKind {
     *     LDB_PAYLOAD_YEAR ships extract(year from that date32 column) instead), out_columns[2..3] =
     *     decimal(p<19) columns shipped as their low 8 bytes.  Tuple = 1 + (n_out_cols - 2) eight-byte words.  The receive region of
     *     every rank is heap[send_offset, + world * send_capacity * tuple bytes): sub-region s belongs to source rank s.
-    *     send_cursors_offset: heap offset of 16 uint64 (zeroed by the caller): [d] = tuples sent to rank d, [8] = overflow flag. */
+    *     send_cursors_offset: heap offset of 16 uint64 (zeroed by the caller): [d] = tuples sent to rank d, [8] = overflow flag.
+    *     The full probe is a semi-join: one tuple per qualifying row with at least one match (K8 emits one per match), so "$payload"
+    *     needs a probe table created LDB_JOIN_UNIQUE (else LDB_ERR_UNSUPPORTED).  A cursor counts every tuple; only the first
+    *     send_capacity of each destination are stored, the rest set the overflow flag. */
    LDB_PIPE_SCAN_PARTITION_SEND = 8,
    /* K11 scan → filters → probe 0 (composite key, int64 payload c; Bloom first) → probe 1 (foreign key → int32 payload g) → the row's
     *     a * (1 - b) - c * d (aggs[0] = LDB_EXPR_MUL_1MINUS_MINUS_PAYMUL) is shipped as {out_columns[0] : 32 | g : 32, lo, hi} (24 bytes)

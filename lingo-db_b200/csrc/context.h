@@ -227,3 +227,8 @@ struct LdbState {
 // reads a join table's error word (synchronises the compute stream) and throws ApiError with the status and message of a
 // non-zero code (runtime.cpp); every caller that reports a join table's failure goes through it
 void ldb_gpu_check_join_error_internal(LdbState* s);
+// fixes the width of aggregate lane `lane` of a group state from the LdbExprKind summed into it (64-bit COL / ONE, else 128-bit);
+// throws ApiError(LDB_ERR_UNSUPPORTED) when an earlier pipeline fixed the other width (runtime.cpp)
+void ldb_gpu_bind_lane_width_internal(LdbState* s, int lane, int expr);
+// merges read a lane at the width of their TARGET: throws ApiError(LDB_ERR_UNSUPPORTED) while one of its aggregate lanes is unbound
+void ldb_gpu_want_bound_lanes_internal(LdbState* s);

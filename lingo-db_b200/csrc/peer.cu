@@ -375,13 +375,15 @@ int ldb_gpu_groupby_allmerge(LdbState* s, LdbComm* c, LdbError* err) {
       if (!s || (s->kind != LDB_STATE_GROUPBY && s->kind != LDB_STATE_SIMPLE)) failPeer(LDB_ERR_INVALID, "not a group state");
       wantConnected(c);
       if (s->ctx != c->ctx) failPeer(LDB_ERR_INVALID, "state and comm belong to different contexts");
+      ldb_gpu_want_bound_lanes_internal(s);
       if (c->world == 1) return;
       const size_t image = (groupImageBytes(s->group.capacity) + 15) & ~size_t(15); // the table allocation carries 16 spare bytes (error word)
       if (image > kSlotBytes) failPeer(LDB_ERR_UNSUPPORTED, "group table image larger than a mailbox slot (capacity <= 1024 groups)");
       LdbContext* ctx = c->ctx;
       LDB_CUDA(cudaSetDevice(ctx->device));
-      ++c->gatherEpochHost;
-      if (ctx->capturing) ctx->capturing->onLaunch.push_back([c] { ++c->gatherEpochHost; }); // every replay bumps the device epoch once more
+      // the mirror follows the device epoch: bumped when the kernel runs (now, or at every replay of a capture), never at capture
+      if (ctx->capturing) ctx->capturing->onLaunch.push_back([c] { ++c->gatherEpochHost; });
+      else ++c->gatherEpochHost;
       ctx->launch("peer_group_allmerge", [&] {
          peerGroupAllMergeKernel<<<c->world, 256, 0, ctx->compute>>>(c->view(), s->group, image);
          peerBumpKernel<<<1, 1, 0, ctx->compute>>>(c->view(), EPOCH_GATHER, EPOCH_MERGE);
@@ -451,6 +453,7 @@ int ldb_gpu_probe_received_groupby(LdbState* ta, LdbState* tb, LdbState* groups,
       if (scale < 0 || scale > 18) failPeer(LDB_ERR_INVALID, "decimal scale out of range");
       wantRange(c, recv_offset, (int64_t) c->world * capacity * 24, "receive region");
       wantRange(c, counts_offset, kMaxPeers * 8, "counts");
+      ldb_gpu_bind_lane_width_internal(groups, 0, LDB_EXPR_MUL_1MINUS); // a * (10^scale - b): a 128-bit sum
       int64_t one = 1;
       for (int i = 0; i < scale; i++) one *= 10;
       LdbContext* ctx = c->ctx;
@@ -469,6 +472,7 @@ int ldb_gpu_probe_received_groupby2(LdbState* table, LdbState* groups, LdbComm* 
       if (!groups || groups->kind != LDB_STATE_GROUPBY || groups->group.nKeys != 2 || groups->group.nAggs != 1) failPeer(LDB_ERR_INVALID, "sink must be a group-by state with two keys and one aggregate");
       wantRange(c, recv_offset, (int64_t) c->world * capacity * 24, "receive region");
       wantRange(c, counts_offset, kMaxPeers * 8, "counts");
+      ldb_gpu_bind_lane_width_internal(groups, 0, LDB_EXPR_MUL_1MINUS_MINUS_PAYMUL); // the shipped K11 sums are 128-bit
       LdbContext* ctx = c->ctx;
       LDB_CUDA(cudaSetDevice(ctx->device));
       uint8_t* user = c->heap + kUserOff;

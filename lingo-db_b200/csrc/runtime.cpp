@@ -757,6 +757,7 @@ int ldb_gpu_groupby_read(LdbState* s, LdbGroupRow* rows, int32_t max_rows, int32
 int ldb_gpu_groupby_merge_rows(LdbState* s, const LdbGroupRow* rows, int32_t n_rows, LdbError* err) {
    return guarded(err, [&] {
       if (!s || (s->kind != LDB_STATE_GROUPBY && s->kind != LDB_STATE_SIMPLE)) fail(LDB_ERR_INVALID, "not a group state");
+      ldb_gpu_want_bound_lanes_internal(s);
       if (n_rows <= 0) return;
       LdbContext* ctx = s->ctx;
       std::vector<int32_t> keys((size_t) n_rows * kMaxKeys);
@@ -790,6 +791,7 @@ int ldb_gpu_groupby_export(LdbState* s, void* dst, LdbError* err) {
 int ldb_gpu_groupby_merge_exported(LdbState* s, const void* src, int32_t n_tables, int32_t skip_index, LdbError* err) {
    return guarded(err, [&] {
       if (!s || (s->kind != LDB_STATE_GROUPBY && s->kind != LDB_STATE_SIMPLE)) fail(LDB_ERR_INVALID, "not a group state");
+      ldb_gpu_want_bound_lanes_internal(s);
       LdbContext* ctx = s->ctx;
       ctx->launch("group_merge", [&] { launchGroupMergeImages(s->group, (const uint8_t*) src, n_tables, skip_index, ctx->compute); });
    });
@@ -1223,6 +1225,14 @@ LdbState* wantSingleKeyTable(LdbState* s, const char* role) {
    return s;
 }
 } // namespace
+} // extern "C"
+void ldb_gpu_bind_lane_width_internal(LdbState* s, int lane, int expr) { bindLaneWidth(s, lane, expr); }
+void ldb_gpu_want_bound_lanes_internal(LdbState* s) {
+   const uint32_t all = (1u << s->group.nAggs) - 1u;
+   if ((s->laneBound & all) != all)
+      fail(LDB_ERR_UNSUPPORTED, "merge target has an aggregate whose width no pipeline fixed yet: a merged lane is read at its target's width (run a pipeline into the state first)");
+}
+extern "C" {
 
 int ldb_gpu_run_pipeline(LdbContext* ctx, const LdbPipelineDesc* d, LdbError* err) {
    return guarded(err, [&] {
@@ -1450,6 +1460,7 @@ int ldb_gpu_run_pipeline(LdbContext* ctx, const LdbPipelineDesc* d, LdbError* er
                if (t->columns[c].precision >= 19 || t->columns[c].scale != 2) fail(LDB_ERR_UNSUPPORTED, "aggregate operands must be decimal(p<19, 2) on the GPU path");
                starValueCols[k] = c;
             }
+            bindLaneWidth(sink, 0, LDB_EXPR_MUL_1MINUS_MINUS_PAYMUL);
             for (auto& b : t->batches) {
                if (b.nRows == 0) continue;
                StarProbeParams p = base;
@@ -1482,6 +1493,8 @@ int ldb_gpu_run_pipeline(LdbContext* ctx, const LdbPipelineDesc* d, LdbError* er
             base.keyStage = sp.add(t, R.col(d->out_columns[0], {LDB_INT32, LDB_DATE32, LDB_FSB4}, "partition key"));
             if (d->out_columns[1] && std::string(d->out_columns[1]) == "$payload") {
                if (!probe || d->probe_bloom_only) fail(LDB_ERR_INVALID, "$payload needs a full probe");
+               // the full probe is a semi-join (one tuple per row with a match): it cannot say WHICH match's payload to ship
+               if (!probe->join.unique) fail(LDB_ERR_UNSUPPORTED, "partition-send ships $payload only from a probe of a unique-key table");
                base.secondStage = -1;
             } else {
                base.secondStage = sp.add(t, R.col(d->out_columns[1], {LDB_INT32, LDB_DATE32, LDB_FSB4}, "second tuple column"));

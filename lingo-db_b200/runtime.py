@@ -315,9 +315,10 @@ def state_destroy(ctx: Context, state):
 # ---------------------------------------------------------------------- generic pipeline call
 def run_pipeline(ctx: Context, kind: str, source: Table, filters=(), keys=(), aggs=(), probes=(), build_key=None, build_payload=None,
                  side=(), sink=None, out_columns=(), out_buffers=(), out_capacity=0, out_count=None, bloom_only=False,
-                 build_key2=None, build_payload_expr="column"):
+                 build_key2=None, build_payload_expr="column", comm=None, send_offset=0, send_capacity=0, send_cursors_offset=0):
     """ldb_gpu_run_pipeline from keyword arguments.  filters: (column, op, value) with value str or int;
-    aggs: (expr, [columns]); probes: (state, key_column)."""
+    aggs: (expr, [columns]); probes: (state, key_column).  comm (a parallel.Comm or its handle) and send_*: the receive regions and
+    cursors of the partition-send pipelines (K10, K11)."""
     keep = []
 
     def b(s):
@@ -367,12 +368,15 @@ def run_pipeline(ctx: Context, kind: str, source: Table, filters=(), keys=(), ag
         d.side_columns[i] = b(c)
     d.sink = sink
     d.n_out_cols = len(out_columns)
-    for i, (c, buf) in enumerate(zip(out_columns, out_buffers)):
+    for i, c in enumerate(out_columns):  # (the partition-send pipelines name columns without buffers)
         d.out_columns[i] = b(c)
+    for i, buf in enumerate(out_buffers):
         d.out_buffers[i] = buf
     d.out_capacity = out_capacity
     d.out_count = out_count
     d.probe_bloom_only = int(bloom_only)
+    d.comm = getattr(comm, "h", comm)
+    d.send_offset, d.send_capacity, d.send_cursors_offset = send_offset, send_capacity, send_cursors_offset
     e = Error()
     check(ctx.L.ldb_gpu_run_pipeline(ctx.h, C.byref(d), C.byref(e)), e)
 
