@@ -198,6 +198,11 @@ SIGNATURES = {
     "ldb_gpu_hashagg_to_table": (C.c_int, [_P, C.c_char_p, C.POINTER(_P), _E]),
     "ldb_gpu_table_order_by": (C.c_int, [_P, C.c_char_p, C.c_int32, C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int64), _E]),
     "ldb_gpu_table_gather": (C.c_int, [_P, C.c_char_p, C.POINTER(C.c_int64), C.c_int64, _P, _P, _E]),
+    "ldb_gpu_table_order_by_keys": (C.c_int, [_P, C.c_int32, C.POINTER(C.c_char_p), C.POINTER(C.c_int32), C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int64), _E]),
+    "ldb_gpu_table_gather_strings": (C.c_int, [_P, C.c_char_p, C.POINTER(C.c_int64), C.c_int64, C.POINTER(C.c_int64), _P, C.c_int64, C.POINTER(C.c_int64), _P, _E]),
+    "ldb_gpu_dict_create": (C.c_int, [_P, C.c_int64, C.c_int64, C.POINTER(_P), _E]),
+    "ldb_gpu_dict_count": (C.c_int, [_P, C.POINTER(C.c_int64), _E]),
+    "ldb_gpu_dict_to_table": (C.c_int, [_P, C.c_char_p, C.POINTER(_P), _E]),
     "ldb_gpu_partition_tuples": (C.c_int, [_P, _P, C.POINTER(_P), C.POINTER(C.c_int32), C.c_int32, C.c_int64, C.c_int32, _P, C.POINTER(_P), C.POINTER(C.c_int64), _E]),
     "ldb_gpu_join_table_insert": (C.c_int, [_P, _P, _P, _P, C.POINTER(_P), C.c_int64, _E]),
     "ldb_gpu_comm_create": (C.c_int, [_P, C.c_int32, C.c_int32, C.c_int64, C.POINTER(_P), _P, _E]),

@@ -216,6 +216,7 @@ struct LdbState {
    ldb::GroupTableDev group{}; // SIMPLE / GROUPBY
    ldb::JoinTableDev join{};   // JOIN_TABLE
    ldb::HashAggDev hashagg{};  // HASHAGG
+   ldb::DictDev dict{};        // DICT
    int32_t aggKinds[ldb::kProgMaxAggs] = {};
    int32_t nSide = 0, nAggs = 0;
    bool selfTimed = false; // created inside a captured query: its scan kernel's self-measured time is harvested at read

@@ -184,6 +184,79 @@ __device__ __forceinline__ uint64_t mix64(uint64_t x) {
    return x;
 }
 
+// ---------------------------------------------------------------- string dictionary (DictDev, program.h)
+// placement hash of a byte string: 8-byte little-endian chunks (the last one zero padded) folded through mix64, seeded with the
+// length.  Internal: codes and results never depend on it.
+__device__ __forceinline__ uint64_t strHash(const uint8_t* s, int32_t n) {
+   uint64_t h = 0x9E3779B97F4A7C15ull ^ ((uint64_t) (uint32_t) n * 0xff51afd7ed558ccdull);
+   for (int32_t i = 0; i < n; i += 8) {
+      uint64_t w = 0;
+      for (int j = 0; j < 8 && i + j < n; j++) w |= (uint64_t) s[i + j] << (8 * j);
+      h = mix64(h ^ w) + 0x632BE59BD9B4E019ull;
+   }
+   return mix64(h);
+}
+__device__ __forceinline__ void dictFail(const DictDev& d, int code) { atomicCAS((unsigned int*) (d.ctr + 2), 0u, (unsigned int) code); }
+// the code of string s[0..n) in dictionary d; absent: inserted when `insert`, else -1.  -2: the dictionary failed (its error word
+// is set, the call reports LDB_ERR_CAPACITY).  A slot is claimed by CAS (empty → tag | kDictWriting); its claimer reserves arena
+// bytes, copies the string, takes a code, writes the entry and publishes tag | code + 1 with one atomic store — or tag | kDictFailed
+// when it cannot, so that no reader waits forever.  A reader that meets its tag waits for the publication, then compares the whole
+// string bytewise (loads through L2: the arena is written by other SMs during the same launch).  A hit takes no atomic.
+__device__ __noinline__ int32_t dictCode(const DictDev& d, const uint8_t* s, int32_t n, int insert) {
+   const uint64_t h = strHash(s, n);
+   const unsigned long long tag = (h >> 32) << 32;
+   uint64_t slot = h & d.mask;
+   const uint64_t limit = d.mask + 1 < 65536 ? d.mask + 1 : 65536;
+   for (uint64_t probes = 0; probes < limit; probes++) {
+      unsigned long long* sp = d.slots + slot;
+      unsigned long long w = *((volatile unsigned long long*) sp);
+      if ((uint32_t) w == 0) {
+         if (!insert) return -1;
+         w = atomicCAS(sp, 0ull, tag | kDictWriting);
+         if (w == 0) {
+            int fail = 0;
+            const unsigned long long off = atomicAdd(d.ctr, (unsigned long long) n);
+            unsigned long long code = 0;
+            if (off + (unsigned long long) n > (unsigned long long) d.arenaCap) {
+               fail = 2;
+            } else {
+               for (int32_t i = 0; i < n; i++) d.arena[off + i] = s[i];
+               code = atomicAdd(d.ctr + 1, 1ull);
+               if (code >= (unsigned long long) d.codeCap) fail = 3;
+            }
+            if (fail) {
+               dictFail(d, fail);
+               atomicExch(sp, tag | kDictFailed);
+               return -2;
+            }
+            d.entryOff[code] = (int64_t) off;
+            d.entryLen[code] = n;
+            __threadfence();
+            atomicExch(sp, tag | (unsigned long long) (code + 1));
+            return (int32_t) code;
+         }
+      }
+      if ((w & 0xffffffff00000000ull) == tag) {
+         while ((uint32_t) w == kDictWriting) {
+            __nanosleep(64);
+            w = *((volatile unsigned long long*) sp);
+         }
+         if ((uint32_t) w == kDictFailed) return -2;
+         __threadfence();
+         const int32_t code = (int32_t) ((uint32_t) w - 1);
+         if (__ldcg(d.entryLen + code) == n) {
+            const uint8_t* a = d.arena + __ldcg(d.entryOff + code);
+            int32_t i = 0;
+            while (i < n && __ldcg(a + i) == s[i]) i++;
+            if (i == n) return code;
+         }
+      }
+      slot = (slot + 1) & d.mask;
+   }
+   dictFail(d, 1);
+   return -2;
+}
+
 // ---------------------------------------------------------------- hash aggregation table
 constexpr uint32_t kSeenBit = 1u, kClaimBit = 1u << 8, kKeyNullBit = 1u << 16;
 __device__ __forceinline__ uint8_t* entryAt(const HashAggDev& t, uint64_t s) { return t.base + s * t.entryBytes; }
@@ -406,6 +479,19 @@ __global__ void __launch_bounds__(256) programKernel(const __grid_constant__ Pro
                         uint64_t k = 0;
                         for (int i = 0; i < 8; i++) k = (k << 8) | (i < n ? c->bytes[b0 + i] : 0);
                         r.v = (s128) (int64_t) k;
+                     }
+                     break;
+                  }
+                  case LDB_OP_STRCODE: { // string → its dictionary code; b = 1 inserts an absent string, b = 0 gives NULL for it
+                     ProgCol tmp;
+                     int64_t at;
+                     const ProgCol* c = cellOf(p.cols[in.a], regs, row, tmp, at);
+                     r.null = !c || colIsNull(*c, at);
+                     if (!r.null) {
+                        const int32_t* off = (const int32_t*) c->data + at;
+                        const int32_t code = dictCode(p.dicts[in.arg], c->bytes + off[0], off[1] - off[0], in.b);
+                        r.null = code < 0;
+                        r.v = code < 0 ? 0 : code;
                      }
                      break;
                   }
@@ -702,6 +788,72 @@ void launchRadixSortPairs(unsigned long long* keys, uint32_t* vals, unsigned lon
       std::swap(vin, vout);
    }
    // 8 passes: the result is back in `keys` / `vals`
+}
+
+// ---------------------------------------------------------------- multi-key ORDER BY, dictionary ranks and export
+// The sort words of one key at the current permutation: an LSD composition of launchRadixSortPairs (stable) sorts by the last key
+// first; a utf8 key is its length word, then its 8-byte chunks from the last to the first.  Zero padding makes a proper prefix tie
+// with its extension on every chunk, and the length pass, run before them, puts the shorter one first: bytewise order with
+// unsigned bytes, the order of LDB_OP_STRCMP.
+__global__ void buildSortWordsKernel(const uint8_t* col, const uint8_t* bytes, int elemBytes, int kind, int chunk, int64_t n, int descending, int first,
+                                     uint32_t* ids, unsigned long long* keys, int32_t* maxLen) {
+   int32_t longest = 0;
+   for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t) gridDim.x * blockDim.x) {
+      const uint32_t row = first ? (uint32_t) i : ids[i];
+      if (first) ids[i] = row;
+      unsigned long long k = 0;
+      if (kind == 0) {
+         const int64_t v = elemBytes == 4 ? (int64_t) ((const int32_t*) col)[row] : *(const int64_t*) (col + (size_t) row * elemBytes);
+         k = (unsigned long long) v ^ 0x8000000000000000ull;
+      } else {
+         const int32_t* off = (const int32_t*) col + row;
+         const int32_t b = off[0], len = off[1] - off[0];
+         if (kind == 1) {
+            k = (unsigned long long) (uint32_t) len;
+            longest = len > longest ? len : longest;
+         } else {
+            for (int j = 0; j < 8; j++) {
+               const int32_t at = chunk * 8 + j;
+               k = (k << 8) | (at < len ? bytes[b + at] : 0u);
+            }
+         }
+      }
+      keys[i] = descending ? ~k : k;
+   }
+   if (kind == 1) {
+      longest = (int32_t) __reduce_max_sync(0xffffffffu, (unsigned) longest);
+      if ((threadIdx.x & 31) == 0 && longest) atomicMax(maxLen, longest);
+   }
+}
+void launchBuildSortWords(const uint8_t* col, const uint8_t* bytes, int elemBytes, int kind, int chunk, int64_t n, int descending, int first,
+                          uint32_t* ids, unsigned long long* keys, int32_t* maxLen, int smCount, cudaStream_t s) {
+   int grid = (int) std::min<int64_t>(std::max<int64_t>((n + 255) / 256, 1), (int64_t) smCount * 8);
+   buildSortWordsKernel<<<grid, 256, 0, s>>>(col, bytes, elemBytes, kind, chunk, n, descending, first, ids, keys, maxLen);
+}
+__global__ void scatterRanksKernel(const uint32_t* ids, int64_t n, int32_t* rank) {
+   for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t) gridDim.x * blockDim.x) rank[ids[i]] = (int32_t) i;
+}
+void launchScatterRanks(const uint32_t* ids, int64_t n, int32_t* rank, int smCount, cudaStream_t s) {
+   int grid = (int) std::min<int64_t>(std::max<int64_t>((n + 255) / 256, 1), (int64_t) smCount * 8);
+   scatterRanksKernel<<<grid, 256, 0, s>>>(ids, n, rank);
+}
+__global__ void dictLengthsKernel(const int32_t* len, int64_t n, uint32_t* offsets) {
+   for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += (int64_t) gridDim.x * blockDim.x) offsets[i] = i < n ? (uint32_t) len[i] : 0u;
+}
+// one warp per code
+__global__ void dictCopyKernel(DictDev d, int64_t n, const uint32_t* offsets, uint8_t* out) {
+   const int lane = threadIdx.x & 31;
+   for (int64_t c = ((int64_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5; c < n; c += ((int64_t) gridDim.x * blockDim.x) >> 5) {
+      const uint8_t* src = d.arena + d.entryOff[c];
+      uint8_t* dst = out + offsets[c];
+      for (int32_t i = lane; i < d.entryLen[c]; i += 32) dst[i] = src[i];
+   }
+}
+void launchDictExport(const DictDev& d, int64_t n, uint32_t* offsets, uint8_t* bytes, int smCount, cudaStream_t s) {
+   int grid = (int) std::min<int64_t>(std::max<int64_t>((n + 256) / 256, 1), (int64_t) smCount * 8);
+   dictLengthsKernel<<<grid, 256, 0, s>>>(d.entryLen, n, offsets);
+   sortScanKernel<<<1, 1024, 0, s>>>(offsets, n + 1); // exclusive: offsets[n] = total bytes
+   if (n) dictCopyKernel<<<(int) std::min<int64_t>((n + 7) / 8, (int64_t) smCount * 16), 256, 0, s>>>(d, n, offsets, bytes);
 }
 
 } // namespace ldb

@@ -66,7 +66,26 @@ struct HashAggDev {
    unsigned long long* count; // groups
    int32_t* error;            // 1 = table full
 };
-// The kernel takes ProgramParams by value (__grid_constant__): 3 176 bytes with the limits above, within the classic 4 096-byte
+// string dictionary (LDB_STATE_DICT): a concurrent hash set of byte strings → dense int32 codes 0..n-1, in HBM
+//   slots[mask + 1]  u64 = {tag:32 (high 32 bits of the string's hash) | state:32}; state 0 empty (the whole word is 0),
+//                    kDictWriting while its claimer copies the string, kDictFailed when the claimer gave up, else code + 1
+//   entryOff/Len     per code: the string's arena offset and length
+//   arena            the strings' bytes, appended in claim order
+//   ctr              [0] arena cursor, [1] next code, [2] low 32 bits: error word (1 directory full or probe bound, 2 arena
+//                    full, 3 code past INT32_MAX)
+struct DictDev {
+   unsigned long long* slots;
+   uint64_t mask;
+   int64_t* entryOff;
+   int32_t* entryLen;
+   uint8_t* arena;
+   unsigned long long* ctr;
+   int64_t arenaCap;
+   int64_t codeCap; // codes 0..codeCap-1 fit the entry arrays and int32
+};
+constexpr uint32_t kDictWriting = 0xffffffffu, kDictFailed = 0xfffffffeu;
+
+// The kernel takes ProgramParams by value (__grid_constant__): 3 432 bytes with the limits above, within the classic 4 096-byte
 // kernel-parameter limit (program_rt.cpp checks it at compile time).
 struct ProgramParams {
    int64_t nRows;
@@ -80,6 +99,7 @@ struct ProgramParams {
    uint8_t strings[kProgMaxStrings][kProgStringBytes];
    int32_t stringLen[kProgMaxStrings];
    JoinTableDev tables[kProgMaxTables];
+   DictDev dicts[kProgMaxTables]; // tables[k] is a string dictionary: dicts[k] (LDB_OP_STRCODE)
    int32_t filterReg; // -1: every row passes
    int32_t sinkKind;  // 1 hash aggregation, 2 join-table build, 3 materialize
    // sink 1
@@ -107,5 +127,13 @@ void launchHashAggExport(const HashAggDev& t, int64_t* const* keyCols, uint8_t* 
 // order-preserving 64-bit sort keys + row ids from one fixed-width column (low 8 bytes of a cell, sign bit flipped; inverted for DESC)
 void launchBuildSortKeys(const uint8_t* col, int elemBytes, int64_t n, int descending, unsigned long long* keys, uint32_t* ids, int smCount, cudaStream_t s);
 void launchRadixSortPairs(unsigned long long* keys, uint32_t* vals, unsigned long long* keysTmp, uint32_t* valsTmp, int64_t n, unsigned int* histScratch, int smCount, cudaStream_t s);
+// multi-key ORDER BY: the 64-bit sort words of one key at the current permutation `ids` (first = 1: ids := 0..n-1 first).
+// kind 0: a fixed-width cell (low 8 bytes, sign bit flipped); kind 1: a utf8 cell's length (the longest is atomicMax'ed into
+// *maxLen); kind 2: bytes [8 chunk, 8 chunk + 8) of a utf8 cell, zero padded, big-endian, unsigned.  DESC inverts the word.
+void launchBuildSortWords(const uint8_t* col, const uint8_t* bytes, int elemBytes, int kind, int chunk, int64_t n, int descending, int first,
+                          uint32_t* ids, unsigned long long* keys, int32_t* maxLen, int smCount, cudaStream_t s);
+void launchScatterRanks(const uint32_t* ids, int64_t n, int32_t* rank, int smCount, cudaStream_t s);
+// dictionary → table: offsets[0..n] (exclusive scan of the lengths) and the bytes of code i at offsets[i]
+void launchDictExport(const DictDev& d, int64_t n, uint32_t* offsets, uint8_t* bytes, int smCount, cudaStream_t s);
 
 } // namespace ldb

@@ -241,6 +241,139 @@ int ldb_gpu_hashagg_to_table(LdbState* s, const char* name, LdbTable** out, LdbE
 
 static_assert(sizeof(ProgramParams) <= 4096, "ProgramParams exceeds the 4 KB kernel-parameter limit");
 
+// ---------------------------------------------------------------- string dictionaries
+static void checkDict(LdbState* s) {
+   if (!s || s->kind != LDB_STATE_DICT) failP(LDB_ERR_INVALID, "not a string dictionary");
+}
+// the dictionary's counters {arena bytes, codes}, after its error word is checked (synchronises)
+static std::pair<int64_t, int64_t> checkDictError(LdbState* s) {
+   unsigned long long c[3] = {0, 0, 0};
+   LDB_CUDA(cudaMemcpyAsync(c, s->dict.ctr, sizeof(c), cudaMemcpyDeviceToHost, s->ctx->compute));
+   s->ctx->syncStream(s->ctx->compute);
+   switch ((uint32_t) c[2]) {
+      case 0: break;
+      case 1: failP(LDB_ERR_CAPACITY, "string dictionary full: more distinct strings than expected_strings allowed (recreate it larger)");
+      case 2: failP(LDB_ERR_CAPACITY, "string dictionary arena full: more string bytes than expected_bytes allowed (recreate it larger)");
+      case 3: failP(LDB_ERR_CAPACITY, "string dictionary: a code would pass INT32_MAX");
+      default: failP(LDB_ERR_CAPACITY, "string dictionary error word " + std::to_string((uint32_t) c[2]));
+   }
+   return {(int64_t) c[0], (int64_t) c[1]};
+}
+
+// row ids of the single-batch table `t` (n rows, n < 2^32) ordered by the keys (column index, descending): device buffer of n
+// uint32 (released by the caller with stagingRelease).  The one place that knows the string order: ORDER BY and dictionary ranks.
+static uint32_t* sortRows(LdbTable* t, const std::vector<std::pair<int, int>>& keys, int64_t n) {
+   LdbContext* ctx = t->ctx;
+   LdbBatch& b = t->batches[0];
+   const size_t rows = (size_t) std::max<int64_t>(n, 1);
+   uint32_t* dv = (uint32_t*) ctx->stagingAlloc(rows * 4);
+   if (n == 0) return dv;
+   unsigned long long* dk = (unsigned long long*) ctx->stagingAlloc(rows * 8);
+   unsigned long long* dk2 = (unsigned long long*) ctx->stagingAlloc(rows * 8);
+   uint32_t* dv2 = (uint32_t*) ctx->stagingAlloc(rows * 4);
+   unsigned int* hist = (unsigned int*) ctx->stagingAlloc((size_t) ((n + 4095) / 4096) * 256 * 4);
+   int32_t* maxLen = (int32_t*) ctx->stagingAlloc(16);
+   int first = 1;
+   auto pass = [&](int c, int kind, int chunk, int desc) {
+      ctx->launch("radix_sort", [&] {
+         launchBuildSortWords((const uint8_t*) b.data[c], (const uint8_t*) b.bytes[c], b.elemBytes[c], kind, chunk, n, desc, first, dv, dk, maxLen, ctx->smCount, ctx->compute);
+         launchRadixSortPairs(dk, dv, dk2, dv2, n, hist, ctx->smCount, ctx->compute);
+      });
+      first = 0;
+   };
+   for (size_t k = keys.size(); k-- > 0;) {
+      const int c = keys[k].first, desc = keys[k].second;
+      if (t->columns[c].type != LDB_UTF8) {
+         pass(c, 0, 0, desc);
+         continue;
+      }
+      int32_t longest = 0;
+      LDB_CUDA(cudaMemsetAsync(maxLen, 0, 4, ctx->compute));
+      pass(c, 1, 0, desc); // lengths: the least significant word of a string
+      LDB_CUDA(cudaMemcpyAsync(&longest, maxLen, 4, cudaMemcpyDeviceToHost, ctx->compute));
+      ctx->syncStream(ctx->compute);
+      for (int chunk = (longest + 7) / 8; chunk-- > 0;) pass(c, 2, chunk, desc);
+   }
+   ctx->syncStream(ctx->compute);
+   for (void* p : {(void*) dk, (void*) dk2, (void*) dv2, (void*) hist, (void*) maxLen}) ctx->stagingRelease(p);
+   return dv;
+}
+
+int ldb_gpu_dict_create(LdbContext* ctx, int64_t expected_strings, int64_t expected_bytes, LdbState** out, LdbError* err) {
+   return guardedP(err, [&] {
+      if (!ctx || !out) failP(LDB_ERR_INVALID, "null argument");
+      if (expected_strings < 0 || expected_bytes < 0) failP(LDB_ERR_INVALID, "negative dictionary size");
+      if (expected_strings > ((int64_t) 1 << 30)) failP(LDB_ERR_UNSUPPORTED, "a dictionary holds at most 2^30 expected strings (codes are int32)");
+      LDB_CUDA(cudaSetDevice(ctx->device));
+      auto* s = new LdbState;
+      s->ctx = ctx;
+      s->kind = LDB_STATE_DICT;
+      ctx->states.push_back(s);
+      auto alloc = [&](size_t bytes) {
+         void* p = ctx->stagingAlloc(std::max<size_t>(bytes, 16));
+         s->allocations.push_back(p);
+         return p;
+      };
+      DictDev& dd = s->dict;
+      const uint64_t cap = nextPow2P((uint64_t) std::max<int64_t>(expected_strings, 8) * 2);
+      dd.mask = cap - 1;
+      dd.slots = (unsigned long long*) alloc(cap * 8);
+      dd.entryOff = (int64_t*) alloc(cap * 8);
+      dd.entryLen = (int32_t*) alloc(cap * 4);
+      dd.arenaCap = std::max<int64_t>(expected_bytes, 1);
+      dd.arena = (uint8_t*) alloc((size_t) dd.arenaCap);
+      dd.ctr = (unsigned long long*) alloc(32);
+      dd.codeCap = std::min<int64_t>((int64_t) cap, (int64_t) INT32_MAX + 1);
+      LDB_CUDA(cudaMemsetAsync(dd.slots, 0, cap * 8, ctx->compute));
+      LDB_CUDA(cudaMemsetAsync(dd.ctr, 0, 32, ctx->compute));
+      *out = s;
+   });
+}
+int ldb_gpu_dict_count(LdbState* s, int64_t* n_strings, LdbError* err) {
+   return guardedP(err, [&] {
+      checkDict(s);
+      if (!n_strings) failP(LDB_ERR_INVALID, "null argument");
+      LDB_CUDA(cudaSetDevice(s->ctx->device));
+      *n_strings = checkDictError(s).second;
+   });
+}
+int ldb_gpu_dict_to_table(LdbState* s, const char* name, LdbTable** out, LdbError* err) {
+   return guardedP(err, [&] {
+      checkDict(s);
+      if (!out) failP(LDB_ERR_INVALID, "null argument");
+      LdbContext* ctx = s->ctx;
+      LDB_CUDA(cudaSetDevice(ctx->device));
+      const std::pair<int64_t, int64_t> used = checkDictError(s);
+      const int64_t bytes = used.first, n = used.second;
+      if (bytes > (int64_t) INT32_MAX) failP(LDB_ERR_UNSUPPORTED, "dictionary strings exceed 2^31 - 1 bytes (utf8 offsets are int32)");
+      uint32_t* offsets = (uint32_t*) ctx->stagingAlloc((size_t) (n + 1) * 4);
+      uint8_t* data = (uint8_t*) ctx->stagingAlloc((size_t) std::max<int64_t>(bytes, 1));
+      int32_t* rank = (int32_t*) ctx->stagingAlloc((size_t) std::max<int64_t>(n, 1) * 4);
+      ctx->launch("dict_export", [&] { launchDictExport(s->dict, n, offsets, data, ctx->smCount, ctx->compute); });
+      auto* t = new LdbTable;
+      t->ctx = ctx;
+      t->name = name ? name : "dictionary";
+      t->columns.push_back({"str", LDB_UTF8, 0, 0});
+      t->columns.push_back({"rank", LDB_INT32, 0, 0});
+      LdbBatch b;
+      b.nRows = n;
+      b.data = {offsets, rank};
+      b.bytes = {data, nullptr};
+      b.elemBytes = {4, 4};
+      b.validity.assign(2, nullptr);
+      b.validityBitOffset.assign(2, 0);
+      b.owned = {offsets, data, rank};
+      t->numRows = n;
+      t->batches.push_back(std::move(b));
+      ctx->tables.push_back(t);
+      uint32_t* ids = sortRows(t, {{0, 0}}, n);
+      if (n) ctx->launch("dict_rank", [&] { launchScatterRanks(ids, n, rank, ctx->smCount, ctx->compute); });
+      ctx->syncStream(ctx->compute);
+      ctx->stagingRelease(ids);
+      *out = t;
+   });
+}
+
 // the pointers of column `ci` of batch `b` (validity bitmap or validity bytes included)
 static void bindColumn(ProgCol& pc, const LdbBatch& b, int ci) {
    pc.data = (const uint8_t*) b.data[ci];
@@ -298,13 +431,21 @@ static void runProgram(LdbContext* ctx, const LdbProgramDesc* d, const LdbProgra
    };
    bool usesRowid = false;
    int eachTable = -1;
+   bool probed[kProgMaxTables] = {}, coded[kProgMaxTables] = {}; // tables[k] read by PROBE / PROBE_EACH, by STRCODE
    for (int i = 0; i < d->n_instr; i++) {
       const LdbInstr& in = d->instr[i];
       if (in.dst >= kProgMaxRegs) failP(LDB_ERR_INVALID, "destination register out of range");
       switch (in.op) {
          case LDB_OP_LOAD:
             wantCol(in.arg, "LOAD");
-            if (colType(in.arg) == LDB_UTF8) failP(LDB_ERR_UNSUPPORTED, "LOAD of a string column (strings are operands of STRCMP / STRLIKE / STRKEY8 only)");
+            if (colType(in.arg) == LDB_UTF8) failP(LDB_ERR_UNSUPPORTED, "LOAD of a string column (strings are operands of STRCMP / STRLIKE / STRKEY8 / STRCODE only)");
+            break;
+         case LDB_OP_STRCODE:
+            if (in.a >= nCols || colType(in.a) != LDB_UTF8) failP(LDB_ERR_INVALID, "STRCODE needs a utf8 column");
+            wantCol(in.a, "STRCODE");
+            if (in.arg < 0 || in.arg >= d->n_tables) failP(LDB_ERR_INVALID, "STRCODE: dictionary index out of range");
+            if (in.b > 1) failP(LDB_ERR_INVALID, "STRCODE: b is 1 (insert) or 0 (lookup only)");
+            coded[in.arg] = true;
             break;
          case LDB_OP_CONST:
             if (in.arg < 0 || in.arg >= d->n_consts) failP(LDB_ERR_INVALID, "CONST: constant index out of range");
@@ -338,6 +479,7 @@ static void runProgram(LdbContext* ctx, const LdbProgramDesc* d, const LdbProgra
          case LDB_OP_PROBE:
             wantReg(in.a, "key");
             if (in.arg < 0 || in.arg >= d->n_tables) failP(LDB_ERR_INVALID, "PROBE: table index out of range");
+            probed[in.arg] = true;
             break;
          case LDB_OP_ROWID: usesRowid = true; break;
          case LDB_OP_PROBE_EACH:
@@ -347,6 +489,7 @@ static void runProgram(LdbContext* ctx, const LdbProgramDesc* d, const LdbProgra
             if (base.eachPc >= 0) failP(LDB_ERR_UNSUPPORTED, "at most one PROBE_EACH per program");
             base.eachPc = i;
             eachTable = in.arg;
+            probed[in.arg] = true;
             break;
          default: failP(LDB_ERR_UNSUPPORTED, "unknown opcode " + std::to_string(in.op));
       }
@@ -366,8 +509,18 @@ static void runProgram(LdbContext* ctx, const LdbProgramDesc* d, const LdbProgra
       memcpy(base.strings[c], d->strings[c], n);
       base.stringLen[c] = (int32_t) n;
    }
+   std::vector<LdbState*> dicts;
    for (int k = 0; k < d->n_tables; k++) {
       LdbState* js = d->tables[k];
+      if (js && js->kind == LDB_STATE_DICT) {
+         if (probed[k]) failP(LDB_ERR_INVALID, "PROBE / PROBE_EACH on a string dictionary (they take join tables)");
+         if (js->ctx != ctx) failP(LDB_ERR_INVALID, "string dictionary belongs to another context");
+         if (ctx->capturing) failP(LDB_ERR_UNSUPPORTED, "string dictionaries are not part of captured queries");
+         base.dicts[k] = js->dict;
+         dicts.push_back(js);
+         continue;
+      }
+      if (coded[k]) failP(LDB_ERR_INVALID, "STRCODE needs a string dictionary, not a join table");
       if (k == eachTable && js && js->kind == LDB_STATE_JOIN_TABLE && !(js->join.stride == 8 || js->join.direct))
          failP(LDB_ERR_UNSUPPORTED, "PROBE_EACH takes a plain single-key or direct-address join table (not a pair table or a group-join map)");
       if (!js || js->kind != LDB_STATE_JOIN_TABLE || js->join.stride == 16) failP(LDB_ERR_INVALID, "PROBE tables are single-key join tables");
@@ -487,16 +640,16 @@ static void runProgram(LdbContext* ctx, const LdbProgramDesc* d, const LdbProgra
    runBatches();
    // a probe run longer than the bound (PROBE_EACH), or a build that could not store a row (table full, the reserved pair, a key or
    // payload outside int32): fail rather than return a truncated match list or a table with rows missing
-   for (LdbState* js : {eachTable >= 0 ? d->tables[eachTable] : nullptr, d->sink_kind == LDB_SINK_JOIN_BUILD ? sink : nullptr}) {
-      if (!js) continue;
-      try {
-         ldb_gpu_check_join_error_internal(js);
-      } catch (...) {
-         ctx->syncStream(ctx->compute);
-         for (void* q : outOwned) ctx->stagingRelease(q);
-         for (void* q : dirs) ctx->stagingRelease(q);
-         throw;
-      }
+   // — and a dictionary that could not take a string
+   try {
+      for (LdbState* js : {eachTable >= 0 ? d->tables[eachTable] : nullptr, d->sink_kind == LDB_SINK_JOIN_BUILD ? sink : nullptr})
+         if (js) ldb_gpu_check_join_error_internal(js);
+      for (LdbState* ds : dicts) checkDictError(ds);
+   } catch (...) {
+      ctx->syncStream(ctx->compute);
+      for (void* q : outOwned) ctx->stagingRelease(q);
+      for (void* q : dirs) ctx->stagingRelease(q);
+      throw;
    }
    if (d->sink_kind == LDB_SINK_MATERIALIZE) {
       unsigned long long n = 0;
@@ -604,6 +757,102 @@ int ldb_gpu_table_gather(LdbTable* t, const char* column, const int64_t* row_ids
          }
       }
       ctx->syncStream(ctx->compute);
+   });
+}
+int ldb_gpu_table_order_by_keys(LdbTable* t, int32_t n_keys, const char* const* columns, const int32_t* descending, int64_t limit, int64_t* row_ids, int64_t* n_out, LdbError* err) {
+   return guardedP(err, [&] {
+      if (!t || !columns || !descending || !row_ids || !n_out) failP(LDB_ERR_INVALID, "null argument");
+      if (n_keys < 1) failP(LDB_ERR_INVALID, "ORDER BY needs at least one key");
+      LdbContext* ctx = t->ctx;
+      std::vector<std::pair<int, int>> keys;
+      for (int k = 0; k < n_keys; k++) {
+         const int c = t->colIndex(columns[k]);
+         if (c < 0) failP(LDB_ERR_INVALID, std::string("unknown column ") + (columns[k] ? columns[k] : "(null)"));
+         const int type = t->columns[c].type;
+         if (type == LDB_FLOAT32 || type == LDB_FLOAT64 || type == LDB_INT8 || type == LDB_INT16) failP(LDB_ERR_UNSUPPORTED, "ORDER BY column must be int32/date32/char(1)/int64/decimal/utf8");
+         keys.push_back({c, descending[k] ? 1 : 0});
+      }
+      if (t->batches.size() != 1) failP(LDB_ERR_UNSUPPORTED, "ORDER BY runs over single-batch tables (materialised results, exported groups)");
+      LdbBatch& b = t->batches[0];
+      const int64_t n = b.nRows;
+      if (n >= (int64_t) 1 << 32) failP(LDB_ERR_UNSUPPORTED, "ORDER BY handles up to 2^32 - 1 rows");
+      LDB_CUDA(cudaSetDevice(ctx->device));
+      ldb_gpu_wait_batch_internal(ctx, &b);
+      uint32_t* ids = sortRows(t, keys, n);
+      const int64_t m = std::min<int64_t>(n, limit < 0 ? n : limit);
+      std::vector<uint32_t> top((size_t) m);
+      if (m) LDB_CUDA(cudaMemcpyAsync(top.data(), ids, (size_t) m * 4, cudaMemcpyDeviceToHost, ctx->compute));
+      ctx->syncStream(ctx->compute);
+      ctx->stagingRelease(ids);
+      for (int64_t i = 0; i < m; i++) row_ids[i] = top[(size_t) i];
+      *n_out = m;
+   });
+}
+int ldb_gpu_table_gather_strings(LdbTable* t, const char* column, const int64_t* row_ids, int64_t n, int64_t* host_offsets, void* host_bytes, int64_t bytes_cap, int64_t* bytes_needed,
+                                 uint8_t* host_valid, LdbError* err) {
+   return guardedP(err, [&] {
+      if (!t || (n > 0 && !row_ids) || !host_offsets || !bytes_needed || n < 0) failP(LDB_ERR_INVALID, "null argument");
+      LdbContext* ctx = t->ctx;
+      const int c = t->colIndex(column);
+      if (c < 0) failP(LDB_ERR_INVALID, "unknown column");
+      if (t->columns[c].type != LDB_UTF8) failP(LDB_ERR_UNSUPPORTED, "gather_strings reads utf8 columns");
+      if (t->batches.size() != 1) failP(LDB_ERR_UNSUPPORTED, "gather runs over single-batch tables");
+      LdbBatch& b = t->batches[0];
+      for (int64_t i = 0; i < n; i++)
+         if (row_ids[i] < 0 || row_ids[i] >= b.nRows) failP(LDB_ERR_INVALID, "row id out of range");
+      LDB_CUDA(cudaSetDevice(ctx->device));
+      ldb_gpu_wait_batch_internal(ctx, &b);
+      // runs of consecutive row ids: [first index, end index) → the run's m + 1 offsets at `at` in `offs`
+      struct Run {
+         int64_t i, j;
+         size_t at;
+      };
+      std::vector<Run> runs;
+      for (int64_t i = 0, j; i < n; i = j) {
+         for (j = i + 1; j < n && row_ids[j] == row_ids[j - 1] + 1;) j++;
+         runs.push_back({i, j, 0});
+      }
+      std::vector<int32_t> offs;
+      for (Run& r : runs) {
+         r.at = offs.size();
+         offs.resize(offs.size() + (size_t) (r.j - r.i) + 1);
+      }
+      for (const Run& r : runs)
+         LDB_CUDA(cudaMemcpyAsync(offs.data() + r.at, (const int32_t*) b.data[c] + row_ids[r.i], (size_t) (r.j - r.i + 1) * 4, cudaMemcpyDeviceToHost, ctx->compute));
+      ctx->syncStream(ctx->compute);
+      int64_t total = 0;
+      for (const Run& r : runs) total += offs[r.at + (size_t) (r.j - r.i)] - offs[r.at];
+      *bytes_needed = total;
+      if (total > bytes_cap) failP(LDB_ERR_CAPACITY, "gather_strings: the strings need more than bytes_cap bytes (see bytes_needed)");
+      if (total > 0 && !host_bytes) failP(LDB_ERR_INVALID, "null argument");
+      const uint8_t* bitmap = c < (int) b.validity.size() ? (const uint8_t*) b.validity[c] : nullptr;
+      const uint8_t* vbytes = c < (int) b.validBytes.size() ? b.validBytes[c] : nullptr;
+      std::vector<std::vector<uint8_t>> bits(host_valid && bitmap && !vbytes ? runs.size() : 0);
+      int64_t pos = 0;
+      host_offsets[0] = 0;
+      for (size_t k = 0; k < runs.size(); k++) {
+         const Run& r = runs[k];
+         const size_t m = (size_t) (r.j - r.i);
+         for (size_t q = 0; q < m; q++) host_offsets[r.i + (int64_t) q + 1] = pos + offs[r.at + q + 1] - offs[r.at];
+         const int64_t len = offs[r.at + m] - offs[r.at];
+         if (len) LDB_CUDA(cudaMemcpyAsync((uint8_t*) host_bytes + pos, (const uint8_t*) b.bytes[c] + offs[r.at], (size_t) len, cudaMemcpyDeviceToHost, ctx->compute));
+         pos += len;
+         if (!host_valid) continue;
+         if (vbytes) {
+            LDB_CUDA(cudaMemcpyAsync(host_valid + r.i, vbytes + row_ids[r.i], m, cudaMemcpyDeviceToHost, ctx->compute));
+         } else if (bitmap) {
+            const int64_t bit0 = b.validityBitOffset[c] + row_ids[r.i];
+            bits[k].resize((size_t) ((bit0 % 8 + (int64_t) m + 7) / 8));
+            LDB_CUDA(cudaMemcpyAsync(bits[k].data(), bitmap + bit0 / 8, bits[k].size(), cudaMemcpyDeviceToHost, ctx->compute));
+         } else {
+            memset(host_valid + r.i, 1, m);
+         }
+      }
+      ctx->syncStream(ctx->compute);
+      for (size_t k = 0; k < bits.size(); k++) {
+         const int64_t bit0 = (b.validityBitOffset[c] + row_ids[runs[k].i]) % 8;
+         for (int64_t q = 0; q < runs[k].j - runs[k].i; q++) host_valid[runs[k].i + q] = (bits[k][(size_t) ((bit0 + q) >> 3)] >> ((bit0 + q) & 7)) & 1u;
+      }
    });
 }
 

@@ -8,6 +8,8 @@ An expression is a nested tuple:
   ("case", cond, a, b)                                       cond is true ? a : b
   ("i2f", a) ("fadd"|"fsub"|"fmul"|"fdiv", a, b) ("fcmp", op, a, b)
   ("strcmp", op, column, "constant") ("like", "prefix"|"suffix"|"contains", column, "text") ("strkey8", column)
+  ("strcode", dict_state, column[, "lookup"])                the string's int32 code in a string dictionary (dict_state): inserted when
+                                                             absent, or with "lookup" NULL when absent; a NULL string gives NULL
   ("year", a)                                                extract(year from date32)
   ("probe", join_table_state, key)                           payload, or NULL when the key is absent (semi / anti / mark / outer joins)
   ("probe_each", join_table_state, key[, "outer"])           payload of EACH match: what follows runs once per match (inner join; "outer":
@@ -15,7 +17,8 @@ An expression is a nested tuple:
                                                              per program; emitted once, never re-evaluated.
   ("rowid",)                                                 the scanned row's number in its table (a build payload for "fetch")
   ("fetch", side_table, row, "column")                       `column` of another table at the row `row` evaluates to (NULL row → NULL);
-                                                             accepted wherever a column name is, also as the column of strcmp / like / strkey8
+                                                             accepted wherever a column name is, also as the column of strcmp / like /
+                                                             strkey8 / strcode
 This is test/bench plumbing over the C-ABI, like runtime.py; in a LingoDB build the sub-operator lowering would emit LdbInstr lists."""
 import ctypes as C
 import struct
@@ -25,7 +28,7 @@ from . import capi
 from .capi import Error, check
 
 OPS = dict(load=1, const=2, add=3, sub=4, mul=5, div=6, neg=7, cmp=8, **{"and": 9, "or": 10, "not": 11}, isnull=12, select=13, i2f=14, fadd=15, fsub=16, fmul=17,
-           fdiv=18, fcmp=19, strcmp=20, strlike=21, year=22, probe=23, strkey8=24, rowid=25, probe_each=26)
+           fdiv=18, fcmp=19, strcmp=20, strlike=21, year=22, probe=23, strkey8=24, rowid=25, probe_each=26, strcode=27)
 CMP = {"=": 0, "!=": 1, "<": 2, "<=": 3, ">": 4, ">=": 5}
 AGG = dict(sum=1, sum_f64=2, count=3, count_star=4, min=5, max=6, min_f64=7, max_f64=8, any=9)
 LIKE = dict(prefix=0, suffix=1, contains=2)
@@ -73,7 +76,7 @@ class Builder:
         for op, dst, a, b, arg in self.instr:
             if op == OPS["load"]:
                 arg = fix(arg)
-            elif op in (OPS["strcmp"], OPS["strlike"], OPS["strkey8"]):
+            elif op in (OPS["strcmp"], OPS["strlike"], OPS["strkey8"], OPS["strcode"]):
                 a = fix(a)
             out.append((op, dst, a, b, arg))
         return out
@@ -136,6 +139,12 @@ class Builder:
             r = self._emit("strlike", self._col(e[2]), LIKE[e[1]], self._string(e[3]))
         elif k == "strkey8":
             r = self._emit("strkey8", self._col(e[1]))
+        elif k == "strcode":
+            if len(e) > 3 and e[3] != "lookup":
+                raise ValueError(f"strcode mode is 'lookup' or omitted, not {e[3]!r}")
+            if e[1] not in self.tables:
+                self.tables.append(e[1])
+            r = self._emit("strcode", self._col(e[2]), int(len(e) <= 3), self.tables.index(e[1]))
         elif k == "probe":
             if e[1] not in self.tables:
                 self.tables.append(e[1])
@@ -304,6 +313,35 @@ class RawTable:
                 out.append(int.from_bytes(raw[i * cell_bytes:(i + 1) * cell_bytes], "little", signed=True))
         return out
 
+    def order_by_keys(self, keys: list, limit=-1):
+        """ORDER BY over [(column, descending), …] (fixed-width or utf8 columns); the first `limit` row ids (all with -1)."""
+        n = self.num_rows
+        names = [c.encode() for c, _ in keys]
+        cols = (C.c_char_p * max(1, len(keys)))(*names)
+        desc = (C.c_int32 * max(1, len(keys)))(*[int(bool(d)) for _, d in keys])
+        ids = (C.c_int64 * max(1, n))()
+        m, e = C.c_int64(), Error()
+        check(self.ctx.L.ldb_gpu_table_order_by_keys(self.h, len(keys), cols, desc, limit, ids, C.byref(m), C.byref(e)), e)
+        return list(ids[: m.value])
+
+    def gather_strings(self, column: str, row_ids: list, decode=True) -> list:
+        """The utf8 cells at `row_ids`: str (bytes with decode=False), None for NULL."""
+        n = len(row_ids)
+        ids = (C.c_int64 * max(1, n))(*row_ids)
+        offs = (C.c_int64 * (n + 1))()
+        valid = (C.c_uint8 * max(1, n))()
+        need, e = C.c_int64(), Error()
+        rc = self.ctx.L.ldb_gpu_table_gather_strings(self.h, column.encode(), ids, n, offs, None, 0, C.byref(need), valid, C.byref(e))
+        if rc == capi.LDB_ERR_CAPACITY and need.value > 0:
+            buf = (C.c_uint8 * need.value)()
+            rc = self.ctx.L.ldb_gpu_table_gather_strings(self.h, column.encode(), ids, n, offs, buf, need.value, C.byref(need), valid, C.byref(e))
+            raw = bytes(buf)
+        else:
+            raw = b""
+        check(rc, e)
+        out = [raw[offs[i]:offs[i + 1]] if valid[i] else None for i in range(n)]
+        return [s.decode() if decode and s is not None else s for s in out]
+
     def destroy(self):
         if self.h:
             self.ctx.L.ldb_gpu_table_destroy(self.h)
@@ -313,4 +351,24 @@ class RawTable:
 def groups_table(ctx, state, name="groups") -> RawTable:
     t, e = C.c_void_p(), Error()
     check(ctx.L.ldb_gpu_hashagg_to_table(state, name.encode(), C.byref(t), C.byref(e)), e)
+    return RawTable(ctx, t)
+
+
+def dict_state(ctx, expected_strings: int, expected_bytes: int) -> C.c_void_p:
+    """A string dictionary for ("strcode", state, column): codes 0..n-1, which string gets which code is unspecified."""
+    s, e = C.c_void_p(), Error()
+    check(ctx.L.ldb_gpu_dict_create(ctx.h, int(expected_strings), int(expected_bytes), C.byref(s), C.byref(e)), e)
+    return s
+
+
+def dict_count(ctx, state) -> int:
+    n, e = C.c_int64(), Error()
+    check(ctx.L.ldb_gpu_dict_count(state, C.byref(n), C.byref(e)), e)
+    return n.value
+
+
+def dict_table(ctx, state, name="dictionary") -> RawTable:
+    """The dictionary as a table, row i = code i: "str" (utf8) and "rank" (int32, the string's position in bytewise order)."""
+    t, e = C.c_void_p(), Error()
+    check(ctx.L.ldb_gpu_dict_to_table(state, name.encode(), C.byref(t), C.byref(e)), e)
     return RawTable(ctx, t)
