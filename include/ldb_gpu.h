@@ -97,6 +97,9 @@ typedef struct LdbTable LdbTable;
 int ldb_gpu_table_create(LdbContext* ctx, const char* name, int32_t n_cols, const LdbColumnSchema* schema, LdbTable** out, LdbError* err);
 /* Append one record batch.  HOST buffers are staged to HBM with asynchronous copies on the context's
  * copy stream (the scan of batch k overlaps the copy of batch k+1); DEVICE buffers are borrowed.
+ * Borrowed DEVICE buffers must not change while the batch belongs to the table (until ldb_gpu_table_clear /
+ * _destroy): the table caches what it derived from them — column min/max statistics and the encoded column copies the
+ * scan pipelines read (ldb_gpu_set_encoded_scan).  To change the data, clear the table and append it again.
  * utf8 columns additionally need `utf8_bytes[col]` = size of buffers[2] (0 for other columns). */
 int ldb_gpu_table_append_batch(LdbTable* t, int64_t n_rows, const LdbArrayView* columns, const int64_t* utf8_bytes, int32_t location, LdbError* err);
 int ldb_gpu_table_clear(LdbTable* t, LdbError* err); /* drop all batches (staging memory is pooled) */
@@ -117,6 +120,14 @@ void ldb_gpu_set_tuning(int32_t stages_build, int32_t stages_probe_agg, int32_t 
  * their filter SHAPE (none / one int32 compare / one int32 range — what the reference's JIT would emit for the same pushed-down predicate);
  * 0 = always the descriptor-driven form.  Results are identical; also settable through LDB_SPECIALISE. */
 void ldb_gpu_set_filter_specialisation(int32_t on);
+/* 1 (default) = scan-reduce / scan-group-by pipelines (Q6, Q1 signatures) read a DEVICE batch from a frame-of-reference copy of its
+ * fixed-width columns (csrc/encode.cu: per 64 Ki-row block a base, values in 1/2/4/8 bytes; Q1 ~12 B/row instead of 76), built
+ * once on the first such pipeline that needs it and freed by ldb_gpu_table_clear / _destroy; 0 = Arrow cells only.  Results are
+ * identical; also settable through LDB_ENCODED_SCAN.  A copy that cannot be allocated, or that would take the context past
+ * LDB_ENCODED_SCAN_MAX_BYTES (environment, read at context creation; default unlimited), leaves its batch in Arrow layout.
+ * Bytes the copies of a context hold now: */
+void ldb_gpu_set_encoded_scan(int32_t on);
+int64_t ldb_gpu_context_encoded_bytes(LdbContext* ctx);
 /* experiment hook: nanoseconds the producer lane / the consumer warps of the warp-specialised tile driver pause between two polls of
  * a tile barrier (0 = poll back to back; also LDB_PRODUCER_SLEEP_NS / LDB_CONSUMER_SLEEP_NS) */
 void ldb_gpu_set_poll_pause(int32_t producer_ns, int32_t consumer_ns);

@@ -153,6 +153,8 @@ SIGNATURES = {
     "ldb_gpu_effective_cpus": (C.c_int32, []),
     "ldb_gpu_set_tuning": (None, [C.c_int32] * 5),
     "ldb_gpu_set_filter_specialisation": (None, [C.c_int32]),
+    "ldb_gpu_set_encoded_scan": (None, [C.c_int32]),
+    "ldb_gpu_context_encoded_bytes": (C.c_int64, [_P]),
     "ldb_gpu_set_poll_pause": (None, [C.c_int32, C.c_int32]),
     "ldb_gpu_launch_count": (C.c_int64, [_P]),
     "ldb_gpu_timer_start": (C.c_int, [_P, _E]),

@@ -104,6 +104,11 @@ struct LdbContext {
    std::atomic<uint64_t> stagingGen{0};      // bumped by ldb_gpu_table_clear: workers order their next write after computeDone
    std::atomic<int64_t> stagingLaunches{0};  // unpack kernels launched by the staging workers
    std::atomic<int64_t> rawStagedRows{0};    // rows the raw copiers shipped uncompressed (the rest was packed)
+   // encoded column copies of DEVICE batches (encode.cu, LdbBatch::enc): built on their own stream, never captured
+   cudaStream_t encodeStream = nullptr;
+   int64_t encodedBytes = 0;              // device bytes the copies hold now
+   int64_t encodedBudget = INT64_MAX;     // LDB_ENCODED_SCAN_MAX_BYTES: beyond it batches are scanned in Arrow layout
+   int64_t encodeLaunches = 0;            // encoder kernels launched (part of ldb_gpu_launch_count)
 
    // Host waits SLEEP instead of spinning (cudaEventBlockingSync): the container's CPU quota is shared with the staging
    // threads and, on a multi-GPU box, with the other ranks — a spinning waiter would burn a whole CPU of it.
@@ -165,6 +170,16 @@ struct LdbBatch {
    std::vector<void*> owned;       // staging buffers to give back on clear
    cudaEvent_t ready = nullptr;    // H2D of this batch finished (null for borrowed device batches)
    std::shared_ptr<ldb::PackedBatch> packed; // columns staged through the compressed staging engine (host wait + worker events)
+   bool borrowed = false;          // appended as LDB_MEM_DEVICE: the caller's buffers, unchanged while the batch belongs to the table
+   // per column: frame-of-reference copy read by the K1/K2 scan instead of the Arrow cells (kernels.h kEncodeTileHeader), empty until
+   // the first such pipeline needs it
+   struct Encoded {
+      uint8_t* data = nullptr;
+      int32_t width = 0, tileRows = 0;
+      int64_t bytes = 0;
+      bool failed = false; // allocation failed or over the budget: this batch is scanned in Arrow layout
+   };
+   std::vector<Encoded> enc;
 };
 struct LdbColumn {
    std::string name;
@@ -209,6 +224,11 @@ struct LdbGraph {
 
 // order the compute stream after the staging of one batch (runtime.cpp)
 void ldb_gpu_wait_batch_internal(LdbContext* ctx, const struct LdbBatch* b);
+// builds the missing encoded copies of columns cols[0..n) of a borrowed DEVICE batch (encode.cu) for tiles of `tileRows` rows;
+// true when every one of them has a copy.  Runs outside any capture and waits for its work on the host.
+bool ldb_gpu_encode_batch_internal(LdbContext* ctx, LdbTable* t, LdbBatch& b, const int* cols, int n, int tileRows);
+// frees the encoded copies of a batch (the caller made sure no queued kernel reads them)
+void ldb_gpu_free_encoded_internal(LdbContext* ctx, LdbBatch& b);
 
 struct LdbState {
    LdbContext* ctx;

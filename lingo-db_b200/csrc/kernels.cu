@@ -57,12 +57,56 @@ struct GlobalTile {
       else return lo64(col, lr) >> 63;
    }
 };
+// Encoded layout (kernels.h kEncodeTileHeader): a column tile is {base of its block, 0} followed by the tile's values packed in W
+// bytes each.  A value is base + the zero-extended field; width and base are uniform per column and tile, so the decode is a
+// shared load of the 32-bit word holding the field, a shift, a mask and an add.  Values come back exactly, so filters, group ids
+// and aggregates run unchanged on them.
+template <>
+struct SmemTile<kDecEncoded> {
+   uint32_t stage;
+   const StagedCols* sc;
+   // the W-byte field of row lr (W <= 4): a field never straddles an aligned 32-bit word
+   __device__ __forceinline__ uint32_t field32(int col, int lr) const {
+      const uint32_t a = stage + (uint32_t) sc->smemOffset[col] + kEncodeTileHeader + ((uint32_t) lr << sc->encShift[col]);
+      return ((uint32_t) ldShared32(a & ~3u) >> ((a & 3u) * 8)) & sc->encMask[col];
+   }
+   __device__ __forceinline__ int32_t i32(int col, int lr) const { // int32 columns are encoded in at most 4 bytes
+      return (int32_t) ((uint32_t) ldShared32(stage + sc->smemOffset[col]) + field32(col, lr));
+   }
+   __device__ __forceinline__ int64_t lo64(int col, int lr) const {
+      const uint32_t h = stage + (uint32_t) sc->smemOffset[col];
+      if (sc->encShift[col] == 3) return (int64_t) ((uint64_t) ldShared64(h) + (uint64_t) ldShared64(h + kEncodeTileHeader + (uint32_t) lr * 8));
+      return (int64_t) ((uint64_t) ldShared64(h) + field32(col, lr));
+   }
+   __device__ __forceinline__ int64_t hi64(int col, int lr) const { return lo64(col, lr) >> 63; }
+};
+template <>
+struct GlobalTile<kDecEncoded> {
+   int64_t rowBase; // first row of a tile
+   const StagedCols* sc;
+   __device__ __forceinline__ const uint8_t* tileStart(int col) const {
+      return sc->base[col] + (rowBase / sc->tileRows) * ((int64_t) kEncodeTileHeader + (int64_t) sc->tileRows * sc->elemBytes[col]);
+   }
+   __device__ __forceinline__ uint64_t field(int col, int lr) const {
+      const uint8_t* p = tileStart(col) + kEncodeTileHeader;
+      switch (sc->elemBytes[col]) {
+         case 1: return __ldg(p + lr);
+         case 2: return __ldg((const uint16_t*) p + lr);
+         case 4: return __ldg((const uint32_t*) p + lr);
+         default: return __ldg((const unsigned long long*) p + lr);
+      }
+   }
+   __device__ __forceinline__ uint64_t base(int col) const { return (uint64_t) __ldg((const long long*) tileStart(col)); }
+   __device__ __forceinline__ int32_t i32(int col, int lr) const { return (int32_t) (uint32_t) (base(col) + field(col, lr)); }
+   __device__ __forceinline__ int64_t lo64(int col, int lr) const { return (int64_t) (base(col) + field(col, lr)); }
+   __device__ __forceinline__ int64_t hi64(int col, int lr) const { return lo64(col, lr) >> 63; }
+};
 __device__ __forceinline__ void issueTile(const StagedCols& sc, uint8_t* smem, uint64_t* bars /* full[] */, int64_t tile, int s) {
    const uint64_t policy = evictFirstPolicy();
    mbarExpectTx(&bars[s], (uint32_t) sc.stageBytes);
    const uint32_t dst = smemAddr(smem) + (uint32_t) s * sc.stageBytes;
    for (int c = 0; c < sc.n; c++) {
-      const uint32_t bytes = (uint32_t) sc.elemBytes[c] * (uint32_t) sc.tileRows;
+      const uint32_t bytes = (uint32_t) sc.elemBytes[c] * (uint32_t) sc.tileRows + (uint32_t) sc.tileHeader;
       bulkLoad(dst + sc.smemOffset[c], sc.base[c] + (size_t) tile * bytes, bytes, &bars[s], policy);
    }
 }
@@ -669,6 +713,7 @@ static Tuning& tuningStorage() {
       x.rptBuild = envInt("LDB_RPT_BUILD", 2, 1, 4);
       x.rptStar = envInt("LDB_RPT_STAR", 2, 1, 4);
       x.specialise = envInt("LDB_SPECIALISE", 1, 0, 1);
+      x.encodedScan = envInt("LDB_ENCODED_SCAN", 1, 0, 1);
       x.producerSleepNs = envInt("LDB_PRODUCER_SLEEP_NS", 0, 0, 2000);
       x.consumerSleepNs = envInt("LDB_CONSUMER_SLEEP_NS", 0, 0, 2000);
       if (x.rptStar == 3) x.rptStar = 2;
@@ -688,6 +733,7 @@ void setTuning(const Tuning& t) {
    x.rptBuild = x.rptBuild >= 4 ? 4 : (x.rptBuild >= 2 ? 2 : 1);
    x.rptStar = x.rptStar >= 4 ? 4 : (x.rptStar >= 2 ? 2 : 1);
    x.specialise = x.specialise ? 1 : 0;
+   x.encodedScan = x.encodedScan ? 1 : 0;
    x.producerSleepNs = x.producerSleepNs < 0 ? 0 : (x.producerSleepNs > 2000 ? 2000 : x.producerSleepNs);
    x.consumerSleepNs = x.consumerSleepNs < 0 ? 0 : (x.consumerSleepNs > 2000 ? 2000 : x.consumerSleepNs);
    tuningStorage() = x;
@@ -899,9 +945,16 @@ static void launchGBd(const GroupByParams& p, int smCount, cudaStream_t s) {
    int grid = persistentGrid(scanGroupByKernel<DB, IN, NK, NV, As...>, p.src.cols, p.src.nRows, smCount, &dyn, kBlock);
    scanGroupByKernel<DB, IN, NK, NV, As...><<<grid, kBlock, dyn, s>>>(p);
 }
-template <int NK, int NV, class... As>
+// ENC: the signature is also compiled for the encoded layout (only without IN lists; scanGroupByEncodable says which)
+template <bool ENC, int NK, int NV, class... As>
 static void launchGB(const GroupByParams& p, int smCount, cudaStream_t s) {
    const bool in = hasInList(p.src.filters);
+   if constexpr (ENC) {
+      if (p.src.cols.decBytes == kDecEncoded) {
+         launchGBd<kDecEncoded, false, NK, NV, As...>(p, smCount, s);
+         return;
+      }
+   }
    if (p.src.cols.decBytes == 8) {
       if (in) launchGBd<8, true, NK, NV, As...>(p, smCount, s);
       else launchGBd<8, false, NK, NV, As...>(p, smCount, s);
@@ -914,27 +967,38 @@ using C0 = Agg<LDB_EXPR_COL, 0>;
 using C1 = Agg<LDB_EXPR_COL, 1>;
 using C2 = Agg<LDB_EXPR_COL, 2>;
 using ONE = Agg<LDB_EXPR_ONE>;
+// the signatures compiled for the encoded layout as well: Q1 and Q6, the two the encoded column copy exists for
+static const char* const kSigQ1 = "k2v4|0:0|0:1|2:1,2|3:1,2,3|0:2|4";
+static const char* const kSigQ6 = "k0v2|1:0,1";
+bool scanGroupByEncodable(const GroupByParams& p) {
+   const std::string sig = signature(p);
+   return (sig == kSigQ1 || sig == kSigQ6) && !hasInList(p.src.filters);
+}
 bool launchScanGroupBy(const GroupByParams& p, int smCount, cudaStream_t s, const char** why) {
    std::string sig = signature(p);
+   if (p.src.cols.decBytes == kDecEncoded && !scanGroupByEncodable(p)) {
+      *why = "group-by pipeline bound to the encoded layout has no encoded instantiation";
+      return false;
+   }
    // Q1 pricing summary: sum(a) sum(b) sum(b*(1-c)) sum(b*(1-c)*(1+d)) sum(c) count   (resources/sql/tpch/1.sql)
-   if (sig == "k2v4|0:0|0:1|2:1,2|3:1,2,3|0:2|4") {
-      launchGB<2, 4, C0, C1, Agg<LDB_EXPR_MUL_1MINUS, 1, 2>, Agg<LDB_EXPR_MUL_1MINUS_1PLUS, 1, 2, 3>, C2, ONE>(p, smCount, s);
+   if (sig == kSigQ1) {
+      launchGB<true, 2, 4, C0, C1, Agg<LDB_EXPR_MUL_1MINUS, 1, 2>, Agg<LDB_EXPR_MUL_1MINUS_1PLUS, 1, 2, 3>, C2, ONE>(p, smCount, s);
    } else if (sig == "k1v4|0:0|0:1|2:1,2|3:1,2,3|0:2|4") {
-      launchGB<1, 4, C0, C1, Agg<LDB_EXPR_MUL_1MINUS, 1, 2>, Agg<LDB_EXPR_MUL_1MINUS_1PLUS, 1, 2, 3>, C2, ONE>(p, smCount, s);
-   } else if (sig == "k0v2|1:0,1") { // Q6 forecast revenue: sum(a*b)
-      launchGB<0, 2, Agg<LDB_EXPR_MUL, 0, 1>>(p, smCount, s);
+      launchGB<false, 1, 4, C0, C1, Agg<LDB_EXPR_MUL_1MINUS, 1, 2>, Agg<LDB_EXPR_MUL_1MINUS_1PLUS, 1, 2, 3>, C2, ONE>(p, smCount, s);
+   } else if (sig == kSigQ6) { // Q6 forecast revenue: sum(a*b)
+      launchGB<true, 0, 2, Agg<LDB_EXPR_MUL, 0, 1>>(p, smCount, s);
    } else if (sig == "k0v2|2:0,1") { // keyless sum(a*(1-b))
-      launchGB<0, 2, Agg<LDB_EXPR_MUL_1MINUS, 0, 1>>(p, smCount, s);
+      launchGB<false, 0, 2, Agg<LDB_EXPR_MUL_1MINUS, 0, 1>>(p, smCount, s);
    } else if (sig == "k0v1|0:0|4") { // keyless sum(a), count
-      launchGB<0, 1, C0, ONE>(p, smCount, s);
+      launchGB<false, 0, 1, C0, ONE>(p, smCount, s);
    } else if (sig == "k1v2|2:0,1") { // group by k: sum(a*(1-b))
-      launchGB<1, 2, Agg<LDB_EXPR_MUL_1MINUS, 0, 1>>(p, smCount, s);
+      launchGB<false, 1, 2, Agg<LDB_EXPR_MUL_1MINUS, 0, 1>>(p, smCount, s);
    } else if (sig == "k2v2|2:0,1") {
-      launchGB<2, 2, Agg<LDB_EXPR_MUL_1MINUS, 0, 1>>(p, smCount, s);
+      launchGB<false, 2, 2, Agg<LDB_EXPR_MUL_1MINUS, 0, 1>>(p, smCount, s);
    } else if (sig == "k1v1|0:0|4") { // group by k: sum(a), count
-      launchGB<1, 1, C0, ONE>(p, smCount, s);
+      launchGB<false, 1, 1, C0, ONE>(p, smCount, s);
    } else if (sig == "k2v1|0:0|4") {
-      launchGB<2, 1, C0, ONE>(p, smCount, s);
+      launchGB<false, 2, 1, C0, ONE>(p, smCount, s);
    } else {
       static thread_local std::string msg;
       msg = "no compiled group-by pipeline for aggregate signature '" + sig + "' (register it in kernels.cu:launchScanGroupBy)";

@@ -93,19 +93,38 @@ struct Tuning {
    int rptStar;                                               // rows per thread of a K9 tile (1, 2 or 4)
    int producerSleepNs, consumerSleepNs;                      // pause between mbarrier polls in the warp-specialised tile driver (0 = poll)
    int specialise;                                            // 1: join pipelines run the filter-shape instantiations (kernels.cu FilterShape), 0: descriptor-driven only
+   int encodedScan;                                           // 1: K1/K2 scan DEVICE batches from their frame-of-reference copy (LdbBatch::enc), 0: Arrow layout only
 };
 const Tuning& tuning();
 void setTuning(const Tuning& t);
+
+// ---- frame-of-reference encoded column copy (encode.cu), read by K1/K2 in place of the Arrow cells of a DEVICE batch.
+// Per column one width W in {1, 2, 4, 8} bytes; per block of kEncodeBlockRows rows a base (the block minimum, int64); a value is
+// stored as (v - base) in W bytes, zero-extended on decode (exact modulo 2^64, so int32 columns and the low 8 bytes of a
+// decimal(p<19) cell come back bit for bit).  The copy is TILE-FRAMED for the K1/K2 tile of kEncodeTileRows rows: tile t of a
+// column starts at t * (kEncodeTileHeader + kEncodeTileRows * W) with a 16-byte header {base of the tile's block, 0} followed by
+// the tile's packed values.  One bulk copy then brings a tile's base with its values, and no thread loads a base from HBM.
+constexpr int64_t kEncodeBlockRows = 65536; // = kPackBlockRows of the compressed staging format: a tile never straddles two blocks
+constexpr int kEncodeTileHeader = 16;
+constexpr int kDecEncoded = 0; // StagedCols::decBytes / kernel DB parameter of the encoded layout
+inline int64_t encodedColumnBytes(int64_t nRows, int width, int tileRows) {
+   const int64_t tiles = (nRows + tileRows - 1) / tileRows;
+   return ((tiles * kEncodeTileHeader + nRows * width) + 15) / 16 * 16;
+}
+
 struct StagedCols {
    int32_t n;
    int32_t tileRows;   // rows per tile = kBlockThreads * rows-per-thread of the kernel
-   int32_t stageBytes; // bytes of one stage = sum(elemBytes) * tileRows
+   int32_t stageBytes; // bytes of one stage = sum(elemBytes * tileRows + tileHeader)
    int32_t useTma;     // 0 when a column base is not 16-byte aligned: tiles are then read with plain loads
-   int32_t decBytes;   // bytes per decimal128 cell as staged: 16 (Arrow layout) or 8 (HOST batch narrowed); selects the kernel instantiation
+   int32_t decBytes;   // bytes per decimal128 cell as staged: 16 (Arrow layout), 8 (HOST batch narrowed) or kDecEncoded; selects the kernel instantiation
+   int32_t tileHeader; // bytes in front of every column tile: kEncodeTileHeader in the encoded layout, else 0
    int32_t producerSleepNs, consumerSleepNs; // pause between mbarrier polls of the producer lane / the consumer warps (0 = plain polling)
    const uint8_t* base[kMaxStagedCols];
-   int32_t elemBytes[kMaxStagedCols];  // 4 (int32/date32/fsb4) or 16 (decimal128)
+   int32_t elemBytes[kMaxStagedCols];  // 4 (int32/date32/fsb4) or 16 (decimal128); the width W in the encoded layout
    int32_t smemOffset[kMaxStagedCols]; // offset of the column inside a stage
+   int32_t encShift[kMaxStagedCols];   // encoded layout: log2(W)
+   uint32_t encMask[kMaxStagedCols];   // encoded layout: mask of the low W bytes of a 32-bit word (W <= 4)
 };
 // LATE-MATERIALISED value columns: a selective probe pipeline (Bloom filter in front, a few percent of the rows survive) streams
 // only its key / filter columns through the TMA tiles; the operands of the aggregate are fetched from HBM by the SURVIVORS
@@ -249,6 +268,13 @@ void launchProbeReceivedGroupBy(const JoinTableDev& tableA, const JoinTableDev& 
 
 // signature → instantiation registry for the group-by kernel; returns false when no compiled shape matches
 bool launchScanGroupBy(const GroupByParams& p, int smCount, cudaStream_t s, const char** why);
+// true when launchScanGroupBy has an instantiation of p's signature for the encoded layout (p.src.cols need not be bound yet)
+bool scanGroupByEncodable(const GroupByParams& p);
+// encoder (encode.cu).  A source column is `n` int32 cells (isI32) or decimal128 cells of which the low 8 bytes are taken.
+// Range pass: blockMin[b] = minimum of block b, *maxRange = max over blocks of (max - min) as unsigned (caller zeroes it).
+void launchEncodeRange(const uint8_t* src, bool isI32, int64_t n, int64_t* blockMin, unsigned long long* maxRange, cudaStream_t s);
+// Pack pass: writes the tile-framed copy (kernels.h, kEncodeTileHeader) of width `width` for tiles of `tileRows` rows
+void launchEncodePack(const uint8_t* src, bool isI32, int64_t n, const int64_t* blockMin, int width, int tileRows, uint8_t* dst, cudaStream_t s);
 void launchScanBuild(const BuildParams& p, int smCount, cudaStream_t s);
 bool launchScanProbeAgg(const ProbeAggParams& p, int smCount, cudaStream_t s, const char** why);
 bool launchScanProbe2GroupBy(const Probe2GroupByParams& p, int smCount, cudaStream_t s, const char** why);

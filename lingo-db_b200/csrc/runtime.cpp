@@ -260,6 +260,7 @@ int ldb_gpu_context_create(int device, LdbContext** out, LdbError* err) {
       LDB_CUDA(cudaEventCreateWithFlags(&ctx->computeDone, cudaEventDisableTiming));
       if (const char* e = getenv("LDB_NARROW_STAGING")) ctx->narrowStaging = atoi(e) != 0;
       if (const char* e = getenv("LDB_PACKED_STAGING")) ctx->packedStaging = atoi(e) != 0;
+      if (const char* e = getenv("LDB_ENCODED_SCAN_MAX_BYTES")) ctx->encodedBudget = std::max<int64_t>(0, atoll(e));
       *out = ctx.release();
    });
 }
@@ -293,6 +294,7 @@ void ldb_gpu_context_destroy(LdbContext* ctx) {
    if (ctx->pinnedScratch) cudaFreeHost(ctx->pinnedScratch);
    cudaStreamDestroy(ctx->compute);
    cudaStreamDestroy(ctx->copy);
+   if (ctx->encodeStream) cudaStreamDestroy(ctx->encodeStream);
    delete ctx;
 }
 int ldb_gpu_device_info(LdbContext* ctx, LdbDeviceInfo* out, LdbError* err) {
@@ -336,13 +338,19 @@ void ldb_gpu_set_filter_specialisation(int32_t on) {
    t.specialise = on ? 1 : 0;
    setTuning(t);
 }
+void ldb_gpu_set_encoded_scan(int32_t on) {
+   Tuning t = tuning();
+   t.encodedScan = on ? 1 : 0;
+   setTuning(t);
+}
+int64_t ldb_gpu_context_encoded_bytes(LdbContext* ctx) { return ctx ? ctx->encodedBytes : 0; }
 void ldb_gpu_set_poll_pause(int32_t producer_ns, int32_t consumer_ns) {
    Tuning t = tuning();
    t.producerSleepNs = producer_ns;
    t.consumerSleepNs = consumer_ns;
    setTuning(t);
 }
-int64_t ldb_gpu_launch_count(LdbContext* ctx) { return ctx ? ctx->launches + ctx->stagingLaunches.load() : 0; }
+int64_t ldb_gpu_launch_count(LdbContext* ctx) { return ctx ? ctx->launches + ctx->stagingLaunches.load() + ctx->encodeLaunches : 0; }
 int ldb_gpu_timer_start(LdbContext* ctx, LdbError* err) {
    return guarded(err, [&] { LDB_CUDA(cudaEventRecord(ctx->timerStart, ctx->compute)); });
 }
@@ -491,6 +499,7 @@ int ldb_gpu_table_append_batch(LdbTable* t, int64_t n_rows, const LdbArrayView* 
       LDB_CUDA(cudaSetDevice(ctx->device));
       LdbBatch b;
       b.nRows = n_rows;
+      b.borrowed = location == LDB_MEM_DEVICE;
       size_t nc = t->columns.size();
       b.data.resize(nc);
       b.bytes.assign(nc, nullptr);
@@ -626,7 +635,11 @@ int ldb_gpu_table_clear(LdbTable* t, LdbError* err) {
       LDB_CUDA(cudaEventRecord(ctx->computeDone, ctx->compute));
       LDB_CUDA(cudaStreamWaitEvent(ctx->copy, ctx->computeDone, 0));
       ctx->stagingGen.fetch_add(1);
+      bool encoded = false;
+      for (auto& b : t->batches) encoded |= !b.enc.empty();
+      if (encoded && !ctx->capturing) ctx->syncStream(ctx->compute); // queued scans may still read the encoded copies freed below
       for (auto& b : t->batches) {
+         ldb_gpu_free_encoded_internal(ctx, b);
          for (void* p : b.owned) ctx->stagingRelease(p);
          if (b.ready) ctx->eventPool.push_back(b.ready);
       }
@@ -1057,6 +1070,24 @@ struct StagePlan {
       }
       if (!out.decBytes) out.decBytes = 16;
    }
+   // the same columns read from the batch's encoded copies (every one of them built by ldb_gpu_encode_batch_internal)
+   void bindEncoded(LdbTable* t, const LdbBatch& b, StagedCols& out, int rowsPerThread) const {
+      bind(t, b, out, rowsPerThread);
+      out.tileHeader = kEncodeTileHeader;
+      int off = 0;
+      for (int i = 0; i < n; i++) {
+         const LdbBatch::Encoded& e = b.enc[colIdx[i]];
+         out.base[i] = e.data;
+         out.elemBytes[i] = e.width;
+         out.smemOffset[i] = off;
+         off += e.width * out.tileRows + kEncodeTileHeader;
+         out.encShift[i] = e.width == 1 ? 0 : e.width == 2 ? 1 : e.width == 4 ? 2 : 3;
+         out.encMask[i] = e.width >= 4 ? ~0u : (1u << (8 * e.width)) - 1u;
+      }
+      out.stageBytes = off;
+      out.useTma = n > 0 ? 1 : 0; // the copies are cudaMalloc'd and every column tile is a multiple of 16 bytes
+      out.decBytes = kDecEncoded;
+   }
 };
 struct FilterPlan {
    FilterSet set{};
@@ -1266,7 +1297,6 @@ int ldb_gpu_run_pipeline(LdbContext* ctx, const LdbPipelineDesc* d, LdbError* er
                GroupByParams p{};
                p.src.nRows = b.nRows;
                bindFilters(fp, b, p.src.filters);
-               sp.bind(t, b, p.src.cols, kRowsPerThreadScan);
                p.nKeys = nKeys;
                for (int k = 0; k < nKeys; k++) p.keyStage[k] = keyStage[k];
                p.nValueCols = ap.nValueCols;
@@ -1274,6 +1304,12 @@ int ldb_gpu_run_pipeline(LdbContext* ctx, const LdbPipelineDesc* d, LdbError* er
                p.nAggs = ap.nAggs;
                for (int a = 0; a < ap.nAggs; a++) p.aggs[a] = ap.aggs[a];
                p.table = sink->group;
+               // a borrowed DEVICE batch is scanned from its frame-of-reference copy (built here on first use); HOST-staged
+               // batches, signatures without an encoded instantiation and copies that could not be allocated use the Arrow cells
+               const bool encoded = tuning().encodedScan && b.borrowed && scanGroupByEncodable(p) &&
+                                    ldb_gpu_encode_batch_internal(ctx, t, b, sp.colIdx, sp.n, kBlockThreads * kRowsPerThreadScan);
+               if (encoded) sp.bindEncoded(t, b, p.src.cols, kRowsPerThreadScan);
+               else sp.bind(t, b, p.src.cols, kRowsPerThreadScan);
                waitBatch(ctx, b);
                bool ok = true;
                ctx->launch(keyless ? "scan_reduce" : "scan_groupby", [&] { ok = launchScanGroupBy(p, ctx->smCount, ctx->compute, &why); });
