@@ -142,9 +142,11 @@ void ldb_gpu_table_destroy(LdbTable* t);
  *   LDB_STATE_JOIN_TABLE  rt::GrowingBuffer + rt::HashIndexedView (GrowingBuffer.cpp:39-113,
  *                         LazyJoinHashtable.cpp:12-34): key → payload multimap; with aggregate
  *                         lanes it is the group-join map of SubOpToControlFlow.cpp:2730-2839.
+ *   LDB_STATE_KEY_JOIN    rt::HashIndexedView over a key TUPLE (db.hash over the tuple, LowerToStd.cpp:1139-1150):
+ *                         1..4 int64 keys → int64 payload, for program pipelines (ldb_gpu_join_table_create_keys).
  * The memory image differs from the CPU objects (open addressing, 32-bit payloads, no tagged
  * pointers): the contract is the same MULTISET of results, not the same bytes (SURVEY §7). */
-enum LdbStateKind { LDB_STATE_SIMPLE = 1, LDB_STATE_GROUPBY = 2, LDB_STATE_JOIN_TABLE = 3, LDB_STATE_HASHAGG = 4, LDB_STATE_DICT = 5 };
+enum LdbStateKind { LDB_STATE_SIMPLE = 1, LDB_STATE_GROUPBY = 2, LDB_STATE_JOIN_TABLE = 3, LDB_STATE_HASHAGG = 4, LDB_STATE_DICT = 5, LDB_STATE_KEY_JOIN = 6 };
 typedef struct LdbState LdbState;
 typedef struct LdbI128 {
    uint64_t lo;
@@ -200,6 +202,16 @@ int ldb_gpu_join_table_create_pair(LdbContext* ctx, int64_t expected_rows, int32
  * fails the build (LDB_ERR_INVALID).  ldb_gpu_table_column_range gives the plan the column's min/max (one streaming pass). */
 int ldb_gpu_join_table_create_direct(LdbContext* ctx, int32_t key_min, int32_t key_max, LdbState** out, LdbError* err);
 int ldb_gpu_table_column_range(LdbTable* t, const char* column, int32_t* min, int32_t* max, LdbError* err);
+/* Key-tuple join table (LDB_STATE_KEY_JOIN): n_keys (1..4) int64 keys → int64 payload, for program pipelines only — built by the
+ * JOIN_BUILD sink (keys from LdbProgramDesc.n_keys / key_regs), read by LDB_OP_PROBE / LDB_OP_PROBE_EACH (keys from consecutive
+ * registers).  The directory holds nextPow2(2 x expected_rows) entries; a build that overflows it fails with LDB_ERR_CAPACITY, as
+ * does an insert that finds no free slot within 65 536 probes (more duplicates of one tuple than that in a multimap).  flags:
+ * LDB_JOIN_UNIQUE = set semantics, a duplicate key tuple is dropped (which of the duplicates' payloads is kept is unspecified);
+ * LDB_JOIN_NO_BLOOM = no Bloom filter.  Without it the table is a multimap: every duplicate is kept.  ldb_gpu_join_table_count,
+ * ldb_gpu_state_destroy, ldb_gpu_register_state and ldb_gpu_find_state take it; the specialised pipelines, serialised steps and every
+ * other join-table entry point refuse it (LDB_ERR_INVALID).  Not for captured queries: creating, building or probing one while a
+ * capture is in progress fails with LDB_ERR_UNSUPPORTED. */
+int ldb_gpu_join_table_create_keys(LdbContext* ctx, int32_t n_keys, int64_t expected_rows, int32_t flags, LdbState** out, LdbError* err);
 int ldb_gpu_join_table_count(LdbState* s, int64_t* n_entries, LdbError* err);
 typedef struct LdbTopKRow {
    int32_t key, side[LDB_MAX_SIDE];
@@ -384,7 +396,10 @@ enum LdbOp {
    LDB_OP_STRCMP = 20, /* dst = columns[a] <b: LDB_EQ..LDB_GTE> strings[arg] */
    LDB_OP_STRLIKE = 21,/* dst = columns[a] LIKE strings[arg]; b = 0 'x%', 1 '%x', 2 '%x%' */
    LDB_OP_YEAR = 22,   /* dst = extract(year from date32 a) */
-   LDB_OP_PROBE = 23,  /* dst = payload of int32 key a in tables[arg]; NULL when absent */
+   LDB_OP_PROBE = 23,  /* dst = payload of int32 key a in tables[arg]; NULL when absent.  On a key-tuple join table of n keys
+                          (LDB_STATE_KEY_JOIN) the key is the tuple of registers a, a+1, …, a+n-1 and the payload comes back as int64; a
+                          NULL component or one outside int64 never matches, and a probe run that reaches the interpreter's bound of
+                          16384 slots fails the call (LDB_ERR_CAPACITY). */
    LDB_OP_STRKEY8 = 24,/* dst = first 8 bytes of columns[a], zero padded, big-endian, as a signed int64 (a group / sort key for short
                           strings: char(n<=8), flags, codes; longer strings take LDB_OP_STRCODE).  It preserves the
                           bytewise string order only while the first byte is below 0x80 (7-bit text): a first byte >= 0x80 makes the
@@ -394,7 +409,8 @@ enum LdbOp {
                              instructions after it, the filter and the sink run once per match.  b = 0 inner join (no match: no tuple),
                              b = 1 left outer join (no match: one tuple with dst NULL).  A NULL key never matches.  At most one per
                              program; later instructions may not overwrite registers written at or before it.  A probe run longer
-                             than the interpreter's bound fails the call (LDB_ERR_CAPACITY) rather than dropping matches. */
+                             than the interpreter's bound fails the call (LDB_ERR_CAPACITY) rather than dropping matches.  On a
+                             key-tuple join table the key is the tuple of registers a .. a+n-1, as for PROBE. */
    LDB_OP_STRCODE = 27 /* dst = int32 code of the utf8 string columns[a] (a source or side column) in the string dictionary tables[arg]
                           (ldb_gpu_dict_create).  b = 1 inserts an absent string, b = 0 only looks up: an absent string gives NULL.  A
                           NULL string gives NULL and is never inserted.  Every instruction runs before the WHERE test, so b = 1 inserts
@@ -425,9 +441,10 @@ typedef struct LdbProgramDesc {
    const LdbI128* consts;
    int32_t n_strings;            /* <= 12, each <= 32 bytes */
    const char* const* strings;
-   int32_t n_tables;             /* <= 4 join tables (single int32 key or direct-address) for LDB_OP_PROBE / LDB_OP_PROBE_EACH, or
-                                    string dictionaries (same context) for LDB_OP_STRCODE; a dictionary is no PROBE table and a
-                                    join table no STRCODE dictionary (LDB_ERR_INVALID) */
+   int32_t n_tables;             /* <= 4 join tables (single int32 key, direct-address, or key-tuple of the same context) for
+                                    LDB_OP_PROBE / LDB_OP_PROBE_EACH, or string dictionaries (same context) for LDB_OP_STRCODE; a
+                                    dictionary is no PROBE table and a join table no STRCODE dictionary (LDB_ERR_INVALID).  A program
+                                    may not probe the key-tuple table it builds (LDB_ERR_INVALID). */
    LdbState* const* tables;
    int32_t filter_reg;           /* the row is kept when this register is TRUE (NULL is not true); -1 = keep all */
    int32_t sink_kind;            /* LdbProgramSink */
@@ -438,7 +455,10 @@ typedef struct LdbProgramDesc {
    LdbProgAgg aggs[LDB_MAX_AGGS];
    /* JOIN_BUILD: payload_reg -1 = 0.  Rows with a NULL key are not inserted; a NULL payload is stored as 0.  The call fails when a
     * row could not be stored: a non-NULL key or payload outside int32 (LDB_ERR_UNSUPPORTED), a table smaller than the build side
-    * (LDB_ERR_CAPACITY), the reserved pair key -1 / payload -1 (LDB_ERR_UNSUPPORTED). */
+    * (LDB_ERR_CAPACITY), the reserved pair key -1 / payload -1 (LDB_ERR_UNSUPPORTED).
+    * Into a key-tuple join table (LDB_STATE_KEY_JOIN) the keys are n_keys / key_regs[] (n_keys must equal the table's key count
+    * and build_key_reg must be -1, else LDB_ERR_INVALID); a row with a NULL key component is not inserted; a non-NULL key or
+    * payload outside int64 fails the call (LDB_ERR_UNSUPPORTED); ROWID payloads have no row limit. */
    int32_t build_key_reg, build_payload_reg;
    /* MATERIALIZE: out_regs → a new DEVICE table (columns "c0".."cN": decimal128(38,0) cells = the raw i128 / double bits in the
     * low 8 bytes, each with a validity byte); capacity = source rows, regrown to the produced row count (one more run of the
@@ -466,7 +486,7 @@ typedef struct LdbProgramJoins {
    const LdbSideColumn* side_columns;
 } LdbProgramJoins;
 /* ldb_gpu_run_program with side columns (joins may be NULL).  A JOIN_BUILD program that uses ROWID is rejected when its source
- * has 2^31 rows or more (join payloads are int32). */
+ * has 2^31 rows or more and its sink is a plain join table (int32 payloads); a key-tuple join table takes int64 payloads. */
 int ldb_gpu_run_program_ex(LdbContext* ctx, const LdbProgramDesc* desc, const LdbProgramJoins* joins, LdbError* err);
 /* hash aggregation state sized for `expected_groups` (the directory holds 2x that; LDB_ERR_CAPACITY when it overflows) */
 int ldb_gpu_hashagg_create(LdbContext* ctx, int32_t n_keys, int32_t n_aggs, const LdbProgAgg* aggs, int64_t expected_groups, LdbState** out, LdbError* err);

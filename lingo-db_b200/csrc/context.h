@@ -237,6 +237,7 @@ struct LdbState {
    ldb::JoinTableDev join{};   // JOIN_TABLE
    ldb::HashAggDev hashagg{};  // HASHAGG
    ldb::DictDev dict{};        // DICT
+   ldb::KeyJoinDev keyJoin{};  // KEY_JOIN
    int32_t aggKinds[ldb::kProgMaxAggs] = {};
    int32_t nSide = 0, nAggs = 0;
    bool selfTimed = false; // created inside a captured query: its scan kernel's self-measured time is harvested at read
@@ -248,6 +249,8 @@ struct LdbState {
 // reads a join table's error word (synchronises the compute stream) and throws ApiError with the status and message of a
 // non-zero code (runtime.cpp); every caller that reports a join table's failure goes through it
 void ldb_gpu_check_join_error_internal(LdbState* s);
+// the same for a key-tuple join table (LDB_STATE_KEY_JOIN, program_rt.cpp)
+void ldb_gpu_check_keyjoin_error_internal(LdbState* s);
 // fixes the width of aggregate lane `lane` of a group state from the LdbExprKind summed into it (64-bit COL / ONE, else 128-bit);
 // throws ApiError(LDB_ERR_UNSUPPORTED) when an earlier pipeline fixed the other width (runtime.cpp)
 void ldb_gpu_bind_lane_width_internal(LdbState* s, int lane, int expr);

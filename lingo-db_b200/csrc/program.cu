@@ -183,6 +183,14 @@ __device__ __forceinline__ uint64_t mix64(uint64_t x) {
    x ^= x >> 33;
    return x;
 }
+// placement hash of a tuple of int64 keys: every key goes through mix64, so correlated tuples ((partkey, suppkey) pairs whose
+// components grow together) do not cluster the way an XOR combine of per-key hashes does.  Shared by the hash-aggregation table (seeded
+// with its key-NULL bits) and the key-tuple join table.
+__device__ __forceinline__ uint64_t keyTupleHash(const int64_t* keys, int n, uint32_t seed) {
+   uint64_t h = 0x9E3779B97F4A7C55ull ^ seed;
+   for (int k = 0; k < n; k++) h = mix64(h ^ (uint64_t) keys[k]) + 0x632BE59BD9B4E019ull * (k + 1);
+   return h;
+}
 
 // ---------------------------------------------------------------- string dictionary (DictDev, program.h)
 // placement hash of a byte string: 8-byte little-endian chunks (the last one zero padded) folded through mix64, seeded with the
@@ -257,6 +265,123 @@ __device__ __noinline__ int32_t dictCode(const DictDev& d, const uint8_t* s, int
    return -2;
 }
 
+// ---------------------------------------------------------------- key-tuple join table (KeyJoinDev, program.h)
+// Kept out of line (__noinline__), like dictCode, and called only from programKernel<true>: programs without a key-tuple table run
+// programKernel<false>, which has none of this code.  The calls take the table descriptor and the key tuple by value and return their
+// results by value: no pointer into the register file or into the kernel parameters escapes into them.
+struct KeyTuple {
+   int64_t k[kProgMaxKeys];
+};
+struct KeyCursor { // a probe run: the next slot, the probes taken, the tuple's tag; `live` false: the run ended (or never started)
+   uint64_t slot;
+   uint32_t probes, tag;
+   bool live;
+};
+struct KeyHit {
+   KeyCursor next;
+   int64_t payload;
+   bool hit;
+};
+__device__ __forceinline__ uint8_t* keyEntry(const KeyJoinDev& t, uint64_t s) { return t.base + s * t.entryBytes; }
+// the entry at e holds exactly the tuple `keys`: 16-byte loads (keys start 16 bytes into an entry; an odd last key reads the entry's
+// padding), through L2 (`coherent`: a build reads entries other SMs publish during the same launch) or the read-only path
+__device__ __forceinline__ bool keysEqual(const KeyJoinDev& t, const uint8_t* e, const KeyTuple& keys, bool coherent) {
+   const longlong2* kp = (const longlong2*) (e + 16);
+   for (int k = 0; k < t.nKeys; k += 2) {
+      const longlong2 w = coherent ? __ldcg(kp + k / 2) : __ldg(kp + k / 2);
+      if (w.x != keys.k[k] || (k + 1 < t.nKeys && w.y != keys.k[k + 1])) return false;
+   }
+   return true;
+}
+// the tuple of registers regs[reg(0)], …, regs[reg(n - 1)]: 0, or bit 0 = a NULL component, bit 1 = a component outside int64
+template <class Reg>
+__device__ __forceinline__ int gatherTuple(const Val* regs, int n, Reg reg, KeyTuple& keys) {
+   int bad = 0;
+   for (int k = 0; k < n; k++) {
+      const Val v = regs[reg(k)];
+      bad |= v.null ? 1 : (v.v != (s128) (int64_t) v.v ? 2 : 0);
+      keys.k[k] = (int64_t) v.v;
+   }
+   return bad;
+}
+// insert: claims an empty slot by CAS (0 → tag | kKeyJoinWriting), writes the payload and the keys, fences and publishes
+// tag | kKeyJoinReady with one atomic store.  A multimap insert skips occupied slots without reading their keys.  A unique insert that
+// meets its own tag waits (__nanosleep) for the publication, then compares the keys and drops a duplicate.  false: not inserted (a
+// duplicate, or error word 1: no empty slot within kKeyJoinInsertBound probes — a full directory, or that many entries sharing one run,
+// e.g. duplicates of one tuple in a multimap).  The bound keeps a build that overflows the table from walking the whole directory for
+// every row; every 1024 probes the insert also gives up once another row has set the error word.
+constexpr uint64_t kKeyJoinInsertBound = 65536;
+__device__ __noinline__ bool keyJoinInsert(const KeyJoinDev t, const KeyTuple keys, int64_t payload) {
+   const uint64_t h = keyTupleHash(keys.k, t.nKeys, 0);
+   const unsigned long long tag = (h >> 32) << 32;
+   uint64_t s = h & t.mask;
+   const uint64_t limit = t.mask + 1 < kKeyJoinInsertBound ? t.mask + 1 : kKeyJoinInsertBound;
+   for (uint64_t probes = 0; probes < limit; probes++) {
+      if ((probes & 1023) == 1023 && *((volatile int32_t*) t.error)) return false; // the call fails already
+      uint8_t* e = keyEntry(t, s);
+      unsigned long long* wp = (unsigned long long*) e;
+      unsigned long long w = *((volatile unsigned long long*) wp);
+      if (w == 0) {
+         w = atomicCAS(wp, 0ull, tag | kKeyJoinWriting);
+         if (w == 0) {
+            int64_t* ep = (int64_t*) e;
+            ep[1] = payload;
+            for (int k = 0; k < t.nKeys; k++) ep[2 + k] = keys.k[k];
+            __threadfence();
+            atomicExch(wp, tag | kKeyJoinReady);
+            if (t.bloom) atomicOr(&t.bloom[(uint32_t) (h >> 32) & t.bloomMask], bloomBits(h));
+            return true;
+         }
+      }
+      if (t.unique && (w & 0xffffffff00000000ull) == tag) {
+         while ((uint32_t) w == kKeyJoinWriting) {
+            __nanosleep(64);
+            w = *((volatile unsigned long long*) wp);
+         }
+         __threadfence();
+         if (keysEqual(t, e, keys, true)) return false;
+      }
+      s = (s + 1) & t.mask;
+   }
+   atomicExch(t.error, 1);
+   return false;
+}
+// the start of a probe run for `keys` (a tuple without NULL or out-of-range components): not live when the Bloom filter rules it out
+__device__ __noinline__ KeyCursor keyJoinStart(const KeyJoinDev t, const KeyTuple keys) {
+   const uint64_t h = keyTupleHash(keys.k, t.nKeys, 0);
+   KeyCursor c{h & t.mask, 0, (uint32_t) (h >> 32), true};
+   if (t.bloom) {
+      const uint32_t bits = bloomBits(h);
+      c.live = (__ldg(&t.bloom[(uint32_t) (h >> 32) & t.bloomMask]) & bits) == bits;
+   }
+   return c;
+}
+// the next entry of `keys` along its probe run from cursor c (PROBE takes the first, PROBE_EACH every one).  The state word (with the tag)
+// and the payload come in one 16-byte load; the keys are loaded only on a tag match.  A program never builds and probes one table, so no
+// probe shares a launch with a build: the loads take the read-only path.  A run that reaches the interpreter's bound in a directory larger
+// than the bound sets the error word (6): the call fails rather than miss a match.
+__device__ __noinline__ KeyHit keyJoinNext(const KeyJoinDev t, const KeyTuple keys, KeyCursor c) {
+   KeyHit r{c, 0, false};
+   while (r.next.probes <= t.mask && r.next.probes < 16384) {
+      const uint8_t* e = keyEntry(t, r.next.slot);
+      const ulonglong2 head = __ldg((const ulonglong2*) e);
+      if (head.x == 0) {
+         r.next.live = false;
+         return r;
+      }
+      r.next.slot = (r.next.slot + 1) & t.mask;
+      r.next.probes++;
+      if ((uint32_t) (head.x >> 32) == r.next.tag && keysEqual(t, e, keys, false)) {
+         r.payload = (int64_t) head.y;
+         r.hit = true;
+         return r;
+      }
+   }
+   if (r.next.probes >= 16384 && t.mask >= 16384) atomicExch(t.error, 6);
+   r.next.live = false;
+   return r;
+}
+
 // ---------------------------------------------------------------- hash aggregation table
 constexpr uint32_t kSeenBit = 1u, kClaimBit = 1u << 8, kKeyNullBit = 1u << 16;
 __device__ __forceinline__ uint8_t* entryAt(const HashAggDev& t, uint64_t s) { return t.base + s * t.entryBytes; }
@@ -264,8 +389,7 @@ __device__ __forceinline__ uint8_t* entryAt(const HashAggDev& t, uint64_t s) { r
 __device__ uint8_t* hashAggFind(const ProgramParams& p, const int64_t* keys, uint32_t keyNulls) {
    const HashAggDev& t = p.agg;
    if (t.nKeys == 0) return t.base; // keyless: the table is one pre-initialised entry
-   uint64_t h = 0x9E3779B97F4A7C55ull ^ keyNulls;
-   for (int k = 0; k < t.nKeys; k++) h = mix64(h ^ (uint64_t) keys[k]) + 0x632BE59BD9B4E019ull * (k + 1);
+   const uint64_t h = keyTupleHash(keys, t.nKeys, keyNulls);
    uint64_t s = h & t.mask;
    const uint64_t limit = t.mask + 1 < 65536 ? t.mask + 1 : 65536;
    for (uint64_t probes = 0; probes < limit; probes++) {
@@ -379,6 +503,10 @@ __device__ void hashAggUpdate(const ProgramParams& p, uint8_t* e, const Val* reg
 // One thread per scanned row.  Without LDB_OP_PROBE_EACH the program, the WHERE test and the sink run once.  With it, the
 // instructions from PROBE_EACH on, the WHERE test and the sink run once per match: the warp keeps iterating together until no lane
 // has a match left (the materialize sink's ballot needs all 32 lanes), and a lane without a tuple in an iteration does not pass.
+// KeyTuples: the instance that also reads and builds key-tuple join tables.  Programs without one run the instance that has none of
+// that code: even an untaken key-tuple build call in the sink made the plain-table build kernel four times slower (register allocation
+// and scheduling of the whole loop change with it).
+template <bool KeyTuples>
 __global__ void __launch_bounds__(256) programKernel(const __grid_constant__ ProgramParams p) {
    unsigned long long inserted = 0;
    for (int64_t base = (int64_t) blockIdx.x * blockDim.x; base < p.nRows; base += (int64_t) gridDim.x * blockDim.x) {
@@ -393,6 +521,7 @@ __global__ void __launch_bounds__(256) programKernel(const __grid_constant__ Pro
       int32_t eachKey = 0;
       uint64_t eachSlot = 0;
       uint32_t eachProbes = 0;
+      KeyCursor eachCur{}; // key-tuple tables
       while (true) {
          bool pass = false;
          if (pending) {
@@ -498,7 +627,15 @@ __global__ void __launch_bounds__(256) programKernel(const __grid_constant__ Pro
                   case LDB_OP_PROBE: { // key → payload of a unique/multimap single-key table; absent key = NULL (semi / anti / mark / outer)
                      const JoinTableDev& t = p.tables[in.arg];
                      r.null = true;
-                     if (!a.null && a.v == (s128) (int32_t) a.v) {
+                     if (KeyTuples && p.keyTables[in.arg].nKeys) { // key-tuple table: the keys are registers a .. a + nKeys - 1
+                        KeyTuple keys;
+                        if (!gatherTuple(regs, p.keyTables[in.arg].nKeys, [&](int k) { return in.a + k; }, keys)) { // NULL / past int64: no match
+                           const KeyCursor c = keyJoinStart(p.keyTables[in.arg], keys);
+                           const KeyHit h = c.live ? keyJoinNext(p.keyTables[in.arg], keys, c) : KeyHit{c, 0, false};
+                           r.v = h.payload;
+                           r.null = !h.hit;
+                        }
+                     } else if (!a.null && a.v == (s128) (int32_t) a.v) {
                         const int32_t key = (int32_t) a.v;
                         if (t.direct) {
                            const int32_t pay = directLoadProg(t, key);
@@ -530,9 +667,16 @@ __global__ void __launch_bounds__(256) programKernel(const __grid_constant__ Pro
                   }
                   case LDB_OP_PROBE_EACH: { // the next match; b = 1: a row without any match yields one tuple with a NULL payload
                      const JoinTableDev& t = p.tables[in.arg];
+                     const bool tuple64 = KeyTuples && p.keyTables[in.arg].nKeys != 0; // key-tuple table: keys in registers a .. a + nKeys - 1,
+                                                                                         // its run in eachCur
+                     KeyTuple eachKeys;
+                     if (tuple64 && eachState != 2 && gatherTuple(regs, p.keyTables[in.arg].nKeys, [&](int k) { return in.a + k; }, eachKeys)) eachState = 2;
                      if (eachState == 0) {
                         eachState = 2; // a NULL key (or one outside int32) never matches
-                        if (!a.null && a.v == (s128) (int32_t) a.v) {
+                        if (tuple64) {
+                           eachCur = keyJoinStart(p.keyTables[in.arg], eachKeys);
+                           if (eachCur.live) eachState = 1;
+                        } else if (!a.null && a.v == (s128) (int32_t) a.v) {
                            eachKey = (int32_t) a.v;
                            const uint64_t h = hashI32(eachKey);
                            eachSlot = h & t.mask;
@@ -544,9 +688,16 @@ __global__ void __launch_bounds__(256) programKernel(const __grid_constant__ Pro
                         }
                      }
                      int32_t pay = 0;
+                     int64_t pay64 = 0;
+                     auto tupleNext = [&] {
+                        const KeyHit h = keyJoinNext(p.keyTables[in.arg], eachKeys, eachCur);
+                        eachCur = h.next;
+                        pay64 = h.payload;
+                        return h.hit;
+                     };
                      r.null = true;
-                     if (eachState == 1 && probeEachNext(t, eachKey, eachSlot, eachProbes, pay)) {
-                        r.v = pay;
+                     if (eachState == 1 && (tuple64 ? tupleNext() : probeEachNext(t, eachKey, eachSlot, eachProbes, pay))) {
+                        r.v = tuple64 ? pay64 : pay;
                         r.null = false;
                      } else {
                         eachState = 2;
@@ -582,7 +733,18 @@ __global__ void __launch_bounds__(256) programKernel(const __grid_constant__ Pro
                if (e) hashAggUpdate(p, e, regs);
             }
          } else if (p.sinkKind == 2) {
-            if (pass) {
+            if (KeyTuples && pass && p.keyBuild.nKeys) { // a key-tuple table: keys from keyReg[], int64 keys and payloads
+               KeyTuple keys;
+               const int bad = gatherTuple(regs, p.nKeys, [&](int k) { return p.keyReg[k]; }, keys);
+               const s128 pay = p.buildPayloadReg >= 0 && !regs[p.buildPayloadReg].null ? regs[p.buildPayloadReg].v : 0;
+               if (bad & 1) {
+                  // a NULL key component never matches: the row is not stored
+               } else if (bad || pay != (s128) (int64_t) pay) {
+                  atomicExch(p.keyBuild.error, 7); // keys and payloads are int64
+               } else if (keyJoinInsert(p.keyBuild, keys, (int64_t) pay)) {
+                  inserted++;
+               }
+            } else if (pass) {
                const Val k = regs[p.buildKeyReg];
                if (!k.null) { // NULL keys never match (SQL join semantics); a NULL payload is stored as 0
                   const s128 pay = p.buildPayloadReg >= 0 && !regs[p.buildPayloadReg].null ? regs[p.buildPayloadReg].v : 0;
@@ -614,12 +776,15 @@ __global__ void __launch_bounds__(256) programKernel(const __grid_constant__ Pro
    }
    if (p.sinkKind == 2) {
       unsigned long long total = warpSum64(inserted);
-      if ((threadIdx.x & 31) == 0 && total) atomicAdd(p.build.count, total);
+      if ((threadIdx.x & 31) == 0 && total) atomicAdd(KeyTuples && p.keyBuild.nKeys ? p.keyBuild.count : p.build.count, total);
    }
 }
 void launchProgram(const ProgramParams& p, int smCount, cudaStream_t s) {
    int grid = (int) std::min<int64_t>(std::max<int64_t>((p.nRows + 255) / 256, 1), (int64_t) smCount * 8);
-   programKernel<<<grid, 256, 0, s>>>(p);
+   bool keyTuples = p.keyBuild.nKeys != 0;
+   for (int k = 0; k < kProgMaxTables; k++) keyTuples |= p.keyTables[k].nKeys != 0;
+   if (keyTuples) programKernel<true><<<grid, 256, 0, s>>>(p);
+   else programKernel<false><<<grid, 256, 0, s>>>(p);
 }
 
 __global__ void hashAggInitKernel(HashAggDev t) {

@@ -84,8 +84,25 @@ struct DictDev {
    int64_t codeCap; // codes 0..codeCap-1 fit the entry arrays and int32
 };
 constexpr uint32_t kDictWriting = 0xffffffffu, kDictFailed = 0xfffffffeu;
+// key-tuple join table (LDB_STATE_KEY_JOIN): 1..4 int64 keys → int64 payload, open addressing in HBM, cap = nextPow2(2 x expected)
+//   entry = { word:u64 = tag:32 (high 32 bits of the tuple's hash) | state:32 (0 empty: the whole word is 0, kKeyJoinWriting,
+//             kKeyJoinReady), payload:i64, keys[nKeys]:i64 } padded to entryBytes = 32 (1-2 keys: one DRAM sector) or 48 (3-4 keys)
+//   error    1 directory full, 6 a probe run reached the interpreter's bound, 7 a build key or payload outside int64
+// nKeys == 0 marks an unused descriptor (the table is a plain join table or a dictionary).
+struct KeyJoinDev {
+   uint8_t* base;
+   uint64_t mask;             // capacity - 1
+   uint32_t* bloom;           // blocked Bloom filter over the key tuples (as JoinTableDev), or null
+   uint32_t bloomMask;
+   int32_t nKeys;
+   uint32_t entryBytes;
+   int32_t unique;            // set semantics: a duplicate tuple is dropped
+   unsigned long long* count; // inserted entries
+   int32_t* error;
+};
+constexpr uint32_t kKeyJoinWriting = 1u, kKeyJoinReady = 2u;
 
-// The kernel takes ProgramParams by value (__grid_constant__): 3 432 bytes with the limits above, within the classic 4 096-byte
+// The kernel takes ProgramParams by value (__grid_constant__): 3 712 bytes with the limits above, within the classic 4 096-byte
 // kernel-parameter limit (program_rt.cpp checks it at compile time).
 struct ProgramParams {
    int64_t nRows;
@@ -100,9 +117,11 @@ struct ProgramParams {
    int32_t stringLen[kProgMaxStrings];
    JoinTableDev tables[kProgMaxTables];
    DictDev dicts[kProgMaxTables]; // tables[k] is a string dictionary: dicts[k] (LDB_OP_STRCODE)
+   KeyJoinDev keyTables[kProgMaxTables]; // tables[k] is a key-tuple join table: keyTables[k] (nKeys > 0; PROBE / PROBE_EACH read its keys
+                                         // from registers a .. a + nKeys - 1)
    int32_t filterReg; // -1: every row passes
    int32_t sinkKind;  // 1 hash aggregation, 2 join-table build, 3 materialize
-   // sink 1
+   // sink 1 (and sink 2 into a key-tuple table: its key registers)
    int32_t nKeys, nAggs;
    int32_t keyReg[kProgMaxKeys];
    ProgAgg aggs[kProgMaxAggs];
@@ -110,6 +129,7 @@ struct ProgramParams {
    // sink 2
    int32_t buildKeyReg, buildPayloadReg;
    JoinTableDev build;
+   KeyJoinDev keyBuild; // nKeys > 0: the build goes into this key-tuple table instead of `build`
    // sink 3: compacted output columns, 16 bytes per value (i128 / double bits in lo) + 1 validity byte
    int32_t nOut;
    int32_t outReg[kProgMaxAggs];

@@ -374,6 +374,63 @@ int ldb_gpu_dict_to_table(LdbState* s, const char* name, LdbTable** out, LdbErro
    });
 }
 
+// ---------------------------------------------------------------- key-tuple join tables
+int ldb_gpu_join_table_create_keys(LdbContext* ctx, int32_t n_keys, int64_t expected_rows, int32_t flags, LdbState** out, LdbError* err) {
+   return guardedP(err, [&] {
+      int devices = 0;
+      if (cudaGetDeviceCount(&devices) != cudaSuccess || devices == 0) {
+         cudaGetLastError();
+         failP(LDB_ERR_NO_DEVICE, "no CUDA device available: the GPU operator runtime has no CPU fallback");
+      }
+      if (!ctx || !out) failP(LDB_ERR_INVALID, "null argument");
+      if (n_keys < 1 || n_keys > kProgMaxKeys) failP(LDB_ERR_INVALID, "a key-tuple join table takes 1..4 keys");
+      if (expected_rows < 0) failP(LDB_ERR_INVALID, "negative expected_rows");
+      if (expected_rows > ((int64_t) 1 << 36)) failP(LDB_ERR_UNSUPPORTED, "a key-tuple join table holds at most 2^36 expected rows");
+      if (ctx->capturing) failP(LDB_ERR_UNSUPPORTED, "key-tuple join tables are not part of captured queries");
+      LDB_CUDA(cudaSetDevice(ctx->device));
+      auto* s = new LdbState;
+      s->ctx = ctx;
+      s->kind = LDB_STATE_KEY_JOIN;
+      ctx->states.push_back(s);
+      auto alloc = [&](size_t bytes) {
+         void* p = ctx->stagingAlloc(std::max<size_t>(bytes, 16));
+         s->allocations.push_back(p);
+         LDB_CUDA(cudaMemsetAsync(p, 0, std::max<size_t>(bytes, 16), ctx->compute));
+         return p;
+      };
+      KeyJoinDev& k = s->keyJoin;
+      const uint64_t cap = nextPow2P((uint64_t) std::max<int64_t>(expected_rows, 8) * 2); // load <= 0.5, like the other join tables
+      k.mask = cap - 1;
+      k.nKeys = n_keys;
+      k.entryBytes = n_keys <= 2 ? 32 : 48; // {word, payload, keys} padded: one 32-byte sector for 1-2 keys
+      k.unique = (flags & LDB_JOIN_UNIQUE) ? 1 : 0;
+      k.base = (uint8_t*) alloc(cap * k.entryBytes);
+      uint8_t* small = (uint8_t*) alloc(16);
+      k.count = (unsigned long long*) small;
+      k.error = (int32_t*) (small + 8);
+      if (cap >= 4096 && !(flags & LDB_JOIN_NO_BLOOM)) { // the plain tables' filter: 8 bits per directory slot
+         const uint64_t words = cap / 4;
+         k.bloom = (uint32_t*) alloc(words * 4);
+         k.bloomMask = (uint32_t) (words - 1);
+      }
+      *out = s;
+   });
+}
+} // extern "C"
+void ldb_gpu_check_keyjoin_error_internal(LdbState* s) {
+   int32_t e = 0;
+   LDB_CUDA(cudaMemcpyAsync(&e, s->keyJoin.error, sizeof(e), cudaMemcpyDeviceToHost, s->ctx->compute));
+   s->ctx->syncStream(s->ctx->compute);
+   switch (e) {
+      case 0: return;
+      case 1: failP(LDB_ERR_CAPACITY, "key-tuple join table full: more build rows than expected_rows allowed, or more than 65536 entries in one probe run (too many duplicates of one key tuple)");
+      case 6: failP(LDB_ERR_CAPACITY, "a probe run of a key-tuple join table is longer than the interpreter's bound of 16384 slots (too many entries share one run)");
+      case 7: failP(LDB_ERR_UNSUPPORTED, "a program join build met a key or payload outside int64 (key-tuple join tables store int64 keys and payloads)");
+      default: failP(LDB_ERR_INVALID, "key-tuple join table error word " + std::to_string(e));
+   }
+}
+extern "C" {
+
 // the pointers of column `ci` of batch `b` (validity bitmap or validity bytes included)
 static void bindColumn(ProgCol& pc, const LdbBatch& b, int ci) {
    pc.data = (const uint8_t*) b.data[ci];
@@ -432,6 +489,13 @@ static void runProgram(LdbContext* ctx, const LdbProgramDesc* d, const LdbProgra
    bool usesRowid = false;
    int eachTable = -1;
    bool probed[kProgMaxTables] = {}, coded[kProgMaxTables] = {}; // tables[k] read by PROBE / PROBE_EACH, by STRCODE
+   if (d->n_tables > 0 && !d->tables) failP(LDB_ERR_INVALID, "null tables list");
+   int tupleKeys[kProgMaxTables] = {}; // tables[k] is a key-tuple join table of this many keys: PROBE reads registers a .. a + n - 1
+   for (int k = 0; k < d->n_tables; k++)
+      if (d->tables[k] && d->tables[k]->kind == LDB_STATE_KEY_JOIN) tupleKeys[k] = d->tables[k]->keyJoin.nKeys;
+   auto wantKeys = [&](const LdbInstr& in) {
+      for (int k = 0; k < std::max(tupleKeys[in.arg], 1); k++) wantReg(in.a + k, "key");
+   };
    for (int i = 0; i < d->n_instr; i++) {
       const LdbInstr& in = d->instr[i];
       if (in.dst >= kProgMaxRegs) failP(LDB_ERR_INVALID, "destination register out of range");
@@ -477,14 +541,14 @@ static void runProgram(LdbContext* ctx, const LdbProgramDesc* d, const LdbProgra
             if (in.op == LDB_OP_STRCMP ? in.b > LDB_GTE : in.b > 2) failP(LDB_ERR_INVALID, "string op: unknown comparison / pattern kind");
             break;
          case LDB_OP_PROBE:
-            wantReg(in.a, "key");
             if (in.arg < 0 || in.arg >= d->n_tables) failP(LDB_ERR_INVALID, "PROBE: table index out of range");
+            wantKeys(in);
             probed[in.arg] = true;
             break;
          case LDB_OP_ROWID: usesRowid = true; break;
          case LDB_OP_PROBE_EACH:
-            wantReg(in.a, "key");
             if (in.arg < 0 || in.arg >= d->n_tables) failP(LDB_ERR_INVALID, "PROBE_EACH: table index out of range");
+            wantKeys(in);
             if (in.b > 1) failP(LDB_ERR_INVALID, "PROBE_EACH: b is 0 (inner) or 1 (left outer)");
             if (base.eachPc >= 0) failP(LDB_ERR_UNSUPPORTED, "at most one PROBE_EACH per program");
             base.eachPc = i;
@@ -509,9 +573,21 @@ static void runProgram(LdbContext* ctx, const LdbProgramDesc* d, const LdbProgra
       memcpy(base.strings[c], d->strings[c], n);
       base.stringLen[c] = (int32_t) n;
    }
-   std::vector<LdbState*> dicts;
+   std::vector<LdbState*> dicts, tupleTables; // tupleTables: key-tuple tables whose error word the run may set
+   auto wantTupleTable = [&](LdbState* js) {
+      if (js->ctx != ctx) failP(LDB_ERR_INVALID, "key-tuple join table belongs to another context");
+      if (ctx->capturing) failP(LDB_ERR_UNSUPPORTED, "key-tuple join tables are not part of captured queries");
+   };
    for (int k = 0; k < d->n_tables; k++) {
       LdbState* js = d->tables[k];
+      if (js && js->kind == LDB_STATE_KEY_JOIN) {
+         if (coded[k]) failP(LDB_ERR_INVALID, "STRCODE needs a string dictionary, not a join table");
+         wantTupleTable(js);
+         if (d->sink_kind == LDB_SINK_JOIN_BUILD && d->sink == js) failP(LDB_ERR_INVALID, "a program may not build a key-tuple join table and probe it");
+         base.keyTables[k] = js->keyJoin;
+         if (probed[k]) tupleTables.push_back(js);
+         continue;
+      }
       if (js && js->kind == LDB_STATE_DICT) {
          if (probed[k]) failP(LDB_ERR_INVALID, "PROBE / PROBE_EACH on a string dictionary (they take join tables)");
          if (js->ctx != ctx) failP(LDB_ERR_INVALID, "string dictionary belongs to another context");
@@ -568,6 +644,21 @@ static void runProgram(LdbContext* ctx, const LdbProgramDesc* d, const LdbProgra
          base.aggs[a] = ProgAgg{d->aggs[a].kind, d->aggs[a].reg};
       }
       base.agg = sink->hashagg;
+   } else if (d->sink_kind == LDB_SINK_JOIN_BUILD && sink && sink->kind == LDB_STATE_KEY_JOIN) {
+      // keys from n_keys / key_regs[]; payloads are int64, so ROWID has no row limit here
+      wantTupleTable(sink);
+      if (d->n_keys != sink->keyJoin.nKeys) failP(LDB_ERR_INVALID, "n_keys differs from the key-tuple join table's key count");
+      if (d->build_key_reg != -1) failP(LDB_ERR_INVALID, "a build into a key-tuple join table takes its keys from key_regs (build_key_reg must be -1)");
+      base.nKeys = d->n_keys;
+      for (int k = 0; k < d->n_keys; k++) {
+         wantReg(d->key_regs[k], "build key");
+         base.keyReg[k] = d->key_regs[k];
+      }
+      if (d->build_payload_reg >= 0) wantReg(d->build_payload_reg, "build payload");
+      base.buildKeyReg = -1;
+      base.buildPayloadReg = d->build_payload_reg;
+      base.keyBuild = sink->keyJoin;
+      tupleTables.push_back(sink);
    } else if (d->sink_kind == LDB_SINK_JOIN_BUILD) {
       if (!sink || sink->kind != LDB_STATE_JOIN_TABLE || sink->join.stride != 8 || sink->join.direct) failP(LDB_ERR_INVALID, "build sink must be a plain single-key join table");
       if (usesRowid && t->numRows > (int64_t) INT32_MAX) failP(LDB_ERR_UNSUPPORTED, "ROWID build payloads are int32: the source has 2^31 rows or more");
@@ -643,7 +734,8 @@ static void runProgram(LdbContext* ctx, const LdbProgramDesc* d, const LdbProgra
    // — and a dictionary that could not take a string
    try {
       for (LdbState* js : {eachTable >= 0 ? d->tables[eachTable] : nullptr, d->sink_kind == LDB_SINK_JOIN_BUILD ? sink : nullptr})
-         if (js) ldb_gpu_check_join_error_internal(js);
+         if (js && js->kind == LDB_STATE_JOIN_TABLE) ldb_gpu_check_join_error_internal(js);
+      for (LdbState* ks : tupleTables) ldb_gpu_check_keyjoin_error_internal(ks); // a full build, a probe run at the bound, a key outside int64
       for (LdbState* ds : dicts) checkDictError(ds);
    } catch (...) {
       ctx->syncStream(ctx->compute);

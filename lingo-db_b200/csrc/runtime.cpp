@@ -968,10 +968,12 @@ void ldb_gpu_check_join_error_internal(LdbState* s) { checkJoinError(s); }
 extern "C" {
 int ldb_gpu_join_table_count(LdbState* s, int64_t* n_entries, LdbError* err) {
    return guarded(err, [&] {
-      if (!s || s->kind != LDB_STATE_JOIN_TABLE) fail(LDB_ERR_INVALID, "not a join table");
-      checkJoinError(s);
+      if (!s || (s->kind != LDB_STATE_JOIN_TABLE && s->kind != LDB_STATE_KEY_JOIN)) fail(LDB_ERR_INVALID, "not a join table");
+      const bool keys = s->kind == LDB_STATE_KEY_JOIN;
+      if (keys) ldb_gpu_check_keyjoin_error_internal(s);
+      else checkJoinError(s);
       unsigned long long c = 0;
-      LDB_CUDA(cudaMemcpyAsync(&c, s->join.count, 8, cudaMemcpyDeviceToHost, s->ctx->compute));
+      LDB_CUDA(cudaMemcpyAsync(&c, keys ? s->keyJoin.count : s->join.count, 8, cudaMemcpyDeviceToHost, s->ctx->compute));
       s->ctx->syncStream(s->ctx->compute);
       *n_entries = (int64_t) c;
    });

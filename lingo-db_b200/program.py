@@ -11,10 +11,12 @@ An expression is a nested tuple:
   ("strcode", dict_state, column[, "lookup"])                the string's int32 code in a string dictionary (dict_state): inserted when
                                                              absent, or with "lookup" NULL when absent; a NULL string gives NULL
   ("year", a)                                                extract(year from date32)
-  ("probe", join_table_state, key)                           payload, or NULL when the key is absent (semi / anti / mark / outer joins)
-  ("probe_each", join_table_state, key[, "outer"])           payload of EACH match: what follows runs once per match (inner join; "outer":
+  ("probe", join_table_state, key, …)                        payload, or NULL when the key is absent (semi / anti / mark / outer joins);
+                                                             a key-tuple table (runtime.join_table_keys) takes one key per component
+  ("probe_each", join_table_state, key, …[, "outer"])        payload of EACH match: what follows runs once per match (inner join; "outer":
                                                              a row without a match yields one tuple with a NULL payload).  At most one
                                                              per program; emitted once, never re-evaluated.
+                                                             The keys of a tuple go to consecutive registers (moves where needed).
   ("rowid",)                                                 the scanned row's number in its table (a build payload for "fetch")
   ("fetch", side_table, row, "column")                       `column` of another table at the row `row` evaluates to (NULL row → NULL);
                                                              accepted wherever a column name is, also as the column of strcmp / like /
@@ -92,6 +94,14 @@ class Builder:
             self.consts.append(v)
         return self.consts.index(v)
 
+    def _keys(self, keys) -> int:
+        """The first of consecutive registers holding the key expressions: as evaluated when they already are consecutive, else
+        copied by moves (SELECT dst, x, x, x: condition, then and else all x) into fresh registers."""
+        regs = [self.expr(k) for k in keys]
+        if all(r == regs[0] + i for i, r in enumerate(regs)):
+            return regs[0]
+        return [self._emit("select", r, r, r) for r in regs][0]
+
     def _string(self, s: str):
         if s not in self.strings:
             self.strings.append(s)
@@ -113,8 +123,11 @@ class Builder:
                 raise ValueError("at most one probe_each per program")
             if e[1] not in self.tables:
                 self.tables.append(e[1])
-            outer = len(e) > 3 and e[3] == "outer"
-            r = self._emit("probe_each", self.expr(e[2]), int(outer), self.tables.index(e[1]))
+            keys = list(e[2:])
+            outer = keys[-1] == "outer"
+            if outer:
+                keys.pop()
+            r = self._emit("probe_each", self._keys(keys), int(outer), self.tables.index(e[1]))
             self._each = r
         elif k == "const":
             r = self._emit("const", arg=self._const(int(e[1])))
@@ -148,7 +161,7 @@ class Builder:
         elif k == "probe":
             if e[1] not in self.tables:
                 self.tables.append(e[1])
-            r = self._emit("probe", self.expr(e[2]), 0, self.tables.index(e[1]))
+            r = self._emit("probe", self._keys(e[2:]), 0, self.tables.index(e[1]))
         else:
             raise ValueError(f"unknown expression {k}")
         if key is not None:
@@ -254,13 +267,22 @@ def decode_groups(raw, n_keys: int, n_aggs: int, f64_aggs=()):
 
 
 def build_join(ctx, table, join_state, key, payload=None, where=None):
+    """key: one expression, or a list of 1..4 key expressions for a key-tuple table (runtime.join_table_keys)."""
     b = Builder()
     f = b.expr(where) if where is not None else -1
-    kr = b.expr(key)
+    tuple_keys = isinstance(key, list)
+    kregs = [b.expr(k) for k in key] if tuple_keys else [b.expr(key)]
     pr = b.expr(payload) if payload is not None else -1
     d, keep = _desc(ctx, table, b, f)
     d.sink_kind, d.sink = SINK_JOIN_BUILD, join_state
-    d.build_key_reg, d.build_payload_reg = kr, pr
+    if tuple_keys:
+        d.n_keys = len(kregs)
+        for i, r in enumerate(kregs):
+            d.key_regs[i] = r
+        d.build_key_reg = -1
+    else:
+        d.build_key_reg = kregs[0]
+    d.build_payload_reg = pr
     _run(ctx, d, b)
 
 

@@ -393,6 +393,14 @@ def join_table_pair(ctx: Context, expected_rows: int, unique: bool = True) -> C.
     return s
 
 
+def join_table_keys(ctx: Context, n_keys: int, expected_rows: int, unique: bool = True, bloom: bool = True) -> C.c_void_p:
+    """A key-tuple join table for program pipelines: 1..4 int64 keys → int64 payload (unique: duplicate tuples are dropped)."""
+    s, e = C.c_void_p(), Error()
+    flags = (1 if unique else 0) | (0 if bloom else 2)
+    check(ctx.L.ldb_gpu_join_table_create_keys(ctx.h, int(n_keys), int(expected_rows), flags, C.byref(s), C.byref(e)), e)
+    return s
+
+
 def join_table_direct(ctx: Context, key_min: int, key_max: int) -> C.c_void_p:
     s, e = C.c_void_p(), Error()
     check(ctx.L.ldb_gpu_join_table_create_direct(ctx.h, int(key_min), int(key_max), C.byref(s), C.byref(e)), e)
