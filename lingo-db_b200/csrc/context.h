@@ -7,6 +7,8 @@
 #include <cuda_runtime.h>
 #include <atomic>
 #include <condition_variable>
+#include <cstdio>
+#include <exception>
 #include <functional>
 #include <map>
 #include <memory>
@@ -34,6 +36,36 @@ struct ApiError : std::runtime_error {
    int code;
    ApiError(int code, const std::string& m) : std::runtime_error(m), code(code) {}
 };
+[[noreturn]] inline void fail(int code, const std::string& m) { throw ApiError(code, m); }
+
+// The body of every C-ABI entry point: no exception leaves an extern "C" function.  The status goes to the return value and,
+// with its message, to `err` when the caller passed one (LDB_OK and an empty message on success).
+template <class Fn>
+int guarded(LdbError* err, const Fn& fn) {
+   auto set = [&](int code, const char* msg) {
+      if (err) {
+         err->code = code;
+         snprintf(err->message, sizeof(err->message), "%s", msg);
+      }
+      return code;
+   };
+   try {
+      fn();
+      return set(LDB_OK, "");
+   } catch (const CudaError& e) {
+      return set(e.code, e.what());
+   } catch (const ApiError& e) {
+      return set(e.code, e.what());
+   } catch (const std::exception& e) {
+      return set(LDB_ERR_INVALID, e.what());
+   }
+}
+
+inline uint64_t nextPow2(uint64_t v) {
+   v--;
+   for (int s = 1; s < 64; s <<= 1) v |= v >> s;
+   return v + 1;
+}
 
 // Host worker pool used while staging HOST batches (narrowing decimal128 → the 8 bytes the kernels read).
 class HostPool {
@@ -158,6 +190,45 @@ struct LdbContext {
       LDB_CUDA(cudaGetLastError());
    }
 };
+
+namespace ldb {
+// The scratch device buffers of one call, from the context's staging pool, given back to it when the scope ends.  A call that
+// returns normally has already waited for the kernels that read them (it reads their results on the host); no wait is added
+// here because some of these calls run inside a graph capture.  A call that throws may leave such kernels queued: then the
+// compute stream is drained first, without throwing (and not while capturing, where nothing runs yet).
+class Scratch {
+   LdbContext* ctx;
+   std::vector<void*> bufs;
+   const int uncaught = std::uncaught_exceptions();
+
+   public:
+   explicit Scratch(LdbContext* c) : ctx(c) {}
+   Scratch(const Scratch&) = delete;
+   Scratch& operator=(const Scratch&) = delete;
+   ~Scratch() {
+      if (bufs.empty()) return;
+      if (std::uncaught_exceptions() > uncaught && !ctx->capturing) {
+         cudaStreamSynchronize(ctx->compute);
+         cudaGetLastError();
+      }
+      for (void* p : bufs) ctx->stagingRelease(p);
+   }
+   template <class T = void>
+   T* alloc(size_t bytes) {
+      bufs.reserve(bufs.size() + 1); // the push_back below cannot throw once the buffer is taken from the pool
+      void* p = ctx->stagingAlloc(bytes);
+      bufs.push_back(p);
+      return (T*) p;
+   }
+   bool empty() const { return bufs.empty(); }
+   // the buffers now belong to the caller (a result table's LdbBatch::owned)
+   std::vector<void*> take() {
+      std::vector<void*> out;
+      out.swap(bufs);
+      return out;
+   }
+};
+} // namespace ldb
 
 struct LdbBatch {
    int64_t nRows = 0;

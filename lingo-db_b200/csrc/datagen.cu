@@ -159,77 +159,61 @@ __global__ void dbgenBytesKernel(int table, int64_t rowBegin, int64_t n, const i
    }
 }
 int gridFor(LdbContext* ctx, int64_t n) { return (int) std::min<int64_t>(std::max<int64_t>((n + 255) / 256, 1), (int64_t) ctx->smCount * 16); }
-template <class Fn>
-int guardedGen(LdbError* err, const Fn& fn) {
-   try {
-      fn();
-      if (err) {
-         err->code = LDB_OK;
-         err->message[0] = 0;
-      }
-      return LDB_OK;
-   } catch (const ldb::CudaError& e) {
-      if (err) {
-         err->code = e.code;
-         snprintf(err->message, sizeof(err->message), "%s", e.what());
-      }
-      return e.code;
-   }
-}
 } // namespace
+using ldb::guarded;
 
 extern "C" {
 int ldb_gpu_datagen_lineitem(LdbContext* ctx, const LdbGenScale* g, int64_t row_begin, int64_t n_rows, const LdbGenLineitemCols* c, LdbError* err) {
-   return guardedGen(err, [&] {
+   return guarded(err, [&] {
       LDB_CUDA(cudaSetDevice(ctx->device));
       lineitemKernel<<<gridFor(ctx, n_rows), 256, 0, ctx->compute>>>(toScale(g), row_begin, n_rows, *c);
       LDB_CUDA(cudaGetLastError());
    });
 }
 int ldb_gpu_datagen_orders(LdbContext* ctx, const LdbGenScale* g, int64_t row_begin, int64_t n_rows, const LdbGenOrdersCols* c, LdbError* err) {
-   return guardedGen(err, [&] {
+   return guarded(err, [&] {
       LDB_CUDA(cudaSetDevice(ctx->device));
       ordersKernel<<<gridFor(ctx, n_rows), 256, 0, ctx->compute>>>(toScale(g), row_begin, n_rows, *c);
       LDB_CUDA(cudaGetLastError());
    });
 }
 int ldb_gpu_datagen_customer_fixed(LdbContext* ctx, const LdbGenScale* g, int64_t row_begin, int64_t n_rows, const LdbGenCustomerCols* c, int32_t* dev_seg_lengths, LdbError* err) {
-   return guardedGen(err, [&] {
+   return guarded(err, [&] {
       LDB_CUDA(cudaSetDevice(ctx->device));
       customerFixedKernel<<<gridFor(ctx, n_rows), 256, 0, ctx->compute>>>(toScale(g), row_begin, n_rows, *c, dev_seg_lengths);
       LDB_CUDA(cudaGetLastError());
    });
 }
 int ldb_gpu_datagen_customer_bytes(LdbContext* ctx, const LdbGenScale* g, int64_t row_begin, int64_t n_rows, const int32_t* dev_offsets, uint8_t* dev_data, LdbError* err) {
-   return guardedGen(err, [&] {
+   return guarded(err, [&] {
       LDB_CUDA(cudaSetDevice(ctx->device));
       customerBytesKernel<<<gridFor(ctx, n_rows), 256, 0, ctx->compute>>>(toScale(g), row_begin, n_rows, dev_offsets, dev_data);
       LDB_CUDA(cudaGetLastError());
    });
 }
 int ldb_gpu_datagen_supplier(LdbContext* ctx, const LdbGenScale* g, int64_t row_begin, int64_t n_rows, const LdbGenSupplierCols* c, LdbError* err) {
-   return guardedGen(err, [&] {
+   return guarded(err, [&] {
       LDB_CUDA(cudaSetDevice(ctx->device));
       supplierKernel<<<gridFor(ctx, n_rows), 256, 0, ctx->compute>>>(toScale(g), row_begin, n_rows, *c);
       LDB_CUDA(cudaGetLastError());
    });
 }
 int ldb_gpu_datagen_part_fixed(LdbContext* ctx, const LdbGenScale* g, int64_t row_begin, int64_t n_rows, const LdbGenPartCols* c, int32_t* dev_name_lengths, LdbError* err) {
-   return guardedGen(err, [&] {
+   return guarded(err, [&] {
       LDB_CUDA(cudaSetDevice(ctx->device));
       partFixedKernel<<<gridFor(ctx, n_rows), 256, 0, ctx->compute>>>(toScale(g), row_begin, n_rows, *c, dev_name_lengths);
       LDB_CUDA(cudaGetLastError());
    });
 }
 int ldb_gpu_datagen_part_bytes(LdbContext* ctx, const LdbGenScale* g, int64_t row_begin, int64_t n_rows, const int32_t* dev_offsets, uint8_t* dev_data, LdbError* err) {
-   return guardedGen(err, [&] {
+   return guarded(err, [&] {
       LDB_CUDA(cudaSetDevice(ctx->device));
       partBytesKernel<<<gridFor(ctx, n_rows), 256, 0, ctx->compute>>>(toScale(g), row_begin, n_rows, dev_offsets, dev_data);
       LDB_CUDA(cudaGetLastError());
    });
 }
 int ldb_gpu_datagen_partsupp(LdbContext* ctx, const LdbGenScale* g, int64_t row_begin, int64_t n_rows, const LdbGenPartsuppCols* c, LdbError* err) {
-   return guardedGen(err, [&] {
+   return guarded(err, [&] {
       LDB_CUDA(cudaSetDevice(ctx->device));
       partsuppKernel<<<gridFor(ctx, n_rows), 256, 0, ctx->compute>>>(toScale(g), row_begin, n_rows, *c);
       LDB_CUDA(cudaGetLastError());
@@ -238,35 +222,35 @@ int ldb_gpu_datagen_partsupp(LdbContext* ctx, const LdbGenScale* g, int64_t row_
 // ---- dbgen-faithful variant
 static ldbdbgen::Scale toDbgenScale(const LdbGenScale* g) { return ldbdbgen::Scale{g->n_orders, g->n_customer, g->n_supplier, g->n_part}; }
 int ldb_gpu_dbgen_line_counts(LdbContext* ctx, const LdbGenScale*, int64_t order_begin, int64_t n_orders, int32_t* dev_counts, LdbError* err) {
-   return guardedGen(err, [&] {
+   return guarded(err, [&] {
       LDB_CUDA(cudaSetDevice(ctx->device));
       dbgenLineCountsKernel<<<gridFor(ctx, n_orders), 256, 0, ctx->compute>>>(order_begin, n_orders, dev_counts);
       LDB_CUDA(cudaGetLastError());
    });
 }
 int ldb_gpu_dbgen_lineitem(LdbContext* ctx, const LdbGenScale* g, int64_t order_begin, int64_t n_orders, const int64_t* dev_first_row, const LdbGenLineitemCols* c, LdbError* err) {
-   return guardedGen(err, [&] {
+   return guarded(err, [&] {
       LDB_CUDA(cudaSetDevice(ctx->device));
       dbgenLineitemKernel<<<gridFor(ctx, n_orders), 256, 0, ctx->compute>>>(toDbgenScale(g), order_begin, n_orders, dev_first_row, *c);
       LDB_CUDA(cudaGetLastError());
    });
 }
 int ldb_gpu_dbgen_orders(LdbContext* ctx, const LdbGenScale* g, int64_t row_begin, int64_t n_rows, const LdbGenOrdersCols* c, LdbError* err) {
-   return guardedGen(err, [&] {
+   return guarded(err, [&] {
       LDB_CUDA(cudaSetDevice(ctx->device));
       dbgenOrdersKernel<<<gridFor(ctx, n_rows), 256, 0, ctx->compute>>>(toDbgenScale(g), row_begin, n_rows, *c);
       LDB_CUDA(cudaGetLastError());
    });
 }
 int ldb_gpu_dbgen_small_fixed(LdbContext* ctx, const LdbGenScale* g, int32_t table, int64_t row_begin, int64_t n_rows, int32_t* dev_key, int32_t* dev_second, uint8_t* dev_decimal, int32_t* dev_lengths, LdbError* err) {
-   return guardedGen(err, [&] {
+   return guarded(err, [&] {
       LDB_CUDA(cudaSetDevice(ctx->device));
       dbgenSmallFixedKernel<<<gridFor(ctx, n_rows), 256, 0, ctx->compute>>>(toDbgenScale(g), table, row_begin, n_rows, dev_key, dev_second, dev_decimal, dev_lengths);
       LDB_CUDA(cudaGetLastError());
    });
 }
 int ldb_gpu_dbgen_bytes(LdbContext* ctx, const LdbGenScale*, int32_t table, int64_t row_begin, int64_t n_rows, const int32_t* dev_offsets, uint8_t* dev_data, LdbError* err) {
-   return guardedGen(err, [&] {
+   return guarded(err, [&] {
       LDB_CUDA(cudaSetDevice(ctx->device));
       dbgenBytesKernel<<<gridFor(ctx, n_rows), 256, 0, ctx->compute>>>(table, row_begin, n_rows, dev_offsets, dev_data);
       LDB_CUDA(cudaGetLastError());

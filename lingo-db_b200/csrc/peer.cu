@@ -194,34 +194,6 @@ __global__ void peerPublishCountsKernel(PeerView v, size_t cursorsOff, size_t co
 using namespace ldb;
 
 // ---------------------------------------------------------------- host side
-namespace {
-template <class Fn>
-int guardedPeer(LdbError* err, const Fn& fn) {
-   auto set = [&](int code, const char* msg) {
-      if (err) {
-         err->code = code;
-         snprintf(err->message, sizeof(err->message), "%s", msg);
-      }
-      return code;
-   };
-   try {
-      fn();
-      if (err) {
-         err->code = LDB_OK;
-         err->message[0] = 0;
-      }
-      return LDB_OK;
-   } catch (const CudaError& e) {
-      return set(e.code, e.what());
-   } catch (const ApiError& e) {
-      return set(e.code, e.what());
-   } catch (const std::exception& e) {
-      return set(LDB_ERR_INVALID, e.what());
-   }
-}
-[[noreturn]] void failPeer(int code, const std::string& m) { throw ApiError(code, m); }
-} // namespace
-
 PeerView LdbComm::view() const {
    PeerView v{};
    v.rank = rank;
@@ -237,10 +209,10 @@ extern "C" {
 int64_t ldb_gpu_comm_reserved_bytes(void) { return (int64_t) kUserOff; }
 
 int ldb_gpu_comm_create(LdbContext* ctx, int32_t rank, int32_t world, int64_t user_bytes, LdbComm** out, uint8_t* handle_out, LdbError* err) {
-   return guardedPeer(err, [&] {
-      if (!ctx || !out || !handle_out) failPeer(LDB_ERR_INVALID, "null argument");
-      if (world < 1 || world > kMaxPeers || rank < 0 || rank >= world) failPeer(LDB_ERR_INVALID, "rank/world out of range (1..8 ranks)");
-      if (user_bytes < 0) failPeer(LDB_ERR_INVALID, "negative heap size");
+   return guarded(err, [&] {
+      if (!ctx || !out || !handle_out) fail(LDB_ERR_INVALID, "null argument");
+      if (world < 1 || world > kMaxPeers || rank < 0 || rank >= world) fail(LDB_ERR_INVALID, "rank/world out of range (1..8 ranks)");
+      if (user_bytes < 0) fail(LDB_ERR_INVALID, "negative heap size");
       LDB_CUDA(cudaSetDevice(ctx->device));
       auto c = std::make_unique<LdbComm>();
       c->ctx = ctx;
@@ -275,8 +247,8 @@ int ldb_gpu_comm_create(LdbContext* ctx, int32_t rank, int32_t world, int64_t us
 
 // all_handles: world x 64 bytes in rank order (exchanged by the caller: torch.distributed all_gather, MPI, a file …)
 int ldb_gpu_comm_connect(LdbComm* c, const uint8_t* all_handles, LdbError* err) {
-   return guardedPeer(err, [&] {
-      if (!c || !all_handles) failPeer(LDB_ERR_INVALID, "null argument");
+   return guarded(err, [&] {
+      if (!c || !all_handles) fail(LDB_ERR_INVALID, "null argument");
       LDB_CUDA(cudaSetDevice(c->ctx->device));
       for (int p = 0; p < c->world; p++) {
          if (p == c->rank) continue;
@@ -293,17 +265,17 @@ int ldb_gpu_comm_connect(LdbComm* c, const uint8_t* all_handles, LdbError* err) 
 
 // single-process variant (tests, one process driving several devices): peers are other LdbComm objects of this process
 int ldb_gpu_comm_connect_local(LdbComm** comms, int32_t n, LdbError* err) {
-   return guardedPeer(err, [&] {
-      if (!comms || n < 1 || n > kMaxPeers) failPeer(LDB_ERR_INVALID, "bad comm list");
+   return guarded(err, [&] {
+      if (!comms || n < 1 || n > kMaxPeers) fail(LDB_ERR_INVALID, "bad comm list");
       for (int i = 0; i < n; i++) {
-         if (!comms[i] || comms[i]->world != n || comms[i]->rank != i) failPeer(LDB_ERR_INVALID, "comm list must hold ranks 0..n-1 of one world");
+         if (!comms[i] || comms[i]->world != n || comms[i]->rank != i) fail(LDB_ERR_INVALID, "comm list must hold ranks 0..n-1 of one world");
          LDB_CUDA(cudaSetDevice(comms[i]->ctx->device));
          for (int p = 0; p < n; p++) {
             if (p == i) continue;
             if (comms[p]->ctx->device != comms[i]->ctx->device) {
                int can = 0;
                LDB_CUDA(cudaDeviceCanAccessPeer(&can, comms[i]->ctx->device, comms[p]->ctx->device));
-               if (!can) failPeer(LDB_ERR_UNSUPPORTED, "devices cannot access each other's memory");
+               if (!can) fail(LDB_ERR_UNSUPPORTED, "devices cannot access each other's memory");
                cudaError_t e = cudaDeviceEnablePeerAccess(comms[p]->ctx->device, 0);
                if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) LDB_CUDA(e);
                cudaGetLastError();
@@ -334,12 +306,12 @@ int32_t ldb_gpu_comm_rank(LdbComm* c) { return c ? c->rank : -1; }
 int32_t ldb_gpu_comm_world(LdbComm* c) { return c ? c->world : 0; }
 
 static void wantConnected(LdbComm* c) {
-   if (!c) failPeer(LDB_ERR_INVALID, "null comm");
-   if (!c->connected && c->world > 1) failPeer(LDB_ERR_INVALID, "comm is not connected to its peers yet");
+   if (!c) fail(LDB_ERR_INVALID, "null comm");
+   if (!c->connected && c->world > 1) fail(LDB_ERR_INVALID, "comm is not connected to its peers yet");
 }
 
 int ldb_gpu_comm_barrier(LdbComm* c, LdbError* err) {
-   return guardedPeer(err, [&] {
+   return guarded(err, [&] {
       wantConnected(c);
       if (c->world == 1) return;
       LdbContext* ctx = c->ctx;
@@ -355,12 +327,12 @@ int ldb_gpu_comm_barrier(LdbComm* c, LdbError* err) {
 // blocks of this collective: block of rank r at result + r * ldb_gpu_comm_slot_bytes().  Valid until the next-but-one gather.
 int64_t ldb_gpu_comm_slot_bytes(void) { return (int64_t) kSlotBytes; }
 int ldb_gpu_comm_allgather_small(LdbComm* c, const void* src, int64_t bytes, void** result, LdbError* err) {
-   return guardedPeer(err, [&] {
+   return guarded(err, [&] {
       wantConnected(c);
-      if (bytes <= 0 || bytes > (int64_t) kSlotBytes || bytes % 16) failPeer(LDB_ERR_INVALID, "all-gather blocks are 16..262144 bytes, multiples of 16");
+      if (bytes <= 0 || bytes > (int64_t) kSlotBytes || bytes % 16) fail(LDB_ERR_INVALID, "all-gather blocks are 16..262144 bytes, multiples of 16");
       LdbContext* ctx = c->ctx;
       LDB_CUDA(cudaSetDevice(ctx->device));
-      if (ctx->capturing) failPeer(LDB_ERR_UNSUPPORTED, "the small all-gather returns a parity-dependent address and cannot be captured");
+      if (ctx->capturing) fail(LDB_ERR_UNSUPPORTED, "the small all-gather returns a parity-dependent address and cannot be captured");
       const unsigned long long epoch = ++c->gatherEpochHost; // mirror of the device counter (every rank issues the same collectives)
       ctx->launch("peer_allgather", [&] {
          peerAllGatherKernel<<<c->world, 256, 0, ctx->compute>>>(c->view(), (const uint8_t*) src, (size_t) bytes);
@@ -371,14 +343,14 @@ int ldb_gpu_comm_allgather_small(LdbComm* c, const void* src, int64_t bytes, voi
 }
 
 int ldb_gpu_groupby_allmerge(LdbState* s, LdbComm* c, LdbError* err) {
-   return guardedPeer(err, [&] {
-      if (!s || (s->kind != LDB_STATE_GROUPBY && s->kind != LDB_STATE_SIMPLE)) failPeer(LDB_ERR_INVALID, "not a group state");
+   return guarded(err, [&] {
+      if (!s || (s->kind != LDB_STATE_GROUPBY && s->kind != LDB_STATE_SIMPLE)) fail(LDB_ERR_INVALID, "not a group state");
       wantConnected(c);
-      if (s->ctx != c->ctx) failPeer(LDB_ERR_INVALID, "state and comm belong to different contexts");
+      if (s->ctx != c->ctx) fail(LDB_ERR_INVALID, "state and comm belong to different contexts");
       ldb_gpu_want_bound_lanes_internal(s);
       if (c->world == 1) return;
       const size_t image = (groupImageBytes(s->group.capacity) + 15) & ~size_t(15); // the table allocation carries 16 spare bytes (error word)
-      if (image > kSlotBytes) failPeer(LDB_ERR_UNSUPPORTED, "group table image larger than a mailbox slot (capacity <= 1024 groups)");
+      if (image > kSlotBytes) fail(LDB_ERR_UNSUPPORTED, "group table image larger than a mailbox slot (capacity <= 1024 groups)");
       LdbContext* ctx = c->ctx;
       LDB_CUDA(cudaSetDevice(ctx->device));
       // the mirror follows the device epoch: bumped when the kernel runs (now, or at every replay of a capture), never at capture
@@ -392,9 +364,9 @@ int ldb_gpu_groupby_allmerge(LdbState* s, LdbComm* c, LdbError* err) {
 }
 
 int ldb_gpu_comm_or_reduce(LdbComm* c, int64_t user_offset, int64_t bytes, LdbError* err) {
-   return guardedPeer(err, [&] {
+   return guarded(err, [&] {
       wantConnected(c);
-      if (user_offset < 0 || bytes < 0 || user_offset % 16 || bytes % 16 || (size_t) (user_offset + bytes) > c->userBytes) failPeer(LDB_ERR_INVALID, "OR-reduce range outside the heap or not 16-byte aligned");
+      if (user_offset < 0 || bytes < 0 || user_offset % 16 || bytes % 16 || (size_t) (user_offset + bytes) > c->userBytes) fail(LDB_ERR_INVALID, "OR-reduce range outside the heap or not 16-byte aligned");
       if (c->world == 1 || bytes == 0) return;
       LdbContext* ctx = c->ctx;
       LDB_CUDA(cudaSetDevice(ctx->device));
@@ -405,25 +377,25 @@ int ldb_gpu_comm_or_reduce(LdbComm* c, int64_t user_offset, int64_t bytes, LdbEr
 }
 
 int ldb_gpu_comm_heap_zero(LdbComm* c, int64_t user_offset, int64_t bytes, LdbError* err) {
-   return guardedPeer(err, [&] {
-      if (!c || user_offset < 0 || bytes < 0 || (size_t) (user_offset + bytes) > c->userBytes) failPeer(LDB_ERR_INVALID, "range outside the comm's user heap");
+   return guarded(err, [&] {
+      if (!c || user_offset < 0 || bytes < 0 || (size_t) (user_offset + bytes) > c->userBytes) fail(LDB_ERR_INVALID, "range outside the comm's user heap");
       LDB_CUDA(cudaSetDevice(c->ctx->device));
       LDB_CUDA(cudaMemsetAsync(c->heap + kUserOff + user_offset, 0, (size_t) bytes, c->ctx->compute));
    });
 }
 int ldb_gpu_comm_heap_read(LdbComm* c, int64_t user_offset, int64_t bytes, void* host_dst, LdbError* err) {
-   return guardedPeer(err, [&] {
-      if (!c || !host_dst || user_offset < 0 || bytes < 0 || (size_t) (user_offset + bytes) > c->userBytes) failPeer(LDB_ERR_INVALID, "range outside the comm's user heap");
+   return guarded(err, [&] {
+      if (!c || !host_dst || user_offset < 0 || bytes < 0 || (size_t) (user_offset + bytes) > c->userBytes) fail(LDB_ERR_INVALID, "range outside the comm's user heap");
       LDB_CUDA(cudaSetDevice(c->ctx->device));
       LDB_CUDA(cudaMemcpyAsync(host_dst, c->heap + kUserOff + user_offset, (size_t) bytes, cudaMemcpyDeviceToHost, c->ctx->compute));
       c->ctx->syncStream(c->ctx->compute);
    });
 }
 static void wantRange(LdbComm* c, int64_t off, int64_t bytes, const char* what) {
-   if (off < 0 || bytes < 0 || off % 16 || (size_t) (off + bytes) > c->userBytes) failPeer(LDB_ERR_CAPACITY, std::string(what) + " outside the comm's user heap (create the comm with a larger heap)");
+   if (off < 0 || bytes < 0 || off % 16 || (size_t) (off + bytes) > c->userBytes) fail(LDB_ERR_CAPACITY, std::string(what) + " outside the comm's user heap (create the comm with a larger heap)");
 }
 int ldb_gpu_comm_publish_counts(LdbComm* c, int64_t cursors_offset, int64_t counts_offset, LdbError* err) {
-   return guardedPeer(err, [&] {
+   return guarded(err, [&] {
       wantConnected(c);
       wantRange(c, cursors_offset, 16 * 8, "cursors");
       wantRange(c, counts_offset, kMaxPeers * 8, "counts");
@@ -433,9 +405,9 @@ int ldb_gpu_comm_publish_counts(LdbComm* c, int64_t cursors_offset, int64_t coun
    });
 }
 int ldb_gpu_join_table_insert_received(LdbState* table, LdbComm* c, int64_t recv_offset, int64_t capacity, int64_t counts_offset, LdbError* err) {
-   return guardedPeer(err, [&] {
+   return guarded(err, [&] {
       wantConnected(c);
-      if (!table || table->kind != LDB_STATE_JOIN_TABLE || table->join.stride != 8 || table->join.direct) failPeer(LDB_ERR_INVALID, "insert target must be a plain single-key join table");
+      if (!table || table->kind != LDB_STATE_JOIN_TABLE || table->join.stride != 8 || table->join.direct) fail(LDB_ERR_INVALID, "insert target must be a plain single-key join table");
       wantRange(c, recv_offset, (int64_t) c->world * capacity * 8, "receive region");
       wantRange(c, counts_offset, kMaxPeers * 8, "counts");
       LdbContext* ctx = c->ctx;
@@ -445,12 +417,12 @@ int ldb_gpu_join_table_insert_received(LdbState* table, LdbComm* c, int64_t recv
    });
 }
 int ldb_gpu_probe_received_groupby(LdbState* ta, LdbState* tb, LdbState* groups, LdbComm* c, int64_t recv_offset, int64_t capacity, int64_t counts_offset, int32_t scale, LdbError* err) {
-   return guardedPeer(err, [&] {
+   return guarded(err, [&] {
       wantConnected(c);
       for (LdbState* t : {ta, tb})
-         if (!t || t->kind != LDB_STATE_JOIN_TABLE || t->join.stride != 8 || t->join.direct) failPeer(LDB_ERR_INVALID, "probe tables must be plain single-key join tables");
-      if (!groups || groups->kind != LDB_STATE_GROUPBY || groups->group.nKeys != 1 || groups->group.nAggs != 1) failPeer(LDB_ERR_INVALID, "sink must be a group-by state with one key and one aggregate");
-      if (scale < 0 || scale > 18) failPeer(LDB_ERR_INVALID, "decimal scale out of range");
+         if (!t || t->kind != LDB_STATE_JOIN_TABLE || t->join.stride != 8 || t->join.direct) fail(LDB_ERR_INVALID, "probe tables must be plain single-key join tables");
+      if (!groups || groups->kind != LDB_STATE_GROUPBY || groups->group.nKeys != 1 || groups->group.nAggs != 1) fail(LDB_ERR_INVALID, "sink must be a group-by state with one key and one aggregate");
+      if (scale < 0 || scale > 18) fail(LDB_ERR_INVALID, "decimal scale out of range");
       wantRange(c, recv_offset, (int64_t) c->world * capacity * 24, "receive region");
       wantRange(c, counts_offset, kMaxPeers * 8, "counts");
       ldb_gpu_bind_lane_width_internal(groups, 0, LDB_EXPR_MUL_1MINUS); // a * (10^scale - b): a 128-bit sum
@@ -466,10 +438,10 @@ int ldb_gpu_probe_received_groupby(LdbState* ta, LdbState* tb, LdbState* groups,
 }
 
 int ldb_gpu_probe_received_groupby2(LdbState* table, LdbState* groups, LdbComm* c, int64_t recv_offset, int64_t capacity, int64_t counts_offset, LdbError* err) {
-   return guardedPeer(err, [&] {
+   return guarded(err, [&] {
       wantConnected(c);
-      if (!table || table->kind != LDB_STATE_JOIN_TABLE || table->join.stride != 8 || table->join.direct) failPeer(LDB_ERR_INVALID, "probe table must be a plain single-key join table");
-      if (!groups || groups->kind != LDB_STATE_GROUPBY || groups->group.nKeys != 2 || groups->group.nAggs != 1) failPeer(LDB_ERR_INVALID, "sink must be a group-by state with two keys and one aggregate");
+      if (!table || table->kind != LDB_STATE_JOIN_TABLE || table->join.stride != 8 || table->join.direct) fail(LDB_ERR_INVALID, "probe table must be a plain single-key join table");
+      if (!groups || groups->kind != LDB_STATE_GROUPBY || groups->group.nKeys != 2 || groups->group.nAggs != 1) fail(LDB_ERR_INVALID, "sink must be a group-by state with two keys and one aggregate");
       wantRange(c, recv_offset, (int64_t) c->world * capacity * 24, "receive region");
       wantRange(c, counts_offset, kMaxPeers * 8, "counts");
       ldb_gpu_bind_lane_width_internal(groups, 0, LDB_EXPR_MUL_1MINUS_MINUS_PAYMUL); // the shipped K11 sums are 128-bit
@@ -484,13 +456,13 @@ int ldb_gpu_probe_received_groupby2(LdbState* table, LdbState* groups, LdbComm* 
 
 // surfaces a timed-out wait (dead or stuck peer); synchronises the compute stream
 int ldb_gpu_comm_check(LdbComm* c, LdbError* err) {
-   return guardedPeer(err, [&] {
-      if (!c) failPeer(LDB_ERR_INVALID, "null comm");
+   return guarded(err, [&] {
+      if (!c) fail(LDB_ERR_INVALID, "null comm");
       LDB_CUDA(cudaSetDevice(c->ctx->device));
       int32_t e = 0;
       LDB_CUDA(cudaMemcpyAsync(&e, c->error, 4, cudaMemcpyDeviceToHost, c->ctx->compute));
       c->ctx->syncStream(c->ctx->compute);
-      if (e) failPeer(LDB_ERR_CUDA, "a peer did not arrive at a collective within the timeout (LDB_PEER_TIMEOUT_MS)");
+      if (e) fail(LDB_ERR_CUDA, "a peer did not arrive at a collective within the timeout (LDB_PEER_TIMEOUT_MS)");
    });
 }
 

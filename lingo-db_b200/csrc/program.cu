@@ -926,18 +926,6 @@ __global__ void __launch_bounds__(kSortThreads) sortScatterKernel(const unsigned
       __syncthreads();
    }
 }
-__global__ void buildSortKeysKernel(const uint8_t* col, int elemBytes, int64_t n, int descending, unsigned long long* keys, uint32_t* ids) {
-   for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t) gridDim.x * blockDim.x) {
-      const int64_t v = elemBytes == 4 ? (int64_t) ((const int32_t*) col)[i] : *(const int64_t*) (col + (size_t) i * elemBytes);
-      const unsigned long long k = (unsigned long long) v ^ 0x8000000000000000ull;
-      keys[i] = descending ? ~k : k;
-      ids[i] = (uint32_t) i;
-   }
-}
-void launchBuildSortKeys(const uint8_t* col, int elemBytes, int64_t n, int descending, unsigned long long* keys, uint32_t* ids, int smCount, cudaStream_t s) {
-   int grid = (int) std::min<int64_t>(std::max<int64_t>((n + 255) / 256, 1), (int64_t) smCount * 8);
-   buildSortKeysKernel<<<grid, 256, 0, s>>>(col, elemBytes, n, descending, keys, ids);
-}
 void launchRadixSortPairs(unsigned long long* keys, uint32_t* vals, unsigned long long* keysTmp, uint32_t* valsTmp, int64_t n, unsigned int* histScratch, int smCount, cudaStream_t s) {
    if (n <= 0) return;
    const int ctas = (int) ((n + kSortItemsPerCta - 1) / kSortItemsPerCta);

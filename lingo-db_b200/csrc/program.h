@@ -144,8 +144,6 @@ void launchHashAggInit(const HashAggDev& t, int smCount, cudaStream_t s);
 // compacts the occupied entries into columnar buffers: keys (int64 + validity byte), aggregates (16 B + validity byte)
 void launchHashAggExport(const HashAggDev& t, int64_t* const* keyCols, uint8_t* const* keyValid, uint8_t* const* aggCols, uint8_t* const* aggValid, unsigned long long* counter, uint32_t countAggMask, int smCount, cudaStream_t s);
 // LSD radix sort of (64-bit key, 32-bit row id) pairs — ORDER BY / top-k over materialised rows (GrowingBuffer::sort, Sorting.cpp)
-// order-preserving 64-bit sort keys + row ids from one fixed-width column (low 8 bytes of a cell, sign bit flipped; inverted for DESC)
-void launchBuildSortKeys(const uint8_t* col, int elemBytes, int64_t n, int descending, unsigned long long* keys, uint32_t* ids, int smCount, cudaStream_t s);
 void launchRadixSortPairs(unsigned long long* keys, uint32_t* vals, unsigned long long* keysTmp, uint32_t* valsTmp, int64_t n, unsigned int* histScratch, int smCount, cudaStream_t s);
 // multi-key ORDER BY: the 64-bit sort words of one key at the current permutation `ids` (first = 1: ids := 0..n-1 first).
 // kind 0: a fixed-width cell (low 8 bytes, sign bit flipped); kind 1: a utf8 cell's length (the longest is atomicMax'ed into

@@ -11,61 +11,33 @@
 using namespace ldb;
 
 namespace {
-template <class Fn>
-int guardedP(LdbError* err, const Fn& fn) {
-   auto set = [&](int code, const char* msg) {
-      if (err) {
-         err->code = code;
-         snprintf(err->message, sizeof(err->message), "%s", msg);
-      }
-      return code;
-   };
-   try {
-      fn();
-      if (err) {
-         err->code = LDB_OK;
-         err->message[0] = 0;
-      }
-      return LDB_OK;
-   } catch (const CudaError& e) {
-      return set(e.code, e.what());
-   } catch (const ApiError& e) {
-      return set(e.code, e.what());
-   } catch (const std::exception& e) {
-      return set(LDB_ERR_INVALID, e.what());
-   }
-}
-[[noreturn]] void failP(int code, const std::string& m) { throw ApiError(code, m); }
-uint64_t nextPow2P(uint64_t v) {
-   v--;
-   for (int s = 1; s < 64; s <<= 1) v |= v >> s;
-   return v + 1;
-}
 bool isCountKind(int k) { return k == LDB_AGG_COUNT || k == LDB_AGG_COUNT_STAR; }
-size_t cellBytes(int type) {
-   switch (type) {
-      case LDB_INT8: return 1;
-      case LDB_INT16: return 2;
-      case LDB_INT32:
-      case LDB_DATE32:
-      case LDB_FSB4:
-      case LDB_FLOAT32:
-      case LDB_UTF8: return 4;
-      case LDB_INT64:
-      case LDB_FLOAT64: return 8;
-      default: return 16;
-   }
-}
 } // namespace
+
+// registers a single-batch table this library made: `b` holds nRows and, per column, data / bytes / elemBytes / validBytes; the table
+// takes over the device buffers of `buffers`
+static LdbTable* addResultTable(LdbContext* ctx, std::string name, std::vector<LdbColumn> columns, LdbBatch b, Scratch& buffers) {
+   auto* t = new LdbTable;
+   t->ctx = ctx;
+   t->name = std::move(name);
+   t->columns = std::move(columns);
+   t->numRows = b.nRows;
+   b.validity.assign(b.data.size(), nullptr);
+   b.validityBitOffset.assign(b.data.size(), 0);
+   b.owned = buffers.take();
+   t->batches.push_back(std::move(b));
+   ctx->tables.push_back(t);
+   return t;
+}
 
 extern "C" {
 
 int ldb_gpu_hashagg_create(LdbContext* ctx, int32_t n_keys, int32_t n_aggs, const LdbProgAgg* aggs, int64_t expected_groups, LdbState** out, LdbError* err) {
-   return guardedP(err, [&] {
-      if (!ctx || !out || (n_aggs > 0 && !aggs)) failP(LDB_ERR_INVALID, "null argument");
-      if (n_keys < 0 || n_keys > kProgMaxKeys || n_aggs < 0 || n_aggs > kProgMaxAggs) failP(LDB_ERR_INVALID, "hash aggregation takes 0..4 keys and 0..8 aggregates");
+   return guarded(err, [&] {
+      if (!ctx || !out || (n_aggs > 0 && !aggs)) fail(LDB_ERR_INVALID, "null argument");
+      if (n_keys < 0 || n_keys > kProgMaxKeys || n_aggs < 0 || n_aggs > kProgMaxAggs) fail(LDB_ERR_INVALID, "hash aggregation takes 0..4 keys and 0..8 aggregates");
       for (int a = 0; a < n_aggs; a++)
-         if (aggs[a].kind < LDB_AGG_SUM || aggs[a].kind > LDB_AGG_ANY) failP(LDB_ERR_INVALID, "unknown aggregate kind");
+         if (aggs[a].kind < LDB_AGG_SUM || aggs[a].kind > LDB_AGG_ANY) fail(LDB_ERR_INVALID, "unknown aggregate kind");
       LDB_CUDA(cudaSetDevice(ctx->device));
       auto* s = new LdbState;
       s->ctx = ctx;
@@ -75,7 +47,7 @@ int ldb_gpu_hashagg_create(LdbContext* ctx, int32_t n_keys, int32_t n_aggs, cons
       h.nKeys = n_keys;
       h.nAggs = n_aggs;
       h.entryBytes = (uint32_t) (48 + 16 * n_aggs);
-      const uint64_t cap = n_keys == 0 ? 1 : nextPow2P((uint64_t) std::max<int64_t>(expected_groups, 8) * 2);
+      const uint64_t cap = n_keys == 0 ? 1 : nextPow2((uint64_t) std::max<int64_t>(expected_groups, 8) * 2);
       h.mask = cap - 1;
       h.base = (uint8_t*) ctx->stagingAlloc(cap * h.entryBytes);
       s->allocations.push_back(h.base);
@@ -112,62 +84,57 @@ int ldb_gpu_hashagg_create(LdbContext* ctx, int32_t n_keys, int32_t n_aggs, cons
    });
 }
 static void checkHashAgg(LdbState* s) {
-   if (!s || s->kind != LDB_STATE_HASHAGG) failP(LDB_ERR_INVALID, "not a hash aggregation state");
+   if (!s || s->kind != LDB_STATE_HASHAGG) fail(LDB_ERR_INVALID, "not a hash aggregation state");
 }
 int ldb_gpu_hashagg_count(LdbState* s, int64_t* n_groups, LdbError* err) {
-   return guardedP(err, [&] {
+   return guarded(err, [&] {
       checkHashAgg(s);
       unsigned long long h[2] = {0, 0};
       LDB_CUDA(cudaMemcpyAsync(h, s->hashagg.count, 16, cudaMemcpyDeviceToHost, s->ctx->compute));
       s->ctx->syncStream(s->ctx->compute);
-      if ((int32_t) h[1]) failP(LDB_ERR_CAPACITY, "hash aggregation table full: more groups than expected_groups allowed");
+      if ((int32_t) h[1]) fail(LDB_ERR_CAPACITY, "hash aggregation table full: more groups than expected_groups allowed");
       *n_groups = (int64_t) h[0];
    });
 }
 
-// export into fresh device columns; returns the row count (synchronises)
+// export into fresh device columns, allocated in `cols`; returns the row count (synchronises before the export, not after)
 struct ExportedGroups {
    int64_t n = 0;
    std::vector<int64_t*> keyCols;
    std::vector<uint8_t*> keyValid, aggCols, aggValid;
 };
-static ExportedGroups exportGroups(LdbState* s, std::vector<void*>& owned) {
+static ExportedGroups exportGroups(LdbState* s, Scratch& cols) {
    LdbContext* ctx = s->ctx;
    auto& h = s->hashagg;
    int64_t n = 0;
    LdbError e;
-   if (ldb_gpu_hashagg_count(s, &n, &e) != LDB_OK) failP(e.code, e.message);
+   if (ldb_gpu_hashagg_count(s, &n, &e) != LDB_OK) fail(e.code, e.message);
    ExportedGroups g;
    g.n = n;
    const size_t rows = (size_t) std::max<int64_t>(n, 1);
-   auto alloc = [&](size_t bytes) {
-      void* p = ctx->stagingAlloc(bytes);
-      owned.push_back(p);
-      return p;
-   };
    for (int k = 0; k < h.nKeys; k++) {
-      g.keyCols.push_back((int64_t*) alloc(rows * 8));
-      g.keyValid.push_back((uint8_t*) alloc(rows));
+      g.keyCols.push_back(cols.alloc<int64_t>(rows * 8));
+      g.keyValid.push_back(cols.alloc<uint8_t>(rows));
    }
    uint32_t countMask = 0;
    for (int a = 0; a < h.nAggs; a++) {
-      g.aggCols.push_back((uint8_t*) alloc(rows * 16));
-      g.aggValid.push_back((uint8_t*) alloc(rows));
+      g.aggCols.push_back(cols.alloc<uint8_t>(rows * 16));
+      g.aggValid.push_back(cols.alloc<uint8_t>(rows));
       if (isCountKind(s->aggKinds[a])) countMask |= 1u << a;
    }
-   unsigned long long* counter = (unsigned long long*) alloc(8);
+   unsigned long long* counter = cols.alloc<unsigned long long>(8);
    LDB_CUDA(cudaMemsetAsync(counter, 0, 8, ctx->compute));
    ctx->launch("hashagg_export", [&] { launchHashAggExport(h, g.keyCols.data(), g.keyValid.data(), g.aggCols.data(), g.aggValid.data(), counter, countMask, ctx->smCount, ctx->compute); });
    return g;
 }
 int ldb_gpu_hashagg_read(LdbState* s, LdbHashAggRow* rows, int64_t max_rows, int64_t* n_rows, LdbError* err) {
-   return guardedP(err, [&] {
+   return guarded(err, [&] {
       checkHashAgg(s);
-      if (!rows || !n_rows) failP(LDB_ERR_INVALID, "null argument");
+      if (!rows || !n_rows) fail(LDB_ERR_INVALID, "null argument");
       LdbContext* ctx = s->ctx;
       LDB_CUDA(cudaSetDevice(ctx->device));
-      std::vector<void*> owned;
-      ExportedGroups g = exportGroups(s, owned);
+      Scratch cols(ctx);
+      ExportedGroups g = exportGroups(s, cols);
       auto& h = s->hashagg;
       const int64_t n = std::min(g.n, max_rows);
       std::vector<std::vector<int64_t>> keys(h.nKeys, std::vector<int64_t>((size_t) n));
@@ -195,26 +162,23 @@ int ldb_gpu_hashagg_read(LdbState* s, LdbHashAggRow* rows, int64_t max_rows, int
          }
       }
       *n_rows = g.n;
-      for (void* p : owned) ctx->stagingRelease(p);
    });
 }
 int ldb_gpu_hashagg_to_table(LdbState* s, const char* name, LdbTable** out, LdbError* err) {
-   return guardedP(err, [&] {
+   return guarded(err, [&] {
       checkHashAgg(s);
-      if (!out) failP(LDB_ERR_INVALID, "null argument");
+      if (!out) fail(LDB_ERR_INVALID, "null argument");
       LdbContext* ctx = s->ctx;
       LDB_CUDA(cudaSetDevice(ctx->device));
-      std::vector<void*> owned;
-      ExportedGroups g = exportGroups(s, owned);
+      Scratch cols(ctx);
+      ExportedGroups g = exportGroups(s, cols);
       ctx->syncStream(ctx->compute);
       auto& h = s->hashagg;
-      auto* t = new LdbTable;
-      t->ctx = ctx;
-      t->name = name ? name : "groups";
+      std::vector<LdbColumn> columns;
       LdbBatch b;
       b.nRows = g.n;
       for (int k = 0; k < h.nKeys; k++) {
-         t->columns.push_back({"k" + std::to_string(k), LDB_INT64, 0, 0});
+         columns.push_back({"k" + std::to_string(k), LDB_INT64, 0, 0});
          b.data.push_back(g.keyCols[k]);
          b.bytes.push_back(nullptr);
          b.elemBytes.push_back(8);
@@ -223,19 +187,13 @@ int ldb_gpu_hashagg_to_table(LdbState* s, const char* name, LdbTable** out, LdbE
       for (int a = 0; a < h.nAggs; a++) {
          const int kind = s->aggKinds[a];
          const bool f64 = kind == LDB_AGG_SUM_F64 || kind == LDB_AGG_MIN_F64 || kind == LDB_AGG_MAX_F64;
-         t->columns.push_back({"a" + std::to_string(a), f64 ? LDB_FLOAT64 : LDB_DECIMAL128, 38, 0});
+         columns.push_back({"a" + std::to_string(a), f64 ? LDB_FLOAT64 : LDB_DECIMAL128, 38, 0});
          b.data.push_back(g.aggCols[a]);
          b.bytes.push_back(nullptr);
          b.elemBytes.push_back(16); // doubles keep the 16-byte stride (bits in the low 8 bytes)
          b.validBytes.push_back(g.aggValid[a]);
       }
-      b.validity.assign(b.data.size(), nullptr);
-      b.validityBitOffset.assign(b.data.size(), 0);
-      b.owned = owned; // the table owns the exported buffers
-      t->numRows = g.n;
-      t->batches.push_back(std::move(b));
-      ctx->tables.push_back(t);
-      *out = t;
+      *out = addResultTable(ctx, name ? name : "groups", std::move(columns), std::move(b), cols);
    });
 }
 
@@ -243,7 +201,7 @@ static_assert(sizeof(ProgramParams) <= 4096, "ProgramParams exceeds the 4 KB ker
 
 // ---------------------------------------------------------------- string dictionaries
 static void checkDict(LdbState* s) {
-   if (!s || s->kind != LDB_STATE_DICT) failP(LDB_ERR_INVALID, "not a string dictionary");
+   if (!s || s->kind != LDB_STATE_DICT) fail(LDB_ERR_INVALID, "not a string dictionary");
 }
 // the dictionary's counters {arena bytes, codes}, after its error word is checked (synchronises)
 static std::pair<int64_t, int64_t> checkDictError(LdbState* s) {
@@ -252,27 +210,28 @@ static std::pair<int64_t, int64_t> checkDictError(LdbState* s) {
    s->ctx->syncStream(s->ctx->compute);
    switch ((uint32_t) c[2]) {
       case 0: break;
-      case 1: failP(LDB_ERR_CAPACITY, "string dictionary full: more distinct strings than expected_strings allowed (recreate it larger)");
-      case 2: failP(LDB_ERR_CAPACITY, "string dictionary arena full: more string bytes than expected_bytes allowed (recreate it larger)");
-      case 3: failP(LDB_ERR_CAPACITY, "string dictionary: a code would pass INT32_MAX");
-      default: failP(LDB_ERR_CAPACITY, "string dictionary error word " + std::to_string((uint32_t) c[2]));
+      case 1: fail(LDB_ERR_CAPACITY, "string dictionary full: more distinct strings than expected_strings allowed (recreate it larger)");
+      case 2: fail(LDB_ERR_CAPACITY, "string dictionary arena full: more string bytes than expected_bytes allowed (recreate it larger)");
+      case 3: fail(LDB_ERR_CAPACITY, "string dictionary: a code would pass INT32_MAX");
+      default: fail(LDB_ERR_CAPACITY, "string dictionary error word " + std::to_string((uint32_t) c[2]));
    }
    return {(int64_t) c[0], (int64_t) c[1]};
 }
 
-// row ids of the single-batch table `t` (n rows, n < 2^32) ordered by the keys (column index, descending): device buffer of n
-// uint32 (released by the caller with stagingRelease).  The one place that knows the string order: ORDER BY and dictionary ranks.
-static uint32_t* sortRows(LdbTable* t, const std::vector<std::pair<int, int>>& keys, int64_t n) {
+// row ids of the single-batch table `t` (n rows, n < 2^32) ordered by the keys (column index, descending): a device buffer of n
+// uint32 in `scratch`, like the sort's temporaries, so the caller waits for the sort before its scope ends.  The one place that
+// knows the string order: ORDER BY and dictionary ranks.
+static uint32_t* sortRows(Scratch& scratch, LdbTable* t, const std::vector<std::pair<int, int>>& keys, int64_t n) {
    LdbContext* ctx = t->ctx;
    LdbBatch& b = t->batches[0];
    const size_t rows = (size_t) std::max<int64_t>(n, 1);
-   uint32_t* dv = (uint32_t*) ctx->stagingAlloc(rows * 4);
+   uint32_t* dv = scratch.alloc<uint32_t>(rows * 4);
    if (n == 0) return dv;
-   unsigned long long* dk = (unsigned long long*) ctx->stagingAlloc(rows * 8);
-   unsigned long long* dk2 = (unsigned long long*) ctx->stagingAlloc(rows * 8);
-   uint32_t* dv2 = (uint32_t*) ctx->stagingAlloc(rows * 4);
-   unsigned int* hist = (unsigned int*) ctx->stagingAlloc((size_t) ((n + 4095) / 4096) * 256 * 4);
-   int32_t* maxLen = (int32_t*) ctx->stagingAlloc(16);
+   unsigned long long* dk = scratch.alloc<unsigned long long>(rows * 8);
+   unsigned long long* dk2 = scratch.alloc<unsigned long long>(rows * 8);
+   uint32_t* dv2 = scratch.alloc<uint32_t>(rows * 4);
+   unsigned int* hist = scratch.alloc<unsigned int>((size_t) ((n + 4095) / 4096) * 256 * 4);
+   int32_t* maxLen = scratch.alloc<int32_t>(16);
    int first = 1;
    auto pass = [&](int c, int kind, int chunk, int desc) {
       ctx->launch("radix_sort", [&] {
@@ -294,16 +253,14 @@ static uint32_t* sortRows(LdbTable* t, const std::vector<std::pair<int, int>>& k
       ctx->syncStream(ctx->compute);
       for (int chunk = (longest + 7) / 8; chunk-- > 0;) pass(c, 2, chunk, desc);
    }
-   ctx->syncStream(ctx->compute);
-   for (void* p : {(void*) dk, (void*) dk2, (void*) dv2, (void*) hist, (void*) maxLen}) ctx->stagingRelease(p);
    return dv;
 }
 
 int ldb_gpu_dict_create(LdbContext* ctx, int64_t expected_strings, int64_t expected_bytes, LdbState** out, LdbError* err) {
-   return guardedP(err, [&] {
-      if (!ctx || !out) failP(LDB_ERR_INVALID, "null argument");
-      if (expected_strings < 0 || expected_bytes < 0) failP(LDB_ERR_INVALID, "negative dictionary size");
-      if (expected_strings > ((int64_t) 1 << 30)) failP(LDB_ERR_UNSUPPORTED, "a dictionary holds at most 2^30 expected strings (codes are int32)");
+   return guarded(err, [&] {
+      if (!ctx || !out) fail(LDB_ERR_INVALID, "null argument");
+      if (expected_strings < 0 || expected_bytes < 0) fail(LDB_ERR_INVALID, "negative dictionary size");
+      if (expected_strings > ((int64_t) 1 << 30)) fail(LDB_ERR_UNSUPPORTED, "a dictionary holds at most 2^30 expected strings (codes are int32)");
       LDB_CUDA(cudaSetDevice(ctx->device));
       auto* s = new LdbState;
       s->ctx = ctx;
@@ -315,7 +272,7 @@ int ldb_gpu_dict_create(LdbContext* ctx, int64_t expected_strings, int64_t expec
          return p;
       };
       DictDev& dd = s->dict;
-      const uint64_t cap = nextPow2P((uint64_t) std::max<int64_t>(expected_strings, 8) * 2);
+      const uint64_t cap = nextPow2((uint64_t) std::max<int64_t>(expected_strings, 8) * 2);
       dd.mask = cap - 1;
       dd.slots = (unsigned long long*) alloc(cap * 8);
       dd.entryOff = (int64_t*) alloc(cap * 8);
@@ -330,63 +287,53 @@ int ldb_gpu_dict_create(LdbContext* ctx, int64_t expected_strings, int64_t expec
    });
 }
 int ldb_gpu_dict_count(LdbState* s, int64_t* n_strings, LdbError* err) {
-   return guardedP(err, [&] {
+   return guarded(err, [&] {
       checkDict(s);
-      if (!n_strings) failP(LDB_ERR_INVALID, "null argument");
+      if (!n_strings) fail(LDB_ERR_INVALID, "null argument");
       LDB_CUDA(cudaSetDevice(s->ctx->device));
       *n_strings = checkDictError(s).second;
    });
 }
 int ldb_gpu_dict_to_table(LdbState* s, const char* name, LdbTable** out, LdbError* err) {
-   return guardedP(err, [&] {
+   return guarded(err, [&] {
       checkDict(s);
-      if (!out) failP(LDB_ERR_INVALID, "null argument");
+      if (!out) fail(LDB_ERR_INVALID, "null argument");
       LdbContext* ctx = s->ctx;
       LDB_CUDA(cudaSetDevice(ctx->device));
       const std::pair<int64_t, int64_t> used = checkDictError(s);
       const int64_t bytes = used.first, n = used.second;
-      if (bytes > (int64_t) INT32_MAX) failP(LDB_ERR_UNSUPPORTED, "dictionary strings exceed 2^31 - 1 bytes (utf8 offsets are int32)");
-      uint32_t* offsets = (uint32_t*) ctx->stagingAlloc((size_t) (n + 1) * 4);
-      uint8_t* data = (uint8_t*) ctx->stagingAlloc((size_t) std::max<int64_t>(bytes, 1));
-      int32_t* rank = (int32_t*) ctx->stagingAlloc((size_t) std::max<int64_t>(n, 1) * 4);
+      if (bytes > (int64_t) INT32_MAX) fail(LDB_ERR_UNSUPPORTED, "dictionary strings exceed 2^31 - 1 bytes (utf8 offsets are int32)");
+      Scratch cols(ctx), scratch(ctx);
+      uint32_t* offsets = cols.alloc<uint32_t>((size_t) (n + 1) * 4);
+      uint8_t* data = cols.alloc<uint8_t>((size_t) std::max<int64_t>(bytes, 1));
+      int32_t* rank = cols.alloc<int32_t>((size_t) std::max<int64_t>(n, 1) * 4);
       ctx->launch("dict_export", [&] { launchDictExport(s->dict, n, offsets, data, ctx->smCount, ctx->compute); });
-      auto* t = new LdbTable;
-      t->ctx = ctx;
-      t->name = name ? name : "dictionary";
-      t->columns.push_back({"str", LDB_UTF8, 0, 0});
-      t->columns.push_back({"rank", LDB_INT32, 0, 0});
       LdbBatch b;
       b.nRows = n;
       b.data = {offsets, rank};
       b.bytes = {data, nullptr};
       b.elemBytes = {4, 4};
-      b.validity.assign(2, nullptr);
-      b.validityBitOffset.assign(2, 0);
-      b.owned = {offsets, data, rank};
-      t->numRows = n;
-      t->batches.push_back(std::move(b));
-      ctx->tables.push_back(t);
-      uint32_t* ids = sortRows(t, {{0, 0}}, n);
+      LdbTable* t = addResultTable(ctx, name ? name : "dictionary", {{"str", LDB_UTF8, 0, 0}, {"rank", LDB_INT32, 0, 0}}, std::move(b), cols);
+      uint32_t* ids = sortRows(scratch, t, {{0, 0}}, n);
       if (n) ctx->launch("dict_rank", [&] { launchScatterRanks(ids, n, rank, ctx->smCount, ctx->compute); });
       ctx->syncStream(ctx->compute);
-      ctx->stagingRelease(ids);
       *out = t;
    });
 }
 
 // ---------------------------------------------------------------- key-tuple join tables
 int ldb_gpu_join_table_create_keys(LdbContext* ctx, int32_t n_keys, int64_t expected_rows, int32_t flags, LdbState** out, LdbError* err) {
-   return guardedP(err, [&] {
+   return guarded(err, [&] {
       int devices = 0;
       if (cudaGetDeviceCount(&devices) != cudaSuccess || devices == 0) {
          cudaGetLastError();
-         failP(LDB_ERR_NO_DEVICE, "no CUDA device available: the GPU operator runtime has no CPU fallback");
+         fail(LDB_ERR_NO_DEVICE, "no CUDA device available: the GPU operator runtime has no CPU fallback");
       }
-      if (!ctx || !out) failP(LDB_ERR_INVALID, "null argument");
-      if (n_keys < 1 || n_keys > kProgMaxKeys) failP(LDB_ERR_INVALID, "a key-tuple join table takes 1..4 keys");
-      if (expected_rows < 0) failP(LDB_ERR_INVALID, "negative expected_rows");
-      if (expected_rows > ((int64_t) 1 << 36)) failP(LDB_ERR_UNSUPPORTED, "a key-tuple join table holds at most 2^36 expected rows");
-      if (ctx->capturing) failP(LDB_ERR_UNSUPPORTED, "key-tuple join tables are not part of captured queries");
+      if (!ctx || !out) fail(LDB_ERR_INVALID, "null argument");
+      if (n_keys < 1 || n_keys > kProgMaxKeys) fail(LDB_ERR_INVALID, "a key-tuple join table takes 1..4 keys");
+      if (expected_rows < 0) fail(LDB_ERR_INVALID, "negative expected_rows");
+      if (expected_rows > ((int64_t) 1 << 36)) fail(LDB_ERR_UNSUPPORTED, "a key-tuple join table holds at most 2^36 expected rows");
+      if (ctx->capturing) fail(LDB_ERR_UNSUPPORTED, "key-tuple join tables are not part of captured queries");
       LDB_CUDA(cudaSetDevice(ctx->device));
       auto* s = new LdbState;
       s->ctx = ctx;
@@ -399,7 +346,7 @@ int ldb_gpu_join_table_create_keys(LdbContext* ctx, int32_t n_keys, int64_t expe
          return p;
       };
       KeyJoinDev& k = s->keyJoin;
-      const uint64_t cap = nextPow2P((uint64_t) std::max<int64_t>(expected_rows, 8) * 2); // load <= 0.5, like the other join tables
+      const uint64_t cap = nextPow2((uint64_t) std::max<int64_t>(expected_rows, 8) * 2); // load <= 0.5, like the other join tables
       k.mask = cap - 1;
       k.nKeys = n_keys;
       k.entryBytes = n_keys <= 2 ? 32 : 48; // {word, payload, keys} padded: one 32-byte sector for 1-2 keys
@@ -423,13 +370,12 @@ void ldb_gpu_check_keyjoin_error_internal(LdbState* s) {
    s->ctx->syncStream(s->ctx->compute);
    switch (e) {
       case 0: return;
-      case 1: failP(LDB_ERR_CAPACITY, "key-tuple join table full: more build rows than expected_rows allowed, or more than 65536 entries in one probe run (too many duplicates of one key tuple)");
-      case 6: failP(LDB_ERR_CAPACITY, "a probe run of a key-tuple join table is longer than the interpreter's bound of 16384 slots (too many entries share one run)");
-      case 7: failP(LDB_ERR_UNSUPPORTED, "a program join build met a key or payload outside int64 (key-tuple join tables store int64 keys and payloads)");
-      default: failP(LDB_ERR_INVALID, "key-tuple join table error word " + std::to_string(e));
+      case 1: fail(LDB_ERR_CAPACITY, "key-tuple join table full: more build rows than expected_rows allowed, or more than 65536 entries in one probe run (too many duplicates of one key tuple)");
+      case 6: fail(LDB_ERR_CAPACITY, "a probe run of a key-tuple join table is longer than the interpreter's bound of 16384 slots (too many entries share one run)");
+      case 7: fail(LDB_ERR_UNSUPPORTED, "a program join build met a key or payload outside int64 (key-tuple join tables store int64 keys and payloads)");
+      default: fail(LDB_ERR_INVALID, "key-tuple join table error word " + std::to_string(e));
    }
 }
-extern "C" {
 
 // the pointers of column `ci` of batch `b` (validity bitmap or validity bytes included)
 static void bindColumn(ProgCol& pc, const LdbBatch& b, int ci) {
@@ -441,126 +387,153 @@ static void bindColumn(ProgCol& pc, const LdbBatch& b, int ci) {
    pc.validBytes = ci < (int) b.validBytes.size() ? b.validBytes[ci] : nullptr;
 }
 
-static void runProgram(LdbContext* ctx, const LdbProgramDesc* d, const LdbProgramJoins* j) {
-   if (!ctx || !d || !d->source) failP(LDB_ERR_INVALID, "null argument");
-   LdbTable* t = d->source;
-   if (t->ctx != ctx) failP(LDB_ERR_INVALID, "table belongs to another context");
+// One run of a program over the batches of its source, filled step by step by runProgram: the kernel parameters every batch
+// shares, where each column comes from, and the states whose error words are read after the launches.
+struct ProgramPlan {
+   LdbContext* ctx;
+   const LdbProgramDesc* d;
+   LdbTable* t; // the source
+   int nCols = 0;
+   ProgramParams base{};
+   std::vector<int> colIdx, rowReg;  // per column: its index in its table; the row register of a side column (-1: a source column)
+   std::vector<LdbTable*> colTable;
+   bool written[kProgMaxRegs] = {}; // registers some instruction writes
+   bool usesRowid = false;
+   int eachTable = -1; // tables[] index PROBE_EACH reads
+   bool probed[kProgMaxTables] = {}, coded[kProgMaxTables] = {}; // tables[k] read by PROBE / PROBE_EACH, by STRCODE
+   std::vector<LdbState*> dicts, tupleTables; // tupleTables: key-tuple tables whose error word the run may set
+
+   ProgramPlan(LdbContext* c, const LdbProgramDesc* desc) : ctx(c), d(desc), t(desc->source) {}
+   int colType(int c) const { return colTable[c]->columns[colIdx[c]].type; }
+   void wantReg(int r, const char* what) const {
+      if (r < 0 || r >= kProgMaxRegs || !written[r]) fail(LDB_ERR_INVALID, std::string("program reads an unwritten or out-of-range register (") + what + ")");
+   }
+   void wantTupleTable(LdbState* js) const {
+      if (js->ctx != ctx) fail(LDB_ERR_INVALID, "key-tuple join table belongs to another context");
+      if (ctx->capturing) fail(LDB_ERR_UNSUPPORTED, "key-tuple join tables are not part of captured queries");
+   }
+};
+
+// the source's and the side tables' columns by name, and the interpreter's limits
+static void resolveColumns(ProgramPlan& p, const LdbProgramJoins* j) {
+   LdbContext* ctx = p.ctx;
+   const LdbProgramDesc* d = p.d;
+   if (p.t->ctx != ctx) fail(LDB_ERR_INVALID, "table belongs to another context");
    if (j && (j->n_side_tables < 0 || j->n_side_columns < 0 || (j->n_side_tables > 0 && !j->side_tables) || (j->n_side_columns > 0 && !j->side_columns)))
-      failP(LDB_ERR_INVALID, "malformed side-table list");
+      fail(LDB_ERR_INVALID, "malformed side-table list");
    const int nSide = j ? j->n_side_columns : 0;
    if (d->n_columns < 0 || d->n_columns + nSide > kProgMaxCols || d->n_instr < 0 || d->n_instr > kProgMaxInstr || d->n_consts < 0 || d->n_consts > kProgMaxConsts ||
        d->n_strings < 0 || d->n_strings > kProgMaxStrings || d->n_tables < 0 || d->n_tables > kProgMaxTables)
-      failP(LDB_ERR_UNSUPPORTED, "program exceeds the interpreter's limits (12 source + side columns, 96 instructions, 24 constants, 12 strings, 4 tables)");
+      fail(LDB_ERR_UNSUPPORTED, "program exceeds the interpreter's limits (12 source + side columns, 96 instructions, 24 constants, 12 strings, 4 tables)");
    LDB_CUDA(cudaSetDevice(ctx->device));
-   const int nCols = d->n_columns + nSide;
-   ProgramParams base{};
-   base.nCols = nCols;
-   base.nInstr = d->n_instr;
-   base.nTables = d->n_tables;
-   base.eachPc = -1;
-   std::vector<int> colIdx((size_t) nCols), rowReg((size_t) nCols, -1);
-   std::vector<LdbTable*> colTable((size_t) nCols, t);
+   p.nCols = d->n_columns + nSide;
+   p.base.nCols = p.nCols;
+   p.base.nInstr = d->n_instr;
+   p.base.nTables = d->n_tables;
+   p.base.eachPc = -1;
+   p.colIdx.assign((size_t) p.nCols, 0);
+   p.rowReg.assign((size_t) p.nCols, -1);
+   p.colTable.assign((size_t) p.nCols, p.t);
    for (int c = 0; c < d->n_columns; c++) {
-      colIdx[c] = t->colIndex(d->columns[c]);
-      if (colIdx[c] < 0) failP(LDB_ERR_INVALID, std::string("unknown column ") + (d->columns[c] ? d->columns[c] : "(null)"));
+      p.colIdx[c] = p.t->colIndex(d->columns[c]);
+      if (p.colIdx[c] < 0) fail(LDB_ERR_INVALID, std::string("unknown column ") + (d->columns[c] ? d->columns[c] : "(null)"));
    }
    for (int k = 0; k < nSide; k++) {
       const LdbSideColumn& sc = j->side_columns[k];
       const int c = d->n_columns + k;
-      if (sc.table < 0 || sc.table >= j->n_side_tables || !j->side_tables[sc.table]) failP(LDB_ERR_INVALID, "side column: side table index out of range");
+      if (sc.table < 0 || sc.table >= j->n_side_tables || !j->side_tables[sc.table]) fail(LDB_ERR_INVALID, "side column: side table index out of range");
       LdbTable* st = j->side_tables[sc.table];
-      if (st->ctx != ctx) failP(LDB_ERR_INVALID, "side table belongs to another context");
-      colIdx[c] = st->colIndex(sc.column);
-      if (colIdx[c] < 0) failP(LDB_ERR_INVALID, std::string("unknown side column ") + (sc.column ? sc.column : "(null)"));
-      if (sc.row_reg < 0 || sc.row_reg >= kProgMaxRegs) failP(LDB_ERR_INVALID, "side column: row register out of range");
-      colTable[c] = st;
-      rowReg[c] = sc.row_reg;
+      if (st->ctx != ctx) fail(LDB_ERR_INVALID, "side table belongs to another context");
+      p.colIdx[c] = st->colIndex(sc.column);
+      if (p.colIdx[c] < 0) fail(LDB_ERR_INVALID, std::string("unknown side column ") + (sc.column ? sc.column : "(null)"));
+      if (sc.row_reg < 0 || sc.row_reg >= kProgMaxRegs) fail(LDB_ERR_INVALID, "side column: row register out of range");
+      p.colTable[c] = st;
+      p.rowReg[c] = sc.row_reg;
    }
-   auto colType = [&](int c) { return colTable[c]->columns[colIdx[c]].type; };
-   // static validation: every register read was written before, every index is in range, types fit the opcode
-   bool written[kProgMaxRegs] = {}, beforeEach[kProgMaxRegs] = {};
-   auto wantReg = [&](int r, const char* what) {
-      if (r < 0 || r >= kProgMaxRegs || !written[r]) failP(LDB_ERR_INVALID, std::string("program reads an unwritten or out-of-range register (") + what + ")");
-   };
+}
+
+// static validation: every register read was written before, every index is in range, types fit the opcode; copies the
+// instructions, constants and string constants into the kernel parameters
+static void validateInstructions(ProgramPlan& p) {
+   const LdbProgramDesc* d = p.d;
+   ProgramParams& base = p.base;
+   bool beforeEach[kProgMaxRegs] = {};
    auto wantCol = [&](int c, const char* what) {
-      if (c < 0 || c >= nCols) failP(LDB_ERR_INVALID, std::string(what) + ": column index out of range");
-      if (rowReg[c] >= 0) wantReg(rowReg[c], "row register of a side column");
+      if (c < 0 || c >= p.nCols) fail(LDB_ERR_INVALID, std::string(what) + ": column index out of range");
+      if (p.rowReg[c] >= 0) p.wantReg(p.rowReg[c], "row register of a side column");
    };
-   bool usesRowid = false;
-   int eachTable = -1;
-   bool probed[kProgMaxTables] = {}, coded[kProgMaxTables] = {}; // tables[k] read by PROBE / PROBE_EACH, by STRCODE
-   if (d->n_tables > 0 && !d->tables) failP(LDB_ERR_INVALID, "null tables list");
+   if (d->n_tables > 0 && !d->tables) fail(LDB_ERR_INVALID, "null tables list");
    int tupleKeys[kProgMaxTables] = {}; // tables[k] is a key-tuple join table of this many keys: PROBE reads registers a .. a + n - 1
    for (int k = 0; k < d->n_tables; k++)
       if (d->tables[k] && d->tables[k]->kind == LDB_STATE_KEY_JOIN) tupleKeys[k] = d->tables[k]->keyJoin.nKeys;
    auto wantKeys = [&](const LdbInstr& in) {
-      for (int k = 0; k < std::max(tupleKeys[in.arg], 1); k++) wantReg(in.a + k, "key");
+      for (int k = 0; k < std::max(tupleKeys[in.arg], 1); k++) p.wantReg(in.a + k, "key");
    };
    for (int i = 0; i < d->n_instr; i++) {
       const LdbInstr& in = d->instr[i];
-      if (in.dst >= kProgMaxRegs) failP(LDB_ERR_INVALID, "destination register out of range");
+      if (in.dst >= kProgMaxRegs) fail(LDB_ERR_INVALID, "destination register out of range");
       switch (in.op) {
          case LDB_OP_LOAD:
             wantCol(in.arg, "LOAD");
-            if (colType(in.arg) == LDB_UTF8) failP(LDB_ERR_UNSUPPORTED, "LOAD of a string column (strings are operands of STRCMP / STRLIKE / STRKEY8 / STRCODE only)");
+            if (p.colType(in.arg) == LDB_UTF8) fail(LDB_ERR_UNSUPPORTED, "LOAD of a string column (strings are operands of STRCMP / STRLIKE / STRKEY8 / STRCODE only)");
             break;
          case LDB_OP_STRCODE:
-            if (in.a >= nCols || colType(in.a) != LDB_UTF8) failP(LDB_ERR_INVALID, "STRCODE needs a utf8 column");
+            if (in.a >= p.nCols || p.colType(in.a) != LDB_UTF8) fail(LDB_ERR_INVALID, "STRCODE needs a utf8 column");
             wantCol(in.a, "STRCODE");
-            if (in.arg < 0 || in.arg >= d->n_tables) failP(LDB_ERR_INVALID, "STRCODE: dictionary index out of range");
-            if (in.b > 1) failP(LDB_ERR_INVALID, "STRCODE: b is 1 (insert) or 0 (lookup only)");
-            coded[in.arg] = true;
+            if (in.arg < 0 || in.arg >= d->n_tables) fail(LDB_ERR_INVALID, "STRCODE: dictionary index out of range");
+            if (in.b > 1) fail(LDB_ERR_INVALID, "STRCODE: b is 1 (insert) or 0 (lookup only)");
+            p.coded[in.arg] = true;
             break;
          case LDB_OP_CONST:
-            if (in.arg < 0 || in.arg >= d->n_consts) failP(LDB_ERR_INVALID, "CONST: constant index out of range");
+            if (in.arg < 0 || in.arg >= d->n_consts) fail(LDB_ERR_INVALID, "CONST: constant index out of range");
             break;
          case LDB_OP_ADD: case LDB_OP_SUB: case LDB_OP_MUL: case LDB_OP_DIV: case LDB_OP_AND: case LDB_OP_OR:
          case LDB_OP_FADD: case LDB_OP_FSUB: case LDB_OP_FMUL: case LDB_OP_FDIV:
-            wantReg(in.a, "a");
-            wantReg(in.b, "b");
+            p.wantReg(in.a, "a");
+            p.wantReg(in.b, "b");
             break;
          case LDB_OP_CMP: case LDB_OP_FCMP:
-            wantReg(in.a, "a");
-            wantReg(in.b, "b");
-            if (in.arg < LDB_EQ || in.arg > LDB_GTE) failP(LDB_ERR_INVALID, "CMP: unknown comparison");
+            p.wantReg(in.a, "a");
+            p.wantReg(in.b, "b");
+            if (in.arg < LDB_EQ || in.arg > LDB_GTE) fail(LDB_ERR_INVALID, "CMP: unknown comparison");
             break;
-         case LDB_OP_NEG: case LDB_OP_NOT: case LDB_OP_ISNULL: case LDB_OP_I2F: case LDB_OP_YEAR: wantReg(in.a, "a"); break;
+         case LDB_OP_NEG: case LDB_OP_NOT: case LDB_OP_ISNULL: case LDB_OP_I2F: case LDB_OP_YEAR: p.wantReg(in.a, "a"); break;
          case LDB_OP_SELECT:
-            wantReg(in.a, "a");
-            wantReg(in.b, "b");
-            wantReg(in.arg, "condition");
+            p.wantReg(in.a, "a");
+            p.wantReg(in.b, "b");
+            p.wantReg(in.arg, "condition");
             break;
          case LDB_OP_STRKEY8:
-            if (in.a >= nCols || colType(in.a) != LDB_UTF8) failP(LDB_ERR_INVALID, "STRKEY8 needs a utf8 column");
+            if (in.a >= p.nCols || p.colType(in.a) != LDB_UTF8) fail(LDB_ERR_INVALID, "STRKEY8 needs a utf8 column");
             wantCol(in.a, "STRKEY8");
             break;
          case LDB_OP_STRCMP: case LDB_OP_STRLIKE:
-            if (in.a >= nCols || colType(in.a) != LDB_UTF8) failP(LDB_ERR_INVALID, "string op needs a utf8 column");
+            if (in.a >= p.nCols || p.colType(in.a) != LDB_UTF8) fail(LDB_ERR_INVALID, "string op needs a utf8 column");
             wantCol(in.a, "string op");
-            if (in.arg < 0 || in.arg >= d->n_strings) failP(LDB_ERR_INVALID, "string constant index out of range");
-            if (in.op == LDB_OP_STRCMP ? in.b > LDB_GTE : in.b > 2) failP(LDB_ERR_INVALID, "string op: unknown comparison / pattern kind");
+            if (in.arg < 0 || in.arg >= d->n_strings) fail(LDB_ERR_INVALID, "string constant index out of range");
+            if (in.op == LDB_OP_STRCMP ? in.b > LDB_GTE : in.b > 2) fail(LDB_ERR_INVALID, "string op: unknown comparison / pattern kind");
             break;
          case LDB_OP_PROBE:
-            if (in.arg < 0 || in.arg >= d->n_tables) failP(LDB_ERR_INVALID, "PROBE: table index out of range");
+            if (in.arg < 0 || in.arg >= d->n_tables) fail(LDB_ERR_INVALID, "PROBE: table index out of range");
             wantKeys(in);
-            probed[in.arg] = true;
+            p.probed[in.arg] = true;
             break;
-         case LDB_OP_ROWID: usesRowid = true; break;
+         case LDB_OP_ROWID: p.usesRowid = true; break;
          case LDB_OP_PROBE_EACH:
-            if (in.arg < 0 || in.arg >= d->n_tables) failP(LDB_ERR_INVALID, "PROBE_EACH: table index out of range");
+            if (in.arg < 0 || in.arg >= d->n_tables) fail(LDB_ERR_INVALID, "PROBE_EACH: table index out of range");
             wantKeys(in);
-            if (in.b > 1) failP(LDB_ERR_INVALID, "PROBE_EACH: b is 0 (inner) or 1 (left outer)");
-            if (base.eachPc >= 0) failP(LDB_ERR_UNSUPPORTED, "at most one PROBE_EACH per program");
+            if (in.b > 1) fail(LDB_ERR_INVALID, "PROBE_EACH: b is 0 (inner) or 1 (left outer)");
+            if (base.eachPc >= 0) fail(LDB_ERR_UNSUPPORTED, "at most one PROBE_EACH per program");
             base.eachPc = i;
-            eachTable = in.arg;
-            probed[in.arg] = true;
+            p.eachTable = in.arg;
+            p.probed[in.arg] = true;
             break;
-         default: failP(LDB_ERR_UNSUPPORTED, "unknown opcode " + std::to_string(in.op));
+         default: fail(LDB_ERR_UNSUPPORTED, "unknown opcode " + std::to_string(in.op));
       }
       // the instructions after PROBE_EACH run once per match: they may not overwrite what the first pass left for the next one
-      if (base.eachPc >= 0 && i > base.eachPc && beforeEach[in.dst]) failP(LDB_ERR_INVALID, "an instruction after PROBE_EACH overwrites a register written at or before it");
-      written[in.dst] = true;
-      if (base.eachPc == i) std::copy(written, written + kProgMaxRegs, beforeEach);
+      if (base.eachPc >= 0 && i > base.eachPc && beforeEach[in.dst]) fail(LDB_ERR_INVALID, "an instruction after PROBE_EACH overwrites a register written at or before it");
+      p.written[in.dst] = true;
+      if (base.eachPc == i) std::copy(p.written, p.written + kProgMaxRegs, beforeEach);
       base.instr[i] = ProgInstr{in.op, in.dst, in.a, in.b, in.arg};
    }
    for (int c = 0; c < d->n_consts; c++) {
@@ -569,122 +542,122 @@ static void runProgram(LdbContext* ctx, const LdbProgramDesc* d, const LdbProgra
    }
    for (int c = 0; c < d->n_strings; c++) {
       const size_t n = d->strings[c] ? strlen(d->strings[c]) : 0;
-      if (n > (size_t) kProgStringBytes) failP(LDB_ERR_UNSUPPORTED, "string constant longer than 32 bytes");
+      if (n > (size_t) kProgStringBytes) fail(LDB_ERR_UNSUPPORTED, "string constant longer than 32 bytes");
       memcpy(base.strings[c], d->strings[c], n);
       base.stringLen[c] = (int32_t) n;
    }
-   std::vector<LdbState*> dicts, tupleTables; // tupleTables: key-tuple tables whose error word the run may set
-   auto wantTupleTable = [&](LdbState* js) {
-      if (js->ctx != ctx) failP(LDB_ERR_INVALID, "key-tuple join table belongs to another context");
-      if (ctx->capturing) failP(LDB_ERR_UNSUPPORTED, "key-tuple join tables are not part of captured queries");
-   };
+}
+
+// the table slots: plain join tables, key-tuple join tables and string dictionaries
+static void bindTables(ProgramPlan& p) {
+   LdbContext* ctx = p.ctx;
+   const LdbProgramDesc* d = p.d;
    for (int k = 0; k < d->n_tables; k++) {
       LdbState* js = d->tables[k];
       if (js && js->kind == LDB_STATE_KEY_JOIN) {
-         if (coded[k]) failP(LDB_ERR_INVALID, "STRCODE needs a string dictionary, not a join table");
-         wantTupleTable(js);
-         if (d->sink_kind == LDB_SINK_JOIN_BUILD && d->sink == js) failP(LDB_ERR_INVALID, "a program may not build a key-tuple join table and probe it");
-         base.keyTables[k] = js->keyJoin;
-         if (probed[k]) tupleTables.push_back(js);
+         if (p.coded[k]) fail(LDB_ERR_INVALID, "STRCODE needs a string dictionary, not a join table");
+         p.wantTupleTable(js);
+         if (d->sink_kind == LDB_SINK_JOIN_BUILD && d->sink == js) fail(LDB_ERR_INVALID, "a program may not build a key-tuple join table and probe it");
+         p.base.keyTables[k] = js->keyJoin;
+         if (p.probed[k]) p.tupleTables.push_back(js);
          continue;
       }
       if (js && js->kind == LDB_STATE_DICT) {
-         if (probed[k]) failP(LDB_ERR_INVALID, "PROBE / PROBE_EACH on a string dictionary (they take join tables)");
-         if (js->ctx != ctx) failP(LDB_ERR_INVALID, "string dictionary belongs to another context");
-         if (ctx->capturing) failP(LDB_ERR_UNSUPPORTED, "string dictionaries are not part of captured queries");
-         base.dicts[k] = js->dict;
-         dicts.push_back(js);
+         if (p.probed[k]) fail(LDB_ERR_INVALID, "PROBE / PROBE_EACH on a string dictionary (they take join tables)");
+         if (js->ctx != ctx) fail(LDB_ERR_INVALID, "string dictionary belongs to another context");
+         if (ctx->capturing) fail(LDB_ERR_UNSUPPORTED, "string dictionaries are not part of captured queries");
+         p.base.dicts[k] = js->dict;
+         p.dicts.push_back(js);
          continue;
       }
-      if (coded[k]) failP(LDB_ERR_INVALID, "STRCODE needs a string dictionary, not a join table");
-      if (k == eachTable && js && js->kind == LDB_STATE_JOIN_TABLE && !(js->join.stride == 8 || js->join.direct))
-         failP(LDB_ERR_UNSUPPORTED, "PROBE_EACH takes a plain single-key or direct-address join table (not a pair table or a group-join map)");
-      if (!js || js->kind != LDB_STATE_JOIN_TABLE || js->join.stride == 16) failP(LDB_ERR_INVALID, "PROBE tables are single-key join tables");
-      base.tables[k] = js->join;
+      if (p.coded[k]) fail(LDB_ERR_INVALID, "STRCODE needs a string dictionary, not a join table");
+      if (k == p.eachTable && js && js->kind == LDB_STATE_JOIN_TABLE && !(js->join.stride == 8 || js->join.direct))
+         fail(LDB_ERR_UNSUPPORTED, "PROBE_EACH takes a plain single-key or direct-address join table (not a pair table or a group-join map)");
+      if (!js || js->kind != LDB_STATE_JOIN_TABLE || js->join.stride == 16) fail(LDB_ERR_INVALID, "PROBE tables are single-key join tables");
+      p.base.tables[k] = js->join;
    }
+}
+
+// materialize output buffers for `rows` rows (+ the row counter) in `out`, replacing the ones it holds
+static void allocOut(ProgramPlan& p, Scratch& out, size_t rows) {
+   for (void* q : out.take()) p.ctx->stagingRelease(q);
+   for (int c = 0; c < p.d->n_out; c++) {
+      p.base.outValues[c] = out.alloc<uint8_t>(rows * 16);
+      p.base.outValid[c] = out.alloc<uint8_t>(rows);
+   }
+   p.base.outCount = out.alloc<unsigned long long>(8);
+   LDB_CUDA(cudaMemsetAsync(p.base.outCount, 0, 8, p.ctx->compute));
+   p.base.outCapacity = (int64_t) rows;
+}
+
+// the filter and the sink: a hash aggregation, a join build (plain or key-tuple table) or materialized rows (buffers in `out`)
+static void bindSink(ProgramPlan& p, Scratch& out) {
+   const LdbProgramDesc* d = p.d;
+   ProgramParams& base = p.base;
    base.filterReg = d->filter_reg;
-   if (d->filter_reg >= 0) wantReg(d->filter_reg, "filter");
+   if (d->filter_reg >= 0) p.wantReg(d->filter_reg, "filter");
    base.sinkKind = d->sink_kind;
    LdbState* sink = d->sink;
-   std::vector<void*> outOwned;
-   std::vector<uint8_t*> outVals, outValid;
-   unsigned long long* outCount = nullptr;
-   // materialize output buffers for `rows` rows (+ the row counter)
-   auto allocOut = [&](size_t rows) {
-      for (void* q : outOwned) ctx->stagingRelease(q);
-      outOwned.clear();
-      outVals.clear();
-      outValid.clear();
-      for (int c = 0; c < d->n_out; c++) {
-         outVals.push_back((uint8_t*) ctx->stagingAlloc(rows * 16));
-         outValid.push_back((uint8_t*) ctx->stagingAlloc(rows));
-         outOwned.push_back(outVals.back());
-         outOwned.push_back(outValid.back());
-         base.outValues[c] = outVals.back();
-         base.outValid[c] = outValid.back();
-      }
-      outCount = (unsigned long long*) ctx->stagingAlloc(8);
-      outOwned.push_back(outCount);
-      LDB_CUDA(cudaMemsetAsync(outCount, 0, 8, ctx->compute));
-      base.outCapacity = (int64_t) rows;
-      base.outCount = outCount;
-   };
    if (d->sink_kind == LDB_SINK_HASHAGG) {
       checkHashAgg(sink);
-      if (sink->ctx != ctx || d->n_keys != sink->hashagg.nKeys || d->n_aggs != sink->hashagg.nAggs) failP(LDB_ERR_INVALID, "key / aggregate count differs from the state's");
+      if (sink->ctx != p.ctx || d->n_keys != sink->hashagg.nKeys || d->n_aggs != sink->hashagg.nAggs) fail(LDB_ERR_INVALID, "key / aggregate count differs from the state's");
       base.nKeys = d->n_keys;
       base.nAggs = d->n_aggs;
       for (int k = 0; k < d->n_keys; k++) {
-         wantReg(d->key_regs[k], "group key");
+         p.wantReg(d->key_regs[k], "group key");
          base.keyReg[k] = d->key_regs[k];
       }
       for (int a = 0; a < d->n_aggs; a++) {
-         if (d->aggs[a].kind != sink->aggKinds[a]) failP(LDB_ERR_INVALID, "aggregate kind differs from the state's");
-         if (d->aggs[a].kind != LDB_AGG_COUNT_STAR) wantReg(d->aggs[a].reg, "aggregate input");
+         if (d->aggs[a].kind != sink->aggKinds[a]) fail(LDB_ERR_INVALID, "aggregate kind differs from the state's");
+         if (d->aggs[a].kind != LDB_AGG_COUNT_STAR) p.wantReg(d->aggs[a].reg, "aggregate input");
          base.aggs[a] = ProgAgg{d->aggs[a].kind, d->aggs[a].reg};
       }
       base.agg = sink->hashagg;
    } else if (d->sink_kind == LDB_SINK_JOIN_BUILD && sink && sink->kind == LDB_STATE_KEY_JOIN) {
       // keys from n_keys / key_regs[]; payloads are int64, so ROWID has no row limit here
-      wantTupleTable(sink);
-      if (d->n_keys != sink->keyJoin.nKeys) failP(LDB_ERR_INVALID, "n_keys differs from the key-tuple join table's key count");
-      if (d->build_key_reg != -1) failP(LDB_ERR_INVALID, "a build into a key-tuple join table takes its keys from key_regs (build_key_reg must be -1)");
+      p.wantTupleTable(sink);
+      if (d->n_keys != sink->keyJoin.nKeys) fail(LDB_ERR_INVALID, "n_keys differs from the key-tuple join table's key count");
+      if (d->build_key_reg != -1) fail(LDB_ERR_INVALID, "a build into a key-tuple join table takes its keys from key_regs (build_key_reg must be -1)");
       base.nKeys = d->n_keys;
       for (int k = 0; k < d->n_keys; k++) {
-         wantReg(d->key_regs[k], "build key");
+         p.wantReg(d->key_regs[k], "build key");
          base.keyReg[k] = d->key_regs[k];
       }
-      if (d->build_payload_reg >= 0) wantReg(d->build_payload_reg, "build payload");
+      if (d->build_payload_reg >= 0) p.wantReg(d->build_payload_reg, "build payload");
       base.buildKeyReg = -1;
       base.buildPayloadReg = d->build_payload_reg;
       base.keyBuild = sink->keyJoin;
-      tupleTables.push_back(sink);
+      p.tupleTables.push_back(sink);
    } else if (d->sink_kind == LDB_SINK_JOIN_BUILD) {
-      if (!sink || sink->kind != LDB_STATE_JOIN_TABLE || sink->join.stride != 8 || sink->join.direct) failP(LDB_ERR_INVALID, "build sink must be a plain single-key join table");
-      if (usesRowid && t->numRows > (int64_t) INT32_MAX) failP(LDB_ERR_UNSUPPORTED, "ROWID build payloads are int32: the source has 2^31 rows or more");
-      wantReg(d->build_key_reg, "build key");
-      if (d->build_payload_reg >= 0) wantReg(d->build_payload_reg, "build payload");
+      if (!sink || sink->kind != LDB_STATE_JOIN_TABLE || sink->join.stride != 8 || sink->join.direct) fail(LDB_ERR_INVALID, "build sink must be a plain single-key join table");
+      if (p.usesRowid && p.t->numRows > (int64_t) INT32_MAX) fail(LDB_ERR_UNSUPPORTED, "ROWID build payloads are int32: the source has 2^31 rows or more");
+      p.wantReg(d->build_key_reg, "build key");
+      if (d->build_payload_reg >= 0) p.wantReg(d->build_payload_reg, "build payload");
       base.buildKeyReg = d->build_key_reg;
       base.buildPayloadReg = d->build_payload_reg;
       base.build = sink->join;
    } else if (d->sink_kind == LDB_SINK_MATERIALIZE) {
-      if (d->n_out < 1 || d->n_out > kProgMaxAggs || !d->out_table) failP(LDB_ERR_INVALID, "materialize needs 1..8 output registers and out_table");
+      if (d->n_out < 1 || d->n_out > kProgMaxAggs || !d->out_table) fail(LDB_ERR_INVALID, "materialize needs 1..8 output registers and out_table");
       base.nOut = d->n_out;
       for (int c = 0; c < d->n_out; c++) {
-         wantReg(d->out_regs[c], "output");
+         p.wantReg(d->out_regs[c], "output");
          base.outReg[c] = d->out_regs[c];
       }
-      allocOut((size_t) std::max<int64_t>(t->numRows, 1));
+      allocOut(p, out, (size_t) std::max<int64_t>(p.t->numRows, 1));
    } else {
-      failP(LDB_ERR_INVALID, "unknown sink kind");
+      fail(LDB_ERR_INVALID, "unknown sink kind");
    }
-   // side columns: bound once for all batches of the source; a multi-batch side table through a device-resident batch directory
-   std::vector<void*> dirs;
-   for (int c = d->n_columns; c < nCols; c++) {
-      LdbTable* st = colTable[c];
-      ProgCol& pc = base.cols[c];
-      pc.type = colType(c);
-      pc.rowReg = rowReg[c];
+}
+
+// side columns: bound once for all batches of the source; a multi-batch side table through a device-resident batch directory
+// (in `dirs`)
+static void bindSideColumns(ProgramPlan& p, Scratch& dirs) {
+   LdbContext* ctx = p.ctx;
+   for (int c = p.d->n_columns; c < p.nCols; c++) {
+      LdbTable* st = p.colTable[c];
+      ProgCol& pc = p.base.cols[c];
+      pc.type = p.colType(c);
+      pc.rowReg = p.rowReg[c];
       std::vector<ProgSideBatch> dir;
       int64_t first = 0;
       const LdbBatch* only = nullptr;
@@ -692,7 +665,7 @@ static void runProgram(LdbContext* ctx, const LdbProgramDesc* d, const LdbProgra
          ldb_gpu_wait_batch_internal(ctx, &b);
          if (b.nRows > 0) {
             ProgCol one{};
-            bindColumn(one, b, colIdx[c]);
+            bindColumn(one, b, p.colIdx[c]);
             dir.push_back(ProgSideBatch{one.data, one.bytes, one.validity, one.validBytes, one.bitOffset, first, one.elemBytes, 0});
             only = &b;
          }
@@ -701,143 +674,142 @@ static void runProgram(LdbContext* ctx, const LdbProgramDesc* d, const LdbProgra
       pc.sideRows = first;
       pc.nBatches = (int32_t) dir.size();
       if (dir.size() == 1) {
-         bindColumn(pc, *only, colIdx[c]);
+         bindColumn(pc, *only, p.colIdx[c]);
       } else if (dir.size() > 1) {
-         void* dd = ctx->stagingAlloc(dir.size() * sizeof(ProgSideBatch));
-         dirs.push_back(dd);
+         ProgSideBatch* dd = dirs.alloc<ProgSideBatch>(dir.size() * sizeof(ProgSideBatch));
          LDB_CUDA(cudaMemcpyAsync(dd, dir.data(), dir.size() * sizeof(ProgSideBatch), cudaMemcpyHostToDevice, ctx->compute));
-         pc.dir = (const ProgSideBatch*) dd;
+         pc.dir = dd;
       }
    }
-   for (int c = 0; c < d->n_columns; c++) base.cols[c].rowReg = -1;
-   auto runBatches = [&] {
-      int64_t first = 0;
-      for (auto& b : t->batches) {
-         const int64_t firstRow = first;
-         first += b.nRows;
-         if (b.nRows == 0) continue;
-         ProgramParams p = base;
-         p.nRows = b.nRows;
-         p.firstRow = firstRow;
-         for (int c = 0; c < d->n_columns; c++) {
-            const int ci = colIdx[c];
-            p.cols[c].type = t->columns[ci].type;
-            bindColumn(p.cols[c], b, ci);
-         }
-         ldb_gpu_wait_batch_internal(ctx, &b);
-         ctx->launch("program", [&] { launchProgram(p, ctx->smCount, ctx->compute); });
+   for (int c = 0; c < p.d->n_columns; c++) p.base.cols[c].rowReg = -1;
+}
+
+// one interpreter launch per non-empty batch of the source
+static void launchBatches(const ProgramPlan& p) {
+   LdbContext* ctx = p.ctx;
+   int64_t first = 0;
+   for (auto& b : p.t->batches) {
+      const int64_t firstRow = first;
+      first += b.nRows;
+      if (b.nRows == 0) continue;
+      ProgramParams pp = p.base;
+      pp.nRows = b.nRows;
+      pp.firstRow = firstRow;
+      for (int c = 0; c < p.d->n_columns; c++) {
+         const int ci = p.colIdx[c];
+         pp.cols[c].type = p.t->columns[ci].type;
+         bindColumn(pp.cols[c], b, ci);
       }
-   };
-   runBatches();
-   // a probe run longer than the bound (PROBE_EACH), or a build that could not store a row (table full, the reserved pair, a key or
-   // payload outside int32): fail rather than return a truncated match list or a table with rows missing
-   // — and a dictionary that could not take a string
-   try {
-      for (LdbState* js : {eachTable >= 0 ? d->tables[eachTable] : nullptr, d->sink_kind == LDB_SINK_JOIN_BUILD ? sink : nullptr})
-         if (js && js->kind == LDB_STATE_JOIN_TABLE) ldb_gpu_check_join_error_internal(js);
-      for (LdbState* ks : tupleTables) ldb_gpu_check_keyjoin_error_internal(ks); // a full build, a probe run at the bound, a key outside int64
-      for (LdbState* ds : dicts) checkDictError(ds);
-   } catch (...) {
-      ctx->syncStream(ctx->compute);
-      for (void* q : outOwned) ctx->stagingRelease(q);
-      for (void* q : dirs) ctx->stagingRelease(q);
-      throw;
-   }
-   if (d->sink_kind == LDB_SINK_MATERIALIZE) {
-      unsigned long long n = 0;
-      LDB_CUDA(cudaMemcpyAsync(&n, outCount, 8, cudaMemcpyDeviceToHost, ctx->compute));
-      ctx->syncStream(ctx->compute);
-      if (n > (unsigned long long) base.outCapacity) { // PROBE_EACH produced more rows than the source has: regrow and run once more
-         allocOut((size_t) n);
-         runBatches();
-         LDB_CUDA(cudaMemcpyAsync(&n, outCount, 8, cudaMemcpyDeviceToHost, ctx->compute));
-         ctx->syncStream(ctx->compute);
-         if (n > (unsigned long long) base.outCapacity) failP(LDB_ERR_INVALID, "materialize: the rerun produced more rows than the first run");
-      }
-      auto* ot = new LdbTable;
-      ot->ctx = ctx;
-      ot->name = t->name + "_out";
-      LdbBatch ob;
-      ob.nRows = (int64_t) n;
-      for (int c = 0; c < d->n_out; c++) {
-         ot->columns.push_back({"c" + std::to_string(c), LDB_DECIMAL128, 38, 0});
-         ob.data.push_back(outVals[c]);
-         ob.bytes.push_back(nullptr);
-         ob.elemBytes.push_back(16);
-         ob.validBytes.push_back(outValid[c]);
-      }
-      ob.validity.assign(ob.data.size(), nullptr);
-      ob.validityBitOffset.assign(ob.data.size(), 0);
-      ob.owned = outOwned;
-      ot->numRows = (int64_t) n;
-      ot->batches.push_back(std::move(ob));
-      ctx->tables.push_back(ot);
-      *d->out_table = ot;
-   }
-   if (!dirs.empty()) {
-      ctx->syncStream(ctx->compute); // the batch directories are read until the last launch ends
-      for (void* q : dirs) ctx->stagingRelease(q);
+      ldb_gpu_wait_batch_internal(ctx, &b);
+      ctx->launch("program", [&] { launchProgram(pp, ctx->smCount, ctx->compute); });
    }
 }
 
+// a probe run longer than the bound (PROBE_EACH), or a build that could not store a row (table full, the reserved pair, a key or
+// payload outside int32): fail rather than return a truncated match list or a table with rows missing
+// — and a dictionary that could not take a string
+static void checkErrorWords(const ProgramPlan& p) {
+   const LdbProgramDesc* d = p.d;
+   for (LdbState* js : {p.eachTable >= 0 ? d->tables[p.eachTable] : nullptr, d->sink_kind == LDB_SINK_JOIN_BUILD ? d->sink : nullptr})
+      if (js && js->kind == LDB_STATE_JOIN_TABLE) ldb_gpu_check_join_error_internal(js);
+   for (LdbState* ks : p.tupleTables) ldb_gpu_check_keyjoin_error_internal(ks); // a full build, a probe run at the bound, a key outside int64
+   for (LdbState* ds : p.dicts) checkDictError(ds);
+}
+
+// the materialized rows as a table that takes over the output buffers of `out` (synchronises)
+static LdbTable* materializeResult(ProgramPlan& p, Scratch& out) {
+   LdbContext* ctx = p.ctx;
+   unsigned long long n = 0;
+   LDB_CUDA(cudaMemcpyAsync(&n, p.base.outCount, 8, cudaMemcpyDeviceToHost, ctx->compute));
+   ctx->syncStream(ctx->compute);
+   if (n > (unsigned long long) p.base.outCapacity) { // PROBE_EACH produced more rows than the source has: regrow and run once more
+      allocOut(p, out, (size_t) n);
+      launchBatches(p);
+      LDB_CUDA(cudaMemcpyAsync(&n, p.base.outCount, 8, cudaMemcpyDeviceToHost, ctx->compute));
+      ctx->syncStream(ctx->compute);
+      if (n > (unsigned long long) p.base.outCapacity) fail(LDB_ERR_INVALID, "materialize: the rerun produced more rows than the first run");
+   }
+   std::vector<LdbColumn> columns;
+   LdbBatch ob;
+   ob.nRows = (int64_t) n;
+   for (int c = 0; c < p.d->n_out; c++) {
+      columns.push_back({"c" + std::to_string(c), LDB_DECIMAL128, 38, 0});
+      ob.data.push_back(p.base.outValues[c]);
+      ob.bytes.push_back(nullptr);
+      ob.elemBytes.push_back(16);
+      ob.validBytes.push_back(p.base.outValid[c]);
+   }
+   return addResultTable(ctx, p.t->name + "_out", std::move(columns), std::move(ob), out);
+}
+
+static void runProgram(LdbContext* ctx, const LdbProgramDesc* d, const LdbProgramJoins* j) {
+   if (!ctx || !d || !d->source) fail(LDB_ERR_INVALID, "null argument");
+   ProgramPlan p(ctx, d);
+   resolveColumns(p, j);
+   validateInstructions(p);
+   bindTables(p);
+   Scratch out(ctx), dirs(ctx);
+   bindSink(p, out);
+   bindSideColumns(p, dirs);
+   launchBatches(p);
+   checkErrorWords(p);
+   if (d->sink_kind == LDB_SINK_MATERIALIZE) *d->out_table = materializeResult(p, out);
+   if (!dirs.empty()) ctx->syncStream(ctx->compute); // the batch directories are read until the last launch ends
+}
+
+// ORDER BY … LIMIT over a single-batch table: the first min(n, limit) row ids (limit < 0: all n) of the stable sort by `keys`
+static void orderRows(LdbTable* t, const std::vector<std::pair<int, int>>& keys, int64_t limit, int64_t* row_ids, int64_t* n_out) {
+   if (t->batches.size() != 1) fail(LDB_ERR_UNSUPPORTED, "ORDER BY runs over single-batch tables (materialised results, exported groups)");
+   LdbContext* ctx = t->ctx;
+   LdbBatch& b = t->batches[0];
+   const int64_t n = b.nRows;
+   if (n >= (int64_t) 1 << 32) fail(LDB_ERR_UNSUPPORTED, "ORDER BY handles up to 2^32 - 1 rows");
+   LDB_CUDA(cudaSetDevice(ctx->device));
+   ldb_gpu_wait_batch_internal(ctx, &b);
+   Scratch scratch(ctx);
+   const uint32_t* ids = sortRows(scratch, t, keys, n);
+   const int64_t m = std::min<int64_t>(n, limit < 0 ? n : limit);
+   std::vector<uint32_t> top((size_t) m);
+   if (m) LDB_CUDA(cudaMemcpyAsync(top.data(), ids, (size_t) m * 4, cudaMemcpyDeviceToHost, ctx->compute));
+   ctx->syncStream(ctx->compute);
+   for (int64_t i = 0; i < m; i++) row_ids[i] = top[(size_t) i];
+   *n_out = m;
+}
+
+extern "C" {
+
 int ldb_gpu_run_program(LdbContext* ctx, const LdbProgramDesc* d, LdbError* err) {
-   return guardedP(err, [&] { runProgram(ctx, d, nullptr); });
+   return guarded(err, [&] { runProgram(ctx, d, nullptr); });
 }
 int ldb_gpu_run_program_ex(LdbContext* ctx, const LdbProgramDesc* d, const LdbProgramJoins* joins, LdbError* err) {
-   return guardedP(err, [&] { runProgram(ctx, d, joins); });
+   return guarded(err, [&] { runProgram(ctx, d, joins); });
 }
 
 // ---------------------------------------------------------------- ORDER BY … LIMIT and result gather
 int ldb_gpu_table_order_by(LdbTable* t, const char* column, int32_t descending, int64_t limit, int64_t* row_ids, int64_t* n_out, LdbError* err) {
-   return guardedP(err, [&] {
-      if (!t || !row_ids || !n_out) failP(LDB_ERR_INVALID, "null argument");
-      LdbContext* ctx = t->ctx;
+   return guarded(err, [&] {
+      if (!t || !row_ids || !n_out) fail(LDB_ERR_INVALID, "null argument");
       const int c = t->colIndex(column);
-      if (c < 0) failP(LDB_ERR_INVALID, "unknown column");
+      if (c < 0) fail(LDB_ERR_INVALID, "unknown column");
       const int type = t->columns[c].type;
-      if (type == LDB_UTF8 || type == LDB_FLOAT32 || type == LDB_FLOAT64 || type == LDB_INT8 || type == LDB_INT16) failP(LDB_ERR_UNSUPPORTED, "ORDER BY column must be int32/date32/char(1)/int64/decimal");
-      if (t->batches.size() != 1) failP(LDB_ERR_UNSUPPORTED, "ORDER BY runs over single-batch tables (materialised results, exported groups)");
-      LdbBatch& b = t->batches[0];
-      const int64_t n = b.nRows;
-      if (n >= (int64_t) 1 << 32) failP(LDB_ERR_UNSUPPORTED, "ORDER BY handles up to 2^32 - 1 rows");
-      LDB_CUDA(cudaSetDevice(ctx->device));
-      ldb_gpu_wait_batch_internal(ctx, &b);
-      const size_t rows = (size_t) std::max<int64_t>(n, 1);
-      unsigned long long* dk = (unsigned long long*) ctx->stagingAlloc(rows * 8);
-      unsigned long long* dk2 = (unsigned long long*) ctx->stagingAlloc(rows * 8);
-      uint32_t* dv = (uint32_t*) ctx->stagingAlloc(rows * 4);
-      uint32_t* dv2 = (uint32_t*) ctx->stagingAlloc(rows * 4);
-      const int ctas = (int) ((n + 4095) / 4096);
-      unsigned int* hist = (unsigned int*) ctx->stagingAlloc((size_t) std::max(ctas, 1) * 256 * 4);
-      if (n) {
-         ctx->launch("radix_sort", [&] {
-            launchBuildSortKeys((const uint8_t*) b.data[c], b.elemBytes[c], n, descending, dk, dv, ctx->smCount, ctx->compute);
-            launchRadixSortPairs(dk, dv, dk2, dv2, n, hist, ctx->smCount, ctx->compute);
-         });
-      }
-      const int64_t m = std::min<int64_t>(n, limit < 0 ? n : limit);
-      std::vector<uint32_t> top((size_t) m);
-      if (m) LDB_CUDA(cudaMemcpyAsync(top.data(), dv, (size_t) m * 4, cudaMemcpyDeviceToHost, ctx->compute));
-      ctx->syncStream(ctx->compute);
-      for (int64_t i = 0; i < m; i++) row_ids[i] = top[(size_t) i];
-      *n_out = m;
-      for (void* p : {(void*) dk, (void*) dk2, (void*) dv, (void*) dv2, (void*) hist}) ctx->stagingRelease(p);
+      if (type == LDB_UTF8 || type == LDB_FLOAT32 || type == LDB_FLOAT64 || type == LDB_INT8 || type == LDB_INT16) fail(LDB_ERR_UNSUPPORTED, "ORDER BY column must be int32/date32/char(1)/int64/decimal");
+      orderRows(t, {{c, descending ? 1 : 0}}, limit, row_ids, n_out);
    });
 }
 int ldb_gpu_table_gather(LdbTable* t, const char* column, const int64_t* row_ids, int64_t n, void* host_dst, uint8_t* host_valid, LdbError* err) {
-   return guardedP(err, [&] {
-      if (!t || !row_ids || !host_dst) failP(LDB_ERR_INVALID, "null argument");
+   return guarded(err, [&] {
+      if (!t || !row_ids || !host_dst) fail(LDB_ERR_INVALID, "null argument");
       LdbContext* ctx = t->ctx;
       const int c = t->colIndex(column);
-      if (c < 0) failP(LDB_ERR_INVALID, "unknown column");
-      if (t->columns[c].type == LDB_UTF8) failP(LDB_ERR_UNSUPPORTED, "gather reads fixed-width columns");
-      if (t->batches.size() != 1) failP(LDB_ERR_UNSUPPORTED, "gather runs over single-batch tables");
+      if (c < 0) fail(LDB_ERR_INVALID, "unknown column");
+      if (t->columns[c].type == LDB_UTF8) fail(LDB_ERR_UNSUPPORTED, "gather reads fixed-width columns");
+      if (t->batches.size() != 1) fail(LDB_ERR_UNSUPPORTED, "gather runs over single-batch tables");
       LdbBatch& b = t->batches[0];
       LDB_CUDA(cudaSetDevice(ctx->device));
       ldb_gpu_wait_batch_internal(ctx, &b);
       const size_t w = (size_t) b.elemBytes[c];
       for (int64_t i = 0; i < n; i++)
-         if (row_ids[i] < 0 || row_ids[i] >= b.nRows) failP(LDB_ERR_INVALID, "row id out of range");
+         if (row_ids[i] < 0 || row_ids[i] >= b.nRows) fail(LDB_ERR_INVALID, "row id out of range");
       // one copy per run of consecutive row ids (a whole column read back in order is one copy)
       for (int64_t i = 0, j; i < n; i = j) {
          for (j = i + 1; j < n && row_ids[j] == row_ids[j - 1] + 1;) j++;
@@ -852,46 +824,32 @@ int ldb_gpu_table_gather(LdbTable* t, const char* column, const int64_t* row_ids
    });
 }
 int ldb_gpu_table_order_by_keys(LdbTable* t, int32_t n_keys, const char* const* columns, const int32_t* descending, int64_t limit, int64_t* row_ids, int64_t* n_out, LdbError* err) {
-   return guardedP(err, [&] {
-      if (!t || !columns || !descending || !row_ids || !n_out) failP(LDB_ERR_INVALID, "null argument");
-      if (n_keys < 1) failP(LDB_ERR_INVALID, "ORDER BY needs at least one key");
-      LdbContext* ctx = t->ctx;
+   return guarded(err, [&] {
+      if (!t || !columns || !descending || !row_ids || !n_out) fail(LDB_ERR_INVALID, "null argument");
+      if (n_keys < 1) fail(LDB_ERR_INVALID, "ORDER BY needs at least one key");
       std::vector<std::pair<int, int>> keys;
       for (int k = 0; k < n_keys; k++) {
          const int c = t->colIndex(columns[k]);
-         if (c < 0) failP(LDB_ERR_INVALID, std::string("unknown column ") + (columns[k] ? columns[k] : "(null)"));
+         if (c < 0) fail(LDB_ERR_INVALID, std::string("unknown column ") + (columns[k] ? columns[k] : "(null)"));
          const int type = t->columns[c].type;
-         if (type == LDB_FLOAT32 || type == LDB_FLOAT64 || type == LDB_INT8 || type == LDB_INT16) failP(LDB_ERR_UNSUPPORTED, "ORDER BY column must be int32/date32/char(1)/int64/decimal/utf8");
+         if (type == LDB_FLOAT32 || type == LDB_FLOAT64 || type == LDB_INT8 || type == LDB_INT16) fail(LDB_ERR_UNSUPPORTED, "ORDER BY column must be int32/date32/char(1)/int64/decimal/utf8");
          keys.push_back({c, descending[k] ? 1 : 0});
       }
-      if (t->batches.size() != 1) failP(LDB_ERR_UNSUPPORTED, "ORDER BY runs over single-batch tables (materialised results, exported groups)");
-      LdbBatch& b = t->batches[0];
-      const int64_t n = b.nRows;
-      if (n >= (int64_t) 1 << 32) failP(LDB_ERR_UNSUPPORTED, "ORDER BY handles up to 2^32 - 1 rows");
-      LDB_CUDA(cudaSetDevice(ctx->device));
-      ldb_gpu_wait_batch_internal(ctx, &b);
-      uint32_t* ids = sortRows(t, keys, n);
-      const int64_t m = std::min<int64_t>(n, limit < 0 ? n : limit);
-      std::vector<uint32_t> top((size_t) m);
-      if (m) LDB_CUDA(cudaMemcpyAsync(top.data(), ids, (size_t) m * 4, cudaMemcpyDeviceToHost, ctx->compute));
-      ctx->syncStream(ctx->compute);
-      ctx->stagingRelease(ids);
-      for (int64_t i = 0; i < m; i++) row_ids[i] = top[(size_t) i];
-      *n_out = m;
+      orderRows(t, keys, limit, row_ids, n_out);
    });
 }
 int ldb_gpu_table_gather_strings(LdbTable* t, const char* column, const int64_t* row_ids, int64_t n, int64_t* host_offsets, void* host_bytes, int64_t bytes_cap, int64_t* bytes_needed,
                                  uint8_t* host_valid, LdbError* err) {
-   return guardedP(err, [&] {
-      if (!t || (n > 0 && !row_ids) || !host_offsets || !bytes_needed || n < 0) failP(LDB_ERR_INVALID, "null argument");
+   return guarded(err, [&] {
+      if (!t || (n > 0 && !row_ids) || !host_offsets || !bytes_needed || n < 0) fail(LDB_ERR_INVALID, "null argument");
       LdbContext* ctx = t->ctx;
       const int c = t->colIndex(column);
-      if (c < 0) failP(LDB_ERR_INVALID, "unknown column");
-      if (t->columns[c].type != LDB_UTF8) failP(LDB_ERR_UNSUPPORTED, "gather_strings reads utf8 columns");
-      if (t->batches.size() != 1) failP(LDB_ERR_UNSUPPORTED, "gather runs over single-batch tables");
+      if (c < 0) fail(LDB_ERR_INVALID, "unknown column");
+      if (t->columns[c].type != LDB_UTF8) fail(LDB_ERR_UNSUPPORTED, "gather_strings reads utf8 columns");
+      if (t->batches.size() != 1) fail(LDB_ERR_UNSUPPORTED, "gather runs over single-batch tables");
       LdbBatch& b = t->batches[0];
       for (int64_t i = 0; i < n; i++)
-         if (row_ids[i] < 0 || row_ids[i] >= b.nRows) failP(LDB_ERR_INVALID, "row id out of range");
+         if (row_ids[i] < 0 || row_ids[i] >= b.nRows) fail(LDB_ERR_INVALID, "row id out of range");
       LDB_CUDA(cudaSetDevice(ctx->device));
       ldb_gpu_wait_batch_internal(ctx, &b);
       // runs of consecutive row ids: [first index, end index) → the run's m + 1 offsets at `at` in `offs`
@@ -915,8 +873,8 @@ int ldb_gpu_table_gather_strings(LdbTable* t, const char* column, const int64_t*
       int64_t total = 0;
       for (const Run& r : runs) total += offs[r.at + (size_t) (r.j - r.i)] - offs[r.at];
       *bytes_needed = total;
-      if (total > bytes_cap) failP(LDB_ERR_CAPACITY, "gather_strings: the strings need more than bytes_cap bytes (see bytes_needed)");
-      if (total > 0 && !host_bytes) failP(LDB_ERR_INVALID, "null argument");
+      if (total > bytes_cap) fail(LDB_ERR_CAPACITY, "gather_strings: the strings need more than bytes_cap bytes (see bytes_needed)");
+      if (total > 0 && !host_bytes) fail(LDB_ERR_INVALID, "null argument");
       const uint8_t* bitmap = c < (int) b.validity.size() ? (const uint8_t*) b.validity[c] : nullptr;
       const uint8_t* vbytes = c < (int) b.validBytes.size() ? b.validBytes[c] : nullptr;
       std::vector<std::vector<uint8_t>> bits(host_valid && bitmap && !vbytes ? runs.size() : 0);

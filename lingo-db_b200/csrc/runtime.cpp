@@ -14,42 +14,6 @@ using namespace ldb;
 
 // ------------------------------------------------------------------------------------------------ helpers
 namespace {
-template <class Fn>
-int guarded(LdbError* err, const Fn& fn) {
-   auto set = [&](int code, const char* msg) {
-      if (err) {
-         err->code = code;
-         snprintf(err->message, sizeof(err->message), "%s", msg);
-      }
-      return code;
-   };
-   try {
-      fn();
-      if (err) {
-         err->code = LDB_OK;
-         err->message[0] = 0;
-      }
-      return LDB_OK;
-   } catch (const CudaError& e) {
-      return set(e.code, e.what());
-   } catch (const ApiError& e) {
-      return set(e.code, e.what());
-   } catch (const std::exception& e) {
-      return set(LDB_ERR_INVALID, e.what());
-   }
-}
-[[noreturn]] void fail(int code, const std::string& m) { throw ApiError(code, m); }
-
-uint64_t nextPow2(uint64_t v) {
-   v--;
-   v |= v >> 1;
-   v |= v >> 2;
-   v |= v >> 4;
-   v |= v >> 8;
-   v |= v >> 16;
-   v |= v >> 32;
-   return v + 1;
-}
 size_t elemWidth(int type) {
    switch (type) {
       case LDB_INT32:
@@ -782,14 +746,13 @@ int ldb_gpu_groupby_merge_rows(LdbState* s, const LdbGroupRow* rows, int32_t n_r
             acc[((size_t) r * kMaxAggs + a) * 2 + 1] = (unsigned long long) rows[r].aggs[a].hi;
          }
       }
-      void* dk = ctx->stagingAlloc(keys.size() * 4);
-      void* da = ctx->stagingAlloc(acc.size() * 8);
+      Scratch scratch(ctx);
+      int32_t* dk = scratch.alloc<int32_t>(keys.size() * 4);
+      unsigned long long* da = scratch.alloc<unsigned long long>(acc.size() * 8);
       LDB_CUDA(cudaMemcpyAsync(dk, keys.data(), keys.size() * 4, cudaMemcpyHostToDevice, ctx->compute));
       LDB_CUDA(cudaMemcpyAsync(da, acc.data(), acc.size() * 8, cudaMemcpyHostToDevice, ctx->compute));
-      ctx->launch("group_merge", [&] { launchGroupMergeRows(s->group, (const int32_t*) dk, (const unsigned long long*) da, n_rows, ctx->compute); });
+      ctx->launch("group_merge", [&] { launchGroupMergeRows(s->group, dk, da, n_rows, ctx->compute); });
       ctx->syncStream(ctx->compute);
-      ctx->stagingRelease(dk);
-      ctx->stagingRelease(da);
    });
 }
 
@@ -935,7 +898,8 @@ int ldb_gpu_table_column_range(LdbTable* t, const char* column, int32_t* mn, int
       }
       LDB_CUDA(cudaSetDevice(ctx->device));
       int32_t init[2] = {INT32_MAX, INT32_MIN};
-      int32_t* d = (int32_t*) ctx->stagingAlloc(8);
+      Scratch scratch(ctx);
+      int32_t* d = scratch.alloc<int32_t>(8);
       LDB_CUDA(cudaMemcpyAsync(d, init, 8, cudaMemcpyHostToDevice, ctx->compute));
       for (auto& b : t->batches) {
          if (b.nRows == 0) continue;
@@ -944,7 +908,6 @@ int ldb_gpu_table_column_range(LdbTable* t, const char* column, int32_t* mn, int
       }
       LDB_CUDA(cudaMemcpyAsync(init, d, 8, cudaMemcpyDeviceToHost, ctx->compute));
       ctx->syncStream(ctx->compute);
-      ctx->stagingRelease(d);
       *mn = init[0];
       *mx = init[1];
       t->ranges[c] = LdbTable::ColumnRange{t->numRows, init[0], init[1]};
@@ -993,12 +956,12 @@ int ldb_gpu_join_table_topk(LdbState* s, int32_t k, LdbTopKRow* rows, int32_t* n
       LdbContext* ctx = s->ctx;
       int blocks = ctx->smCount * 2;
       size_t bytes = sizeof(TopKRowDev) * (size_t) blocks * k;
-      void* d = ctx->stagingAlloc(bytes);
-      ctx->launch("join_topk", [&] { launchJoinTopK(s->join, k, (s->is64Mask & 1u) != 0, (TopKRowDev*) d, &blocks, ctx->smCount, ctx->compute); });
+      Scratch scratch(ctx);
+      TopKRowDev* d = scratch.alloc<TopKRowDev>(bytes);
+      ctx->launch("join_topk", [&] { launchJoinTopK(s->join, k, (s->is64Mask & 1u) != 0, d, &blocks, ctx->smCount, ctx->compute); });
       std::vector<TopKRowDev> h((size_t) blocks * k);
       LDB_CUDA(cudaMemcpyAsync(h.data(), d, bytes, cudaMemcpyDeviceToHost, ctx->compute));
       ctx->syncStream(ctx->compute);
-      ctx->stagingRelease(d);
       std::vector<TopKRowDev> valid;
       for (auto& r : h)
          if (r.valid) valid.push_back(r);
@@ -1627,7 +1590,8 @@ int ldb_gpu_partition_tuples(LdbContext* ctx, const int32_t* keys, const void* c
       for (int c = 0; c < n_payload_cols; c++)
          if (payload_widths[c] != 4 && payload_widths[c] != 8 && payload_widths[c] != 16) fail(LDB_ERR_INVALID, "payload width must be 4, 8 or 16");
       LDB_CUDA(cudaSetDevice(ctx->device));
-      unsigned long long* counts = (unsigned long long*) ctx->stagingAlloc(64 * 8);
+      Scratch scratch(ctx);
+      unsigned long long* counts = scratch.alloc<unsigned long long>(64 * 8);
       LDB_CUDA(cudaMemsetAsync(counts, 0, 64 * 8, ctx->compute));
       if (n_rows > 0) ctx->launch("partition", [&] { launchPartitionHistogram(keys, n_rows, n_parts, counts, ctx->smCount, ctx->compute); });
       unsigned long long h[64];
@@ -1644,7 +1608,6 @@ int ldb_gpu_partition_tuples(LdbContext* ctx, const int32_t* keys, const void* c
       LDB_CUDA(cudaMemcpyAsync(counts, cursor, 64 * 8, cudaMemcpyHostToDevice, ctx->compute));
       if (n_rows > 0) ctx->launch("partition", [&] { launchPartitionScatter(keys, payload_cols, payload_widths, n_payload_cols, n_rows, n_parts, counts, out_keys, out_payload_cols, ctx->smCount, ctx->compute); });
       ctx->syncStream(ctx->compute);
-      ctx->stagingRelease(counts);
    });
 }
 int ldb_gpu_join_table_insert(LdbContext* ctx, LdbState* table, const int32_t* keys, const int32_t* payloads, const int32_t* const* side_cols, int64_t n_rows, LdbError* err) {
@@ -1659,17 +1622,15 @@ int ldb_gpu_join_table_insert(LdbContext* ctx, LdbState* table, const int32_t* k
 int ldb_gpu_hash_i64(LdbContext* ctx, const int64_t* a, const int64_t* b, int64_t n, uint64_t* out, LdbError* err) {
    return guarded(err, [&] {
       LDB_CUDA(cudaSetDevice(ctx->device));
-      void* da = ctx->stagingAlloc(n * 8);
-      void* db = b ? ctx->stagingAlloc(n * 8) : nullptr;
-      void* dout = ctx->stagingAlloc(n * 8);
+      Scratch scratch(ctx);
+      int64_t* da = scratch.alloc<int64_t>(n * 8);
+      int64_t* db = b ? scratch.alloc<int64_t>(n * 8) : nullptr;
+      uint64_t* dout = scratch.alloc<uint64_t>(n * 8);
       LDB_CUDA(cudaMemcpyAsync(da, a, n * 8, cudaMemcpyHostToDevice, ctx->compute));
       if (b) LDB_CUDA(cudaMemcpyAsync(db, b, n * 8, cudaMemcpyHostToDevice, ctx->compute));
-      ctx->launch("hash", [&] { launchHashI64((const int64_t*) da, (const int64_t*) db, n, (uint64_t*) dout, ctx->compute); });
+      ctx->launch("hash", [&] { launchHashI64(da, db, n, dout, ctx->compute); });
       LDB_CUDA(cudaMemcpyAsync(out, dout, n * 8, cudaMemcpyDeviceToHost, ctx->compute));
       ctx->syncStream(ctx->compute);
-      ctx->stagingRelease(da);
-      if (db) ctx->stagingRelease(db);
-      ctx->stagingRelease(dout);
    });
 }
 

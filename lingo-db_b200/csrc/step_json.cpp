@@ -303,30 +303,6 @@ std::string fromHex(const char* hex) {
    for (size_t i = 0; i < n / 2; i++) out[i] = (char) (nib(hex[2 * i]) * 16 + nib(hex[2 * i + 1]));
    return out;
 }
-template <class Fn>
-int guardedS(LdbError* err, const Fn& fn) {
-   auto set = [&](int code, const char* msg) {
-      if (err) {
-         err->code = code;
-         snprintf(err->message, sizeof(err->message), "%s", msg);
-      }
-      return code;
-   };
-   try {
-      fn();
-      if (err) {
-         err->code = LDB_OK;
-         err->message[0] = 0;
-      }
-      return LDB_OK;
-   } catch (const ldb::CudaError& e) {
-      return set(e.code, e.what());
-   } catch (const ldb::ApiError& e) {
-      return set(e.code, e.what());
-   } catch (const std::exception& e) {
-      return set(LDB_ERR_INVALID, e.what());
-   }
-}
 void check(int rc, const LdbError& e) {
    if (rc != LDB_OK) throw ldb::ApiError(rc, e.message);
 }
@@ -336,7 +312,7 @@ extern "C" {
 
 // structure check only — no device needed (the compiler side can validate what it emits)
 int ldb_gpu_step_validate(const char* json, LdbError* err) {
-   return guardedS(err, [&] {
+   return ldb::guarded(err, [&] {
       if (!json) throw ldb::ApiError(LDB_ERR_INVALID, "null argument");
       Step st;
       parseStep(parseJson(json), st);
@@ -344,7 +320,7 @@ int ldb_gpu_step_validate(const char* json, LdbError* err) {
 }
 // name → handle registries of the context (states a step created or the caller registered)
 int ldb_gpu_register_state(LdbContext* ctx, const char* name, LdbState* s, LdbError* err) {
-   return guardedS(err, [&] {
+   return ldb::guarded(err, [&] {
       if (!ctx || !name || !s) throw ldb::ApiError(LDB_ERR_INVALID, "null argument");
       ctx->namedStates[name] = s;
    });
@@ -355,7 +331,7 @@ LdbState* ldb_gpu_find_state(LdbContext* ctx, const char* name) {
    return it == ctx->namedStates.end() ? nullptr : it->second;
 }
 int ldb_gpu_run_step(LdbContext* ctx, const char* json, LdbError* err) {
-   return guardedS(err, [&] {
+   return ldb::guarded(err, [&] {
       if (!ctx || !json) throw ldb::ApiError(LDB_ERR_INVALID, "null argument");
       Step st;
       parseStep(parseJson(json), st);
@@ -386,7 +362,7 @@ int ldb_gpu_run_step(LdbContext* ctx, const char* json, LdbError* err) {
 // the same document hex-encoded, as the reference ships its serialised descriptions (utility::serializeToHexString →
 // DataSource::get, DataSourceIteration.cpp:57-88)
 int ldb_gpu_run_step_hex(LdbContext* ctx, const char* hex, LdbError* err) {
-   return guardedS(err, [&] {
+   return ldb::guarded(err, [&] {
       if (!hex) throw ldb::ApiError(LDB_ERR_INVALID, "null argument");
       const std::string json = fromHex(hex);
       LdbError e;
