@@ -154,6 +154,9 @@ __device__ __forceinline__ int64_t ldShared64(uint32_t addr) {
    asm volatile("ld.shared.s64 %0, [%1];" : "=l"(v) : "r"(addr));
    return v;
 }
+__device__ __forceinline__ void ldShared64x2(uint32_t addr, int64_t& a, int64_t& b) { // addr 16-byte aligned
+   asm volatile("ld.shared.v2.s64 {%0, %1}, [%2];" : "=l"(a), "=l"(b) : "r"(addr));
+}
 
 // ---------------------------------------------------------------- blocked Bloom filter of the join tables
 // Three bit positions inside the 32-bit filter word that (h >> 32) selects, from a second multiply of the hash.  (Deriving them from the

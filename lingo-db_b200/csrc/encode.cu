@@ -16,8 +16,8 @@ __device__ __forceinline__ int64_t encodeSource(const uint8_t* src, bool isI32, 
    return isI32 ? (int64_t) ((const int32_t*) src)[r] : ((const int64_t*) src)[2 * r]; // decimal128: its low 8 bytes
 }
 
-// one CTA per block: blockMin[b] and the largest (max - min) of all blocks
-__global__ void encodeRangeKernel(const uint8_t* src, bool isI32, int64_t n, int64_t* blockMin, unsigned long long* maxRange) {
+// one CTA per block: blockMin[b], blockRange[b] = max - min, and the largest range of all blocks
+__global__ void encodeRangeKernel(const uint8_t* src, bool isI32, int64_t n, int64_t* blockMin, int64_t* blockRange, unsigned long long* maxRange) {
    __shared__ int64_t sLo[32], sHi[32];
    const int64_t r0 = (int64_t) blockIdx.x * kEncodeBlockRows, r1 = min(n, r0 + kEncodeBlockRows);
    int64_t lo = LLONG_MAX, hi = LLONG_MIN;
@@ -42,12 +42,15 @@ __global__ void encodeRangeKernel(const uint8_t* src, bool isI32, int64_t n, int
          hi = max(hi, sHi[w]);
       }
       blockMin[blockIdx.x] = lo;
+      blockRange[blockIdx.x] = (int64_t) ((uint64_t) hi - (uint64_t) lo);
       atomicMax(maxRange, (unsigned long long) ((uint64_t) hi - (uint64_t) lo));
    }
 }
 
-// one thread per row: the value's offset from its block minimum in `width` bytes, and the header of every tile
-__global__ void encodePackKernel(const uint8_t* src, bool isI32, int64_t n, const int64_t* blockMin, int width, int tileRows, uint8_t* dst) {
+// one thread per row: the value's offset from its block minimum in `width` bytes, and the header {block min, block range} of every
+// tile — the range bounds every value of the tile, so K1/K2 can prove per tile that its products fit 64 bits
+__global__ void encodePackKernel(const uint8_t* src, bool isI32, int64_t n, const int64_t* blockMin, const int64_t* blockRange, int width, int tileRows,
+                                 uint8_t* dst) {
    const int64_t tileStride = kEncodeTileHeader + (int64_t) tileRows * width;
    for (int64_t r = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (int64_t) gridDim.x * blockDim.x) {
       const int64_t t = r / tileRows, lr = r - t * tileRows;
@@ -55,7 +58,7 @@ __global__ void encodePackKernel(const uint8_t* src, bool isI32, int64_t n, cons
       uint8_t* tile = dst + t * tileStride;
       if (lr == 0) {
          ((int64_t*) tile)[0] = base;
-         ((int64_t*) tile)[1] = 0;
+         ((int64_t*) tile)[1] = blockRange[r / kEncodeBlockRows];
       }
       const uint64_t d = (uint64_t) encodeSource(src, isI32, r) - (uint64_t) base;
       uint8_t* p = tile + kEncodeTileHeader + lr * width;
@@ -68,13 +71,14 @@ __global__ void encodePackKernel(const uint8_t* src, bool isI32, int64_t n, cons
    }
 }
 
-void launchEncodeRange(const uint8_t* src, bool isI32, int64_t n, int64_t* blockMin, unsigned long long* maxRange, cudaStream_t s) {
+void launchEncodeRange(const uint8_t* src, bool isI32, int64_t n, int64_t* blockMin, int64_t* blockRange, unsigned long long* maxRange, cudaStream_t s) {
    const int64_t blocks = (n + kEncodeBlockRows - 1) / kEncodeBlockRows;
-   encodeRangeKernel<<<(unsigned) blocks, 256, 0, s>>>(src, isI32, n, blockMin, maxRange);
+   encodeRangeKernel<<<(unsigned) blocks, 256, 0, s>>>(src, isI32, n, blockMin, blockRange, maxRange);
 }
-void launchEncodePack(const uint8_t* src, bool isI32, int64_t n, const int64_t* blockMin, int width, int tileRows, uint8_t* dst, cudaStream_t s) {
+void launchEncodePack(const uint8_t* src, bool isI32, int64_t n, const int64_t* blockMin, const int64_t* blockRange, int width, int tileRows, uint8_t* dst,
+                      cudaStream_t s) {
    const int64_t grid = std::min<int64_t>((n + 255) / 256, 8192);
-   encodePackKernel<<<(unsigned) grid, 256, 0, s>>>(src, isI32, n, blockMin, width, tileRows, dst);
+   encodePackKernel<<<(unsigned) grid, 256, 0, s>>>(src, isI32, n, blockMin, blockRange, width, tileRows, dst);
 }
 
 static int encodedWidth(uint64_t range) { return range < (1ull << 8) ? 1 : range < (1ull << 16) ? 2 : range < (1ull << 32) ? 4 : 8; }
@@ -119,16 +123,17 @@ bool ldb_gpu_encode_batch_internal(LdbContext* ctx, LdbTable* t, LdbBatch& b, co
       LDB_CUDA(cudaStreamWaitEvent(s, ctx->computeDone, 0));
    }
    void* scratch = nullptr;
-   const size_t scratchBytes = (size_t) nTodo * (size_t) blocks * 8 + (size_t) nTodo * 8;
+   const size_t scratchBytes = (size_t) nTodo * (size_t) blocks * 16 + (size_t) nTodo * 8;
    if (cudaMalloc(&scratch, scratchBytes) != cudaSuccess) return failAll();
    int64_t* blockMin = (int64_t*) scratch;
-   unsigned long long* maxRange = (unsigned long long*) (blockMin + (size_t) nTodo * blocks);
+   int64_t* blockRange = blockMin + (size_t) nTodo * blocks;
+   unsigned long long* maxRange = (unsigned long long*) (blockRange + (size_t) nTodo * blocks);
    uint64_t range[kMaxStagedCols];
    try {
       LDB_CUDA(cudaMemsetAsync(maxRange, 0, (size_t) nTodo * 8, s));
       for (int k = 0; k < nTodo; k++) {
          const bool isI32 = t->columns[todo[k]].type != LDB_DECIMAL128;
-         launchEncodeRange((const uint8_t*) b.data[todo[k]], isI32, rows, blockMin + (size_t) k * blocks, maxRange + k, s);
+         launchEncodeRange((const uint8_t*) b.data[todo[k]], isI32, rows, blockMin + (size_t) k * blocks, blockRange + (size_t) k * blocks, maxRange + k, s);
          LDB_CUDA(cudaGetLastError());
       }
       LDB_CUDA(cudaMemcpyAsync(range, maxRange, (size_t) nTodo * 8, cudaMemcpyDeviceToHost, s));
@@ -147,7 +152,8 @@ bool ldb_gpu_encode_batch_internal(LdbContext* ctx, LdbTable* t, LdbBatch& b, co
             continue;
          }
          const bool isI32 = t->columns[todo[k]].type != LDB_DECIMAL128;
-         launchEncodePack((const uint8_t*) b.data[todo[k]], isI32, rows, blockMin + (size_t) k * blocks, width, tileRows, (uint8_t*) data, s);
+         launchEncodePack((const uint8_t*) b.data[todo[k]], isI32, rows, blockMin + (size_t) k * blocks, blockRange + (size_t) k * blocks, width, tileRows,
+                          (uint8_t*) data, s);
          LDB_CUDA(cudaGetLastError());
          ctx->encodeLaunches++;
          e.data = (uint8_t*) data;

@@ -22,6 +22,7 @@
 #include <map>
 #include <mutex>
 #include <string>
+#include <type_traits>
 
 namespace ldb {
 
@@ -57,7 +58,7 @@ struct GlobalTile {
       else return lo64(col, lr) >> 63;
    }
 };
-// Encoded layout (kernels.h kEncodeTileHeader): a column tile is {base of its block, 0} followed by the tile's values packed in W
+// Encoded layout (kernels.h kEncodeTileHeader): a column tile is {base of its block, max - base} followed by the tile's values packed in W
 // bytes each.  A value is base + the zero-extended field; width and base are uniform per column and tile, so the decode is a
 // shared load of the 32-bit word holding the field, a shift, a mask and an add.  Values come back exactly, so filters, group ids
 // and aggregates run unchanged on them.
@@ -73,12 +74,15 @@ struct SmemTile<kDecEncoded> {
    __device__ __forceinline__ int32_t i32(int col, int lr) const { // int32 columns are encoded in at most 4 bytes
       return (int32_t) ((uint32_t) ldShared32(stage + sc->smemOffset[col]) + field32(col, lr));
    }
-   __device__ __forceinline__ int64_t lo64(int col, int lr) const {
-      const uint32_t h = stage + (uint32_t) sc->smemOffset[col];
-      if (sc->encShift[col] == 3) return (int64_t) ((uint64_t) ldShared64(h) + (uint64_t) ldShared64(h + kEncodeTileHeader + (uint32_t) lr * 8));
-      return (int64_t) ((uint64_t) ldShared64(h) + field32(col, lr));
+   // the zero-extended field of row lr, any W
+   __device__ __forceinline__ uint64_t field(int col, int lr) const {
+      if (sc->encShift[col] == 3) return (uint64_t) ldShared64(stage + (uint32_t) sc->smemOffset[col] + kEncodeTileHeader + (uint32_t) lr * 8);
+      return field32(col, lr);
    }
+   __device__ __forceinline__ int64_t lo64(int col, int lr) const { return (int64_t) ((uint64_t) ldShared64(stage + (uint32_t) sc->smemOffset[col]) + field(col, lr)); }
    __device__ __forceinline__ int64_t hi64(int col, int lr) const { return lo64(col, lr) >> 63; }
+   // the tile header: every value of the tile lies in [base, base + range]
+   __device__ __forceinline__ void header(int col, int64_t& base, int64_t& range) const { ldShared64x2(stage + (uint32_t) sc->smemOffset[col], base, range); }
 };
 template <>
 struct GlobalTile<kDecEncoded> {
@@ -650,6 +654,41 @@ __device__ __forceinline__ i128 evalAggDyn(const AggSpec& a, const int64_t* v, i
    }
 }
 
+// Per-tile 64-bit path of the encoded scan.  Value column c of a tile lies in [lo[c], hi[c]] (its block's min and max, from the
+// tile header).  A product aggregate qualifies when each of its operands lies in [0, 2^31) and the largest product of the bounds is
+// below 2^61: every row's product is then an exact non-negative int64, and maxRow grows to that bound.
+template <class A>
+__device__ __forceinline__ bool aggBound64(const int64_t* lo, const int64_t* hi, int64_t one, uint64_t& maxRow) {
+   if constexpr (A::is64) {
+      return true; // a column sum or a count wraps at 64 bits on every path
+   } else {
+      constexpr int64_t k31 = 1ll << 31;
+      const int64_t xl = lo[A::a], xh = hi[A::a];
+      const int64_t yl = A::expr == LDB_EXPR_MUL ? lo[A::b] : one - hi[A::b], yh = A::expr == LDB_EXPR_MUL ? hi[A::b] : one - lo[A::b];
+      bool ok = xl >= 0 && xh < k31 && yl >= 0 && yh < k31;
+      uint64_t m = (uint64_t) xh * (uint64_t) yh; // < 2^62 when ok
+      if constexpr (A::expr == LDB_EXPR_MUL_1MINUS_1PLUS) {
+         const int64_t zl = one + lo[A::c], zh = one + hi[A::c];
+         ok &= zl >= 0 && zh < k31;
+         ok &= __umul64hi(m, (uint64_t) zh) == 0;
+         m *= (uint64_t) zh;
+      }
+      ok &= m < (1ull << 61);
+      if (m > maxRow) maxRow = m;
+      return ok;
+   }
+}
+// the aggregate's value for one row of a tile that aggBound64 admitted
+template <class A>
+__device__ __forceinline__ int64_t evalAgg64(const int64_t* v, int64_t one) {
+   auto u32 = [](int64_t x) { return (uint64_t) (uint32_t) x; };
+   if constexpr (A::expr == LDB_EXPR_COL) return v[A::a];
+   else if constexpr (A::expr == LDB_EXPR_MUL) return (int64_t) (u32(v[A::a]) * u32(v[A::b]));
+   else if constexpr (A::expr == LDB_EXPR_MUL_1MINUS) return (int64_t) (u32(v[A::a]) * u32(one - v[A::b]));
+   else if constexpr (A::expr == LDB_EXPR_MUL_1MINUS_1PLUS) return (int64_t) (u32(v[A::a]) * u32(one - v[A::b]) * u32(one + v[A::c]));
+   else return 1;
+}
+
 // compile-time aggregate list: every index below is a constant after inlining, so v[]/acc[] live in registers
 template <int... Is>
 struct Seq {};
@@ -668,6 +707,22 @@ struct Aggs {
       ((v[Is] = evalAgg<As, FAST>(vals, one)), ...);
    }
    static __device__ __forceinline__ bool fits32(const int64_t* vals, int64_t one) { return ((aggOperandBits<As>(vals, one) | ...) >> 31) == 0; }
+   static __device__ __forceinline__ bool bound64(const int64_t* lo, const int64_t* hi, int64_t one, uint64_t& maxRow) {
+      return (aggBound64<As>(lo, hi, one, maxRow) & ...);
+   }
+   template <int... Is>
+   static __device__ __forceinline__ void eval64(int64_t* q, const int64_t* vals, int64_t one, Seq<Is...>) {
+      ((q[Is] = evalAgg64<As>(vals, one)), ...);
+   }
+   // 64-bit aggregates add into acc as always, the products of the i128 ones into acc64 (folded into acc by fold64)
+   template <int... Is>
+   static __device__ __forceinline__ void accumulate64(i128* acc, int64_t* acc64, const int64_t* q, Seq<Is...>) {
+      ((As::is64 ? (void) (acc[Is].lo += (uint64_t) q[Is]) : (void) (acc64[Is] += q[Is])), ...);
+   }
+   template <int... Is>
+   static __device__ __forceinline__ void fold64(i128* acc, int64_t* acc64, Seq<Is...>) {
+      ((As::is64 ? (void) 0 : (void) (acc[Is] = add128(acc[Is], i128{(uint64_t) acc64[Is], 0}), acc64[Is] = 0)), ...);
+   }
    template <int... Is>
    static __device__ __forceinline__ void accumulate(i128* acc, const i128* v, Seq<Is...>) {
       ((As::is64 ? (void) (acc[Is].lo += v[Is].lo) : (void) (acc[Is] = add128(acc[Is], v[Is]))), ...);
@@ -747,7 +802,11 @@ extern __shared__ __align__(128) uint8_t dynSmem[];
 // reference's 1024-slot per-worker pre-aggregation cache (PreAggregationHashtable.cpp:46-60) collapses to
 // this for small domains; further groups use shared-memory atomics, and only a CTA that meets
 // more than LG groups touches the HBM table per row.  One flush per CTA at the end.
-template <int DB, bool IN, int NK, int NV, class... As>
+// Encoded full tiles (DB == kDecEncoded) with a shaped filter take their own path: the launcher stages value columns first, then the
+// keys, then the filter's column (launchGB), so their layout is read from the parameter block at constant offsets; each column's tile header is
+// loaded once per tile; and a tile whose header bounds prove every product a non-negative int64 below 2^61 (aggBound64) skips the
+// per-row 32-bit vote and sums those products in 64-bit registers (acc64).
+template <int DB, bool IN, int FS, int NK, int NV, class... As>
 __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_constant__ GroupByParams p) {
    using AL = Aggs<As...>;
    constexpr int N = AL::N;
@@ -777,10 +836,17 @@ __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_cons
    __syncthreads();
 
    i128 acc[GREG][N];
+   // products of the i128 aggregates from proven tiles; `room` is what every acc64 can still take (the same in every thread: a thread
+   // adds at most kRowsPerThreadScan rows of a tile, each at most the tile's maxRow), so acc64 never exceeds INT64_MAX
+   int64_t acc64[GREG][N];
+   int64_t room = INT64_MAX;
 #pragma unroll
    for (int g = 0; g < GREG; g++)
 #pragma unroll
-      for (int a = 0; a < N; a++) acc[g][a] = i128{0, 0};
+      for (int a = 0; a < N; a++) {
+         acc[g][a] = i128{0, 0};
+         acc64[g][a] = 0;
+      }
    const int64_t one = 100; // 10^scale of decimal(12,2); checked on the host
    // keys of the register-resident groups live in registers too (refreshed when the CTA registers a new key)
    int32_t rk0[GREG], rk1[GREG];
@@ -788,14 +854,8 @@ __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_cons
 #pragma unroll
    for (int g = 0; g < GREG; g++) rk0[g] = rk1[g] = 0;
 
-   forEachRowUniform<kRowsPerThreadScan, DB>(p.src.cols, p.src.nRows, dynSmem, bars, [&](const auto& tile, int lr, int64_t row, bool valid) {
-      int64_t vals[NV];
-#pragma unroll
-      for (int c = 0; c < NV; c++) vals[c] = tile.lo64(p.valueStage[c], lr);
-      int32_t k0 = 0, k1 = 0;
-      if constexpr (NK > 0) k0 = tile.i32(p.keyStage[0], lr);
-      if constexpr (NK > 1) k1 = tile.i32(p.keyStage[1], lr);
-      const bool pass = valid & evalFilters<IN>(p.src.filters, tile, lr, row);
+   // CTA-local group id of a row's keys (warp-collective: every lane calls it)
+   auto groupOf = [&](int32_t k0, int32_t k1, bool pass) {
       int id = 0;
       if constexpr (NK > 0) {
          // Resolve the CTA-local group id under WARP-UNIFORM control flow.  (A per-lane spin lock
@@ -858,11 +918,9 @@ __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_cons
             }
          }
       }
-      // expressions: 32-bit multiplies when every lane's operands allow it, else the general i128 path
-      i128 v[N];
-      if (__all_sync(0xffffffffu, !pass || AL::fits32(vals, one))) AL::template eval<true>(v, vals, one, typename AL::S{});
-      else AL::template eval<false>(v, vals, one, typename AL::S{});
-      if (!pass) return;
+      return id;
+   };
+   auto add = [&](int id, const i128* v, int32_t k0, int32_t k1) {
       if (id >= 0 && id < GREG) {
 #pragma unroll
          for (int g = 0; g < GREG; g++)
@@ -874,9 +932,108 @@ __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_cons
          int slot = groupLookupOrInsert(p.table, kk);
          if (slot >= 0) AL::globalAdd(p.table, slot, v, typename AL::S{});
       }
+   };
+   auto generalRow = [&](const auto& tile, int lr, int64_t row, bool valid) {
+      int64_t vals[NV];
+#pragma unroll
+      for (int c = 0; c < NV; c++) vals[c] = tile.lo64(p.valueStage[c], lr);
+      int32_t k0 = 0, k1 = 0;
+      if constexpr (NK > 0) k0 = tile.i32(p.keyStage[0], lr);
+      if constexpr (NK > 1) k1 = tile.i32(p.keyStage[1], lr);
+      const bool pass = valid & evalFilters<IN, FS>(p.src.filters, tile, lr, row);
+      const int id = groupOf(k0, k1, pass);
+      // expressions: 32-bit multiplies when every lane's operands allow it, else the general i128 path
+      i128 v[N];
+      if (__all_sync(0xffffffffu, !pass || AL::fits32(vals, one))) AL::template eval<true>(v, vals, one, typename AL::S{});
+      else AL::template eval<false>(v, vals, one, typename AL::S{});
+      if (pass) add(id, v, k0, k1);
+   };
+   auto encodedTile = [&](const SmemTile<kDecEncoded>& tile, int64_t rowBase) {
+      const StagedCols& sc = p.src.cols;
+      constexpr int FC = NV + NK; // staged index of a shaped filter's column
+      int64_t vb[NV], lo[NV], hi[NV];
+#pragma unroll
+      for (int c = 0; c < NV; c++) {
+         int64_t range;
+         tile.header(c, vb[c], range);
+         // a column with a wide range or base gets bounds no operand test passes (and no bound arithmetic overflows)
+         const bool small = (uint64_t) range < (1ull << 31) && vb[c] > -(1ll << 40) && vb[c] < (1ll << 40);
+         lo[c] = small ? vb[c] : -(1ll << 62);
+         hi[c] = small ? vb[c] + range : (1ll << 62);
+      }
+      uint32_t kb[NK > 0 ? NK : 1], fb = 0;
+#pragma unroll
+      for (int k = 0; k < NK; k++) kb[k] = (uint32_t) ldShared32(tile.stage + (uint32_t) sc.smemOffset[NV + k]);
+      if constexpr (FS == FS_I32_ONE || FS == FS_I32_RANGE) fb = (uint32_t) ldShared32(tile.stage + (uint32_t) sc.smemOffset[FC]);
+      uint64_t maxRow = 0;
+      const bool proven = AL::bound64(lo, hi, one, maxRow);
+      if (proven) {
+         const int64_t need = (int64_t) maxRow * kRowsPerThreadScan;
+         if (need > room) {
+#pragma unroll
+            for (int g = 0; g < GREG; g++) AL::fold64(acc[g], acc64[g], typename AL::S{});
+            room = INT64_MAX;
+         }
+         room -= need;
+      }
+#pragma unroll
+      for (int j = 0; j < kRowsPerThreadScan; j++) {
+         const int lr = j * kBlock + threadIdx.x;
+         int64_t vals[NV];
+#pragma unroll
+         for (int c = 0; c < NV; c++) vals[c] = (int64_t) ((uint64_t) vb[c] + tile.field(c, lr));
+         int32_t k0 = 0, k1 = 0;
+         if constexpr (NK > 0) k0 = (int32_t) (kb[0] + tile.field32(NV, lr));
+         if constexpr (NK > 1) k1 = (int32_t) (kb[1] + tile.field32(NV + 1, lr));
+         bool pass;
+         if constexpr (FS == FS_I32_ONE || FS == FS_I32_RANGE) {
+            const FilterCol& f = p.src.filters.c[0];
+            const int32_t x = (int32_t) (fb + tile.field32(FC, lr));
+            pass = cmpMask32(x, (int32_t) f.valA, f.maskA);
+            if constexpr (FS == FS_I32_RANGE) pass &= cmpMask32(x, (int32_t) f.valB, f.maskB);
+         } else {
+            pass = evalFilters<IN, FS>(p.src.filters, tile, lr, rowBase + lr);
+         }
+         const int id = groupOf(k0, k1, pass);
+         if (proven) {
+            int64_t q[N];
+            AL::eval64(q, vals, one, typename AL::S{});
+            if (!pass) continue;
+            if (id >= 0 && id < GREG) {
+#pragma unroll
+               for (int g = 0; g < GREG; g++)
+                  if (id == g) AL::accumulate64(acc[g], acc64[g], q, typename AL::S{});
+            } else {
+               i128 v[N];
+#pragma unroll
+               for (int a = 0; a < N; a++) v[a] = i128{(uint64_t) q[a], 0}; // what evalAgg gives: products are >= 0 here
+               add(id, v, k0, k1);
+            }
+         } else {
+            i128 v[N];
+            if (__all_sync(0xffffffffu, !pass || AL::fits32(vals, one))) AL::template eval<true>(v, vals, one, typename AL::S{});
+            else AL::template eval<false>(v, vals, one, typename AL::S{});
+            if (pass) add(id, v, k0, k1);
+         }
+      }
+   };
+   forEachTileUniform<kRowsPerThreadScan, DB>(p.src.cols, p.src.nRows, dynSmem, bars, [&](const auto& tile, int64_t rowBase, int rows) {
+      // the descriptor-driven filter costs more per row than the tile path saves (Q6 measured slower), so it keeps the row path
+      if constexpr (std::is_same_v<std::decay_t<decltype(tile)>, SmemTile<kDecEncoded>> && FS != FS_GENERIC) {
+         encodedTile(tile, rowBase);
+      } else {
+#pragma unroll
+         for (int j = 0; j < kRowsPerThreadScan; j++) {
+            const int lr = j * kBlock + threadIdx.x;
+            const bool valid = lr < rows;
+            generalRow(tile, valid ? lr : 0, rowBase + (valid ? lr : 0), valid);
+         }
+      }
    });
    // ---- flush: registers → warp sums → shared → one HBM atomic per (CTA, group, aggregate)
    __syncthreads();
+#pragma unroll
+   for (int g = 0; g < GREG; g++) AL::fold64(acc[g], acc64[g], typename AL::S{});
    const int lane = threadIdx.x & 31;
 #pragma unroll
    for (int g = 0; g < GREG; g++) AL::warpFlush(sAcc[g], acc[g], lane, typename AL::S{});
@@ -939,28 +1096,69 @@ static bool hasInList(const FilterSet& f) { // "rare" filters: IN lists and LIKE
       if (f.c[i].nIn > 0 || f.c[i].kind == COL_UTF8_CONTAINS) return true;
    return false;
 }
-template <int DB, bool IN, int NK, int NV, class... As>
+template <int DB, bool IN, int FS, int NK, int NV, class... As>
 static void launchGBd(const GroupByParams& p, int smCount, cudaStream_t s) {
    size_t dyn;
-   int grid = persistentGrid(scanGroupByKernel<DB, IN, NK, NV, As...>, p.src.cols, p.src.nRows, smCount, &dyn, kBlock);
-   scanGroupByKernel<DB, IN, NK, NV, As...><<<grid, kBlock, dyn, s>>>(p);
+   int grid = persistentGrid(scanGroupByKernel<DB, IN, FS, NK, NV, As...>, p.src.cols, p.src.nRows, smCount, &dyn, kBlock);
+   scanGroupByKernel<DB, IN, FS, NK, NV, As...><<<grid, kBlock, dyn, s>>>(p);
 }
-// ENC: the signature is also compiled for the encoded layout (only without IN lists; scanGroupByEncodable says which)
-template <bool ENC, int NK, int NV, class... As>
+// The encoded instance reads its columns' layout at constant indices: value column c is staged column c, key k is NV + k, and a
+// shaped filter's column is NV + NK.  Permutes the staged columns (and every index into them) into that order; returns the filter
+// shape the permuted parameters can run under.  Keys and values are distinct staged columns (scanGroupByEncodable).
+static int toSignatureOrder(GroupByParams& p) {
+   const StagedCols src = p.src.cols;
+   int order[kMaxStagedCols], pos[kMaxStagedCols], n = 0;
+   auto place = [&](int c) {
+      for (int i = 0; i < n; i++)
+         if (order[i] == c) return;
+      order[n++] = c;
+   };
+   for (int v = 0; v < p.nValueCols; v++) place(p.valueStage[v]);
+   for (int k = 0; k < p.nKeys; k++) place(p.keyStage[k]);
+   if (p.src.filters.n > 0 && p.src.filters.c[0].staged >= 0) place(p.src.filters.c[0].staged);
+   for (int c = 0; c < src.n; c++) place(c);
+   StagedCols& sc = p.src.cols;
+   for (int i = 0; i < n; i++) {
+      pos[order[i]] = i;
+      sc.base[i] = src.base[order[i]];
+      sc.elemBytes[i] = src.elemBytes[order[i]];
+      sc.smemOffset[i] = src.smemOffset[order[i]];
+      sc.encShift[i] = src.encShift[order[i]];
+      sc.encMask[i] = src.encMask[order[i]];
+   }
+   for (int v = 0; v < p.nValueCols; v++) p.valueStage[v] = pos[p.valueStage[v]];
+   for (int k = 0; k < p.nKeys; k++) p.keyStage[k] = pos[p.keyStage[k]];
+   for (int f = 0; f < p.src.filters.n; f++)
+      if (p.src.filters.c[f].staged >= 0) p.src.filters.c[f].staged = pos[p.src.filters.c[f].staged];
+   const int fs = filterShape(p.src.filters);
+   if ((fs == FS_I32_ONE || fs == FS_I32_RANGE) && p.src.filters.c[0].staged != p.nValueCols + p.nKeys) return FS_GENERIC; // e.g. a filter on a key
+   return fs;
+}
+// ENC: the signature is also compiled for the encoded layout (only without IN lists; scanGroupByEncodable says which); ENC_ONE: and
+// for the one-int32-constant filter shape (Q1's l_shipdate <= date), otherwise the encoded instance evaluates the filter descriptor
+template <bool ENC, bool ENC_ONE, int NK, int NV, class... As>
 static void launchGB(const GroupByParams& p, int smCount, cudaStream_t s) {
    const bool in = hasInList(p.src.filters);
    if constexpr (ENC) {
       if (p.src.cols.decBytes == kDecEncoded) {
-         launchGBd<kDecEncoded, false, NK, NV, As...>(p, smCount, s);
+         GroupByParams q = p;
+         const int fs = toSignatureOrder(q);
+         if constexpr (ENC_ONE) {
+            if (fs == FS_I32_ONE) {
+               launchGBd<kDecEncoded, false, FS_I32_ONE, NK, NV, As...>(q, smCount, s);
+               return;
+            }
+         }
+         launchGBd<kDecEncoded, false, FS_GENERIC, NK, NV, As...>(q, smCount, s);
          return;
       }
    }
    if (p.src.cols.decBytes == 8) {
-      if (in) launchGBd<8, true, NK, NV, As...>(p, smCount, s);
-      else launchGBd<8, false, NK, NV, As...>(p, smCount, s);
+      if (in) launchGBd<8, true, FS_GENERIC, NK, NV, As...>(p, smCount, s);
+      else launchGBd<8, false, FS_GENERIC, NK, NV, As...>(p, smCount, s);
    } else {
-      if (in) launchGBd<16, true, NK, NV, As...>(p, smCount, s);
-      else launchGBd<16, false, NK, NV, As...>(p, smCount, s);
+      if (in) launchGBd<16, true, FS_GENERIC, NK, NV, As...>(p, smCount, s);
+      else launchGBd<16, false, FS_GENERIC, NK, NV, As...>(p, smCount, s);
    }
 }
 using C0 = Agg<LDB_EXPR_COL, 0>;
@@ -972,7 +1170,15 @@ static const char* const kSigQ1 = "k2v4|0:0|0:1|2:1,2|3:1,2,3|0:2|4";
 static const char* const kSigQ6 = "k0v2|1:0,1";
 bool scanGroupByEncodable(const GroupByParams& p) {
    const std::string sig = signature(p);
-   return (sig == kSigQ1 || sig == kSigQ6) && !hasInList(p.src.filters);
+   if ((sig != kSigQ1 && sig != kSigQ6) || hasInList(p.src.filters)) return false;
+   // the encoded instance stages every key and value column once (toSignatureOrder)
+   int stage[kMaxKeys + kMaxValueCols], n = 0;
+   for (int k = 0; k < p.nKeys; k++) stage[n++] = p.keyStage[k];
+   for (int v = 0; v < p.nValueCols; v++) stage[n++] = p.valueStage[v];
+   for (int i = 0; i < n; i++)
+      for (int j = 0; j < i; j++)
+         if (stage[i] == stage[j]) return false;
+   return true;
 }
 bool launchScanGroupBy(const GroupByParams& p, int smCount, cudaStream_t s, const char** why) {
    std::string sig = signature(p);
@@ -982,23 +1188,23 @@ bool launchScanGroupBy(const GroupByParams& p, int smCount, cudaStream_t s, cons
    }
    // Q1 pricing summary: sum(a) sum(b) sum(b*(1-c)) sum(b*(1-c)*(1+d)) sum(c) count   (resources/sql/tpch/1.sql)
    if (sig == kSigQ1) {
-      launchGB<true, 2, 4, C0, C1, Agg<LDB_EXPR_MUL_1MINUS, 1, 2>, Agg<LDB_EXPR_MUL_1MINUS_1PLUS, 1, 2, 3>, C2, ONE>(p, smCount, s);
+      launchGB<true, true, 2, 4, C0, C1, Agg<LDB_EXPR_MUL_1MINUS, 1, 2>, Agg<LDB_EXPR_MUL_1MINUS_1PLUS, 1, 2, 3>, C2, ONE>(p, smCount, s);
    } else if (sig == "k1v4|0:0|0:1|2:1,2|3:1,2,3|0:2|4") {
-      launchGB<false, 1, 4, C0, C1, Agg<LDB_EXPR_MUL_1MINUS, 1, 2>, Agg<LDB_EXPR_MUL_1MINUS_1PLUS, 1, 2, 3>, C2, ONE>(p, smCount, s);
+      launchGB<false, false, 1, 4, C0, C1, Agg<LDB_EXPR_MUL_1MINUS, 1, 2>, Agg<LDB_EXPR_MUL_1MINUS_1PLUS, 1, 2, 3>, C2, ONE>(p, smCount, s);
    } else if (sig == kSigQ6) { // Q6 forecast revenue: sum(a*b)
-      launchGB<true, 0, 2, Agg<LDB_EXPR_MUL, 0, 1>>(p, smCount, s);
+      launchGB<true, false, 0, 2, Agg<LDB_EXPR_MUL, 0, 1>>(p, smCount, s);
    } else if (sig == "k0v2|2:0,1") { // keyless sum(a*(1-b))
-      launchGB<false, 0, 2, Agg<LDB_EXPR_MUL_1MINUS, 0, 1>>(p, smCount, s);
+      launchGB<false, false, 0, 2, Agg<LDB_EXPR_MUL_1MINUS, 0, 1>>(p, smCount, s);
    } else if (sig == "k0v1|0:0|4") { // keyless sum(a), count
-      launchGB<false, 0, 1, C0, ONE>(p, smCount, s);
+      launchGB<false, false, 0, 1, C0, ONE>(p, smCount, s);
    } else if (sig == "k1v2|2:0,1") { // group by k: sum(a*(1-b))
-      launchGB<false, 1, 2, Agg<LDB_EXPR_MUL_1MINUS, 0, 1>>(p, smCount, s);
+      launchGB<false, false, 1, 2, Agg<LDB_EXPR_MUL_1MINUS, 0, 1>>(p, smCount, s);
    } else if (sig == "k2v2|2:0,1") {
-      launchGB<false, 2, 2, Agg<LDB_EXPR_MUL_1MINUS, 0, 1>>(p, smCount, s);
+      launchGB<false, false, 2, 2, Agg<LDB_EXPR_MUL_1MINUS, 0, 1>>(p, smCount, s);
    } else if (sig == "k1v1|0:0|4") { // group by k: sum(a), count
-      launchGB<false, 1, 1, C0, ONE>(p, smCount, s);
+      launchGB<false, false, 1, 1, C0, ONE>(p, smCount, s);
    } else if (sig == "k2v1|0:0|4") {
-      launchGB<false, 2, 1, C0, ONE>(p, smCount, s);
+      launchGB<false, false, 2, 1, C0, ONE>(p, smCount, s);
    } else {
       static thread_local std::string msg;
       msg = "no compiled group-by pipeline for aggregate signature '" + sig + "' (register it in kernels.cu:launchScanGroupBy)";

@@ -102,8 +102,8 @@ void setTuning(const Tuning& t);
 // Per column one width W in {1, 2, 4, 8} bytes; per block of kEncodeBlockRows rows a base (the block minimum, int64); a value is
 // stored as (v - base) in W bytes, zero-extended on decode (exact modulo 2^64, so int32 columns and the low 8 bytes of a
 // decimal(p<19) cell come back bit for bit).  The copy is TILE-FRAMED for the K1/K2 tile of kEncodeTileRows rows: tile t of a
-// column starts at t * (kEncodeTileHeader + kEncodeTileRows * W) with a 16-byte header {base of the tile's block, 0} followed by
-// the tile's packed values.  One bulk copy then brings a tile's base with its values, and no thread loads a base from HBM.
+// column starts at t * (kEncodeTileHeader + kEncodeTileRows * W) with a 16-byte header {base of the tile's block, max - min of that
+// block} followed by the tile's packed values.  One bulk copy then brings a tile's base with its values, and no thread loads a base from HBM.
 constexpr int64_t kEncodeBlockRows = 65536; // = kPackBlockRows of the compressed staging format: a tile never straddles two blocks
 constexpr int kEncodeTileHeader = 16;
 constexpr int kDecEncoded = 0; // StagedCols::decBytes / kernel DB parameter of the encoded layout
@@ -271,10 +271,12 @@ bool launchScanGroupBy(const GroupByParams& p, int smCount, cudaStream_t s, cons
 // true when launchScanGroupBy has an instantiation of p's signature for the encoded layout (p.src.cols need not be bound yet)
 bool scanGroupByEncodable(const GroupByParams& p);
 // encoder (encode.cu).  A source column is `n` int32 cells (isI32) or decimal128 cells of which the low 8 bytes are taken.
-// Range pass: blockMin[b] = minimum of block b, *maxRange = max over blocks of (max - min) as unsigned (caller zeroes it).
-void launchEncodeRange(const uint8_t* src, bool isI32, int64_t n, int64_t* blockMin, unsigned long long* maxRange, cudaStream_t s);
+// Range pass: blockMin[b] = minimum of block b, blockRange[b] = its max - min, *maxRange = max over blocks of (max - min) as unsigned
+// (caller zeroes it).
+void launchEncodeRange(const uint8_t* src, bool isI32, int64_t n, int64_t* blockMin, int64_t* blockRange, unsigned long long* maxRange, cudaStream_t s);
 // Pack pass: writes the tile-framed copy (kernels.h, kEncodeTileHeader) of width `width` for tiles of `tileRows` rows
-void launchEncodePack(const uint8_t* src, bool isI32, int64_t n, const int64_t* blockMin, int width, int tileRows, uint8_t* dst, cudaStream_t s);
+void launchEncodePack(const uint8_t* src, bool isI32, int64_t n, const int64_t* blockMin, const int64_t* blockRange, int width, int tileRows, uint8_t* dst,
+                      cudaStream_t s);
 void launchScanBuild(const BuildParams& p, int smCount, cudaStream_t s);
 bool launchScanProbeAgg(const ProbeAggParams& p, int smCount, cudaStream_t s, const char** why);
 bool launchScanProbe2GroupBy(const Probe2GroupByParams& p, int smCount, cudaStream_t s, const char** why);
