@@ -185,6 +185,8 @@ SIGNATURES = {
     "ldb_gpu_table_column_range": (C.c_int, [_P, C.c_char_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), _E]),
     "ldb_gpu_join_table_create_keys": (C.c_int, [_P, C.c_int32, C.c_int64, C.c_int32, C.POINTER(_P), _E]),
     "ldb_gpu_join_table_count": (C.c_int, [_P, C.POINTER(C.c_int64), _E]),
+    "ldb_gpu_join_table_marks": (C.c_int, [_P, C.c_int32, C.c_char_p, C.POINTER(_P), _E]),
+    "ldb_gpu_join_table_clear_marks": (C.c_int, [_P, _E]),
     "ldb_gpu_join_table_bloom": (C.c_int, [_P, C.POINTER(_P), C.POINTER(C.c_int64), _E]),
     "ldb_gpu_join_table_topk": (C.c_int, [_P, C.c_int32, C.POINTER(TopKRow), C.POINTER(C.c_int32), _E]),
     "ldb_gpu_run_pipeline": (C.c_int, [_P, C.POINTER(PipelineDesc), _E]),

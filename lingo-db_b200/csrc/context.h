@@ -314,6 +314,8 @@ struct LdbState {
    bool selfTimed = false; // created inside a captured query: its scan kernel's self-measured time is harvested at read
    uint32_t is64Mask = 0;   // aggregates that are 64-bit sums (COL / ONE): normalised to a sign-extended i64 on read
    uint32_t laneBound = 0;  // aggregates whose width (64 / 128 bits) a pipeline fixed already: a later one must agree
+   uint8_t* marks = nullptr; // JOIN_TABLE / KEY_JOIN: one marker byte per directory slot (program.h), from the first program that marks
+                             // the table; also in `allocations`
    std::vector<void*> allocations;
 };
 

@@ -506,7 +506,9 @@ __device__ void hashAggUpdate(const ProgramParams& p, uint8_t* e, const Val* reg
 // KeyTuples: the instance that also reads and builds key-tuple join tables.  Programs without one run the instance that has none of
 // that code: even an untaken key-tuple build call in the sink made the plain-table build kernel four times slower (register allocation
 // and scheduling of the whole loop change with it).
-template <bool KeyTuples>
+// Marks: the instance that also runs LDB_OP_MARK and records, per table, the slot the latest PROBE / PROBE_EACH matched.  For the
+// same reason only programs with a MARK run it; with Marks false none of that code is compiled in.
+template <bool KeyTuples, bool Marks>
 __global__ void __launch_bounds__(256) programKernel(const __grid_constant__ ProgramParams p) {
    unsigned long long inserted = 0;
    for (int64_t base = (int64_t) blockIdx.x * blockDim.x; base < p.nRows; base += (int64_t) gridDim.x * blockDim.x) {
@@ -522,6 +524,10 @@ __global__ void __launch_bounds__(256) programKernel(const __grid_constant__ Pro
       uint64_t eachSlot = 0;
       uint32_t eachProbes = 0;
       KeyCursor eachCur{}; // key-tuple tables
+      // Marks: the directory slot of the entry the latest PROBE / PROBE_EACH of tables[k] matched for this tuple (kNoSlot: none)
+      uint64_t hitSlot[Marks ? kProgMaxTables : 1];
+      if (Marks)
+         for (int k = 0; k < kProgMaxTables; k++) hitSlot[k] = kNoSlot;
       while (true) {
          bool pass = false;
          if (pending) {
@@ -627,6 +633,7 @@ __global__ void __launch_bounds__(256) programKernel(const __grid_constant__ Pro
                   case LDB_OP_PROBE: { // key → payload of a unique/multimap single-key table; absent key = NULL (semi / anti / mark / outer)
                      const JoinTableDev& t = p.tables[in.arg];
                      r.null = true;
+                     if (Marks) hitSlot[in.arg] = kNoSlot;
                      if (KeyTuples && p.keyTables[in.arg].nKeys) { // key-tuple table: the keys are registers a .. a + nKeys - 1
                         KeyTuple keys;
                         if (!gatherTuple(regs, p.keyTables[in.arg].nKeys, [&](int k) { return in.a + k; }, keys)) { // NULL / past int64: no match
@@ -634,6 +641,7 @@ __global__ void __launch_bounds__(256) programKernel(const __grid_constant__ Pro
                            const KeyHit h = c.live ? keyJoinNext(p.keyTables[in.arg], keys, c) : KeyHit{c, 0, false};
                            r.v = h.payload;
                            r.null = !h.hit;
+                           if (Marks && h.hit) hitSlot[in.arg] = (h.next.slot - 1) & p.keyTables[in.arg].mask; // the cursor is past the hit
                         }
                      } else if (!a.null && a.v == (s128) (int32_t) a.v) {
                         const int32_t key = (int32_t) a.v;
@@ -642,6 +650,7 @@ __global__ void __launch_bounds__(256) programKernel(const __grid_constant__ Pro
                            if (pay != kDirectEmpty) {
                               r.v = pay;
                               r.null = false;
+                              if (Marks) hitSlot[in.arg] = (uint32_t) key - (uint32_t) t.keyMin;
                            }
                         } else {
                            const uint64_t h = hashI32(key);
@@ -657,6 +666,7 @@ __global__ void __launch_bounds__(256) programKernel(const __grid_constant__ Pro
                               if ((int32_t) (uint32_t) e == key) {
                                  r.v = (s128) (int32_t) ((uint32_t) (e >> 32) & (t.stride == 32 ? 0x7fffffffu : 0xffffffffu));
                                  r.null = false;
+                                 if (Marks) hitSlot[in.arg] = s;
                                  break;
                               }
                               s = (s + 1) & t.mask;
@@ -696,9 +706,13 @@ __global__ void __launch_bounds__(256) programKernel(const __grid_constant__ Pro
                         return h.hit;
                      };
                      r.null = true;
+                     if (Marks) hitSlot[in.arg] = kNoSlot;
                      if (eachState == 1 && (tuple64 ? tupleNext() : probeEachNext(t, eachKey, eachSlot, eachProbes, pay))) {
                         r.v = tuple64 ? pay64 : pay;
                         r.null = false;
+                        if (Marks) // the cursors are past the hit; a direct-address table has one slot per key
+                           hitSlot[in.arg] = tuple64 ? (eachCur.slot - 1) & p.keyTables[in.arg].mask
+                                                     : t.direct ? (uint64_t) ((uint32_t) eachKey - (uint32_t) t.keyMin) : (eachSlot - 1) & t.mask;
                      } else {
                         eachState = 2;
                         pending = false;
@@ -707,7 +721,17 @@ __global__ void __launch_bounds__(256) programKernel(const __grid_constant__ Pro
                      eachEmitted = true;
                      break;
                   }
-                  default: r.null = true;
+                  default:
+                     if (Marks && in.op == LDB_OP_MARK) { // marks the entry the latest probe of tables[arg] matched, when a is TRUE
+                        const uint64_t slot = hitSlot[in.arg];
+                        r.v = !a.null && a.v != 0 && slot != kNoSlot;
+                        if (r.v != 0) { // check, then store: idempotent, and other threads write the byte in the same launch
+                           volatile uint8_t* m = p.marks[in.arg] + slot;
+                           if (*m == 0) *m = 1;
+                        }
+                     } else {
+                        r.null = true;
+                     }
                }
                if (!tuple) break;
                regs[in.dst] = r;
@@ -781,10 +805,72 @@ __global__ void __launch_bounds__(256) programKernel(const __grid_constant__ Pro
 }
 void launchProgram(const ProgramParams& p, int smCount, cudaStream_t s) {
    int grid = (int) std::min<int64_t>(std::max<int64_t>((p.nRows + 255) / 256, 1), (int64_t) smCount * 8);
-   bool keyTuples = p.keyBuild.nKeys != 0;
-   for (int k = 0; k < kProgMaxTables; k++) keyTuples |= p.keyTables[k].nKeys != 0;
-   if (keyTuples) programKernel<true><<<grid, 256, 0, s>>>(p);
-   else programKernel<false><<<grid, 256, 0, s>>>(p);
+   bool keyTuples = p.keyBuild.nKeys != 0, marks = false;
+   for (int k = 0; k < kProgMaxTables; k++) {
+      keyTuples |= p.keyTables[k].nKeys != 0;
+      marks |= p.marks[k] != nullptr;
+   }
+   if (marks) {
+      if (keyTuples) programKernel<true, true><<<grid, 256, 0, s>>>(p);
+      else programKernel<false, true><<<grid, 256, 0, s>>>(p);
+   } else {
+      if (keyTuples) programKernel<true, false><<<grid, 256, 0, s>>>(p);
+      else programKernel<false, false><<<grid, 256, 0, s>>>(p);
+   }
+}
+
+// ---------------------------------------------------------------- join-table markers
+// One thread per directory slot: an occupancy test for the table's kind, the marker test, then a warp-aggregated append (one atomic
+// per warp), as hashAggExportKernel.  Runs after the launches that built and marked the table: plain loads.
+__global__ void __launch_bounds__(256) joinMarksKernel(JoinTableDev t, KeyJoinDev k, const uint8_t* marks, int which, MarkScanOut o, unsigned long long* counter) {
+   const uint64_t slots = k.nKeys ? k.mask + 1 : t.direct ? (uint64_t) t.range : t.mask + 1;
+   const int nKeys = k.nKeys ? k.nKeys : 1;
+   for (uint64_t base = (uint64_t) blockIdx.x * blockDim.x; base < slots; base += (uint64_t) gridDim.x * blockDim.x) {
+      const uint64_t s = base + threadIdx.x;
+      bool occ = false;
+      int64_t key[kProgMaxKeys] = {};
+      int64_t pay = 0;
+      if (s < slots) {
+         if (k.nKeys) {
+            const uint8_t* e = k.base + s * k.entryBytes;
+            const ulonglong2 head = *(const ulonglong2*) e;
+            occ = (uint32_t) head.x == kKeyJoinReady;
+            pay = (int64_t) head.y;
+#pragma unroll
+            for (int j = 0; j < kProgMaxKeys; j++)
+               if (j < k.nKeys) key[j] = ((const int64_t*) (e + 16))[j];
+         } else if (t.direct) {
+            const int32_t v = ((const int32_t*) t.base)[s];
+            occ = v != kDirectEmpty;
+            key[0] = (int64_t) s + t.keyMin;
+            pay = v;
+         } else {
+            const unsigned long long e = *(const unsigned long long*) (t.base + s * t.stride);
+            occ = e != ~0ull;
+            key[0] = (int32_t) (uint32_t) e;
+            pay = (int32_t) (uint32_t) (e >> 32);
+         }
+      }
+      const bool marked = occ && marks && marks[s];
+      const bool take = occ && (which < 0 || (which == 1) == marked);
+      const unsigned m = __ballot_sync(0xffffffffu, take);
+      if (!m) continue;
+      const int lane = threadIdx.x & 31, leader = __ffs(m) - 1;
+      unsigned long long pos = 0;
+      if (lane == leader) pos = atomicAdd(counter, (unsigned long long) __popc(m));
+      pos = __shfl_sync(0xffffffffu, pos, leader) + __popc(m & ((1u << lane) - 1));
+      if (!take || pos >= (unsigned long long) o.capacity) continue;
+#pragma unroll
+      for (int j = 0; j < kProgMaxKeys; j++)
+         if (j < nKeys) o.keyCols[j][pos] = key[j];
+      o.payload[pos] = pay;
+      if (o.marked) o.marked[pos] = marked ? 1 : 0;
+   }
+}
+void launchJoinMarks(const JoinTableDev& t, const KeyJoinDev& k, const uint8_t* marks, int which, const MarkScanOut& o, unsigned long long* counter, int smCount, cudaStream_t s) {
+   const uint64_t slots = k.nKeys ? k.mask + 1 : t.direct ? (uint64_t) t.range : t.mask + 1;
+   const int grid = (int) std::min<uint64_t>((slots + 255) / 256, (uint64_t) smCount * 8);
+   joinMarksKernel<<<grid < 1 ? 1 : grid, 256, 0, s>>>(t, k, marks, which, o, counter);
 }
 
 __global__ void hashAggInitKernel(HashAggDev t) {

@@ -102,7 +102,13 @@ struct KeyJoinDev {
 };
 constexpr uint32_t kKeyJoinWriting = 1u, kKeyJoinReady = 2u;
 
-// The kernel takes ProgramParams by value (__grid_constant__): 3 712 bytes with the limits above, within the classic 4 096-byte
+// Join-table markers (LDB_OP_MARK): one byte per directory slot of a plain single-key table (mask + 1 slots), per key of a
+// direct-address table (range slots) or per entry of a key-tuple table (mask + 1 slots); 0 = unmarked.  Entries never move under open
+// addressing, so a marker stays with its entry while more rows are inserted.  Allocated zeroed by the first program that marks the
+// table, freed with it; a table without markers reads as all unmarked.
+constexpr uint64_t kNoSlot = ~0ull;
+
+// The kernel takes ProgramParams by value (__grid_constant__): 3 744 bytes with the limits above, within the classic 4 096-byte
 // kernel-parameter limit (program_rt.cpp checks it at compile time).
 struct ProgramParams {
    int64_t nRows;
@@ -137,7 +143,20 @@ struct ProgramParams {
    uint8_t* outValid[kProgMaxAggs];
    int64_t outCapacity;
    unsigned long long* outCount;
+   // LDB_OP_MARK: the markers of tables[k] when an instruction marks it, else null.  Last, so that the fields every other instance
+   // reads keep their offsets; any non-null entry selects the kernel instance that has the MARK code.
+   uint8_t* marks[kProgMaxTables];
 };
+// the entries of one join table (a key-tuple table when k.nKeys > 0, else the plain or direct-address table t) selected by their
+// markers: which = 1 marked, 0 unmarked, -1 all (and `marked` gets 0 / 1).  Per selected entry, at a position counted by `counter`:
+// its keys (keyCols[0..n)), its payload, its marker.  Positions at or past `capacity` are counted but not written.
+struct MarkScanOut {
+   int64_t* keyCols[kProgMaxKeys];
+   int64_t* payload;
+   int32_t* marked; // null unless which = -1
+   int64_t capacity;
+};
+void launchJoinMarks(const JoinTableDev& t, const KeyJoinDev& k, const uint8_t* marks, int which, const MarkScanOut& o, unsigned long long* counter, int smCount, cudaStream_t s);
 
 void launchProgram(const ProgramParams& p, int smCount, cudaStream_t s);
 void launchHashAggInit(const HashAggDev& t, int smCount, cudaStream_t s);

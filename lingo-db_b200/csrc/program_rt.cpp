@@ -401,6 +401,7 @@ struct ProgramPlan {
    bool usesRowid = false;
    int eachTable = -1; // tables[] index PROBE_EACH reads
    bool probed[kProgMaxTables] = {}, coded[kProgMaxTables] = {}; // tables[k] read by PROBE / PROBE_EACH, by STRCODE
+   bool marked[kProgMaxTables] = {};                             // tables[k] marked by MARK
    std::vector<LdbState*> dicts, tupleTables; // tupleTables: key-tuple tables whose error word the run may set
 
    ProgramPlan(LdbContext* c, const LdbProgramDesc* desc) : ctx(c), d(desc), t(desc->source) {}
@@ -528,6 +529,12 @@ static void validateInstructions(ProgramPlan& p) {
             p.eachTable = in.arg;
             p.probed[in.arg] = true;
             break;
+         case LDB_OP_MARK:
+            if (in.arg < 0 || in.arg >= d->n_tables) fail(LDB_ERR_INVALID, "MARK: table index out of range");
+            if (!p.probed[in.arg]) fail(LDB_ERR_INVALID, "MARK: no earlier PROBE / PROBE_EACH of the program reads the table it marks");
+            p.wantReg(in.a, "MARK condition");
+            p.marked[in.arg] = true;
+            break;
          default: fail(LDB_ERR_UNSUPPORTED, "unknown opcode " + std::to_string(in.op));
       }
       // the instructions after PROBE_EACH run once per match: they may not overwrite what the first pass left for the next one
@@ -548,12 +555,43 @@ static void validateInstructions(ProgramPlan& p) {
    }
 }
 
+// ---------------------------------------------------------------- join-table markers (program.h)
+// the tables that keep markers: plain single-key, direct-address and key-tuple join tables
+static bool markable(const LdbState* s) {
+   return s && (s->kind == LDB_STATE_KEY_JOIN || (s->kind == LDB_STATE_JOIN_TABLE && (s->join.stride == 8 || s->join.direct)));
+}
+static void checkMarkable(LdbState* s) {
+   if (s->kind != LDB_STATE_JOIN_TABLE && s->kind != LDB_STATE_KEY_JOIN) fail(LDB_ERR_INVALID, "not a join table");
+   if (!markable(s)) fail(LDB_ERR_INVALID, "markers are kept for plain single-key, direct-address and key-tuple join tables (not pair tables or group-join maps)");
+   if (s->ctx->capturing) fail(LDB_ERR_UNSUPPORTED, "join-table markers are not part of captured queries");
+}
+static uint64_t markSlots(const LdbState* s) {
+   if (s->kind == LDB_STATE_KEY_JOIN) return s->keyJoin.mask + 1;
+   return s->join.direct ? (uint64_t) s->join.range : s->join.mask + 1;
+}
+// tables[k] is marked by a MARK instruction: its markers, allocated zeroed on first use
+static void bindMarks(ProgramPlan& p, int k) {
+   LdbState* js = p.d->tables[k];
+   if (!markable(js)) fail(LDB_ERR_INVALID, "MARK takes a plain single-key, direct-address or key-tuple join table (not a pair table, a group-join map or a dictionary)");
+   if (js->ctx != p.ctx) fail(LDB_ERR_INVALID, "MARK: the join table belongs to another context");
+   if (p.d->sink_kind == LDB_SINK_JOIN_BUILD && p.d->sink == js) fail(LDB_ERR_INVALID, "MARK: a program may not mark the join table it builds");
+   if (p.ctx->capturing) fail(LDB_ERR_UNSUPPORTED, "programs with MARK are not part of captured queries");
+   if (!js->marks) {
+      const size_t bytes = std::max<size_t>(markSlots(js), 16);
+      js->marks = (uint8_t*) p.ctx->stagingAlloc(bytes);
+      js->allocations.push_back(js->marks);
+      LDB_CUDA(cudaMemsetAsync(js->marks, 0, bytes, p.ctx->compute));
+   }
+   p.base.marks[k] = js->marks;
+}
+
 // the table slots: plain join tables, key-tuple join tables and string dictionaries
 static void bindTables(ProgramPlan& p) {
    LdbContext* ctx = p.ctx;
    const LdbProgramDesc* d = p.d;
    for (int k = 0; k < d->n_tables; k++) {
       LdbState* js = d->tables[k];
+      if (p.marked[k]) bindMarks(p, k);
       if (js && js->kind == LDB_STATE_KEY_JOIN) {
          if (p.coded[k]) fail(LDB_ERR_INVALID, "STRCODE needs a string dictionary, not a join table");
          p.wantTupleTable(js);
@@ -590,7 +628,7 @@ static void allocOut(ProgramPlan& p, Scratch& out, size_t rows) {
    p.base.outCapacity = (int64_t) rows;
 }
 
-// the filter and the sink: a hash aggregation, a join build (plain or key-tuple table) or materialized rows (buffers in `out`)
+// the filter and the sink: a hash aggregation, a join build (plain or key-tuple table), materialized rows (buffers in `out`) or none
 static void bindSink(ProgramPlan& p, Scratch& out) {
    const LdbProgramDesc* d = p.d;
    ProgramParams& base = p.base;
@@ -644,6 +682,8 @@ static void bindSink(ProgramPlan& p, Scratch& out) {
          base.outReg[c] = d->out_regs[c];
       }
       allocOut(p, out, (size_t) std::max<int64_t>(p.t->numRows, 1));
+   } else if (d->sink_kind == LDB_SINK_NONE) { // effects only (MARK, STRCODE inserts)
+      if (sink) fail(LDB_ERR_INVALID, "LDB_SINK_NONE takes no sink state (sink must be NULL)");
    } else {
       fail(LDB_ERR_INVALID, "unknown sink kind");
    }
@@ -783,6 +823,63 @@ int ldb_gpu_run_program(LdbContext* ctx, const LdbProgramDesc* d, LdbError* err)
 }
 int ldb_gpu_run_program_ex(LdbContext* ctx, const LdbProgramDesc* d, const LdbProgramJoins* joins, LdbError* err) {
    return guarded(err, [&] { runProgram(ctx, d, joins); });
+}
+
+// ---------------------------------------------------------------- join-table markers
+int ldb_gpu_join_table_marks(LdbState* s, int32_t which, const char* name, LdbTable** out, LdbError* err) {
+   return guarded(err, [&] {
+      if (!s || !out) fail(LDB_ERR_INVALID, "null argument");
+      if (which < -1 || which > 1) fail(LDB_ERR_INVALID, "which is 1 (marked entries), 0 (unmarked entries) or -1 (all entries and a marked column)");
+      checkMarkable(s);
+      LdbContext* ctx = s->ctx;
+      LDB_CUDA(cudaSetDevice(ctx->device));
+      int64_t n = 0;
+      LdbError e;
+      if (ldb_gpu_join_table_count(s, &n, &e) != LDB_OK) fail(e.code, e.message); // the table's error word first
+      const bool tuple = s->kind == LDB_STATE_KEY_JOIN;
+      const int nKeys = tuple ? s->keyJoin.nKeys : 1;
+      const size_t rows = (size_t) std::max<int64_t>(n, 1);
+      Scratch cols(ctx), scratch(ctx);
+      MarkScanOut o{};
+      std::vector<LdbColumn> columns;
+      LdbBatch b;
+      auto add = [&](const std::string& column, int32_t type, void* data, int32_t elemBytes) {
+         columns.push_back({column, type, 0, 0});
+         b.data.push_back(data);
+         b.bytes.push_back(nullptr);
+         b.elemBytes.push_back(elemBytes);
+         b.validBytes.push_back(nullptr);
+      };
+      for (int k = 0; k < nKeys; k++) {
+         o.keyCols[k] = cols.alloc<int64_t>(rows * 8);
+         add(tuple ? "k" + std::to_string(k) : "key", LDB_INT64, o.keyCols[k], 8);
+      }
+      o.payload = cols.alloc<int64_t>(rows * 8);
+      add("payload", LDB_INT64, o.payload, 8);
+      if (which < 0) {
+         o.marked = cols.alloc<int32_t>(rows * 4);
+         add("marked", LDB_INT32, o.marked, 4);
+      }
+      o.capacity = n;
+      unsigned long long* counter = scratch.alloc<unsigned long long>(8);
+      LDB_CUDA(cudaMemsetAsync(counter, 0, 8, ctx->compute));
+      ctx->launch("join_marks", [&] { launchJoinMarks(tuple ? JoinTableDev{} : s->join, tuple ? s->keyJoin : KeyJoinDev{}, s->marks, which, o, counter, ctx->smCount, ctx->compute); });
+      unsigned long long got = 0;
+      LDB_CUDA(cudaMemcpyAsync(&got, counter, 8, cudaMemcpyDeviceToHost, ctx->compute));
+      ctx->syncStream(ctx->compute);
+      if (got > (unsigned long long) n) fail(LDB_ERR_INVALID, "the join table holds more entries than its count");
+      b.nRows = (int64_t) got;
+      *out = addResultTable(ctx, name ? name : "marks", std::move(columns), std::move(b), cols);
+   });
+}
+int ldb_gpu_join_table_clear_marks(LdbState* s, LdbError* err) {
+   return guarded(err, [&] {
+      if (!s) fail(LDB_ERR_INVALID, "null argument");
+      checkMarkable(s);
+      if (!s->marks) return;
+      LDB_CUDA(cudaSetDevice(s->ctx->device));
+      LDB_CUDA(cudaMemsetAsync(s->marks, 0, markSlots(s), s->ctx->compute));
+   });
 }
 
 // ---------------------------------------------------------------- ORDER BY … LIMIT and result gather

@@ -17,6 +17,12 @@ An expression is a nested tuple:
                                                              a row without a match yields one tuple with a NULL payload).  At most one
                                                              per program; emitted once, never re-evaluated.
                                                              The keys of a tuple go to consecutive registers (moves where needed).
+  ("mark", probe, cond)                                      probe: a ("probe", …) or ("probe_each", …) expression.  When cond is TRUE
+                                                             and that probe matched, marks the matched build entry; TRUE when it
+                                                             marked, else FALSE.  Runs whether WHERE keeps the tuple or not (the
+                                                             residual join predicate goes into cond).  A "probe" marks one of a
+                                                             multimap key's entries, "probe_each" every one it walks.  join_marks
+                                                             reads the markers: reversed semi / anti / mark joins, right / full outer
   ("rowid",)                                                 the scanned row's number in its table (a build payload for "fetch")
   ("fetch", side_table, row, "column")                       `column` of another table at the row `row` evaluates to (NULL row → NULL);
                                                              accepted wherever a column name is, also as the column of strcmp / like /
@@ -30,11 +36,12 @@ from . import capi
 from .capi import Error, check
 
 OPS = dict(load=1, const=2, add=3, sub=4, mul=5, div=6, neg=7, cmp=8, **{"and": 9, "or": 10, "not": 11}, isnull=12, select=13, i2f=14, fadd=15, fsub=16, fmul=17,
-           fdiv=18, fcmp=19, strcmp=20, strlike=21, year=22, probe=23, strkey8=24, rowid=25, probe_each=26, strcode=27)
+           fdiv=18, fcmp=19, strcmp=20, strlike=21, year=22, probe=23, strkey8=24, rowid=25, probe_each=26, strcode=27, mark=28)
 CMP = {"=": 0, "!=": 1, "<": 2, "<=": 3, ">": 4, ">=": 5}
 AGG = dict(sum=1, sum_f64=2, count=3, count_star=4, min=5, max=6, min_f64=7, max_f64=8, any=9)
 LIKE = dict(prefix=0, suffix=1, contains=2)
-SINK_HASHAGG, SINK_JOIN_BUILD, SINK_MATERIALIZE = 1, 2, 3
+SINK_HASHAGG, SINK_JOIN_BUILD, SINK_MATERIALIZE, SINK_NONE = 1, 2, 3, 4
+MARKED, UNMARKED, ALL = 1, 0, -1  # join_marks: which entries
 
 
 class Builder:
@@ -162,6 +169,19 @@ class Builder:
             if e[1] not in self.tables:
                 self.tables.append(e[1])
             r = self._emit("probe", self._keys(e[2:]), 0, self.tables.index(e[1]))
+        elif k == "mark":
+            probe = e[1] if len(e) == 3 else None
+            if not (isinstance(probe, tuple) and probe and probe[0] in ("probe", "probe_each")):
+                raise ValueError("mark takes a probe or probe_each expression and a condition")
+            if probe[1] in self.tables and any(i[0] == OPS["strcode"] and i[4] == self.tables.index(probe[1]) for i in self.instr):
+                raise ValueError("mark: the probed table is a string dictionary")
+            c = self.expr(e[2])
+            p = self.expr(probe)  # after the condition: the probe the mark refers to is the table's latest one
+            t = self.tables.index(probe[1])
+            last = [i for i in self.instr if i[0] in (OPS["probe"], OPS["probe_each"]) and i[4] == t][-1]
+            if last[1] != p:
+                raise ValueError("mark: another probe of the same table runs between the probe and the mark")
+            r = self._emit("mark", c, 0, t)
         else:
             raise ValueError(f"unknown expression {k}")
         if key is not None:
@@ -300,6 +320,32 @@ def materialize(ctx, table, outs: list, where=None) -> C.c_void_p:
     d.out_table = C.pointer(out)
     _run(ctx, d, b)
     return out
+
+
+def run_effects(ctx, table, effects: list):
+    """A program with no sink (LDB_SINK_NONE): evaluates the expressions in `effects` — ("mark", …), ("strcode", …) inserts — on every
+    row of `table` and produces nothing else."""
+    b = Builder()
+    for x in effects:
+        b.expr(x)
+    d, keep = _desc(ctx, table, b, -1)
+    d.sink_kind = SINK_NONE
+    _run(ctx, d, b)
+
+
+def join_marks(ctx, state, which: int, name="marks") -> "RawTable":
+    """The entries of a join table by their markers (which: MARKED, UNMARKED or ALL) as a DEVICE table: "key" (or "k0".."k{n-1}" for a
+    key-tuple table) and "payload", int64 (gather with cell_bytes=8); with ALL also "marked", int32 0 / 1 (cell_bytes=4).  Row order
+    is unspecified."""
+    t, e = C.c_void_p(), Error()
+    check(ctx.L.ldb_gpu_join_table_marks(state, int(which), name.encode(), C.byref(t), C.byref(e)), e)
+    return RawTable(ctx, t)
+
+
+def clear_marks(ctx, state):
+    """Unmarks every entry of a join table."""
+    e = Error()
+    check(ctx.L.ldb_gpu_join_table_clear_marks(state, C.byref(e)), e)
 
 
 class RawTable:
