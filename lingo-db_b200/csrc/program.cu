@@ -105,10 +105,10 @@ __device__ __forceinline__ const ProgCol* cellOf(const ProgCol& c, const Val* re
    at -= b.firstRow;
    return &tmp;
 }
-// LDB_OP_PROBE_EACH: the next match of `key` along its linear-probe run, resuming at slot `s` after `probes` probes.  false: the run
-// ended.  A run that reaches the probe bound of a table larger than the bound sets the table's error word (6) instead of ending
-// early with a truncated match list.
-__device__ bool probeEachNext(const JoinTableDev& t, int32_t key, uint64_t& s, uint32_t& probes, int32_t& payload) {
+// LDB_OP_PROBE_EACH / LDB_OP_EXISTS: the next match of `key` along its linear-probe run, resuming at slot `s` after `probes` probes.
+// false: the run ended.  A run that reaches the probe bound of a table larger than the bound sets the table's error word (6 for
+// PROBE_EACH, 8 for EXISTS) instead of ending early with a truncated match list.
+__device__ bool probeEachNext(const JoinTableDev& t, int32_t key, uint64_t& s, uint32_t& probes, int32_t& payload, int boundError = 6) {
    if (t.direct) {
       if (probes++) return false; // one slot per key
       payload = directLoadProg(t, key);
@@ -124,7 +124,7 @@ __device__ bool probeEachNext(const JoinTableDev& t, int32_t key, uint64_t& s, u
          return true;
       }
    }
-   if (probes >= 16384 && t.mask >= 16384) atomicExch(t.error, 6);
+   if (probes >= 16384 && t.mask >= 16384) atomicExch(t.error, boundError);
    return false;
 }
 __device__ __forceinline__ bool cmpI(s128 a, s128 b, int op) {
@@ -508,7 +508,12 @@ __device__ void hashAggUpdate(const ProgramParams& p, uint8_t* e, const Val* reg
 // and scheduling of the whole loop change with it).
 // Marks: the instance that also runs LDB_OP_MARK and records, per table, the slot the latest PROBE / PROBE_EACH matched.  For the
 // same reason only programs with a MARK run it; with Marks false none of that code is compiled in.
-template <bool KeyTuples, bool Marks>
+// Exists: the instance that also runs LDB_OP_EXISTS, again launched only for programs that contain one.  The walk over a key's matches
+// is a state machine on the program counter: EXISTS takes the first match and runs its residual block (a key without a match runs it
+// once with dst NULL, so that a warp's lanes stay together); at the block's last instruction the walk either jumps back to the block's
+// first instruction with the next match or writes the verdict and falls through.  Its cursor
+// (ex*) is separate from PROBE_EACH's, because an EXISTS after a PROBE_EACH walks while the PROBE_EACH run is still open.
+template <bool KeyTuples, bool Marks, bool Exists>
 __global__ void __launch_bounds__(256) programKernel(const __grid_constant__ ProgramParams p) {
    unsigned long long inserted = 0;
    for (int64_t base = (int64_t) blockIdx.x * blockDim.x; base < p.nRows; base += (int64_t) gridDim.x * blockDim.x) {
@@ -528,13 +533,35 @@ __global__ void __launch_bounds__(256) programKernel(const __grid_constant__ Pro
       uint64_t hitSlot[Marks ? kProgMaxTables : 1];
       if (Marks)
          for (int k = 0; k < kProgMaxTables; k++) hitSlot[k] = kNoSlot;
+      // Exists: the EXISTS at exPc walks its key's matches while exEnd (its block's last instruction) is >= 0
+      int exPc = 0, exEnd = -1;
+      bool exMiss = false; // the key has no match: the block runs once for nothing
+      int32_t exKey = 0;
+      uint64_t exSlot = 0;
+      uint32_t exProbes = 0;
+      KeyCursor exCur{};
+      KeyTuple exKeys;
+      // the next match of the walk: its payload in `pay`; false: the run ended
+      auto exNext = [&](const ProgInstr& ex, int64_t& pay) {
+         if (KeyTuples && p.keyTables[ex.arg].nKeys) {
+            const KeyHit h = keyJoinNext(p.keyTables[ex.arg], exKeys, exCur);
+            exCur = h.next;
+            pay = h.payload;
+            return h.hit;
+         }
+         int32_t pay32 = 0;
+         const bool hit = probeEachNext(p.tables[ex.arg], exKey, exSlot, exProbes, pay32, 8);
+         pay = pay32;
+         return hit;
+      };
       while (true) {
          bool pass = false;
          if (pending) {
             bool tuple = true;
             for (int pc = start; pc < p.nInstr; pc++) {
                const ProgInstr in = p.instr[pc];
-               const Val a = regs[in.a], b = regs[in.b];
+               // EXISTS's b is its block length (up to 94), not a register: never an index into regs
+               const Val a = regs[in.a], b = regs[Exists && in.op == LDB_OP_EXISTS ? 0 : in.b];
                Val r;
                r.v = 0;
                r.null = false;
@@ -729,12 +756,59 @@ __global__ void __launch_bounds__(256) programKernel(const __grid_constant__ Pro
                            volatile uint8_t* m = p.marks[in.arg] + slot;
                            if (*m == 0) *m = 1;
                         }
+                     } else if (Exists && in.op == LDB_OP_EXISTS) { // the walk starts: the key's first match, or FALSE and past the block
+                        bool live = false;
+                        if (KeyTuples && p.keyTables[in.arg].nKeys) {
+                           if (!gatherTuple(regs, p.keyTables[in.arg].nKeys, [&](int k) { return in.a + k; }, exKeys)) { // NULL / past int64: no match
+                              exCur = keyJoinStart(p.keyTables[in.arg], exKeys);
+                              live = exCur.live;
+                           }
+                        } else if (!a.null && a.v == (s128) (int32_t) a.v) {
+                           const JoinTableDev& t = p.tables[in.arg];
+                           exKey = (int32_t) a.v;
+                           const uint64_t h = hashI32(exKey);
+                           exSlot = h & t.mask;
+                           exProbes = 0;
+                           live = true;
+                           if (!t.direct && t.bloom) {
+                              const uint32_t bits = bloomBits(h);
+                              live = (__ldg(&t.bloom[(uint32_t) (h >> 32) & t.bloomMask]) & bits) == bits;
+                           }
+                        }
+                        int64_t pay = 0;
+                        const bool hit = live && exNext(in, pay);
+                        if (in.b == 0) {
+                           r.v = hit; // no residual: a match is enough
+                        } else { // the block runs with dst = this match's payload.  Without a match it runs once too, with dst NULL and
+                                 // its residual ignored: the lanes of a warp stay on the same instructions (skipping the block made the
+                                 // interpreter run the two instruction streams one after the other, 5x slower at half the rows matching)
+                           r.v = pay;
+                           r.null = !hit;
+                           exMiss = !hit;
+                           exPc = pc;
+                           exEnd = pc + in.b;
+                        }
                      } else {
                         r.null = true;
                      }
                }
                if (!tuple) break;
                regs[in.dst] = r;
+               if (Exists && pc == exEnd) { // the last instruction of an EXISTS block wrote the residual r: TRUE ends the walk, else the next match
+                  const ProgInstr ex = p.instr[exPc];
+                  Val v{0, false};
+                  int64_t pay = 0;
+                  if (exMiss) {
+                     // no match at all: FALSE
+                  } else if (!r.null && r.v != 0) {
+                     v.v = 1;
+                  } else if (exNext(ex, pay)) {
+                     v.v = pay; // back to the block's first instruction with dst = the next match's payload
+                     pc = exPc;
+                  }
+                  if (pc != exPc) exEnd = -1;
+                  regs[ex.dst] = v;
+               }
             }
             pass = tuple;
             if (tuple && p.filterReg >= 0) { // WHERE: NULL is not true
@@ -810,12 +884,22 @@ void launchProgram(const ProgramParams& p, int smCount, cudaStream_t s) {
       keyTuples |= p.keyTables[k].nKeys != 0;
       marks |= p.marks[k] != nullptr;
    }
-   if (marks) {
-      if (keyTuples) programKernel<true, true><<<grid, 256, 0, s>>>(p);
-      else programKernel<false, true><<<grid, 256, 0, s>>>(p);
+   bool exists = false;
+   for (int i = 0; i < p.nInstr; i++) exists |= p.instr[i].op == LDB_OP_EXISTS;
+   if (exists) {
+      if (marks) {
+         if (keyTuples) programKernel<true, true, true><<<grid, 256, 0, s>>>(p);
+         else programKernel<false, true, true><<<grid, 256, 0, s>>>(p);
+      } else {
+         if (keyTuples) programKernel<true, false, true><<<grid, 256, 0, s>>>(p);
+         else programKernel<false, false, true><<<grid, 256, 0, s>>>(p);
+      }
+   } else if (marks) {
+      if (keyTuples) programKernel<true, true, false><<<grid, 256, 0, s>>>(p);
+      else programKernel<false, true, false><<<grid, 256, 0, s>>>(p);
    } else {
-      if (keyTuples) programKernel<true, false><<<grid, 256, 0, s>>>(p);
-      else programKernel<false, false><<<grid, 256, 0, s>>>(p);
+      if (keyTuples) programKernel<true, false, false><<<grid, 256, 0, s>>>(p);
+      else programKernel<false, false, false><<<grid, 256, 0, s>>>(p);
    }
 }
 

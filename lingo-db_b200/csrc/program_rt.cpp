@@ -402,12 +402,17 @@ struct ProgramPlan {
    int eachTable = -1; // tables[] index PROBE_EACH reads
    bool probed[kProgMaxTables] = {}, coded[kProgMaxTables] = {}; // tables[k] read by PROBE / PROBE_EACH, by STRCODE
    bool marked[kProgMaxTables] = {};                             // tables[k] marked by MARK
+   bool existed[kProgMaxTables] = {};                            // tables[k] read by EXISTS
+   // registers written inside an EXISTS block that has ended (they hold whatever its last match left), and the dst registers of ended
+   // EXISTS (a verdict there, not a row); a later write outside a block clears both
+   bool blockOnly[kProgMaxRegs] = {}, verdict[kProgMaxRegs] = {};
    std::vector<LdbState*> dicts, tupleTables; // tupleTables: key-tuple tables whose error word the run may set
 
    ProgramPlan(LdbContext* c, const LdbProgramDesc* desc) : ctx(c), d(desc), t(desc->source) {}
    int colType(int c) const { return colTable[c]->columns[colIdx[c]].type; }
    void wantReg(int r, const char* what) const {
       if (r < 0 || r >= kProgMaxRegs || !written[r]) fail(LDB_ERR_INVALID, std::string("program reads an unwritten or out-of-range register (") + what + ")");
+      if (blockOnly[r]) fail(LDB_ERR_INVALID, std::string("a register written inside an EXISTS block is read after the block (") + what + ")");
    }
    void wantTupleTable(LdbState* js) const {
       if (js->ctx != ctx) fail(LDB_ERR_INVALID, "key-tuple join table belongs to another context");
@@ -459,9 +464,14 @@ static void validateInstructions(ProgramPlan& p) {
    const LdbProgramDesc* d = p.d;
    ProgramParams& base = p.base;
    bool beforeEach[kProgMaxRegs] = {};
+   // EXISTS: the last instruction of the block being read (-1: none), the EXISTS's dst, the registers written before it and inside it
+   int exEnd = -1, exDst = 0;
+   bool beforeExists[kProgMaxRegs] = {}, inBlock[kProgMaxRegs] = {};
+   bool probedInBlock[kProgMaxTables] = {}; // tables[k] probed inside an EXISTS block (which also runs for keys without a match)
    auto wantCol = [&](int c, const char* what) {
       if (c < 0 || c >= p.nCols) fail(LDB_ERR_INVALID, std::string(what) + ": column index out of range");
       if (p.rowReg[c] >= 0) p.wantReg(p.rowReg[c], "row register of a side column");
+      if (p.rowReg[c] >= 0 && p.verdict[p.rowReg[c]]) fail(LDB_ERR_INVALID, "a side column reads an EXISTS result as its row after the EXISTS block (it holds the verdict there)");
    };
    if (d->n_tables > 0 && !d->tables) fail(LDB_ERR_INVALID, "null tables list");
    int tupleKeys[kProgMaxTables] = {}; // tables[k] is a key-tuple join table of this many keys: PROBE reads registers a .. a + n - 1
@@ -473,6 +483,11 @@ static void validateInstructions(ProgramPlan& p) {
    for (int i = 0; i < d->n_instr; i++) {
       const LdbInstr& in = d->instr[i];
       if (in.dst >= kProgMaxRegs) fail(LDB_ERR_INVALID, "destination register out of range");
+      if (exEnd >= 0) { // inside an EXISTS block: it re-runs per match and must end at its last instruction
+         if (in.op == LDB_OP_EXISTS) fail(LDB_ERR_INVALID, "EXISTS blocks do not nest (an EXISTS inside another EXISTS's block)");
+         if (in.op == LDB_OP_PROBE_EACH || in.op == LDB_OP_MARK || (in.op == LDB_OP_STRCODE && in.b == 1))
+            fail(LDB_ERR_INVALID, "an EXISTS block may not contain PROBE_EACH, MARK or an inserting STRCODE (it runs once per match)");
+      }
       switch (in.op) {
          case LDB_OP_LOAD:
             wantCol(in.arg, "LOAD");
@@ -518,6 +533,7 @@ static void validateInstructions(ProgramPlan& p) {
             if (in.arg < 0 || in.arg >= d->n_tables) fail(LDB_ERR_INVALID, "PROBE: table index out of range");
             wantKeys(in);
             p.probed[in.arg] = true;
+            if (exEnd >= 0) probedInBlock[in.arg] = true;
             break;
          case LDB_OP_ROWID: p.usesRowid = true; break;
          case LDB_OP_PROBE_EACH:
@@ -532,14 +548,38 @@ static void validateInstructions(ProgramPlan& p) {
          case LDB_OP_MARK:
             if (in.arg < 0 || in.arg >= d->n_tables) fail(LDB_ERR_INVALID, "MARK: table index out of range");
             if (!p.probed[in.arg]) fail(LDB_ERR_INVALID, "MARK: no earlier PROBE / PROBE_EACH of the program reads the table it marks");
+            if (probedInBlock[in.arg]) fail(LDB_ERR_INVALID, "MARK: the table it marks is probed inside an EXISTS block");
             p.wantReg(in.a, "MARK condition");
             p.marked[in.arg] = true;
+            break;
+         case LDB_OP_EXISTS:
+            if (in.arg < 0 || in.arg >= d->n_tables) fail(LDB_ERR_INVALID, "EXISTS: table index out of range");
+            wantKeys(in);
+            if (i + in.b >= d->n_instr) fail(LDB_ERR_INVALID, "EXISTS: its residual block of b instructions runs past the end of the program");
+            p.existed[in.arg] = true;
             break;
          default: fail(LDB_ERR_UNSUPPORTED, "unknown opcode " + std::to_string(in.op));
       }
       // the instructions after PROBE_EACH run once per match: they may not overwrite what the first pass left for the next one
       if (base.eachPc >= 0 && i > base.eachPc && beforeEach[in.dst]) fail(LDB_ERR_INVALID, "an instruction after PROBE_EACH overwrites a register written at or before it");
+      if (exEnd >= 0) { // the block re-runs per match: what was written before the EXISTS (its dst included) must survive it
+         if (beforeExists[in.dst]) fail(LDB_ERR_INVALID, "an instruction of an EXISTS block overwrites a register written before the EXISTS");
+         inBlock[in.dst] = true;
+      } else {
+         p.blockOnly[in.dst] = p.verdict[in.dst] = false;
+      }
       p.written[in.dst] = true;
+      if (in.op == LDB_OP_EXISTS) {
+         std::copy(p.written, p.written + kProgMaxRegs, beforeExists);
+         std::fill(inBlock, inBlock + kProgMaxRegs, false);
+         exDst = in.dst;
+         exEnd = in.b ? i + in.b : -1;
+         if (!in.b) p.verdict[in.dst] = true;
+      } else if (i == exEnd) { // the block ends: after it, its registers and the EXISTS's dst as a row are off limits
+         for (int r = 0; r < kProgMaxRegs; r++) p.blockOnly[r] |= inBlock[r];
+         p.verdict[exDst] = true;
+         exEnd = -1;
+      }
       if (base.eachPc == i) std::copy(p.written, p.written + kProgMaxRegs, beforeEach);
       base.instr[i] = ProgInstr{in.op, in.dst, in.a, in.b, in.arg};
    }
@@ -591,16 +631,19 @@ static void bindTables(ProgramPlan& p) {
    const LdbProgramDesc* d = p.d;
    for (int k = 0; k < d->n_tables; k++) {
       LdbState* js = d->tables[k];
+      // the table's error word (a probe run at the bound) is read back after the launch, which a captured query cannot do
+      if (p.existed[k] && ctx->capturing) fail(LDB_ERR_UNSUPPORTED, "programs with EXISTS are not part of captured queries (the probe-run bound is checked after the launch)");
       if (p.marked[k]) bindMarks(p, k);
       if (js && js->kind == LDB_STATE_KEY_JOIN) {
          if (p.coded[k]) fail(LDB_ERR_INVALID, "STRCODE needs a string dictionary, not a join table");
          p.wantTupleTable(js);
          if (d->sink_kind == LDB_SINK_JOIN_BUILD && d->sink == js) fail(LDB_ERR_INVALID, "a program may not build a key-tuple join table and probe it");
          p.base.keyTables[k] = js->keyJoin;
-         if (p.probed[k]) p.tupleTables.push_back(js);
+         if (p.probed[k] || p.existed[k]) p.tupleTables.push_back(js);
          continue;
       }
       if (js && js->kind == LDB_STATE_DICT) {
+         if (p.existed[k]) fail(LDB_ERR_INVALID, "EXISTS on a string dictionary (it takes a join table)");
          if (p.probed[k]) fail(LDB_ERR_INVALID, "PROBE / PROBE_EACH on a string dictionary (they take join tables)");
          if (js->ctx != ctx) fail(LDB_ERR_INVALID, "string dictionary belongs to another context");
          if (ctx->capturing) fail(LDB_ERR_UNSUPPORTED, "string dictionaries are not part of captured queries");
@@ -611,6 +654,8 @@ static void bindTables(ProgramPlan& p) {
       if (p.coded[k]) fail(LDB_ERR_INVALID, "STRCODE needs a string dictionary, not a join table");
       if (k == p.eachTable && js && js->kind == LDB_STATE_JOIN_TABLE && !(js->join.stride == 8 || js->join.direct))
          fail(LDB_ERR_UNSUPPORTED, "PROBE_EACH takes a plain single-key or direct-address join table (not a pair table or a group-join map)");
+      if (p.existed[k] && js && js->kind == LDB_STATE_JOIN_TABLE && !(js->join.stride == 8 || js->join.direct))
+         fail(LDB_ERR_UNSUPPORTED, "EXISTS takes a plain single-key, direct-address or key-tuple join table (not a pair table or a group-join map)");
       if (!js || js->kind != LDB_STATE_JOIN_TABLE || js->join.stride == 16) fail(LDB_ERR_INVALID, "PROBE tables are single-key join tables");
       p.base.tables[k] = js->join;
    }
@@ -745,13 +790,15 @@ static void launchBatches(const ProgramPlan& p) {
    }
 }
 
-// a probe run longer than the bound (PROBE_EACH), or a build that could not store a row (table full, the reserved pair, a key or
-// payload outside int32): fail rather than return a truncated match list or a table with rows missing
+// a probe run longer than the bound (PROBE_EACH, EXISTS), or a build that could not store a row (table full, the reserved pair, a key
+// or payload outside int32): fail rather than return a truncated match list, a verdict that missed a match or a table with rows missing
 // — and a dictionary that could not take a string
 static void checkErrorWords(const ProgramPlan& p) {
    const LdbProgramDesc* d = p.d;
    for (LdbState* js : {p.eachTable >= 0 ? d->tables[p.eachTable] : nullptr, d->sink_kind == LDB_SINK_JOIN_BUILD ? d->sink : nullptr})
       if (js && js->kind == LDB_STATE_JOIN_TABLE) ldb_gpu_check_join_error_internal(js);
+   for (int k = 0; k < d->n_tables; k++)
+      if (p.existed[k] && k != p.eachTable && d->tables[k]->kind == LDB_STATE_JOIN_TABLE) ldb_gpu_check_join_error_internal(d->tables[k]);
    for (LdbState* ks : p.tupleTables) ldb_gpu_check_keyjoin_error_internal(ks); // a full build, a probe run at the bound, a key outside int64
    for (LdbState* ds : p.dicts) checkDictError(ds);
 }

@@ -924,6 +924,7 @@ static void checkJoinError(LdbState* s) {
    if (e == 5) fail(LDB_ERR_INVALID, "key outside the declared range of a direct-address table");
    if (e == 6) fail(LDB_ERR_CAPACITY, "PROBE_EACH: a probe run is longer than the interpreter's bound of 16384 slots (an overfull join table)");
    if (e == 7) fail(LDB_ERR_UNSUPPORTED, "a program join build met a key or payload outside int32 (join tables store int32 keys and payloads)");
+   if (e == 8) fail(LDB_ERR_CAPACITY, "EXISTS: a probe run is longer than the interpreter's bound of 16384 slots (an overfull join table)");
    if (e != 0) fail(LDB_ERR_INVALID, "join table error word " + std::to_string(e));
 }
 } // extern "C"

@@ -23,6 +23,18 @@ An expression is a nested tuple:
                                                              residual join predicate goes into cond).  A "probe" marks one of a
                                                              multimap key's entries, "probe_each" every one it walks.  join_marks
                                                              reads the markers: reversed semi / anti / mark joins, right / full outer
+  ("exists", join_table_state, key, …, cond)                 TRUE when some match of the key satisfies cond, else FALSE (never NULL):
+                                                             semi join (WHERE it), anti join (WHERE ("not", it)), mark join (its value).
+                                                             cond is the residual, evaluated once per match in probe-run order until one
+                                                             is TRUE; inside it ("match", join_table_state) is the current match's
+                                                             payload (a "fetch" row).  cond None: TRUE when the key has any match.  No
+                                                             exists, probe_each, mark or inserting strcode inside cond; what cond
+                                                             evaluates stays inside it (re-evaluated if used again after it).
+  ("probe_each", join_table_state, key, …, "outer", ("on", cond))
+                                                             left outer join with the residual cond (("match", join_table_state) as in
+                                                             exists): each match that satisfies cond, or one tuple with a NULL payload
+                                                             when none does.  Emitted as exists + a key NULLed when it fails + an outer
+                                                             probe_each, with (cond OR payload IS NULL) ANDed into the WHERE.
   ("rowid",)                                                 the scanned row's number in its table (a build payload for "fetch")
   ("fetch", side_table, row, "column")                       `column` of another table at the row `row` evaluates to (NULL row → NULL);
                                                              accepted wherever a column name is, also as the column of strcmp / like /
@@ -36,7 +48,7 @@ from . import capi
 from .capi import Error, check
 
 OPS = dict(load=1, const=2, add=3, sub=4, mul=5, div=6, neg=7, cmp=8, **{"and": 9, "or": 10, "not": 11}, isnull=12, select=13, i2f=14, fadd=15, fsub=16, fmul=17,
-           fdiv=18, fcmp=19, strcmp=20, strlike=21, year=22, probe=23, strkey8=24, rowid=25, probe_each=26, strcode=27, mark=28)
+           fdiv=18, fcmp=19, strcmp=20, strlike=21, year=22, probe=23, strkey8=24, rowid=25, probe_each=26, strcode=27, mark=28, exists=29)
 CMP = {"=": 0, "!=": 1, "<": 2, "<=": 3, ">": 4, ">=": 5}
 AGG = dict(sum=1, sum_f64=2, count=3, count_star=4, min=5, max=6, min_f64=7, max_f64=8, any=9)
 LIKE = dict(prefix=0, suffix=1, contains=2)
@@ -49,6 +61,9 @@ class Builder:
         self.instr, self.columns, self.consts, self.strings, self.tables = [], [], [], [], []
         self.side_tables, self.side_columns = [], []  # side tables (handles); side columns as (side table index, column, row register)
         self._cache, self._rows, self._next, self._each = {}, {}, 0, None
+        # _match = (table handle, register of the current match) while a residual compiles; _on = the registers to AND into the WHERE
+        # (outer probe_each with a residual)
+        self._match, self._on = None, []
 
     def _reg(self):
         r = self._next
@@ -114,11 +129,53 @@ class Builder:
             self.strings.append(s)
         return self.strings.index(s)
 
+    def _residual(self, table, match: int, cond) -> int:
+        """cond with ("match", table) = register `match`.  What it evaluates is cached only while it compiles: inside an exists block
+        it is re-evaluated per match, so a later use must not read it after the block."""
+        saved = dict(self._cache), dict(self._rows)
+        self._match = (_handle(table), match)
+        try:
+            return self.expr(cond)
+        finally:
+            self._cache, self._rows = saved
+            self._match = None
+
+    def _exists(self, table, key: int, cond) -> int:
+        """EXISTS over the keys from register `key` on, its residual block right after it (b = the block's length)"""
+        if table not in self.tables:
+            self.tables.append(table)
+        at = len(self.instr)
+        r = self._emit("exists", key, 0, self.tables.index(table))
+        if cond is None:
+            return r
+        res = self._residual(table, r, cond)
+        if len(self.instr) == at + 1 or self.instr[-1][1] != res:  # the residual is the block's last write; an empty block means none
+            self._emit("select", res, res, res)
+        n = len(self.instr) - at - 1
+        if n > 255:
+            raise ValueError("exists: the residual takes more than 255 instructions")
+        op, dst, a, _, arg = self.instr[at]
+        self.instr[at] = (op, dst, a, n, arg)
+        return r
+
+    def where(self, f: int) -> int:
+        """the WHERE register: f (-1: none) ANDed with the conditions outer probe_each residuals add, emitted last"""
+        for r in self._on:
+            f = r if f < 0 else self._emit("and", f, r)
+        self._on = []
+        return f
+
     def expr(self, e) -> int:
-        key = repr(e) if not (isinstance(e, tuple) and e and e[0] == "probe") else None
+        key = repr(e) if not (isinstance(e, tuple) and e and e[0] in ("probe", "match")) else None
         if key is not None and key in self._cache:
             return self._cache[key]
         k = e[0]
+        if self._match is not None and (k in ("exists", "probe_each", "mark") or (k == "strcode" and len(e) <= 3)):
+            raise ValueError(f"{k} inside the condition of an exists or an outer probe_each (no nesting, no effects per match)")
+        if k == "match":
+            if self._match is None or _handle(e[1]) != self._match[0]:
+                raise ValueError("match: only inside the condition of an exists or an outer probe_each, naming its join table")
+            return self._match[1]
         if k == "col":
             r = self._emit("load", arg=self._col(e[1]))
         elif k == "fetch":
@@ -131,10 +188,23 @@ class Builder:
             if e[1] not in self.tables:
                 self.tables.append(e[1])
             keys = list(e[2:])
+            on = keys.pop()[1] if isinstance(keys[-1], tuple) and len(keys[-1]) == 2 and keys[-1][0] == "on" else None
             outer = keys[-1] == "outer"
             if outer:
                 keys.pop()
-            r = self._emit("probe_each", self._keys(keys), int(outer), self.tables.index(e[1]))
+            if on is None:
+                r = self._emit("probe_each", self._keys(keys), int(outer), self.tables.index(e[1]))
+            elif not outer:
+                raise ValueError("probe_each: a residual ('on', cond) takes the outer form (an inner join's residual is a WHERE term)")
+            else:  # v = EXISTS(k, cond); k' = v ? k : NULL; PROBE_EACH(k', outer); WHERE (cond[match] OR payload IS NULL)
+                k0 = self._keys(keys)
+                v = self._exists(e[1], k0, on)
+                null = self.expr(("div", ("const", 0), ("const", 0)))
+                kn = [self._emit("select", k0 + i, null, v) for i in range(len(keys))]
+                r = self._emit("probe_each", kn[0], 1, self.tables.index(e[1]))
+                self._each = r
+                res = self._residual(e[1], r, on)
+                self._on.append(self._emit("or", res, self._emit("isnull", r)))
             self._each = r
         elif k == "const":
             r = self._emit("const", arg=self._const(int(e[1])))
@@ -165,6 +235,10 @@ class Builder:
             if e[1] not in self.tables:
                 self.tables.append(e[1])
             r = self._emit("strcode", self._col(e[2]), int(len(e) <= 3), self.tables.index(e[1]))
+        elif k == "exists":
+            if len(e) < 4:
+                raise ValueError("exists takes a join table, its keys and a condition (None: no residual)")
+            r = self._exists(e[1], self._keys(e[2:-1]), e[-1])
         elif k == "probe":
             if e[1] not in self.tables:
                 self.tables.append(e[1])
@@ -191,6 +265,7 @@ class Builder:
 
 def _desc(ctx, table, b: Builder, filter_reg: int):
     keep = []
+    filter_reg = b.where(filter_reg)
     d = capi.ProgramDesc()
     d.source = table.h
     cols = [c.encode() for c in b.columns]
