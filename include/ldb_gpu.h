@@ -548,12 +548,15 @@ int ldb_gpu_hashagg_read(LdbState* s, LdbHashAggRow* rows, int64_t max_rows, int
 int ldb_gpu_hashagg_to_table(LdbState* s, const char* name, LdbTable** out, LdbError* err);
 /* ORDER BY <column> [DESC] LIMIT k over a DEVICE/staged table (GrowingBuffer::sort + Heap, GrowingBuffer.cpp:54-78): an LSD radix
  * sort of (order-preserving 64-bit key, row id) on the device; returns the first `limit` row ids (ties keep row order: stable).
- * column types: int32/date32/fsb4/int64/decimal(p<19). */
+ * column types: int32/date32/fsb4/int64/decimal of any precision, ordered by its full value (a 16-byte cell takes two sort passes:
+ * low word, then high word).  A materialized column holding double bits (the materialize sink does not record register types)
+ * orders by its bit pattern. */
 int ldb_gpu_table_order_by(LdbTable* t, const char* column, int32_t descending, int64_t limit, int64_t* row_ids, int64_t* n_out, LdbError* err);
 /* read back `n` cells of a fixed-width column at the given row ids (result materialisation of small outputs) */
 int ldb_gpu_table_gather(LdbTable* t, const char* column, const int64_t* row_ids, int64_t n, void* host_dst /* n * cell bytes */, uint8_t* host_valid /* n, may be NULL */, LdbError* err);
 /* ORDER BY k1 [DESC], k2 [DESC], … LIMIT over a single-batch table of fewer than 2^32 rows: an LSD composition of the stable radix
- * sort (the last key first), so ties on every key keep row order.  Fixed-width keys: the types ldb_gpu_table_order_by takes.  utf8
+ * sort (the last key first), so ties on every key keep row order.  Fixed-width keys: the types ldb_gpu_table_order_by takes, in its
+ * order (decimals of any precision by their full value; a 16-byte cell costs two sort passes, other fixed-width keys one).  utf8
  * keys order bytewise with unsigned bytes, a proper prefix first (the order of LDB_OP_STRCMP); a utf8 key costs one sort pass for
  * its lengths plus one per 8 bytes of its LONGEST string.  Validity is not consulted: a NULL sorts by the cell it holds.  Returns
  * the first `limit` row ids (all with limit < 0).  Unknown column: LDB_ERR_INVALID. */

@@ -1117,7 +1117,8 @@ void launchRadixSortPairs(unsigned long long* keys, uint32_t* vals, unsigned lon
 // The sort words of one key at the current permutation: an LSD composition of launchRadixSortPairs (stable) sorts by the last key
 // first; a utf8 key is its length word, then its 8-byte chunks from the last to the first.  Zero padding makes a proper prefix tie
 // with its extension on every chunk, and the length pass, run before them, puts the shorter one first: bytewise order with
-// unsigned bytes, the order of LDB_OP_STRCMP.
+// unsigned bytes, the order of LDB_OP_STRCMP.  A 16-byte cell (an i128) is two words the same way: chunk 0 its low word, unsigned,
+// then chunk 1 its high word with the sign bit flipped.
 __global__ void buildSortWordsKernel(const uint8_t* col, const uint8_t* bytes, int elemBytes, int kind, int chunk, int64_t n, int descending, int first,
                                      uint32_t* ids, unsigned long long* keys, int32_t* maxLen) {
    int32_t longest = 0;
@@ -1125,7 +1126,10 @@ __global__ void buildSortWordsKernel(const uint8_t* col, const uint8_t* bytes, i
       const uint32_t row = first ? (uint32_t) i : ids[i];
       if (first) ids[i] = row;
       unsigned long long k = 0;
-      if (kind == 0) {
+      if (kind == 0 && elemBytes == 16) {
+         const unsigned long long* w = (const unsigned long long*) (col + (size_t) row * 16);
+         k = chunk ? w[1] ^ 0x8000000000000000ull : w[0];
+      } else if (kind == 0) {
          const int64_t v = elemBytes == 4 ? (int64_t) ((const int32_t*) col)[row] : *(const int64_t*) (col + (size_t) row * elemBytes);
          k = (unsigned long long) v ^ 0x8000000000000000ull;
       } else {

@@ -243,7 +243,8 @@ static uint32_t* sortRows(Scratch& scratch, LdbTable* t, const std::vector<std::
    for (size_t k = keys.size(); k-- > 0;) {
       const int c = keys[k].first, desc = keys[k].second;
       if (t->columns[c].type != LDB_UTF8) {
-         pass(c, 0, 0, desc);
+         if (b.elemBytes[c] == 16) pass(c, 0, 0, desc); // an i128 cell: its low word first, then the high word
+         pass(c, 0, b.elemBytes[c] == 16 ? 1 : 0, desc);
          continue;
       }
       int32_t longest = 0;

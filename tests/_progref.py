@@ -10,10 +10,25 @@ are the op comments of include/ldb_gpu.h ("program pipelines"), restated:
   - YEAR is the proleptic Gregorian year of `date32` days since 1970-01-01 (`datetime` where it reaches, the 400-year cycle beyond);
   - strings compare bytewise (shorter first on a common prefix); STRKEY8 is the first 8 bytes, zero padded, read big-endian as a
     signed int64;
-  - PROBE is the payload of the key's match (NULL when absent, when the key is NULL or outside int32); PROBE_EACH yields one tuple
-    per match (a NULL key never matches; "outer": a row without a match yields one tuple with a NULL payload);
+  - a join table (Join) is its kind and a multimap from key tuple to payloads.  A plain table takes one int32 key (outside int32:
+    no match), a direct-address table one key in [min, max], a key-tuple table n int64 keys (a NULL component, or one outside
+    int64, never matches); a NULL key never matches;
+  - PROBE is the payload of the key's match (NULL when absent).  On a multimap key with several matches it is any one of them: a
+    OneOf value, which compares equal to each of its members and takes part in no arithmetic;  PROBE_EACH yields one tuple per match
+    ("outer": a row without a match yields one tuple with a NULL payload; "outer" + ("on", cond): each match whose cond is TRUE, or
+    exactly one NULL tuple when none is);
+  - EXISTS (t, keys…, cond) is TRUE when some match of the keys has a TRUE cond (("match", t) = that match's payload; NULL is not
+    TRUE; cond None: any match), else FALSE, never NULL;
+  - MARK (probe, cond) is TRUE exactly when cond is TRUE and the probe matched, else FALSE.  Its effect is recorded in the table's
+    Join.marks (MarkModel): through PROBE_EACH every walked match with a TRUE cond (with ("on", c) the walk reaches every match of a
+    key that has one passing c, the rejected ones too: WHERE drops their tuples, not the MARK), through PROBE on a key with one entry that entry,
+    through PROBE on a multimap key at least one of the key's entries;
+  - STRCODE is the string's code in a dictionary whose string → code map is read back after the run (`dicts`): codes are
+    unspecified, so the map is an input; lookups of absent strings are NULL; inserting STRCODEs record their non-NULL strings in
+    `inserted` (their key set must be the dictionary's);
   - ROWID is the row's number in its table; FETCH reads a side table's column at a row number, and a NULL or out-of-range row
-    reads NULL.
+    reads NULL;
+  - ORDER BY (order_rows) is a stable sort over the full i128 cell.
 Values: int for integer-typed results, float for doubles, None for NULL."""
 import datetime
 import math
@@ -140,15 +155,101 @@ class Side:
         self.n = len(next(iter(cols.values()))) if cols else 0
 
 
-# ---------------------------------------------------------------------------------------------------- evaluator
-class Evaluator:
-    """Evaluates expressions column-wise over `cols` (column → list).  `joins` maps a join table's handle value to its multimap
-    {key: [payloads]}; `sides` maps a side table's handle value to a Side."""
+# ---------------------------------------------------------------------------------------------------- joins
+class OneOf(frozenset):
+    """PROBE of a multimap key with several matches: the payload is one of these, which one is not determined"""
 
-    def __init__(self, cols: Dict[str, list], joins: Optional[dict] = None, sides: Optional[dict] = None, first_row: int = 0):
-        self.cols, self.joins, self.sides = cols, joins or {}, sides or {}
+
+class MarkModel:
+    """The markers a join table must end up with: `must` entries marked, for every key in `some` at least one of its entries, and no
+    entry outside those two (an entry = its payload, a build row id)."""
+
+    def __init__(self):
+        self.must, self.some = set(), set()
+
+    def check(self, join: "Join", marked: set, what=""):
+        allowed = set(self.must)
+        for k in self.some:
+            allowed |= set(join.by.get(k, []))
+        assert self.must <= marked, (what, "entries that should be marked are not", sorted(self.must - marked)[:10])
+        assert marked <= allowed, (what, "entries marked that no qualifying probe reached", sorted(marked - allowed)[:10], len(marked), len(allowed))
+        missing = [k for k in self.some if not marked & set(join.by.get(k, []))]
+        assert not missing, (what, "keys probed with a TRUE condition but none of their entries marked", missing[:10])
+
+
+class Join:
+    """A join table's model: kind "plain" (one int32 key), "direct" (one int32 key in [lo, hi]) or "tuple" (n_keys int64 keys), and
+    its entries as a multimap {key tuple: [payloads]}; `marks` accumulates MARK effects until cleared."""
+
+    def __init__(self, kind: str, entries, n_keys: int = 1, lo: Optional[int] = None, hi: Optional[int] = None):
+        self.kind, self.n_keys, self.lo, self.hi = kind, n_keys, lo, hi
+        self.by: Dict[tuple, list] = {}
+        for k, p in entries:
+            k = k if isinstance(k, tuple) else (k,)
+            if None not in k:
+                self.by.setdefault(k, []).append(p)
+        self.marks = MarkModel()
+
+    def hits(self, keys) -> list:
+        if len(keys) != self.n_keys or any(k is None for k in keys):
+            return []
+        if self.kind == "tuple":
+            if not all(I64_MIN <= k <= I64_MAX for k in keys):
+                return []
+        elif not I32_MIN <= keys[0] <= I32_MAX or (self.kind == "direct" and not self.lo <= keys[0] <= self.hi):
+            return []
+        return self.by.get(tuple(keys), [])
+
+    def clear_marks(self):
+        self.marks = MarkModel()
+
+
+def as_join(j) -> Join:
+    """the older form of a plain table, {key: [payloads]}, as a Join"""
+    return j if isinstance(j, Join) else Join("plain", [(k, p) for k, ps in j.items() for p in ps])
+
+
+def check_dictionary(strings: list, ranks: list, keys: set) -> Dict[bytes, int]:
+    """A dictionary read back as rows (row i = code i: its string and rank) against the strings its inserting STRCODEs saw: the codes
+    are a bijection onto 0..n-1, the key set is exactly `keys`, and the rank is the bytewise order.  Returns the string → code map."""
+    assert None not in strings and len(set(strings)) == len(strings), "two codes for one string"
+    assert set(strings) == keys, ("dictionary keys", sorted(set(strings) ^ keys)[:10])
+    order = sorted(range(len(strings)), key=lambda i: strings[i])
+    assert [ranks[i] for i in order] == list(range(len(strings))), "ranks are not the bytewise order"
+    return {s: i for i, s in enumerate(strings)}
+
+
+def order_rows(values: list, descending: bool = False) -> list:
+    """ORDER BY one column of cells (ints: the i128, or a double's bits): the row numbers of a stable sort"""
+    return sorted(range(len(values)), key=lambda i: -values[i] if descending else values[i])
+
+
+# ---------------------------------------------------------------------------------------------------- evaluator
+def _split_probe(e):
+    """("probe_each", t, keys…[, "outer"[, ("on", cond)]]) → (keys, outer, cond)"""
+    keys, on = list(e[2:]), None
+    if keys and isinstance(keys[-1], tuple) and len(keys[-1]) == 2 and keys[-1][0] == "on":
+        on = keys.pop()[1]
+    outer = bool(keys) and keys[-1] == "outer"
+    if outer:
+        keys.pop()
+    return keys, outer, on
+
+
+class Evaluator:
+    """Evaluates expressions column-wise over `cols` (column → list).  `joins` maps a join table's handle value to its Join (or, for a
+    plain table, its multimap {key: [payloads]}); `sides` maps a side table's handle value to a Side; `dicts` a dictionary's handle
+    value to its string → code map."""
+
+    def __init__(self, cols: Dict[str, list], joins: Optional[dict] = None, sides: Optional[dict] = None, first_row: int = 0,
+                 dicts: Optional[dict] = None):
+        self.cols, self.sides = cols, sides or {}
+        self.joins = {h: as_join(j) for h, j in (joins or {}).items()}
+        self.dicts = dicts or {}
+        self.inserted: Dict[object, set] = {}
         self.n = len(next(iter(cols.values()))) if cols else 0
         self.first_row = first_row
+        self._each_key = None
 
     @staticmethod
     def _h(t):
@@ -178,20 +279,23 @@ class Evaluator:
                 each = f
         src = list(range(self.n))
         memo = {}
+        self._each_key, self._walked = None, None
         if each is not None:
-            keys = self._eval(each[2], memo, src)
-            mm = self.joins[self._h(each[1])]
-            outer = len(each) > 3 and each[3] == "outer"
+            kexprs, outer, on = _split_probe(each)
+            keys = list(zip(*[self._eval(k, memo, src) for k in kexprs]))
+            hits = [self.joins[self._h(each[1])].hits(k) for k in keys]
+            if on is not None:  # the walk covers every match of a key with a passing one (WHERE drops the rejected ones' tuples)
+                passing = self._passing(each[1], on, memo, src, hits)
+                self._walked = [(r, hs) for r, hs, ok in zip(src, hits, passing) if ok]
+                hits = passing
             s2, pay = [], []
-            for r, k in zip(src, keys):
-                hits = mm.get(k, []) if k is not None and I32_MIN <= k <= I32_MAX else []
-                if not hits and outer:
-                    hits = [None]
-                for p in hits:
+            for r, hs in zip(src, hits):
+                for p in hs or ([None] if outer else []):
                     s2.append(r)
                     pay.append(p)
             src = s2
-            memo = {repr(each): pay}
+            self._each_key = repr(each)
+            memo = {self._each_key: pay}
         outs = [self._eval(e, memo, src) for e in exprs]
         if where is not None:
             w = self._eval(where, memo, src)
@@ -280,17 +384,67 @@ class Evaluator:
         if k == "year":
             return [None if x is None else year_of_days(x) for x in ev(e[1])]
         if k == "probe":
-            mm = self.joins[self._h(e[1])]
+            j = self.joins[self._h(e[1])]
             out = []
-            for x in ev(e[2]):
-                hits = mm.get(x, []) if x is not None and I32_MIN <= x <= I32_MAX else []
-                if len(hits) > 1:
-                    raise ValueError("PROBE of a key with several matches: the payload is not determined")
-                out.append(hits[0] if hits else None)
+            for keys in zip(*[ev(x) for x in e[2:]]):
+                hits = j.hits(keys)
+                out.append(None if not hits else hits[0] if len(hits) == 1 else OneOf(hits))
             return out
         if k == "probe_each":
             raise ValueError("probe_each is expanded by run()")
+        if k == "match":
+            return memo[f"match:{self._h(e[1])}"]
+        if k == "exists":
+            j = self.joins[self._h(e[1])]
+            hits = [j.hits(keys) for keys in zip(*[ev(x) for x in e[2:-1]])]
+            if e[-1] is not None:
+                hits = self._passing(e[1], e[-1], memo, src, hits)
+            return [int(bool(h)) for h in hits]
+        if k == "mark":
+            probe = e[1]
+            c = ev(e[2])
+            j = self.joins[self._h(probe[1])]
+            if probe[0] == "probe_each":
+                out = [int(_truth(x) is True and p is not None) for x, p in zip(c, ev(probe))]
+                if self._walked is None:
+                    j.marks.must |= {p for p, v in zip(ev(probe), out) if v}
+                    return out
+                # with ("on", cond) the walk also reaches the matches cond rejects: MARK runs on their tuples too
+                wsrc = [r for r, hs in self._walked for _ in hs]
+                wpay = [p for _, hs in self._walked for p in hs]
+                wc = self._eval(e[2], {self._each_key: wpay}, wsrc)
+                j.marks.must |= {p for p, x in zip(wpay, wc) if _truth(x) is True}
+                return out
+            out = []
+            for keys, x in zip(zip(*[ev(k) for k in probe[2:]]), c):
+                hits = j.hits(keys)
+                out.append(int(_truth(x) is True and bool(hits)))
+                if out[-1] and len(hits) == 1:
+                    j.marks.must.add(hits[0])
+                elif out[-1]:
+                    j.marks.some.add(tuple(keys))
+            return out
+        if k == "strcode":
+            h = self._h(e[1])
+            d = self.dicts.get(h, {})
+            ss = self._column(e[2], memo, src)
+            if len(e) <= 3:
+                self.inserted.setdefault(h, set()).update(s for s in ss if s is not None)
+            return [None if s is None else d.get(s) for s in ss]
         raise ValueError(f"unknown expression {k}")
+
+    def _passing(self, table, cond, memo, src, hits) -> list:
+        """per tuple, the matches in `hits` whose cond is TRUE, cond evaluated once per (tuple, match) with ("match", table) = the match"""
+        idx = [i for i, hs in enumerate(hits) for _ in hs]
+        sub = {f"match:{self._h(table)}": [p for hs in hits for p in hs]}
+        if self._each_key in memo:  # what PROBE_EACH expanded stays in reach of the residual
+            sub[self._each_key] = [memo[self._each_key][i] for i in idx]
+        c = self._eval(cond, sub, [src[i] for i in idx])
+        out = [[] for _ in hits]
+        for i, p, v in zip(idx, sub[f"match:{self._h(table)}"], c):
+            if _truth(v) is True:
+                out[i].append(p)
+        return out
 
 
 def cell(v) -> Optional[int]:
@@ -306,6 +460,8 @@ def same_cell(got: Optional[int], want) -> bool:
     """bit-for-bit equality of a materialized cell with a reference value; any NaN equals any NaN"""
     if want is None or got is None:
         return got is None and want is None
+    if isinstance(want, OneOf):
+        return got in want
     if isinstance(want, float) and math.isnan(want):
         return got >> 64 == 0 and math.isnan(bits_f64(got))
     return got == cell(want)
@@ -470,7 +626,7 @@ INT_CONSTS = [0, 1, -1, 2, 7, -3, 100, I8_MIN, I8_MAX, I16_MAX, I32_MIN, I32_MAX
 FLOAT_CONSTS = [0.0, -0.0, 1.0, -2.5, 0.1, math.inf, -math.inf, math.nan, 5e-324, 1e308]
 DATE_CONSTS = [0, -1, 10957, 11016, -719162, 2932896, -25508]
 CMP_OPS = ["=", "!=", "<", "<=", ">", ">="]
-LIMITS = dict(regs=48, instr=96, columns=12, consts=24, strings=12)
+LIMITS = dict(regs=48, instr=96, columns=12, consts=24, strings=12, tables=4)
 
 
 class ProgramGen:
@@ -561,17 +717,19 @@ class ProgramGen:
 
 
 def usage(exprs: list, where=None) -> dict:
-    """registers / instructions / columns / constants / strings one Builder needs for these outputs (registers: None = over 48)"""
+    """registers / instructions / columns / constants / strings / tables one Builder needs for these outputs (registers: None = over
+    48, or a program the builder refuses)"""
     from lingodb_b200 import program as P
     b = P.Builder()
     try:
-        if where is not None:
-            b.expr(where)
+        f = b.expr(where) if where is not None else -1
         for e in exprs:
             b.expr(e)
+        b.where(f)  # with the conditions an outer probe_each with a residual ANDs into the WHERE
     except ValueError:
         return dict(regs=None)
-    return dict(regs=b._next, instr=len(b.instr), columns=len(b.columns) + len(b.side_columns), consts=len(b.consts), strings=len(b.strings))
+    return dict(regs=b._next, instr=len(b.instr), columns=len(b.columns) + len(b.side_columns), consts=len(b.consts), strings=len(b.strings),
+                tables=len(b.tables))
 
 
 def fits(exprs: list, where=None) -> bool:

@@ -399,7 +399,17 @@ def test_probe_and_probe_each_against_a_multimap(gpu_ctx, join_tables, kind):
 
 
 # ---------------------------------------------------------------------------------------------------- 5. ORDER BY
-ORDER_COLUMNS = [("i32", "int32", 0, 0), ("i64", "int64", 0, 0), ("dt", "date32", 0, 0), ("dn", "decimal128", 18, 2)]
+ORDER_COLUMNS = [("i32", "int32", 0, 0), ("i64", "int64", 0, 0), ("dt", "date32", 0, 0), ("dn", "decimal128", 18, 2), ("dw", "decimal128", 38, 0)]
+ORDER_WIDE = [1 << 64, 1, -1, -(1 << 64), R.I128_MIN, R.I128_MAX]  # the low word alone puts 2^64 before 1 and -2^64 after -1
+
+
+def _wide_words(rng, n):
+    """(high, low) words of decimal128 values over the whole i128 range with heavy ties on both words: the first rows are ORDER_WIDE"""
+    hi = np.where(rng.random(n) < 0.6, rng.integers(-2, 2, n), rng.choice(np.array([R.I64_MIN, R.I64_MAX, rng.integers(-2**63, 2**63 - 1)]), n)).astype(np.int64)
+    lo = np.where(rng.random(n) < 0.6, rng.choice(np.array([0, 1, 1 << 63, (1 << 64) - 1], np.uint64), n), rng.integers(0, 2**64 - 1, n, np.uint64, endpoint=True))
+    for i, v in enumerate(ORDER_WIDE[:n]):
+        hi[i], lo[i] = v >> 64, v & ((1 << 64) - 1)
+    return hi, lo.astype(np.uint64)
 
 
 @pytest.mark.parametrize("n", [0, 1, 4095, 4096, 4097, 3 * 4096 + 1, 1_000_003])
@@ -411,13 +421,17 @@ def test_order_by_is_a_stable_sort(gpu_ctx, n):
             "dn": np.where(rng.random(n) < 0.7, small * 10**17, rng.integers(-10**18 + 1, 10**18, n)).astype(np.int64)}
     dcells = np.zeros((n, 2), np.int64)
     dcells[:, 0], dcells[:, 1] = vals["dn"], vals["dn"] >> 63
+    hi, lo = _wide_words(rng, n)
+    wcells = np.zeros((n, 2), np.uint64)
+    wcells[:, 0], wcells[:, 1] = lo, hi.view(np.uint64)
     tab = runtime.Table(gpu_ctx, f"ord{n}", R.specs_of(ORDER_COLUMNS))
-    tab.append_host({"i32": vals["i32"], "i64": vals["i64"], "dt": vals["dt"], "dn": dcells.view(np.uint8).reshape(n, 16)}, n)
+    tab.append_host({"i32": vals["i32"], "i64": vals["i64"], "dt": vals["dt"], "dn": dcells.view(np.uint8).reshape(n, 16),
+                     "dw": wcells.view(np.uint8).reshape(n, 16)}, n)
     raw = P.RawTable(gpu_ctx, tab.h)
-    for c in vals:
-        v = vals[c]
-        asc = np.argsort(v, kind="stable")
-        desc = np.argsort(~v, kind="stable")  # ~v = -v - 1: reverses the order without overflow
+    rows = np.arange(n)
+    orders = {c: (np.argsort(v, kind="stable"), np.argsort(~v, kind="stable")) for c, v in vals.items()}  # ~v = -v - 1: reversed, no overflow
+    orders["dw"] = (np.lexsort((rows, lo, hi)), np.lexsort((rows, ~lo, ~hi)))  # i128 order: the high word, then the low word unsigned
+    for c, (asc, desc) in orders.items():
         for descending, order in ((False, asc), (True, desc)):
             for limit in sorted({0, 1, n, n + 5}):
                 ids = raw.order_by(c, descending=descending, limit=limit)

@@ -92,6 +92,96 @@ def test_probe_fetch_and_expansion():
     assert outs == [[1, 2, 3]]
 
 
+def test_probe_on_every_table_kind():
+    plain = R.Join("plain", [(1, 10), (2, 20), (2, 21), (R.I32_MAX, 30)])
+    direct = R.Join("direct", [(k, 100 + k) for k in range(-2, 3)], lo=-2, hi=2)
+    tup = R.Join("tuple", [((1, R.I64_MAX), 7), ((1, R.I64_MIN), 8), ((0, 0), 9), ((0, 0), 10)], n_keys=2)
+    ev = R.Evaluator({"k": [1, R.I32_MAX, R.I32_MAX + 1, None, 3, -2, 2], "a": [1, 1, 1, None, 0, 0, 1 << 64],
+                      "b": [R.I64_MAX, R.I64_MIN, 0, 0, 0, 0, 0]}, joins={1: plain, 2: direct, 3: tup})
+    assert ev.eval(("probe", 1, col("k"))) == [10, 30, None, None, None, None, R.OneOf([20, 21])]
+    assert ev.eval(("probe", 2, col("k"))) == [101, None, None, None, None, 98, 102]  # outside [min, max]: no match
+    # a NULL component, or one outside int64 (2^64), never matches; a multimap key's payload is any of its entries
+    assert ev.eval(("probe", 3, col("a"), col("b"))) == [7, 8, None, None, R.OneOf([9, 10]), R.OneOf([9, 10]), None]
+    assert R.same_cell(21, R.OneOf([20, 21])) and not R.same_cell(22, R.OneOf([20, 21])) and not R.same_cell(None, R.OneOf([20]))
+    outs, src = ev.run([("probe_each", 3, col("a"), col("b"), "outer")])
+    assert src == [0, 1, 2, 3, 4, 4, 5, 5, 6] and outs[0] == [7, 8, None, None, 9, 10, 9, 10, None]
+
+
+def test_exists_and_the_outer_join_with_a_residual():
+    mm = R.Join("plain", [(1, 0), (1, 1), (1, 2), (2, 3), (3, 4)])
+    side = R.Side({"v": [None, None, 5, None, 1]})  # key 1: NULL, NULL, then TRUE; key 2: NULL only; key 3: FALSE
+    ev = R.Evaluator({"k": [1, 2, 3, 4, None], "x": [5, 5, 5, 5, 5]}, joins={9: mm}, sides={8: side})
+    cond = ("cmp", "=", ("fetch", 8, ("match", 9), "v"), col("x"))
+    assert ev.eval(("exists", 9, col("k"), cond)) == [1, 0, 0, 0, 0]  # NULL is not TRUE; never NULL
+    assert ev.eval(("exists", 9, col("k"), None)) == [1, 1, 1, 0, 0]
+    assert ev.eval(("not", ("exists", 9, col("k"), cond))) == [0, 1, 1, 1, 1]
+    outs, src = ev.run([("rowid",), ("exists", 9, col("k"), cond)], where=("exists", 9, col("k"), None))
+    assert outs == [[0, 1, 2], [1, 0, 0]]
+    # each passing match, or exactly one NULL tuple
+    m = ("probe_each", 9, col("k"), "outer", ("on", cond))
+    outs, src = ev.run([("rowid",), m, ("fetch", 8, m, "v")])
+    assert src == [0, 1, 2, 3, 4] and outs[1] == [2, None, None, None, None] and outs[2] == [5, None, None, None, None]
+    # a residual that reads the PROBE_EACH payload, and an EXISTS keyed by a value fetched through it
+    e = ("probe_each", 9, col("k"))
+    inner = ("exists", 9, ("add", ("fetch", 8, e, "v"), const(-4)), ("cmp", "!=", ("match", 9), e))
+    outs, src = ev.run([e, inner])
+    assert src == [0, 0, 0, 1, 2] and outs == [[0, 1, 2, 3, 4], [0, 0, 1, 0, 0]]  # v = 5 → key 1, whose matches 0, 1 differ from 2
+
+
+def test_mark_values_and_effects():
+    mm = R.Join("plain", [(1, 0), (1, 1), (2, 2)])
+    uq = R.Join("tuple", [((1, 1 << 40), 5), ((2, 0), 6)], n_keys=2)
+    ev = R.Evaluator({"k": [1, 2, 3, None, 1], "c": [1, None, 1, 1, 0]}, joins={1: mm, 2: uq})
+    t = ("cmp", "=", col("c"), const(1))  # TRUE, NULL, TRUE, TRUE, FALSE
+    # through PROBE on a multimap: at least one entry of key 1; key 2's condition is NULL, key 3 has no entry
+    assert ev.eval(("mark", ("probe", 1, col("k")), t)) == [1, 0, 0, 0, 0]
+    assert mm.marks.must == set() and mm.marks.some == {(1,)}
+    mm.marks.check(mm, {0})
+    mm.marks.check(mm, {0, 1})
+    for bad in (set(), {2}, {0, 2}):
+        with pytest.raises(AssertionError):
+            mm.marks.check(mm, bad)
+    # through PROBE_EACH: every walked match with a TRUE condition
+    outs, _ = ev.run([("mark", ("probe_each", 1, col("k")), t)])
+    assert outs == [[1, 1, 0, 0, 0]] and mm.marks.must == {0, 1}  # rows 0 (two matches), 1 (NULL condition), 4 (two, FALSE)
+    with pytest.raises(AssertionError):
+        mm.marks.check(mm, {0})
+    mm.marks.check(mm, {0, 1})
+    # through an outer PROBE_EACH with a residual: the walk reaches the rejected matches of a key with a passing one
+    mm.clear_marks()
+    on = ("probe_each", 1, col("k"), "outer", ("on", ("cmp", "=", ("match", 1), const(1))))
+    outs, src = ev.run([on, ("mark", on, const(1))])
+    assert outs == [[1, None, None, None, 1], [1, 0, 0, 0, 1]] and mm.marks.must == {0, 1}  # entry 0 is walked, not kept
+    # through PROBE of a key-tuple table: the one entry; markers accumulate until cleared
+    ev2 = R.Evaluator({"a": [1, 2, 2], "b": [1 << 40, 0, 1 << 64]}, joins={2: uq})
+    assert ev2.eval(("mark", ("probe", 2, col("a"), col("b")), const(1))) == [1, 1, 0]
+    assert ev2.eval(("mark", ("probe", 2, col("a"), col("b")), ("cmp", "=", col("a"), const(1)))) == [1, 0, 0]
+    assert uq.marks.must == {5, 6}
+    uq.clear_marks()
+    assert uq.marks.must == set()
+
+
+def test_string_codes():
+    d = {b"a": 1, b"bc": 0}
+    ev = R.Evaluator({"s": [b"a", b"bc", b"zz", None], "i": [1, 0, 1, 1]}, dicts={4: d})
+    assert ev.eval(("strcode", 4, "s", "lookup")) == [1, 0, None, None]  # absent strings are NULL
+    assert ev.inserted == {}
+    outs, src = ev.run([("strcode", 4, "s")], where=("cmp", "=", col("i"), const(1)))
+    assert ev.inserted == {4: {b"a", b"bc", b"zz"}}  # what the inserting STRCODE saw, WHERE or not
+    assert R.check_dictionary([b"bc", b"a"], [1, 0], {b"a", b"bc"}) == d
+    for strings, ranks, keys in (([b"bc", b"a"], [0, 1], {b"a", b"bc"}), ([b"a", b"a"], [0, 1], {b"a"}), ([b"a"], [0], {b"a", b"b"})):
+        with pytest.raises(AssertionError):
+            R.check_dictionary(strings, ranks, keys)
+
+
+def test_order_by_is_a_stable_sort_over_the_whole_i128():
+    vals = [1 << 64, 1, -1, -(1 << 64), R.I128_MIN, R.I128_MAX]
+    assert R.order_rows(vals) == [4, 3, 2, 1, 0, 5]
+    assert R.order_rows(vals, descending=True) == [5, 0, 1, 2, 3, 4]
+    ties = [2, -(1 << 64), 2, 1 << 64, -(1 << 64)]
+    assert R.order_rows(ties) == [1, 4, 0, 2, 3] and R.order_rows(ties, descending=True) == [3, 0, 2, 1, 4]
+
+
 def test_aggregates():
     assert R.group_by(0, [], [("count_star", None), ("sum", []), ("min", [])]) == {(): [0, None, None]}
     g = R.group_by(4, [[1, None, 1, None]], [("min", [-5, None, 3, None]), ("count", [1, None, 2, None]), ("max", [R.I64_MIN - 1, 2, None, None])])
