@@ -619,6 +619,28 @@ int ldb_gpu_comm_allgather_small(LdbComm* comm, const void* dev_src, int64_t byt
  * and folds the peers' images into its own table — ONE kernel instead of export + all-gather + merge.  Afterwards every
  * rank holds the full result.  SIMPLE and GROUPBY states (capacity <= 1024). */
 int ldb_gpu_groupby_allmerge(LdbState* s, LdbComm* comm, LdbError* err);
+/* Partitioned merge of program hash aggregations across the ranks of `comm` (rt::PreAggregationHashtable::merge,
+ * PreAggregationHashtable.cpp:76-153, across GPUs).  Collective: every rank calls it in the same order.
+ * `local` and `owned` are two distinct LDB_STATE_HASHAGG states of comm's context with the same key count and the same aggregate
+ * kinds in the same order (else LDB_ERR_INVALID).  `local` is only read.
+ *   Keyed states (1..4 keys): every group of `local` goes to its owner rank ((h >> 32) * world) >> 32, h = the hash that places
+ *   the group in its table (low bits place, high bits own), and is folded into the owner's `owned`.  Afterwards the ranks' `owned`
+ *   states hold disjoint sets of groups whose union is the aggregation over every rank's input.  Groups already in `owned` (an
+ *   earlier exchange, say) stay and accumulate.
+ *   Keyless states: every rank's entry goes to every rank (an all-reduce): every rank's `owned` holds the one row.
+ * Combine, per aggregate, from a received entry into the owner's: COUNT / COUNT_STAR add; the others only when the received entry
+ * has seen a value: SUM adds at 128 bits, SUM_F64 adds the doubles, MIN / MAX (_F64) keep the better value, ANY takes the received
+ * value when the owner's entry has none yet.  NULL-ness of aggregates and keys comes through.
+ * Receive region: recv_offset is a user-heap offset, identical on every rank.  Source s owns `capacity` entries of 48 + 16 n_aggs
+ * bytes at recv_offset + s * capacity * entry_bytes; behind the world * capacity entries the call keeps 2 * 8 * 8 bytes of
+ * cursors and counts.  A region outside the user heap or an offset that is not a multiple of 16: LDB_ERR_INVALID.
+ * Overflow: a source with more than `capacity` groups for one rank writes the first `capacity` and counts the rest; nothing
+ * outside the claimed ranges is written.  Every rank that received too many fails with LDB_ERR_CAPACITY, naming the largest
+ * per-source count (retry with that capacity, into fresh `owned` states: the other ranks have merged); its `owned` is then
+ * unspecified.  An `owned` directory that fills up fails through ldb_gpu_hashagg_count ("table full").
+ * The call reads the received counts on the host (it synchronises the compute stream): inside a captured query it fails with
+ * LDB_ERR_UNSUPPORTED before enqueueing anything.  Ranks of one process must call it from one thread each. */
+int ldb_gpu_hashagg_exchange(LdbState* local, LdbState* owned, LdbComm* comm, int64_t recv_offset, int64_t capacity, LdbError* err);
 /* zero / read back (synchronising) a range of this rank's user heap */
 int ldb_gpu_comm_heap_zero(LdbComm* comm, int64_t user_offset, int64_t bytes, LdbError* err);
 int ldb_gpu_comm_heap_read(LdbComm* comm, int64_t user_offset, int64_t bytes, void* host_dst, LdbError* err);

@@ -15,6 +15,7 @@
 #include "context.h"
 #include "device_utils.cuh"
 #include "peer.h"
+#include "program.h"
 
 #include <algorithm>
 #include <cstring>
@@ -237,6 +238,7 @@ int ldb_gpu_comm_create(LdbContext* ctx, int32_t rank, int32_t world, int64_t us
       LDB_CUDA(cudaFuncGetAttributes(&fa, peerGroupAllMergeKernel));
       LDB_CUDA(cudaFuncGetAttributes(&fa, peerOrReduceKernel));
       LDB_CUDA(cudaFuncGetAttributes(&fa, peerPublishCountsKernel));
+      loadHashAggExchangeKernels();
       cudaIpcMemHandle_t h;
       LDB_CUDA(cudaIpcGetMemHandle(&h, c->heap));
       static_assert(sizeof(h) == LDB_IPC_HANDLE_BYTES, "cudaIpcMemHandle_t is 64 bytes");
@@ -451,6 +453,72 @@ int ldb_gpu_probe_received_groupby2(LdbState* table, LdbState* groups, LdbComm* 
       ctx->launch("join_probe_received_groupby", [&] {
          launchProbeReceivedGroupBy2(table->join, groups->group, user + recv_offset, c->world, capacity, (const unsigned long long*) (user + counts_offset), ctx->smCount, ctx->compute);
       });
+   });
+}
+
+// Partitioned merge of program hash aggregations (include/ldb_gpu.h).  User-heap layout from recv_offset: the receive region (world
+// sub-regions of `capacity` entries, program.h HashAggShip), then this rank's cursors u64[kMaxPeers], then its counts u64[kMaxPeers].
+// barrier (nobody still merges an earlier exchange out of the region) → zero cursors → send → publish counts → barrier → host read of
+// the counts (overflow check) → merge.
+static_assert(kMaxPeers == sizeof(HashAggShip::recv) / sizeof(uint8_t*), "HashAggShip holds one receive region per peer");
+int ldb_gpu_hashagg_exchange(LdbState* local, LdbState* owned, LdbComm* c, int64_t recv_offset, int64_t capacity, LdbError* err) {
+   return guarded(err, [&] {
+      if (!local || !owned || !c) fail(LDB_ERR_INVALID, "null argument");
+      if (local->kind != LDB_STATE_HASHAGG || owned->kind != LDB_STATE_HASHAGG) fail(LDB_ERR_INVALID, "the exchange takes two hash aggregation states");
+      if (local == owned) fail(LDB_ERR_INVALID, "local and owned must be two distinct states");
+      if (local->ctx != c->ctx || owned->ctx != c->ctx) fail(LDB_ERR_INVALID, "states and comm belong to different contexts");
+      const HashAggDev& lt = local->hashagg;
+      const HashAggDev& ot = owned->hashagg;
+      if (lt.nKeys != ot.nKeys) fail(LDB_ERR_INVALID, "local and owned have different key counts");
+      if (lt.nAggs != ot.nAggs) fail(LDB_ERR_INVALID, "local and owned have different aggregate counts");
+      for (int a = 0; a < lt.nAggs; a++)
+         if (local->aggKinds[a] != owned->aggKinds[a]) fail(LDB_ERR_INVALID, "local and owned have different aggregate kinds");
+      wantConnected(c);
+      const int64_t entry = (int64_t) lt.entryBytes, tail = 2 * 8 * kMaxPeers;
+      const int64_t user = (int64_t) c->userBytes;
+      if (capacity < 0 || recv_offset < 0 || recv_offset % 16 || recv_offset > user || capacity > (user - recv_offset) / entry / c->world ||
+          (int64_t) c->world * capacity * entry + tail > user - recv_offset)
+         fail(LDB_ERR_INVALID, "receive region outside the comm's user heap or not 16-byte aligned");
+      LdbContext* ctx = c->ctx;
+      if (ctx->capturing) fail(LDB_ERR_UNSUPPORTED, "the hash aggregation exchange reads the received counts on the host and cannot be captured");
+      LDB_CUDA(cudaSetDevice(ctx->device));
+      const size_t cursorsOff = (size_t) recv_offset + (size_t) c->world * (size_t) capacity * (size_t) entry, countsOff = cursorsOff + 8 * kMaxPeers;
+      uint8_t* heap = c->heap + kUserOff;
+      HashAggShip x{};
+      for (int d = 0; d < c->world; d++) x.recv[d] = c->peerHeap[d] + kUserOff + recv_offset;
+      x.cursors = (unsigned long long*) (heap + cursorsOff);
+      x.counts = (const unsigned long long*) (heap + countsOff);
+      x.capacity = capacity;
+      x.rank = c->rank;
+      x.world = c->world;
+      for (int a = 0; a < lt.nAggs; a++) x.kinds[a] = local->aggKinds[a];
+      // the counts are read into pinned memory (allocated before the first barrier): a copy into pageable memory blocks inside the driver
+      // while this rank's barrier waits for the peers, and a peer of the same process could then not launch its own barrier
+      unsigned long long* counts = (unsigned long long*) ctx->scratch();
+      int32_t* timedOut = (int32_t*) (counts + kMaxPeers);
+      auto barrier = [&] {
+         if (c->world == 1) return;
+         ctx->launch("peer_barrier", [&] {
+            peerBarrierKernel<<<c->world, 32, 0, ctx->compute>>>(c->view());
+            peerBumpKernel<<<1, 1, 0, ctx->compute>>>(c->view(), EPOCH_BARRIER, -1);
+         });
+      };
+      barrier();
+      ctx->launch("hashagg_send", [&] {
+         LDB_CUDA(cudaMemsetAsync(x.cursors, 0, 8 * kMaxPeers, ctx->compute));
+         launchHashAggSend(lt, x, ctx->smCount, ctx->compute);
+         peerPublishCountsKernel<<<1, 32, 0, ctx->compute>>>(c->view(), kUserOff + cursorsOff, kUserOff + countsOff);
+      });
+      barrier();
+      LDB_CUDA(cudaMemcpyAsync(counts, x.counts, 8 * (size_t) c->world, cudaMemcpyDeviceToHost, ctx->compute));
+      LDB_CUDA(cudaMemcpyAsync(timedOut, c->error, 4, cudaMemcpyDeviceToHost, ctx->compute));
+      ctx->syncStream(ctx->compute);
+      if (*timedOut) fail(LDB_ERR_CUDA, "a peer did not arrive at a collective within the timeout (LDB_PEER_TIMEOUT_MS)");
+      const unsigned long long most = *std::max_element(counts, counts + c->world);
+      if (most > (unsigned long long) capacity)
+         fail(LDB_ERR_CAPACITY, "hash aggregation exchange: a source sent this rank " + std::to_string(most) + " groups, more than the receive capacity " +
+                                   std::to_string(capacity) + "; retry with capacity " + std::to_string(most));
+      ctx->launch("hashagg_merge", [&] { launchHashAggMerge(ot, x, most, ctx->smCount, ctx->compute); });
    });
 }
 

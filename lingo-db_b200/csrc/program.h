@@ -162,6 +162,21 @@ void launchProgram(const ProgramParams& p, int smCount, cudaStream_t s);
 void launchHashAggInit(const HashAggDev& t, int smCount, cudaStream_t s);
 // compacts the occupied entries into columnar buffers: keys (int64 + validity byte), aggregates (16 B + validity byte)
 void launchHashAggExport(const HashAggDev& t, int64_t* const* keyCols, uint8_t* const* keyValid, uint8_t* const* aggCols, uint8_t* const* aggValid, unsigned long long* counter, uint32_t countAggMask, int smCount, cudaStream_t s);
+// Exchange of hash aggregations across the ranks of a comm (ldb_gpu_hashagg_exchange, peer.cu).  Received entries are table entries
+// as above, copied whole (state, flags with the seen / claim / key-NULL bits, keys, aggregates): source s's j-th entry sits at
+// recv[d] + (s * capacity + j) * entryBytes of rank d.  The owner of a group is ((h >> 32) * world) >> 32 for its placement hash h.
+struct HashAggShip {
+   uint8_t* recv[8];                  // every rank's receive region (peer-mapped; own at [rank]), kMaxPeers entries
+   unsigned long long* cursors;       // send: this rank's per-destination position counters, zeroed before
+   const unsigned long long* counts;  // merge: the entries source s sent this rank, published by the sources
+   int64_t capacity;                  // entries per source sub-region
+   int32_t rank, world;
+   int32_t kinds[kProgMaxAggs];       // the aggregates' LdbAggKind
+};
+void launchHashAggSend(const HashAggDev& local, const HashAggShip& x, int smCount, cudaStream_t s);
+// maxReceived: the largest min(counts[s], capacity) (sizes the grid)
+void launchHashAggMerge(const HashAggDev& owned, const HashAggShip& x, uint64_t maxReceived, int smCount, cudaStream_t s);
+void loadHashAggExchangeKernels(); // loads both kernels now (collective launches must not wait for a lazy module load)
 // LSD radix sort of (64-bit key, 32-bit row id) pairs — ORDER BY / top-k over materialised rows (GrowingBuffer::sort, Sorting.cpp)
 void launchRadixSortPairs(unsigned long long* keys, uint32_t* vals, unsigned long long* keysTmp, uint32_t* valsTmp, int64_t n, unsigned int* histScratch, int smCount, cudaStream_t s);
 // multi-key ORDER BY: the 64-bit sort words of one key at the current permutation `ids` (first = 1: ids := 0..n-1 first).

@@ -97,6 +97,7 @@ class Comm:
     def __init__(self, ctx, rank: int, world: int, user_bytes: int = 0, exchange=None, connect: bool = True):
         from . import capi
         self.ctx, self.rank, self.world, self.L = ctx, rank, world, ctx.L
+        self._local = None  # local_group: what the ranks of this process share (host barrier, per-rank counts)
         self.h = C.c_void_p()
         handle = (C.c_uint8 * 64)()
         e = capi.Error()
@@ -121,6 +122,11 @@ class Comm:
         arr = (C.c_void_p * len(comms))(*[c.h for c in comms])
         e = capi.Error()
         capi.check(comms[0].L.ldb_gpu_comm_connect_local(arr, len(comms), C.byref(e)), e)
+        import threading
+        import types
+        shared = types.SimpleNamespace(barrier=threading.Barrier(len(comms)), counts=[0] * len(comms))
+        for c in comms:
+            c._local = shared
         return comms
 
     def close(self):
@@ -138,6 +144,50 @@ class Comm:
         from . import capi
         e = capi.Error()
         capi.check(self.L.ldb_gpu_groupby_allmerge(state, self.h, C.byref(e)), e)
+
+    def hashagg_exchange(self, local, owned, capacity: int = None, recv_offset: int = 0):
+        """Partitioned merge of program hash aggregations (ldb_gpu_hashagg_exchange): every group of `local` is folded into `owned` on
+        the rank that owns its key hash, so the ranks' `owned` states hold disjoint groups whose union is the whole aggregation; a
+        keyless state is merged on every rank.  Collective, and it waits for the peers on the host: the ranks of one process call it
+        from one thread each.  The receive region starts at user-heap offset `recv_offset`; without a `capacity` it holds the largest
+        group count of any rank's `local` per source (found by a host barrier in one process, a small all-gather across processes)."""
+        from . import capi
+        e = capi.Error()
+        if capacity is None:
+            n = C.c_int64()
+            capi.check(self.L.ldb_gpu_hashagg_count(local, C.byref(n), C.byref(e)), e)
+            capacity = max(self._gather_counts(int(n.value)))
+        capi.check(self.L.ldb_gpu_hashagg_exchange(local, owned, self.h, int(recv_offset), int(capacity), C.byref(e)), e)
+
+    def _gather_counts(self, n: int) -> List[int]:
+        """every rank's `n`, in rank order"""
+        if self.world == 1:
+            return [n]
+        if self._local is not None:
+            self._local.counts[self.rank] = n
+            self._local.barrier.wait()
+            out = list(self._local.counts)
+            self._local.barrier.wait()  # nobody overwrites its count before every rank has read them all
+            return out
+        import torch
+
+        from . import capi
+        # no device-wide synchronisation and no pageable copy here: the all-gather kernel waits for the peers, and a device-wide wait
+        # would also wait for that kernel.  The block is pinned host memory the kernel reads through unified addressing; the result
+        # comes back into pinned memory on a stream of its own.
+        dev = torch.device("cuda", self.ctx.device)
+        block = torch.tensor([n, 0], dtype=torch.int64).pin_memory()
+        res, e = C.c_void_p(), capi.Error()
+        capi.check(self.L.ldb_gpu_comm_allgather_small(self.h, C.c_void_p(block.data_ptr()), 16, C.byref(res), C.byref(e)), e)
+        self.ctx.synchronize()
+        slot = int(self.L.ldb_gpu_comm_slot_bytes())
+        out = torch.empty(2 * self.world, dtype=torch.int64).pin_memory()
+        side = torch.cuda.Stream(dev)
+        with torch.cuda.stream(side):
+            for r in range(self.world):
+                out[2 * r: 2 * r + 2].view(torch.int32).copy_(_device_view(res.value + r * slot, 4, dev), non_blocking=True)
+        side.synchronize()
+        return [int(out[2 * r]) for r in range(self.world)]
 
     def check(self):
         from . import capi
