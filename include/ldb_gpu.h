@@ -463,7 +463,12 @@ enum LdbOp {
                             WHERE (residual' OR ISNULL(m)) AND user_where, residual' = the residual against the PROBE_EACH match m.
                           A probe row yields exactly its matches that pass the residual, or one NULL-extended tuple when none does. */
 };
-/* SUM wraps at 128 bits; MIN / MAX compare signed 128-bit values; the _F64 kinds work on doubles */
+/* SUM wraps at 128 bits; MIN / MAX compare signed 128-bit values; the _F64 kinds work on doubles.
+ * SUM_F64 adds in an unspecified order, starting from +0.0: any NaN input, or both +inf and -inf, gives NaN; else an infinite input
+ * gives that infinity; else the result is within gamma_m * sum|x| of the exact sum of the m inputs (gamma_m = m u / (1 - m u),
+ * u = 2^-53), and a zero result is +0.0.  Finite inputs whose sum overflows may give ±inf or NaN depending on the order.
+ * MIN_F64 / MAX_F64 are deterministic to the bit: NaN inputs are ignored unless every non-NULL input is NaN (the result is then
+ * NaN), -0.0 orders below +0.0, ±inf are ordinary values. */
 enum LdbAggKind { LDB_AGG_SUM = 1, LDB_AGG_SUM_F64 = 2, LDB_AGG_COUNT = 3, LDB_AGG_COUNT_STAR = 4, LDB_AGG_MIN = 5, LDB_AGG_MAX = 6,
                   LDB_AGG_MIN_F64 = 7, LDB_AGG_MAX_F64 = 8, LDB_AGG_ANY = 9 };
 typedef struct LdbInstr {

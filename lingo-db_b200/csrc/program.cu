@@ -414,8 +414,8 @@ __device__ __forceinline__ uint8_t* hashAggFindIn(const HashAggDev& t, const Kin
                      hi = ~0ull >> 1;
                      break;
                   case LDB_AGG_MAX: hi = 1ull << 63; break; // INT128_MIN
-                  case LDB_AGG_MIN_F64: lo = (unsigned long long) __double_as_longlong(INFINITY); break;
-                  case LDB_AGG_MAX_F64: lo = (unsigned long long) __double_as_longlong(-INFINITY); break;
+                  case LDB_AGG_MIN_F64:
+                  case LDB_AGG_MAX_F64: lo = kF64MinMaxIdentity; break;
                   default: break;
                }
                ea[2 * a] = lo;
@@ -457,10 +457,24 @@ __device__ __forceinline__ void atomicMinMax128(unsigned long long* cell, s128 x
       cur = prev;
    }
 }
-// MIN / MAX of a double cell: a CAS loop that ends once the cell holds a value at least as good as d
+// The order MIN_F64 / MAX_F64 keep (include/ldb_gpu.h, LdbAggKind): NaN loses to every other value, -0.0 orders below +0.0, ±inf
+// are ordinary values.  So the result does not depend on the order of the updates, and a group whose non-NULL inputs are all NaN ends
+// at NaN.  For non-NaN doubles the integer key b ^ ((b >> 63) & INT64_MAX) of the bits b orders like the values, with -0.0 < +0.0.
+__device__ __forceinline__ long long f64OrderKey(double x) {
+   const long long b = __double_as_longlong(x);
+   return b ^ ((b >> 63) & 0x7fffffffffffffffll);
+}
+__device__ __forceinline__ bool f64Better(double d, unsigned long long cur, bool isMin) {
+   const double c = __longlong_as_double((long long) cur);
+   if (isnan(d)) return false;
+   if (isnan(c)) return true;
+   return isMin ? f64OrderKey(d) < f64OrderKey(c) : f64OrderKey(d) > f64OrderKey(c);
+}
+// MIN / MAX of a double cell: a CAS loop that ends once the cell holds a value at least as good as d.  The cell only ever gets
+// better, so a "not better" decision on the plain 8-byte read stays true.
 __device__ __forceinline__ void atomicMinMaxF64(unsigned long long* lo, double d, bool isMin) {
    unsigned long long cur = *((volatile unsigned long long*) lo);
-   while (isMin ? d < __longlong_as_double((long long) cur) : d > __longlong_as_double((long long) cur)) {
+   while (f64Better(d, cur, isMin)) {
       const unsigned long long prev = atomicCAS(lo, cur, (unsigned long long) __double_as_longlong(d));
       if (prev == cur) break;
       cur = prev;

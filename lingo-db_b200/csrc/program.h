@@ -20,6 +20,8 @@ constexpr int kProgStringBytes = 32;
 constexpr int kProgMaxTables = 4;
 constexpr int kProgMaxKeys = 4;
 constexpr int kProgMaxAggs = 8;
+// the identity of MIN_F64 / MAX_F64 cells: the canonical quiet NaN, which every other value replaces (program.cu, f64Better)
+constexpr uint64_t kF64MinMaxIdentity = 0x7ff8000000000000ull;
 
 // one batch of a side table (the device-resident batch directory of a side column over a multi-batch table)
 struct ProgSideBatch {

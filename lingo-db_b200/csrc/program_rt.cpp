@@ -63,15 +63,14 @@ int ldb_gpu_hashagg_create(LdbContext* ctx, int32_t n_keys, int32_t n_aggs, cons
          *(uint32_t*) e.data() = 2;
          unsigned long long* ea = (unsigned long long*) (e.data() + 48);
          for (int a = 0; a < n_aggs; a++) {
-            double inf = 1.0 / 0.0, ninf = -inf;
             switch (aggs[a].kind) {
                case LDB_AGG_MIN: // INT128_MAX
                   ea[2 * a] = ~0ull;
                   ea[2 * a + 1] = ~0ull >> 1;
                   break;
                case LDB_AGG_MAX: ea[2 * a + 1] = 1ull << 63; break; // INT128_MIN
-               case LDB_AGG_MIN_F64: memcpy(&ea[2 * a], &inf, 8); break;
-               case LDB_AGG_MAX_F64: memcpy(&ea[2 * a], &ninf, 8); break;
+               case LDB_AGG_MIN_F64:
+               case LDB_AGG_MAX_F64: ea[2 * a] = kF64MinMaxIdentity; break;
                default: break;
             }
          }

@@ -34,6 +34,8 @@ import datetime
 import math
 import random
 import struct
+import sys
+from fractions import Fraction
 from typing import Dict, List, Optional
 
 import numpy as np
@@ -462,12 +464,135 @@ def same_cell(got: Optional[int], want) -> bool:
         return got is None and want is None
     if isinstance(want, OneOf):
         return got in want
+    if isinstance(want, (F64Sum, F64Exact)):
+        return got >> 64 == 0 and want == bits_f64(got)
     if isinstance(want, float) and math.isnan(want):
         return got >> 64 == 0 and math.isnan(bits_f64(got))
     return got == cell(want)
 
 
 # ---------------------------------------------------------------------------------------------------- aggregates
+# The double aggregates are modelled by rules that do not depend on the order in which the device adds or compares the inputs:
+#   SUM_F64 over a group's non-NULL inputs x_1..x_m: NaN when some input is NaN or both +inf and -inf occur; else that infinity when one
+#     occurs; else any double within gamma_m * sum|x_i| of the exact sum S (gamma_m = m u / (1 - m u), u = 2^-53), the error bound of
+#     recursive summation in any order and over any addition tree (addition does not round on underflow, so subnormals need no extra
+#     term).  The sum starts from +0.0 and x + (-x) is +0.0, so a zero result is +0.0.
+#   MIN_F64 / MAX_F64: NaN inputs are ignored unless every non-NULL input is NaN (then NaN); -0.0 orders below +0.0; ±inf are ordinary
+#     values.  Deterministic to the bit.
+#   Overflow: a group whose finite inputs have sum|x| <= DBL_MAX / 2 cannot overflow in any order.  Beyond that the model answers only
+#     for finite inputs of one sign and no infinite input: finite when |S| + bound <= DBL_MAX (every partial sum is a sub-sum of one
+#     sign), that sign's infinity when |S| - bound > DBL_MAX (every order overflows).  Any other overflow depends on the order and
+#     raises ValueError: tests deliberately do not assert it.
+U_F64 = Fraction(1, 1 << 53)
+DBL_MAX = sys.float_info.max
+_M53 = (1 << 26) - 1
+
+
+def exact_sum(xs) -> Fraction:
+    """the exact sum of finite doubles (each x = M * 2^(e-53) with an integer |M| < 2^53; the numerators add over a 2^-1127 grid)"""
+    xs = np.asarray(xs, dtype=np.float64)
+    if xs.size == 0:
+        return Fraction(0)
+    if xs.size < 256:
+        total = 0
+        for x in xs.tolist():
+            n, d = x.as_integer_ratio()
+            total += n << (1127 - d.bit_length() + 1)
+        return Fraction(total, 1 << 1127)
+    m, e = np.frexp(xs)
+    mant = (m * 2.0 ** 53).astype(np.int64)
+    order = np.argsort(e, kind="stable")
+    e, mant = e[order], mant[order]
+    exps, starts = np.unique(e, return_index=True)
+    his, los = np.add.reduceat(mant >> 26, starts), np.add.reduceat(mant & _M53, starts)  # segment sums stay far inside int64
+    total = sum(((int(h) << 26) + int(lo)) << (int(x) + 1074) for x, h, lo in zip(exps, his, los))
+    return Fraction(total, 1 << 1127)
+
+
+def sum_bound(m: int, abs_sum: Fraction) -> Fraction:
+    """gamma_m * sum|x|: how far a double sum of m inputs, added in any order, can be from the exact sum"""
+    g = m * U_F64
+    return g / (1 - g) * abs_sum
+
+
+class F64Sum(float):
+    """A SUM_F64 result: the float is the correctly rounded exact sum (or NaN / ±inf); `==` accepts a double by the SUM_F64 rule above."""
+
+    def __new__(cls, value: float, exact: Optional[Fraction] = None, bound: Optional[Fraction] = None):
+        o = super().__new__(cls, value)
+        o.exact, o.bound = exact, bound
+        return o
+
+    def __eq__(self, other):
+        if not isinstance(other, float):
+            return False
+        if self.exact is None:  # NaN or ±inf
+            return math.isnan(other) if math.isnan(self) else other == float(self)
+        if not math.isfinite(other):
+            return False
+        if other == 0.0 and math.copysign(1.0, other) < 0:
+            return False  # a zero sum is +0.0
+        return abs(Fraction(other) - self.exact) <= self.bound
+
+    def __ne__(self, other):
+        return not self.__eq__(other)
+
+    __hash__ = float.__hash__
+
+    def __repr__(self):
+        return f"F64Sum({float(self)!r}, ±{float(self.bound or 0):.3g})"
+
+
+class F64Exact(float):
+    """A MIN_F64 / MAX_F64 result: `==` is bit-for-bit equality with a double (any NaN equals any NaN)."""
+
+    def __eq__(self, other):
+        if not isinstance(other, float):
+            return False
+        return (math.isnan(self) and math.isnan(other)) or f64_bits(other) == f64_bits(self)
+
+    def __ne__(self, other):
+        return not self.__eq__(other)
+
+    __hash__ = float.__hash__
+
+    def __repr__(self):
+        return f"F64Exact({float(self)!r})"
+
+
+def f64_sum(vs: list) -> F64Sum:
+    """SUM_F64 of a group's non-NULL inputs (at least one)"""
+    if any(math.isnan(v) for v in vs) or (math.inf in vs and -math.inf in vs):
+        return F64Sum(math.nan)
+    fin = [v for v in vs if math.isfinite(v)]
+    s, a = exact_sum(fin), exact_sum(np.abs(np.asarray(fin, dtype=np.float64)))
+    bound = sum_bound(len(vs), a)
+    if len(fin) < len(vs):
+        if a > Fraction(DBL_MAX) / 2:
+            raise ValueError("SUM_F64: finite inputs that may overflow next to an infinite one depend on the order")
+        return F64Sum(math.inf if math.inf in vs else -math.inf)
+    if a <= Fraction(DBL_MAX) / 2:
+        return F64Sum(float(s), s, bound)
+    if all(v >= 0 for v in fin) or all(v <= 0 for v in fin):
+        if abs(s) + bound <= Fraction(DBL_MAX):  # every partial sum is a sub-sum of one sign: none reaches |S| + bound
+            return F64Sum(float(s), s, bound)
+        if abs(s) - bound > Fraction(DBL_MAX):
+            return F64Sum(math.inf if s > 0 else -math.inf)
+    raise ValueError("SUM_F64: an overflow that depends on the order is not modelled")
+
+
+def _f64_order(x: float):
+    return (x, math.copysign(1.0, x))  # -0.0 before +0.0
+
+
+def f64_min_max(vs: list, is_min: bool) -> F64Exact:
+    """MIN_F64 / MAX_F64 of a group's non-NULL inputs (at least one)"""
+    xs = [v for v in vs if not math.isnan(v)]
+    if not xs:
+        return F64Exact(math.nan)
+    return F64Exact((min if is_min else max)(xs, key=_f64_order))
+
+
 def aggregate(kind: str, values: list):
     """one aggregate over a group's inputs (None = NULL input, skipped); None when no input was seen (COUNT: 0)"""
     if kind == "count_star":
@@ -480,10 +605,12 @@ def aggregate(kind: str, values: list):
     if kind == "sum":
         return wrap128(sum(vs))
     if kind == "sum_f64":
-        return f64(math.fsum(vs))
-    if kind in ("min", "min_f64"):
+        return f64_sum(vs)
+    if kind in ("min_f64", "max_f64"):
+        return f64_min_max(vs, kind == "min_f64")
+    if kind == "min":
         return min(vs)
-    if kind in ("max", "max_f64"):
+    if kind == "max":
         return max(vs)
     if kind == "any":
         return set(vs)

@@ -188,7 +188,81 @@ def test_aggregates():
     assert g == {(1,): [-5, 2, R.I64_MIN - 1], (None,): [None, 0, 2]}
 
 
+def test_sum_f64_specials():
+    s = lambda vs: R.aggregate("sum_f64", vs)
+    nan, inf = math.nan, math.inf
+    for vs in ([1.0, nan], [nan], [inf, -inf], [-inf, 2.0, inf], [nan, inf]):
+        assert s(vs) == nan and s(vs) == -nan and s(vs) != inf and s(vs) != 0.0, vs
+    assert s([inf, 1.0, -5e-324]) == inf and s([inf, 1.0]) != -inf and s([inf]) != nan and s([inf]) != R.DBL_MAX
+    assert s([-inf, -inf, 3.0]) == -inf and s([-inf]) != inf
+    assert s([None, 1.0]) is not None and R.aggregate("sum_f64", [None, None]) is None
+    assert not s([1.0]).__eq__(None) and s([1.0]) != 1  # only doubles compare equal
+
+
+def test_sum_f64_error_bound():
+    s = lambda vs: R.aggregate("sum_f64", vs)
+    # exact sums: bound gamma_2 * 3 = 6.7e-16 admits one ulp of 3 (4.4e-16), not two
+    assert s([1.0, 2.0]) == 3.0 and s([1.0, 2.0]) == 3.0 + 2.0 ** -51 and s([1.0, 2.0]) != 3.0 + 2.0 ** -50 and s([1.0, 2.0]) != 3.0 - 2.0 ** -50
+    # a rounding sum: S = 1 + 2^-52; left to right gives 1.0 (two ties to even), the other order gives S; both are within the bound
+    r = s([1.0, 2.0 ** -53, 2.0 ** -53])
+    assert r.exact == 1 + R.Fraction(1, 1 << 52) and r == 1.0 and r == 1.0 + 2.0 ** -52 and r != 1.0 + 2.0 ** -50
+    # catastrophic cancellation: S = 1, sum|x| = 2e16 + 1, bound gamma_3 * (2e16 + 1) = 6.66; 1e16 + 1 rounds to 1e16, so 0.0 is a result
+    r = s([1e16, 1.0, -1e16])
+    assert r == 1.0 and r == 0.0 and r == 6.0 and r != 8.0 and r != -8.0 and 6.6 < float(r.bound) < 6.7
+    # a zero sum is +0.0: the sum starts from +0.0 and x + (-x) is +0.0
+    assert s([-0.0]) == 0.0 and s([-0.0]) != -0.0 and s([-0.0, -0.0]) != -0.0 and s([2.5, -2.5]) != -0.0 and s([-0.0, 0.0]) == 0.0
+    # subnormals add without rounding: 3 * 2^-1074 exactly
+    assert s([5e-324] * 3) == 1.5e-323 and s([5e-324] * 3) != 1e-323 and s([5e-324, -5e-324, 5e-324]) == 5e-324
+    # the bound grows with m and sum|x|: 2^20 inputs of 1 + 2^-30 at 2^-53 each
+    r = s([1.0 + 2.0 ** -30] * (1 << 20))
+    assert r.exact == (1 << 20) + R.Fraction(1, 1 << 10) and r.bound == R.sum_bound(1 << 20, r.exact)
+    assert 2.0 ** -14 < float(r.bound) < 2.0 ** -12
+    assert r == float(r.exact) + 2.0 ** -14 and r != float(r.exact) + 2.0 ** -12 and r != float(r.exact) - 1.0  # one update lost is off by ~1
+
+
+def test_sum_f64_overflow():
+    s = lambda vs: R.aggregate("sum_f64", vs)
+    big = R.DBL_MAX
+    assert s([big, big]) == math.inf and s([big, big]) != big and s([-big, -big * 0.75]) == -math.inf
+    assert s([big * 0.51, big * 0.5]) == math.inf  # |S| - bound > DBL_MAX: every order overflows
+    assert s([big / 4, big / 8]) == big * 0.375  # sum|x| <= DBL_MAX / 2: finite in every order
+    assert s([big * 0.3, big * 0.3, big * 0.3]) == big * 0.9 and s([-big * 0.7, -0.0]) == -big * 0.7  # one sign, |S| + bound <= DBL_MAX: finite
+    for vs in ([big, -big, big], [big * 0.6, big * 0.5, -1.0], [math.inf, big, big], [big * 0.6, -big * 0.1], [big, big * 1e-17]):
+        with pytest.raises(ValueError):  # the order decides whether it overflows: not modelled
+            s(vs)
+
+
+def test_exact_sum_is_exact():
+    rng = __import__("random").Random(5)
+    for n in (0, 1, 7, 255, 256, 3000):
+        xs = [rng.choice([1.0, -1.0]) * rng.random() * 2.0 ** rng.randrange(-1074, 1000) for _ in range(n)] + [5e-324, -0.0, R.DBL_MAX / 4]
+        assert R.exact_sum(xs) == sum(map(R.Fraction, xs), R.Fraction(0)), n
+    assert R.exact_sum([R.DBL_MAX] * 300 + [-R.DBL_MAX] * 299) == R.Fraction(R.DBL_MAX)
+
+
+def test_min_max_f64_ignore_nan_and_order_signed_zeros():
+    mn = lambda vs: R.aggregate("min_f64", vs)
+    mx = lambda vs: R.aggregate("max_f64", vs)
+    nan, inf = math.nan, math.inf
+    assert mn([nan, 1.0, nan]) == 1.0 and mx([nan, 1.0, nan]) == 1.0 and mn([nan, 1.0]) != nan
+    assert mn([nan, nan]) == nan and mx([nan]) == nan and mn([nan]) != inf and mx([nan]) != -inf
+    for vs in ([0.0, -0.0], [-0.0, 0.0], [0.0, -0.0, 0.0, nan]):
+        assert mn(vs) == -0.0 and mn(vs) != 0.0 and mx(vs) == 0.0 and mx(vs) != -0.0, vs
+    assert mn([inf, -inf, nan, 3.0]) == -inf and mx([nan, inf, -inf]) == inf and mn([inf, nan]) == inf and mx([-inf]) == -inf
+    assert mn([5e-324, 0.0]) == 0.0 and mn([-5e-324, -0.0]) == -5e-324 and mx([1.0]) != 1.0 + 2.0 ** -52
+    assert mn([None, nan, None]) == nan and mn([None]) is None
+    # the result does not depend on the input order, to the bit
+    vals = [nan, 0.0, -0.0, 5.0, nan, -0.0, 0.0]
+    for k in range(len(vals)):
+        rot = vals[k:] + vals[:k]
+        assert R.f64_bits(mn(rot)) == R.f64_bits(-0.0) and R.f64_bits(mx(rot)) == R.f64_bits(5.0)
+        assert R.f64_bits(mx([x for x in rot if x != 5.0])) == R.f64_bits(0.0)
+
+
 def test_cells_compare_bit_for_bit():
+    assert R.same_cell(R.f64_bits(0.0), R.aggregate("sum_f64", [1.0, -1.0])) and not R.same_cell(R.f64_bits(-0.0), R.aggregate("sum_f64", [-0.0]))
+    assert R.same_cell(R.f64_bits(-0.0), R.aggregate("min_f64", [0.0, -0.0])) and not R.same_cell(R.f64_bits(0.0), R.aggregate("min_f64", [0.0, -0.0]))
+    assert R.same_cell(R.f64_bits(math.nan), R.aggregate("max_f64", [math.nan])) and not R.same_cell(1 << 64, R.aggregate("max_f64", [0.0]))
     assert R.same_cell(R.f64_bits(math.nan) | 1, math.nan)
     assert not R.same_cell(R.f64_bits(0.0), -0.0)
     assert R.same_cell(-1, -1) and not R.same_cell((1 << 128) - 1, 1)
