@@ -157,7 +157,9 @@ __device__ __forceinline__ int64_t ldShared64(uint32_t addr) {
 __device__ __forceinline__ void ldShared64x2(uint32_t addr, int64_t& a, int64_t& b) { // addr 16-byte aligned
    asm volatile("ld.shared.v2.s64 {%0, %1}, [%2];" : "=l"(a), "=l"(b) : "r"(addr));
 }
-
+__device__ __forceinline__ void ldShared32x2(uint32_t addr, uint32_t& a, uint32_t& b) { // addr 8-byte aligned
+   asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(a), "=r"(b) : "r"(addr));
+}
 // ---------------------------------------------------------------- blocked Bloom filter of the join tables
 // Three bit positions inside the 32-bit filter word that (h >> 32) selects, from a second multiply of the hash.  (Deriving them from the
 // low hash word with one 32-bit multiply saves four instructions per probe but raised the false-positive rate enough to slow K9

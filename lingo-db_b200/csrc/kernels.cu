@@ -81,8 +81,6 @@ struct SmemTile<kDecEncoded> {
    }
    __device__ __forceinline__ int64_t lo64(int col, int lr) const { return (int64_t) ((uint64_t) ldShared64(stage + (uint32_t) sc->smemOffset[col]) + field(col, lr)); }
    __device__ __forceinline__ int64_t hi64(int col, int lr) const { return lo64(col, lr) >> 63; }
-   // the tile header: every value of the tile lies in [base, base + range]
-   __device__ __forceinline__ void header(int col, int64_t& base, int64_t& range) const { ldShared64x2(stage + (uint32_t) sc->smemOffset[col], base, range); }
 };
 template <>
 struct GlobalTile<kDecEncoded> {
@@ -105,13 +103,16 @@ struct GlobalTile<kDecEncoded> {
    __device__ __forceinline__ int64_t lo64(int col, int lr) const { return (int64_t) (base(col) + field(col, lr)); }
    __device__ __forceinline__ int64_t hi64(int col, int lr) const { return lo64(col, lr) >> 63; }
 };
-__device__ __forceinline__ void issueTile(const StagedCols& sc, uint8_t* smem, uint64_t* bars /* full[] */, int64_t tile, int s) {
+// A stage holds F consecutive tiles (stage `stage` = tiles stage * F ..): the F tiles of a column are contiguous in HBM and in shared
+// memory (column c from F * smemOffset[c]), so each column still takes one bulk copy.
+template <int F = 1>
+__device__ __forceinline__ void issueTile(const StagedCols& sc, uint8_t* smem, uint64_t* bars /* full[] */, int64_t stage, int s) {
    const uint64_t policy = evictFirstPolicy();
-   mbarExpectTx(&bars[s], (uint32_t) sc.stageBytes);
-   const uint32_t dst = smemAddr(smem) + (uint32_t) s * sc.stageBytes;
+   mbarExpectTx(&bars[s], (uint32_t) (F * sc.stageBytes));
+   const uint32_t dst = smemAddr(smem) + (uint32_t) (s * F * sc.stageBytes);
    for (int c = 0; c < sc.n; c++) {
-      const uint32_t bytes = (uint32_t) sc.elemBytes[c] * (uint32_t) sc.tileRows + (uint32_t) sc.tileHeader;
-      bulkLoad(dst + sc.smemOffset[c], sc.base[c] + (size_t) tile * bytes, bytes, &bars[s], policy);
+      const uint32_t bytes = F * ((uint32_t) sc.elemBytes[c] * (uint32_t) sc.tileRows + (uint32_t) sc.tileHeader);
+      bulkLoad(dst + F * sc.smemOffset[c], sc.base[c] + (size_t) stage * bytes, bytes, &bars[s], policy);
    }
 }
 // fnTile(tile, rowBase, rowsInTile) is called once per tile by every CONSUMER thread (threadIdx.x < kBlock), warps converged.
@@ -177,11 +178,17 @@ __device__ __forceinline__ void forEachTile(const StagedCols& sc, int64_t n, uin
 // Non-specialised variant for the arithmetic-bound group-by kernel (K1/K2): every row costs the same, so the CTA-wide
 // barrier is cheap (stall_barrier 0.1 per issue) and a 9th warp would only cost registers (2 CTAs x 288 threads
 // cap the kernel at 112 registers → spills).  One elected thread issues the copies, __syncthreads() recycles a stage.
-template <int kRowsPerThread, int DB, int kStages = ldb::kStages, class Fn>
+// With F > 1 a TMA stage is F tiles (fnTile gets F * kTileRows rows); the full tiles after the last full stage and the partial
+// tail tile are read tile by tile through GlobalTile, one CTA each, continuing the round robin of the stages.
+template <int kRowsPerThread, int DB, int kStages = ldb::kStages, int F = 1, class Fn>
 __device__ __forceinline__ void forEachTileUniform(const StagedCols& sc, int64_t n, uint8_t* smem, TileBarriers* bars, const Fn& fnTile) {
    constexpr int kTileRows = kRowsPerThread * kBlock;
    const int64_t nFull = n / kTileRows;
+   int64_t done = nFull, turns = nFull; // tiles read by the loops below, and the round-robin turns they took
    if (sc.useTma) {
+      const int64_t nStages = nFull / F;
+      done = nStages * F;
+      turns = nStages;
       if (threadIdx.x == 0) {
          for (int s = 0; s < kStages; s++) mbarInit(&bars->full[s], 1);
          mbarInitFence();
@@ -190,18 +197,18 @@ __device__ __forceinline__ void forEachTileUniform(const StagedCols& sc, int64_t
       if (threadIdx.x == 0) {
          for (int s = 0; s < kStages; s++) {
             int64_t t = (int64_t) blockIdx.x + (int64_t) s * gridDim.x;
-            if (t < nFull) issueTile(sc, smem, bars->full, t, s);
+            if (t < nStages) issueTile<F>(sc, smem, bars->full, t, s);
          }
       }
       int it = 0;
-      for (int64_t t = blockIdx.x; t < nFull; t += gridDim.x, it++) {
+      for (int64_t t = blockIdx.x; t < nStages; t += gridDim.x, it++) {
          const int s = it % kStages;
          mbarWait(&bars->full[s], (uint32_t) (it / kStages) & 1u);
-         SmemTile<DB> tile{smemAddr(smem) + (uint32_t) s * sc.stageBytes, &sc};
-         fnTile(tile, t * kTileRows, kTileRows);
+         SmemTile<DB> tile{smemAddr(smem) + (uint32_t) (s * F * sc.stageBytes), &sc};
+         fnTile(tile, t * F * kTileRows, F * kTileRows);
          __syncthreads(); // every thread is done with stage s → refill it
          const int64_t nt = t + (int64_t) kStages * gridDim.x;
-         if (threadIdx.x == 0 && nt < nFull) issueTile(sc, smem, bars->full, nt, s);
+         if (threadIdx.x == 0 && nt < nStages) issueTile<F>(sc, smem, bars->full, nt, s);
       }
    } else {
       for (int64_t t = blockIdx.x; t < nFull; t += gridDim.x) {
@@ -210,10 +217,11 @@ __device__ __forceinline__ void forEachTileUniform(const StagedCols& sc, int64_t
          __syncthreads(); // same contract as the TMA path: no thread starts the next tile before all finished this one
       }
    }
-   if (nFull * kTileRows < n && (int64_t) blockIdx.x == nFull % gridDim.x) {
+   const int64_t nTiles = (n + kTileRows - 1) / kTileRows;
+   for (int64_t t = done + ((int64_t) blockIdx.x + gridDim.x - turns % gridDim.x) % gridDim.x; t < nTiles; t += gridDim.x) {
       __syncthreads();
-      GlobalTile<DB> tile{nFull * kTileRows, &sc};
-      fnTile(tile, nFull * kTileRows, (int) (n - nFull * kTileRows));
+      GlobalTile<DB> tile{t * kTileRows, &sc};
+      fnTile(tile, t * kTileRows, (int) min(n - t * kTileRows, (int64_t) kTileRows));
    }
 }
 template <int kRowsPerThread, int DB, class Fn>
@@ -654,10 +662,11 @@ __device__ __forceinline__ i128 evalAggDyn(const AggSpec& a, const int64_t* v, i
    }
 }
 
-// Per-tile 64-bit path of the encoded scan.  Value column c of a tile lies in [lo[c], hi[c]] (its block's min and max, from the
+// Per-stage 64-bit path of the encoded scan.  Value column c of a stage lies in [lo[c], hi[c]] (its block's min and max, from the
 // tile header).  A product aggregate qualifies when each of its operands lies in [0, 2^31) and the largest product of the bounds is
-// below 2^61: every row's product is then an exact non-negative int64, and maxRow grows to that bound.
-template <class A>
+// below 2^63 / R (R = rows a thread adds per stage): every row's product is then an exact non-negative int64, R of them still sum
+// below 2^63, and maxRow grows to that bound.
+template <class A, int R>
 __device__ __forceinline__ bool aggBound64(const int64_t* lo, const int64_t* hi, int64_t one, uint64_t& maxRow) {
    if constexpr (A::is64) {
       return true; // a column sum or a count wraps at 64 bits on every path
@@ -673,7 +682,7 @@ __device__ __forceinline__ bool aggBound64(const int64_t* lo, const int64_t* hi,
          ok &= __umul64hi(m, (uint64_t) zh) == 0;
          m *= (uint64_t) zh;
       }
-      ok &= m < (1ull << 61);
+      ok &= m < (1ull << 63) / R;
       if (m > maxRow) maxRow = m;
       return ok;
    }
@@ -707,8 +716,9 @@ struct Aggs {
       ((v[Is] = evalAgg<As, FAST>(vals, one)), ...);
    }
    static __device__ __forceinline__ bool fits32(const int64_t* vals, int64_t one) { return ((aggOperandBits<As>(vals, one) | ...) >> 31) == 0; }
+   template <int R>
    static __device__ __forceinline__ bool bound64(const int64_t* lo, const int64_t* hi, int64_t one, uint64_t& maxRow) {
-      return (aggBound64<As>(lo, hi, one, maxRow) & ...);
+      return (aggBound64<As, R>(lo, hi, one, maxRow) & ...);
    }
    template <int... Is>
    static __device__ __forceinline__ void eval64(int64_t* q, const int64_t* vals, int64_t one, Seq<Is...>) {
@@ -802,14 +812,38 @@ extern __shared__ __align__(128) uint8_t dynSmem[];
 // reference's 1024-slot per-worker pre-aggregation cache (PreAggregationHashtable.cpp:46-60) collapses to
 // this for small domains; further groups use shared-memory atomics, and only a CTA that meets
 // more than LG groups touches the HBM table per row.  One flush per CTA at the end.
-// Encoded full tiles (DB == kDecEncoded) with a shaped filter take their own path: the launcher stages value columns first, then the
-// keys, then the filter's column (launchGB), so their layout is read from the parameter block at constant offsets; each column's tile header is
-// loaded once per tile; and a tile whose header bounds prove every product a non-negative int64 below 2^61 (aggBound64) skips the
-// per-row 32-bit vote and sums those products in 64-bit registers (acc64).
+// Encoded batches with the one-int32-constant filter (Q1) take their own STAGE path (encodedStages): the launcher stages value columns
+// first, then the keys, then the filter's column (launchGB), so their layout is read from the parameter block at constant offsets.  A TMA
+// stage holds kEncFrames consecutive 512-row tiles, which share one header per column (kernels.h), so the headers are read and the
+// 64-bit proof runs once per stage; each thread takes 2 * kEncFrames rows of one tile in runs of 2 adjacent rows, whose fields come from one
+// shared load per column (runs of 4 spilled under the 128-register cap); the filter and the key compares run on the raw fields (constant
+// and keys rebased once per stage); and a stage whose header bounds prove every product a non-negative int64 below
+// 2^63 / rows-per-thread (aggBound64) skips the per-row 32-bit vote and sums those products in 64-bit registers (acc64).  The per-stage
+// cost, paid per 512 rows before, is paid per 512 * kEncFrames rows, and kEncStages - 1 stages stay in flight per CTA while it works on one.
+constexpr int kEncFrames = 4, kEncStages = 3;
+template <int DB, int FS>
+constexpr bool encodedStages = DB == kDecEncoded && FS == FS_I32_ONE;
+// the W-byte fields (W = 1 << sh <= 4) of 2 adjacent rows from shared address a (2W-byte aligned), zero-extended: one shared load
+__device__ __forceinline__ void encodedFields2(uint32_t a, int sh, uint32_t (&x)[2]) {
+   if (sh == 0) {
+      uint16_t v;
+      asm volatile("ld.shared.u16 %0, [%1];" : "=h"(v) : "r"(a));
+      x[0] = v & 0xffu;
+      x[1] = v >> 8;
+   } else if (sh == 1) {
+      const uint32_t v = (uint32_t) ldShared32(a);
+      x[0] = v & 0xffffu;
+      x[1] = v >> 16;
+   } else {
+      ldShared32x2(a, x[0], x[1]);
+   }
+}
 template <int DB, bool IN, int FS, int NK, int NV, class... As>
 __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_constant__ GroupByParams p) {
    using AL = Aggs<As...>;
    constexpr int N = AL::N;
+   constexpr bool kStaged = encodedStages<DB, FS>;
+   constexpr int F = kStaged ? kEncFrames : 1;
    constexpr int GREG = NK == 0 ? 1 : 4; // register-resident groups
    constexpr int LG = 16;                // CTA-local groups (registers + shared)
    __shared__ int32_t sKeys[LG][kMaxKeys];
@@ -836,8 +870,8 @@ __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_cons
    __syncthreads();
 
    i128 acc[GREG][N];
-   // products of the i128 aggregates from proven tiles; `room` is what every acc64 can still take (the same in every thread: a thread
-   // adds at most kRowsPerThreadScan rows of a tile, each at most the tile's maxRow), so acc64 never exceeds INT64_MAX
+   // products of the i128 aggregates from proven stages; `room` is what every acc64 can still take (the same in every thread: a thread
+   // adds at most 2 * F rows of a stage, each at most the stage's maxRow), so acc64 never exceeds INT64_MAX
    int64_t acc64[GREG][N];
    int64_t room = INT64_MAX;
 #pragma unroll
@@ -948,27 +982,32 @@ __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_cons
       else AL::template eval<false>(v, vals, one, typename AL::S{});
       if (pass) add(id, v, k0, k1);
    };
-   auto encodedTile = [&](const SmemTile<kDecEncoded>& tile, int64_t rowBase) {
+   auto encodedStage = [&](uint32_t stage) {
       const StagedCols& sc = p.src.cols;
-      constexpr int FC = NV + NK; // staged index of a shaped filter's column
+      constexpr int FC = NV + NK;                  // staged index of the filter's column
+      constexpr int R = kRowsPerThreadScan * F;    // rows of a thread
+      constexpr int kTileRows = kRowsPerThreadScan * kBlock;
+      constexpr int kFrameThreads = kBlock / F;    // threads per tile of the stage
+      constexpr int kRun = 2;                      // adjacent rows decoded together
+      // column c's F tiles lie from stage + F * smemOffset[c]; their headers are equal (kernels.h), tile 0's stands for all
+      auto col = [&](int c) { return stage + (uint32_t) (F * sc.smemOffset[c]); };
       int64_t vb[NV], lo[NV], hi[NV];
 #pragma unroll
       for (int c = 0; c < NV; c++) {
          int64_t range;
-         tile.header(c, vb[c], range);
+         ldShared64x2(col(c), vb[c], range);
          // a column with a wide range or base gets bounds no operand test passes (and no bound arithmetic overflows)
          const bool small = (uint64_t) range < (1ull << 31) && vb[c] > -(1ll << 40) && vb[c] < (1ll << 40);
          lo[c] = small ? vb[c] : -(1ll << 62);
          hi[c] = small ? vb[c] + range : (1ll << 62);
       }
-      uint32_t kb[NK > 0 ? NK : 1], fb = 0;
+      uint32_t kb[2] = {0, 0};
 #pragma unroll
-      for (int k = 0; k < NK; k++) kb[k] = (uint32_t) ldShared32(tile.stage + (uint32_t) sc.smemOffset[NV + k]);
-      if constexpr (FS == FS_I32_ONE || FS == FS_I32_RANGE) fb = (uint32_t) ldShared32(tile.stage + (uint32_t) sc.smemOffset[FC]);
+      for (int k = 0; k < NK; k++) kb[k] = (uint32_t) ldShared32(col(NV + k));
       uint64_t maxRow = 0;
-      const bool proven = AL::bound64(lo, hi, one, maxRow);
+      const bool proven = AL::template bound64<R>(lo, hi, one, maxRow);
       if (proven) {
-         const int64_t need = (int64_t) maxRow * kRowsPerThreadScan;
+         const int64_t need = (int64_t) maxRow * R;
          if (need > room) {
 #pragma unroll
             for (int g = 0; g < GREG; g++) AL::fold64(acc[g], acc64[g], typename AL::S{});
@@ -976,51 +1015,99 @@ __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_cons
          }
          room -= need;
       }
+      // `v cmp C` on the raw field x = v - base in [0, 2^32) is `flo <= x <= fhi`, negated for != (mask 5)
+      uint32_t flo, fhi;
+      bool finv;
+      {
+         const FilterCol& f = p.src.filters.c[0];
+         const int64_t t = (int64_t) (int32_t) f.valA - (int64_t) ldShared32(col(FC));
+         finv = f.maskA == 5u;
+         const uint32_t m = finv ? 2u : f.maskA;
+         const int64_t l = (m & 1u) ? 0 : (m & 2u) ? t : t + 1, h = (m & 4u) ? 0xffffffffll : (m & 2u) ? t : t - 1;
+         const int64_t lc = l < 0 ? 0 : l, hc = h > 0xffffffffll ? 0xffffffffll : h;
+         flo = lc > hc ? 1u : (uint32_t) lc;
+         fhi = lc > hc ? 0u : (uint32_t) hc;
+      }
+      // the register-resident keys, rebased like the key fields (exact: the decode is base + field modulo 2^32); absolute again
+      // around the general lookup and at the end of the stage
+      auto rebase = [&](uint32_t sign) {
 #pragma unroll
-      for (int j = 0; j < kRowsPerThreadScan; j++) {
-         const int lr = j * kBlock + threadIdx.x;
-         int64_t vals[NV];
-#pragma unroll
-         for (int c = 0; c < NV; c++) vals[c] = (int64_t) ((uint64_t) vb[c] + tile.field(c, lr));
-         int32_t k0 = 0, k1 = 0;
-         if constexpr (NK > 0) k0 = (int32_t) (kb[0] + tile.field32(NV, lr));
-         if constexpr (NK > 1) k1 = (int32_t) (kb[1] + tile.field32(NV + 1, lr));
-         bool pass;
-         if constexpr (FS == FS_I32_ONE || FS == FS_I32_RANGE) {
-            const FilterCol& f = p.src.filters.c[0];
-            const int32_t x = (int32_t) (fb + tile.field32(FC, lr));
-            pass = cmpMask32(x, (int32_t) f.valA, f.maskA);
-            if constexpr (FS == FS_I32_RANGE) pass &= cmpMask32(x, (int32_t) f.valB, f.maskB);
-         } else {
-            pass = evalFilters<IN, FS>(p.src.filters, tile, lr, rowBase + lr);
+         for (int g = 0; g < GREG; g++) {
+            rk0[g] = (int32_t) ((uint32_t) rk0[g] + sign * kb[0]);
+            rk1[g] = (int32_t) ((uint32_t) rk1[g] + sign * kb[1]);
          }
-         const int id = groupOf(k0, k1, pass);
-         if (proven) {
-            int64_t q[N];
-            AL::eval64(q, vals, one, typename AL::S{});
-            if (!pass) continue;
-            if (id >= 0 && id < GREG) {
+      };
+      rebase(~0u);
+      const uint32_t frame = threadIdx.x / kFrameThreads, ft = threadIdx.x % kFrameThreads;
+#pragma unroll 1
+      for (int run = 0; run < R / kRun; run++) {
+         // rows r0 .. r0 + kRun - 1 of tile `frame`: the lanes of a warp read consecutive kRun * W bytes, conflict-free at any W
+         const uint32_t r0 = (run * kFrameThreads + ft) * kRun;
+         auto fields = [&](int c, uint32_t (&x)[kRun]) {
+            const int sh = sc.encShift[c];
+            encodedFields2(col(c) + frame * (kEncodeTileHeader + ((uint32_t) kTileRows << sh)) + kEncodeTileHeader + (r0 << sh), sh, x);
+         };
+         // filter and keys first: only the values stay live while the rows are summed
+         uint32_t xk[2][kRun], xf[kRun];
+#pragma unroll
+         for (int i = 0; i < kRun; i++) xk[0][i] = xk[1][i] = 0;
+#pragma unroll
+         for (int k = 0; k < NK; k++) fields(NV + k, xk[k]);
+         fields(FC, xf);
+         bool pass[kRun];
+         int id[kRun];
+#pragma unroll
+         for (int i = 0; i < kRun; i++) {
+            pass[i] = ((xf[i] >= flo) & (xf[i] <= fhi)) != finv;
+            id[i] = NK > 0 ? -1 : 0;
+            if constexpr (NK > 0) {
 #pragma unroll
                for (int g = 0; g < GREG; g++)
-                  if (id == g) AL::accumulate64(acc[g], acc64[g], q, typename AL::S{});
+                  if (g < rcnt && xk[0][i] == (uint32_t) rk0[g] && xk[1][i] == (uint32_t) rk1[g]) id[i] = g;
+               if (__any_sync(0xffffffffu, pass[i] && id[i] < 0)) { // a key outside the register-resident set: look it up as absolute keys
+                  rebase(1u);
+                  id[i] = groupOf((int32_t) (kb[0] + xk[0][i]), (int32_t) (kb[1] + xk[1][i]), pass[i]);
+                  rebase(~0u);
+               }
+            }
+         }
+         uint32_t xv[NV][kRun];
+#pragma unroll
+         for (int c = 0; c < NV; c++) fields(c, xv[c]);
+#pragma unroll
+         for (int i = 0; i < kRun; i++) {
+            const int32_t k0 = (int32_t) (kb[0] + xk[0][i]), k1 = (int32_t) (kb[1] + xk[1][i]);
+            int64_t vals[NV];
+#pragma unroll
+            for (int c = 0; c < NV; c++) vals[c] = (int64_t) ((uint64_t) vb[c] + xv[c][i]);
+            if (proven) {
+               int64_t q[N];
+               AL::eval64(q, vals, one, typename AL::S{});
+               // a one-hot test per group: an `id == g` test here was folded into a dynamically indexed acc[id], which lives in local memory
+               const uint32_t hot = pass[i] && id[i] >= 0 && id[i] < GREG ? 1u << id[i] : 0u;
+#pragma unroll
+               for (int g = 0; g < GREG; g++)
+                  if (hot >> g & 1u) AL::accumulate64(acc[g], acc64[g], q, typename AL::S{});
+               if (pass[i] && !hot) {
+                  i128 v[N];
+#pragma unroll
+                  for (int a = 0; a < N; a++) v[a] = i128{(uint64_t) q[a], 0}; // what evalAgg gives: products are >= 0 here
+                  add(id[i], v, k0, k1);
+               }
             } else {
                i128 v[N];
-#pragma unroll
-               for (int a = 0; a < N; a++) v[a] = i128{(uint64_t) q[a], 0}; // what evalAgg gives: products are >= 0 here
-               add(id, v, k0, k1);
+               if (__all_sync(0xffffffffu, !pass[i] || AL::fits32(vals, one))) AL::template eval<true>(v, vals, one, typename AL::S{});
+               else AL::template eval<false>(v, vals, one, typename AL::S{});
+               if (pass[i]) add(id[i], v, k0, k1);
             }
-         } else {
-            i128 v[N];
-            if (__all_sync(0xffffffffu, !pass || AL::fits32(vals, one))) AL::template eval<true>(v, vals, one, typename AL::S{});
-            else AL::template eval<false>(v, vals, one, typename AL::S{});
-            if (pass) add(id, v, k0, k1);
          }
       }
+      rebase(1u);
    };
-   forEachTileUniform<kRowsPerThreadScan, DB>(p.src.cols, p.src.nRows, dynSmem, bars, [&](const auto& tile, int64_t rowBase, int rows) {
-      // the descriptor-driven filter costs more per row than the tile path saves (Q6 measured slower), so it keeps the row path
-      if constexpr (std::is_same_v<std::decay_t<decltype(tile)>, SmemTile<kDecEncoded>> && FS != FS_GENERIC) {
-         encodedTile(tile, rowBase);
+   forEachTileUniform<kRowsPerThreadScan, DB, kStaged ? kEncStages : kStages, F>(p.src.cols, p.src.nRows, dynSmem, bars, [&](const auto& tile, int64_t rowBase, int rows) {
+      // the descriptor-driven filter costs more per row than the stage path saves (Q6 measured slower), so it keeps the row path
+      if constexpr (std::is_same_v<std::decay_t<decltype(tile)>, SmemTile<kDecEncoded>> && kStaged) {
+         encodedStage(tile.stage);
       } else {
 #pragma unroll
          for (int j = 0; j < kRowsPerThreadScan; j++) {
@@ -1099,8 +1186,22 @@ static bool hasInList(const FilterSet& f) { // "rare" filters: IN lists and LIKE
 template <int DB, bool IN, int FS, int NK, int NV, class... As>
 static void launchGBd(const GroupByParams& p, int smCount, cudaStream_t s) {
    size_t dyn;
-   int grid = persistentGrid(scanGroupByKernel<DB, IN, FS, NK, NV, As...>, p.src.cols, p.src.nRows, smCount, &dyn, kBlock);
+   constexpr int tiles = encodedStages<DB, FS> ? kEncStages * kEncFrames : kStages; // tiles held in shared memory
+   int grid = persistentGrid(scanGroupByKernel<DB, IN, FS, NK, NV, As...>, p.src.cols, p.src.nRows, smCount, &dyn, kBlock, tiles);
    scanGroupByKernel<DB, IN, FS, NK, NV, As...><<<grid, kBlock, dyn, s>>>(p);
+}
+// The stage path reads fields of at most 4 bytes (an 8-byte field is a value column no product proof admits) and must fit its stages in
+// one CTA's shared memory; other encoded batches take the instance with the descriptor-driven filter.
+template <class K>
+static bool encodedStagesFit(K kernel, const StagedCols& sc) {
+   for (int c = 0; c < sc.n; c++)
+      if (sc.elemBytes[c] > 4) return false;
+   int dev = 0, optin = 0;
+   cudaFuncAttributes fa{};
+   cudaGetDevice(&dev);
+   cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+   cudaFuncGetAttributes(&fa, kernel);
+   return (int64_t) kEncStages * kEncFrames * sc.stageBytes + (int64_t) fa.sharedSizeBytes <= optin;
 }
 // The encoded instance reads its columns' layout at constant indices: value column c is staged column c, key k is NV + k, and a
 // shaped filter's column is NV + NK.  Permutes the staged columns (and every index into them) into that order; returns the filter
@@ -1144,7 +1245,7 @@ static void launchGB(const GroupByParams& p, int smCount, cudaStream_t s) {
          GroupByParams q = p;
          const int fs = toSignatureOrder(q);
          if constexpr (ENC_ONE) {
-            if (fs == FS_I32_ONE) {
+            if (fs == FS_I32_ONE && encodedStagesFit(scanGroupByKernel<kDecEncoded, false, FS_I32_ONE, NK, NV, As...>, q.src.cols)) {
                launchGBd<kDecEncoded, false, FS_I32_ONE, NK, NV, As...>(q, smCount, s);
                return;
             }

@@ -105,6 +105,9 @@ void setTuning(const Tuning& t);
 // column starts at t * (kEncodeTileHeader + kEncodeTileRows * W) with a 16-byte header {base of the tile's block, max - min of that
 // block} followed by the tile's packed values.  One bulk copy then brings a tile's base with its values, and no thread loads a base from HBM.
 constexpr int64_t kEncodeBlockRows = 65536; // = kPackBlockRows of the compressed staging format: a tile never straddles two blocks
+// Invariant of the format: the headers of the kEncodeBlockRows / tileRows (= 128) tiles of one block are equal.  A run of F tiles
+// starting at a multiple of F, F dividing 128, thus lies in one block and shares one header — the encoded Q1 scan reads F tiles of a
+// column with one bulk copy and one header (kernels.cu kEncFrames).
 constexpr int kEncodeTileHeader = 16;
 constexpr int kDecEncoded = 0; // StagedCols::decBytes / kernel DB parameter of the encoded layout
 inline int64_t encodedColumnBytes(int64_t nRows, int width, int tileRows) {
