@@ -555,16 +555,21 @@ int ldb_gpu_hashagg_to_table(LdbState* s, const char* name, LdbTable** out, LdbE
  * sort of (order-preserving 64-bit key, row id) on the device; returns the first `limit` row ids (ties keep row order: stable).
  * column types: int32/date32/fsb4/int64/decimal of any precision, ordered by its full value (a 16-byte cell takes two sort passes:
  * low word, then high word).  A materialized column holding double bits (the materialize sink does not record register types)
- * orders by its bit pattern. */
+ * orders by its bit pattern.  NULLs (validity bytes or an Arrow bitmap) sort after every value, first with DESC, and tie with each
+ * other (SQL's ASC NULLS LAST / DESC NULLS FIRST); a nullable column costs one more, single-digit, sort pass. */
 int ldb_gpu_table_order_by(LdbTable* t, const char* column, int32_t descending, int64_t limit, int64_t* row_ids, int64_t* n_out, LdbError* err);
-/* read back `n` cells of a fixed-width column at the given row ids (result materialisation of small outputs) */
+/* read back `n` cells of a fixed-width column of a single-batch table at the given row ids (result materialisation of small
+ * outputs); host_valid[i] = 0 for NULL (validity bytes or an Arrow bitmap, at its bit offset).  A cell is the column's width, and
+ * decimal128 cells are always 16 bytes (an 8-byte staged cell of a narrow decimal is sign-extended).  Exported group keys are 8
+ * bytes, their aggregates 16 (doubles: bits in the low 8 bytes); materialised columns are 16. */
 int ldb_gpu_table_gather(LdbTable* t, const char* column, const int64_t* row_ids, int64_t n, void* host_dst /* n * cell bytes */, uint8_t* host_valid /* n, may be NULL */, LdbError* err);
 /* ORDER BY k1 [DESC], k2 [DESC], … LIMIT over a single-batch table of fewer than 2^32 rows: an LSD composition of the stable radix
  * sort (the last key first), so ties on every key keep row order.  Fixed-width keys: the types ldb_gpu_table_order_by takes, in its
  * order (decimals of any precision by their full value; a 16-byte cell costs two sort passes, other fixed-width keys one).  utf8
  * keys order bytewise with unsigned bytes, a proper prefix first (the order of LDB_OP_STRCMP); a utf8 key costs one sort pass for
- * its lengths plus one per 8 bytes of its LONGEST string.  Validity is not consulted: a NULL sorts by the cell it holds.  Returns
- * the first `limit` row ids (all with limit < 0).  Unknown column: LDB_ERR_INVALID. */
+ * its lengths plus one per 8 bytes of its LONGEST non-NULL string.  On every key a NULL compares greater than any value and equal
+ * to another NULL, and DESC swaps the operands: ASC puts a key's NULLs last, DESC first, and rows NULL on a key are ordered by the
+ * keys after it.  Returns the first `limit` row ids (all with limit < 0).  Unknown column: LDB_ERR_INVALID. */
 int ldb_gpu_table_order_by_keys(LdbTable* t, int32_t n_keys, const char* const* columns, const int32_t* descending, int64_t limit, int64_t* row_ids, int64_t* n_out, LdbError* err);
 /* read back `n` utf8 cells of a single-batch table at the given row ids: string i is host_bytes[host_offsets[i] ..
  * host_offsets[i + 1]), host_valid[i] (may be NULL) = 0 for NULL.  One copy per run of consecutive row ids.  When the strings need

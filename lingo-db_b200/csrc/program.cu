@@ -1140,7 +1140,7 @@ void loadHashAggExchangeKernels() {
    cudaFuncGetAttributes(&fa, hashAggMergeKernel);
 }
 
-// ---------------------------------------------------------------- radix sort (64-bit keys, 32-bit values), 8 passes of 8 bits
+// ---------------------------------------------------------------- radix sort (64-bit keys, 32-bit values), up to 8 passes of 8 bits
 // (GrowingBuffer::sort → parallel sort of the materialised tuples, GrowingBuffer.cpp:54-78, Sorting.cpp; here LSD radix on an
 //  order-preserving 64-bit key the host builds from the ORDER BY columns).  Stable; HBM-bound: 2 x (12 B read + 12 B write) per pass.
 constexpr int kSortThreads = 256;
@@ -1220,21 +1220,21 @@ __global__ void __launch_bounds__(kSortThreads) sortScatterKernel(const unsigned
       __syncthreads();
    }
 }
-void launchRadixSortPairs(unsigned long long* keys, uint32_t* vals, unsigned long long* keysTmp, uint32_t* valsTmp, int64_t n, unsigned int* histScratch, int smCount, cudaStream_t s) {
+void launchRadixSortPairs(unsigned long long* keys, uint32_t* vals, unsigned long long* keysTmp, uint32_t* valsTmp, int64_t n, unsigned int* histScratch, int smCount, cudaStream_t s,
+                          int digits) {
    if (n <= 0) return;
    const int ctas = (int) ((n + kSortItemsPerCta - 1) / kSortItemsPerCta);
    unsigned long long* kin = keys;
    unsigned long long* kout = keysTmp;
    uint32_t* vin = vals;
    uint32_t* vout = valsTmp;
-   for (int pass = 0; pass < 8; pass++) {
+   for (int pass = 0; pass < digits; pass++) {
       sortHistKernel<<<ctas, kSortThreads, 0, s>>>(kin, n, pass * 8, histScratch);
       sortScanKernel<<<1, 1024, 0, s>>>(histScratch, (int64_t) ctas * 256);
       sortScatterKernel<<<ctas, kSortThreads, 0, s>>>(kin, vin, kout, vout, n, pass * 8, histScratch);
       std::swap(kin, kout);
       std::swap(vin, vout);
    }
-   // 8 passes: the result is back in `keys` / `vals`
 }
 
 // ---------------------------------------------------------------- multi-key ORDER BY, dictionary ranks and export
@@ -1242,15 +1242,22 @@ void launchRadixSortPairs(unsigned long long* keys, uint32_t* vals, unsigned lon
 // first; a utf8 key is its length word, then its 8-byte chunks from the last to the first.  Zero padding makes a proper prefix tie
 // with its extension on every chunk, and the length pass, run before them, puts the shorter one first: bytewise order with
 // unsigned bytes, the order of LDB_OP_STRCMP.  A 16-byte cell (an i128) is two words the same way: chunk 0 its low word, unsigned,
-// then chunk 1 its high word with the sign bit flipped.
-__global__ void buildSortWordsKernel(const uint8_t* col, const uint8_t* bytes, int elemBytes, int kind, int chunk, int64_t n, int descending, int first,
-                                     uint32_t* ids, unsigned long long* keys, int32_t* maxLen) {
+// then chunk 1 its high word with the sign bit flipped.  A nullable key ends with its NULL flag (kind 3), the most significant
+// word of the key: NULLs, which tie on every value word, go last, and DESC's inversion puts them first.
+__global__ void buildSortWordsKernel(const uint8_t* col, const uint8_t* bytes, int elemBytes, SortValidity valid, int kind, int chunk, int64_t n, int descending,
+                                     int first, uint32_t* ids, unsigned long long* keys, int32_t* maxLen) {
    int32_t longest = 0;
    for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t) gridDim.x * blockDim.x) {
       const uint32_t row = first ? (uint32_t) i : ids[i];
       if (first) ids[i] = row;
+      const int64_t bit = valid.bitOffset + row;
+      const bool isNull = valid.bytes ? !valid.bytes[row] : valid.bitmap ? !((valid.bitmap[bit >> 3] >> (bit & 7)) & 1) : false;
       unsigned long long k = 0;
-      if (kind == 0 && elemBytes == 16) {
+      if (kind == 3) {
+         k = isNull;
+      } else if (isNull) {
+         // k = 0: every NULL gets the same value word
+      } else if (kind == 0 && elemBytes == 16) {
          const unsigned long long* w = (const unsigned long long*) (col + (size_t) row * 16);
          k = chunk ? w[1] ^ 0x8000000000000000ull : w[0];
       } else if (kind == 0) {
@@ -1276,10 +1283,10 @@ __global__ void buildSortWordsKernel(const uint8_t* col, const uint8_t* bytes, i
       if ((threadIdx.x & 31) == 0 && longest) atomicMax(maxLen, longest);
    }
 }
-void launchBuildSortWords(const uint8_t* col, const uint8_t* bytes, int elemBytes, int kind, int chunk, int64_t n, int descending, int first,
+void launchBuildSortWords(const uint8_t* col, const uint8_t* bytes, int elemBytes, SortValidity valid, int kind, int chunk, int64_t n, int descending, int first,
                           uint32_t* ids, unsigned long long* keys, int32_t* maxLen, int smCount, cudaStream_t s) {
    int grid = (int) std::min<int64_t>(std::max<int64_t>((n + 255) / 256, 1), (int64_t) smCount * 8);
-   buildSortWordsKernel<<<grid, 256, 0, s>>>(col, bytes, elemBytes, kind, chunk, n, descending, first, ids, keys, maxLen);
+   buildSortWordsKernel<<<grid, 256, 0, s>>>(col, bytes, elemBytes, valid, kind, chunk, n, descending, first, ids, keys, maxLen);
 }
 __global__ void scatterRanksKernel(const uint32_t* ids, int64_t n, int32_t* rank) {
    for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t) gridDim.x * blockDim.x) rank[ids[i]] = (int32_t) i;

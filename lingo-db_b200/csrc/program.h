@@ -179,12 +179,22 @@ void launchHashAggSend(const HashAggDev& local, const HashAggShip& x, int smCoun
 // maxReceived: the largest min(counts[s], capacity) (sizes the grid)
 void launchHashAggMerge(const HashAggDev& owned, const HashAggShip& x, uint64_t maxReceived, int smCount, cudaStream_t s);
 void loadHashAggExchangeKernels(); // loads both kernels now (collective launches must not wait for a lazy module load)
-// LSD radix sort of (64-bit key, 32-bit row id) pairs — ORDER BY / top-k over materialised rows (GrowingBuffer::sort, Sorting.cpp)
-void launchRadixSortPairs(unsigned long long* keys, uint32_t* vals, unsigned long long* keysTmp, uint32_t* valsTmp, int64_t n, unsigned int* histScratch, int smCount, cudaStream_t s);
+// LSD radix sort of (64-bit key, 32-bit row id) pairs — ORDER BY / top-k over materialised rows (GrowingBuffer::sort, Sorting.cpp):
+// its lowest `digits` 8-bit digits, one pass each.  After an even number of passes the result is in keys / vals, after an odd
+// number in keysTmp / valsTmp.
+void launchRadixSortPairs(unsigned long long* keys, uint32_t* vals, unsigned long long* keysTmp, uint32_t* valsTmp, int64_t n, unsigned int* histScratch, int smCount, cudaStream_t s,
+                          int digits = 8);
+// a key column's validity: one byte per row, or else an Arrow bitmap read from bit `bitOffset` (both null: no NULLs)
+struct SortValidity {
+   const uint8_t* bytes;
+   const uint8_t* bitmap;
+   int64_t bitOffset;
+};
 // multi-key ORDER BY: the 64-bit sort words of one key at the current permutation `ids` (first = 1: ids := 0..n-1 first).
 // kind 0: a fixed-width cell (low 8 bytes, sign bit flipped); kind 1: a utf8 cell's length (the longest is atomicMax'ed into
-// *maxLen); kind 2: bytes [8 chunk, 8 chunk + 8) of a utf8 cell, zero padded, big-endian, unsigned.  DESC inverts the word.
-void launchBuildSortWords(const uint8_t* col, const uint8_t* bytes, int elemBytes, int kind, int chunk, int64_t n, int descending, int first,
+// *maxLen); kind 2: bytes [8 chunk, 8 chunk + 8) of a utf8 cell, zero padded, big-endian, unsigned; kind 3: 1 for a NULL, else 0.
+// A NULL cell's word is 0 in kinds 0-2 (NULLs tie on the value; a NULL string leaves *maxLen alone).  DESC inverts the word.
+void launchBuildSortWords(const uint8_t* col, const uint8_t* bytes, int elemBytes, SortValidity valid, int kind, int chunk, int64_t n, int descending, int first,
                           uint32_t* ids, unsigned long long* keys, int32_t* maxLen, int smCount, cudaStream_t s);
 void launchScatterRanks(const uint32_t* ids, int64_t n, int32_t* rank, int smCount, cudaStream_t s);
 // dictionary → table: offsets[0..n] (exclusive scan of the lengths) and the bytes of code i at offsets[i]

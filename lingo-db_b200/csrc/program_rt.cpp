@@ -7,6 +7,7 @@
 #include <algorithm>
 #include <cstdio>
 #include <cstring>
+#include <deque>
 
 using namespace ldb;
 
@@ -232,26 +233,36 @@ static uint32_t* sortRows(Scratch& scratch, LdbTable* t, const std::vector<std::
    unsigned int* hist = scratch.alloc<unsigned int>((size_t) ((n + 4095) / 4096) * 256 * 4);
    int32_t* maxLen = scratch.alloc<int32_t>(16);
    int first = 1;
+   SortValidity valid{};
    auto pass = [&](int c, int kind, int chunk, int desc) {
+      const int digits = kind == 3 ? 1 : 8; // the NULL flag is the lowest digit
       ctx->launch("radix_sort", [&] {
-         launchBuildSortWords((const uint8_t*) b.data[c], (const uint8_t*) b.bytes[c], b.elemBytes[c], kind, chunk, n, desc, first, dv, dk, maxLen, ctx->smCount, ctx->compute);
-         launchRadixSortPairs(dk, dv, dk2, dv2, n, hist, ctx->smCount, ctx->compute);
+         launchBuildSortWords((const uint8_t*) b.data[c], (const uint8_t*) b.bytes[c], b.elemBytes[c], valid, kind, chunk, n, desc, first, dv, dk, maxLen, ctx->smCount, ctx->compute);
+         launchRadixSortPairs(dk, dv, dk2, dv2, n, hist, ctx->smCount, ctx->compute, digits);
       });
+      if (digits % 2) {
+         std::swap(dk, dk2);
+         std::swap(dv, dv2);
+      }
       first = 0;
    };
    for (size_t k = keys.size(); k-- > 0;) {
       const int c = keys[k].first, desc = keys[k].second;
+      valid.bytes = c < (int) b.validBytes.size() ? b.validBytes[c] : nullptr;
+      valid.bitmap = c < (int) b.validity.size() && !valid.bytes ? (const uint8_t*) b.validity[c] : nullptr;
+      valid.bitOffset = valid.bitmap ? b.validityBitOffset[c] : 0;
       if (t->columns[c].type != LDB_UTF8) {
          if (b.elemBytes[c] == 16) pass(c, 0, 0, desc); // an i128 cell: its low word first, then the high word
          pass(c, 0, b.elemBytes[c] == 16 ? 1 : 0, desc);
-         continue;
+      } else {
+         int32_t longest = 0;
+         LDB_CUDA(cudaMemsetAsync(maxLen, 0, 4, ctx->compute));
+         pass(c, 1, 0, desc); // lengths: the least significant word of a string
+         LDB_CUDA(cudaMemcpyAsync(&longest, maxLen, 4, cudaMemcpyDeviceToHost, ctx->compute));
+         ctx->syncStream(ctx->compute);
+         for (int chunk = (longest + 7) / 8; chunk-- > 0;) pass(c, 2, chunk, desc);
       }
-      int32_t longest = 0;
-      LDB_CUDA(cudaMemsetAsync(maxLen, 0, 4, ctx->compute));
-      pass(c, 1, 0, desc); // lengths: the least significant word of a string
-      LDB_CUDA(cudaMemcpyAsync(&longest, maxLen, 4, cudaMemcpyDeviceToHost, ctx->compute));
-      ctx->syncStream(ctx->compute);
-      for (int chunk = (longest + 7) / 8; chunk-- > 0;) pass(c, 2, chunk, desc);
+      if (valid.bytes || valid.bitmap) pass(c, 3, 0, desc); // NULL last (ASC) / first (DESC), NULLs tied
    }
    return dv;
 }
@@ -863,6 +874,46 @@ static void orderRows(LdbTable* t, const std::vector<std::pair<int, int>>& keys,
    *n_out = m;
 }
 
+// the validity of gathered rows, one run of consecutive row ids at a time, into host_valid (1 = not NULL): one byte per row
+// (tables this library made) is copied, an Arrow bitmap has the bytes that hold the run's bits copied and is decoded by finish()
+// once the stream has been synchronised, a column without either is all valid
+class GatherValidity {
+ public:
+   GatherValidity(const LdbBatch& b, int c, uint8_t* hostValid) : hostValid_(hostValid) {
+      bytes_ = c < (int) b.validBytes.size() ? b.validBytes[c] : nullptr;
+      bitmap_ = c < (int) b.validity.size() && !bytes_ ? (const uint8_t*) b.validity[c] : nullptr;
+      bitOffset_ = bitmap_ ? b.validityBitOffset[c] : 0;
+   }
+   // rows row .. row + m - 1 → host_valid[i .. i + m)
+   void run(int64_t i, int64_t row, int64_t m, cudaStream_t s) {
+      if (!hostValid_) return;
+      if (bytes_) {
+         LDB_CUDA(cudaMemcpyAsync(hostValid_ + i, bytes_ + row, (size_t) m, cudaMemcpyDeviceToHost, s));
+      } else if (bitmap_) {
+         const int64_t bit0 = bitOffset_ + row;
+         runs_.push_back({i, m, bit0 % 8, std::vector<uint8_t>((size_t) ((bit0 % 8 + m + 7) / 8))});
+         LDB_CUDA(cudaMemcpyAsync(runs_.back().bits.data(), bitmap_ + bit0 / 8, runs_.back().bits.size(), cudaMemcpyDeviceToHost, s));
+      } else {
+         memset(hostValid_ + i, 1, (size_t) m);
+      }
+   }
+   void finish() {
+      for (const Run& r : runs_)
+         for (int64_t q = 0; q < r.m; q++) hostValid_[r.i + q] = (r.bits[(size_t) ((r.bit0 + q) >> 3)] >> ((r.bit0 + q) & 7)) & 1u;
+   }
+
+ private:
+   struct Run {
+      int64_t i, m, bit0;
+      std::vector<uint8_t> bits;
+   };
+   uint8_t* hostValid_;
+   const uint8_t* bytes_;
+   const uint8_t* bitmap_;
+   int64_t bitOffset_;
+   std::deque<Run> runs_; // a deque: the bytes of earlier runs stay put while later runs are added
+};
+
 extern "C" {
 
 int ldb_gpu_run_program(LdbContext* ctx, const LdbProgramDesc* d, LdbError* err) {
@@ -954,17 +1005,24 @@ int ldb_gpu_table_gather(LdbTable* t, const char* column, const int64_t* row_ids
       const size_t w = (size_t) b.elemBytes[c];
       for (int64_t i = 0; i < n; i++)
          if (row_ids[i] < 0 || row_ids[i] >= b.nRows) fail(LDB_ERR_INVALID, "row id out of range");
+      // a decimal128 cell staged as 8 bytes (narrowed or packed HOST staging) is read into `narrow` and widened below
+      const bool widen = t->columns[c].type == LDB_DECIMAL128 && w == 8;
+      std::vector<int64_t> narrow(widen ? (size_t) n : 0);
+      uint8_t* dst = widen ? (uint8_t*) narrow.data() : (uint8_t*) host_dst;
+      GatherValidity valid(b, c, host_valid);
       // one copy per run of consecutive row ids (a whole column read back in order is one copy)
       for (int64_t i = 0, j; i < n; i = j) {
          for (j = i + 1; j < n && row_ids[j] == row_ids[j - 1] + 1;) j++;
          const size_t m = (size_t) (j - i);
-         LDB_CUDA(cudaMemcpyAsync((uint8_t*) host_dst + (size_t) i * w, (const uint8_t*) b.data[c] + (size_t) row_ids[i] * w, m * w, cudaMemcpyDeviceToHost, ctx->compute));
-         if (host_valid) {
-            if (c < (int) b.validBytes.size() && b.validBytes[c]) LDB_CUDA(cudaMemcpyAsync(host_valid + i, b.validBytes[c] + row_ids[i], m, cudaMemcpyDeviceToHost, ctx->compute));
-            else memset(host_valid + i, 1, m);
-         }
+         LDB_CUDA(cudaMemcpyAsync(dst + (size_t) i * w, (const uint8_t*) b.data[c] + (size_t) row_ids[i] * w, m * w, cudaMemcpyDeviceToHost, ctx->compute));
+         valid.run(i, row_ids[i], (int64_t) m, ctx->compute);
       }
       ctx->syncStream(ctx->compute);
+      valid.finish();
+      for (size_t i = 0; i < narrow.size(); i++) {
+         const int64_t cell[2] = {narrow[i], narrow[i] >> 63};
+         memcpy((uint8_t*) host_dst + i * 16, cell, 16);
+      }
    });
 }
 int ldb_gpu_table_order_by_keys(LdbTable* t, int32_t n_keys, const char* const* columns, const int32_t* descending, int64_t limit, int64_t* row_ids, int64_t* n_out, LdbError* err) {
@@ -1019,34 +1077,19 @@ int ldb_gpu_table_gather_strings(LdbTable* t, const char* column, const int64_t*
       *bytes_needed = total;
       if (total > bytes_cap) fail(LDB_ERR_CAPACITY, "gather_strings: the strings need more than bytes_cap bytes (see bytes_needed)");
       if (total > 0 && !host_bytes) fail(LDB_ERR_INVALID, "null argument");
-      const uint8_t* bitmap = c < (int) b.validity.size() ? (const uint8_t*) b.validity[c] : nullptr;
-      const uint8_t* vbytes = c < (int) b.validBytes.size() ? b.validBytes[c] : nullptr;
-      std::vector<std::vector<uint8_t>> bits(host_valid && bitmap && !vbytes ? runs.size() : 0);
+      GatherValidity valid(b, c, host_valid);
       int64_t pos = 0;
       host_offsets[0] = 0;
-      for (size_t k = 0; k < runs.size(); k++) {
-         const Run& r = runs[k];
+      for (const Run& r : runs) {
          const size_t m = (size_t) (r.j - r.i);
          for (size_t q = 0; q < m; q++) host_offsets[r.i + (int64_t) q + 1] = pos + offs[r.at + q + 1] - offs[r.at];
          const int64_t len = offs[r.at + m] - offs[r.at];
          if (len) LDB_CUDA(cudaMemcpyAsync((uint8_t*) host_bytes + pos, (const uint8_t*) b.bytes[c] + offs[r.at], (size_t) len, cudaMemcpyDeviceToHost, ctx->compute));
          pos += len;
-         if (!host_valid) continue;
-         if (vbytes) {
-            LDB_CUDA(cudaMemcpyAsync(host_valid + r.i, vbytes + row_ids[r.i], m, cudaMemcpyDeviceToHost, ctx->compute));
-         } else if (bitmap) {
-            const int64_t bit0 = b.validityBitOffset[c] + row_ids[r.i];
-            bits[k].resize((size_t) ((bit0 % 8 + (int64_t) m + 7) / 8));
-            LDB_CUDA(cudaMemcpyAsync(bits[k].data(), bitmap + bit0 / 8, bits[k].size(), cudaMemcpyDeviceToHost, ctx->compute));
-         } else {
-            memset(host_valid + r.i, 1, m);
-         }
+         valid.run(r.i, row_ids[r.i], (int64_t) m, ctx->compute);
       }
       ctx->syncStream(ctx->compute);
-      for (size_t k = 0; k < bits.size(); k++) {
-         const int64_t bit0 = (b.validityBitOffset[c] + row_ids[runs[k].i]) % 8;
-         for (int64_t q = 0; q < runs[k].j - runs[k].i; q++) host_valid[runs[k].i + q] = (bits[k][(size_t) ((bit0 + q) >> 3)] >> ((bit0 + q) & 7)) & 1u;
-      }
+      valid.finish();
    });
 }
 

@@ -172,9 +172,9 @@ class Table:
         self._keep.append(chunk)
         self._append(n_rows, bufs, capi.MEM_HOST, sizes, valids, offset)
 
-    def append_device(self, tensors: Dict[str, object], n_rows: int):
+    def append_device(self, tensors: Dict[str, object], n_rows: int, offset: int = 0):
         """tensors: column → torch CUDA tensor (or (offsets, bytes) pair for utf8), and optionally "<column>$valid" → the column's
-        Arrow validity bitmap as a uint8 CUDA tensor; borrowed."""
+        Arrow validity bitmap as a uint8 CUDA tensor; borrowed.  `offset` as in append_host."""
         bufs, sizes, valids = {}, {}, {}
         for c in self.columns:
             v = tensors[c.name]
@@ -186,7 +186,7 @@ class Table:
             else:
                 bufs[c.name] = v.data_ptr()
         self._keep.append(tensors)
-        self._append(n_rows, bufs, capi.MEM_DEVICE, sizes, valids)
+        self._append(n_rows, bufs, capi.MEM_DEVICE, sizes, valids, offset)
 
     def clear(self):
         e = Error()

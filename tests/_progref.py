@@ -28,7 +28,8 @@ are the op comments of include/ldb_gpu.h ("program pipelines"), restated:
     `inserted` (their key set must be the dictionary's);
   - ROWID is the row's number in its table; FETCH reads a side table's column at a row number, and a NULL or out-of-range row
     reads NULL;
-  - ORDER BY (order_rows) is a stable sort over the full i128 cell.
+  - ORDER BY (reference_order, order_rows) is a stable sort over the full i128 cell or the bytes of a string, NULLs last (ASC) or
+    first (DESC).
 Values: int for integer-typed results, float for doubles, None for NULL."""
 import datetime
 import math
@@ -221,9 +222,23 @@ def check_dictionary(strings: list, ranks: list, keys: set) -> Dict[bytes, int]:
     return {s: i for i, s in enumerate(strings)}
 
 
+def reference_order(columns, keys: list) -> list:
+    """ORDER BY over `keys`, [(column, descending), …] into `columns` (a list or dict of cell lists, None for NULL): the row numbers
+    in the reference's order.  Integers, dates, fsb4 and decimals compare by their full signed value, strings (bytes) bytewise with
+    unsigned bytes and a proper prefix first.  A NULL compares greater than any value and equal to another NULL; DESC swaps the
+    operands, so it also puts NULLs first.  Rows equal on every key keep row order (the library's sort is stable).
+    Built as the LSD composition of stable sorts, the last key first; sorting reversed keeps ties in order."""
+    n = len(columns[keys[0][0]]) if keys else 0
+    order = list(range(n))
+    for c, descending in reversed(keys):
+        cells = columns[c]
+        order.sort(key=lambda i: (1, 0) if cells[i] is None else (0, cells[i]), reverse=bool(descending))
+    return order
+
+
 def order_rows(values: list, descending: bool = False) -> list:
-    """ORDER BY one column of cells (ints: the i128, or a double's bits): the row numbers of a stable sort"""
-    return sorted(range(len(values)), key=lambda i: -values[i] if descending else values[i])
+    """ORDER BY one column of cells (ints: the i128, or a double's bits; None: NULL): the row numbers of a stable sort"""
+    return reference_order([values], [(0, descending)])
 
 
 # ---------------------------------------------------------------------------------------------------- evaluator

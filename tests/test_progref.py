@@ -182,6 +182,28 @@ def test_order_by_is_a_stable_sort_over_the_whole_i128():
     assert R.order_rows(ties) == [1, 4, 0, 2, 3] and R.order_rows(ties, descending=True) == [3, 0, 2, 1, 4]
 
 
+def test_reference_order_puts_nulls_last_ascending_and_first_descending():
+    vals = [3, None, -1, None, 3, R.I128_MIN]
+    assert R.reference_order([vals], [(0, False)]) == [5, 2, 0, 4, 1, 3]
+    assert R.reference_order([vals], [(0, True)]) == [1, 3, 0, 4, 2, 5]
+    assert R.order_rows(vals) == [5, 2, 0, 4, 1, 3] and R.order_rows(vals, descending=True) == [1, 3, 0, 4, 2, 5]
+    assert R.reference_order([[]], [(0, False)]) == [] and R.reference_order([[None] * 3], [(0, True)]) == [0, 1, 2]
+
+
+def test_reference_order_lets_the_next_key_decide_between_nulls():
+    cols = {"a": [None, 1, None, None, 1], "b": [5, 0, -2, 5, None]}
+    assert R.reference_order(cols, [("a", False), ("b", False)]) == [1, 4, 2, 0, 3]
+    assert R.reference_order(cols, [("a", False), ("b", True)]) == [4, 1, 0, 3, 2]
+    assert R.reference_order(cols, [("a", True), ("b", False)]) == [2, 0, 3, 1, 4]
+    assert R.reference_order(cols, [("b", True), ("a", True)]) == [4, 0, 3, 1, 2]
+
+
+def test_reference_order_of_strings_is_bytewise_with_null_after_the_empty_string():
+    s = [b"b", None, b"", b"a\x80", b"a\x7f", b"a", b"\xff", b"a\0", None, b""]
+    assert R.reference_order([s], [(0, False)]) == [2, 9, 5, 7, 4, 3, 0, 6, 1, 8]
+    assert R.reference_order([s], [(0, True)]) == [1, 8, 6, 0, 3, 4, 7, 5, 2, 9]
+
+
 def test_aggregates():
     assert R.group_by(0, [], [("count_star", None), ("sum", []), ("min", [])]) == {(): [0, None, None]}
     g = R.group_by(4, [[1, None, 1, None]], [("min", [-5, None, 3, None]), ("count", [1, None, 2, None]), ("max", [R.I64_MIN - 1, 2, None, None])])
