@@ -651,6 +651,36 @@ int ldb_gpu_groupby_allmerge(LdbState* s, LdbComm* comm, LdbError* err);
  * The call reads the received counts on the host (it synchronises the compute stream): inside a captured query it fails with
  * LDB_ERR_UNSUPPORTED before enqueueing anything.  Ranks of one process must call it from one thread each. */
 int ldb_gpu_hashagg_exchange(LdbState* local, LdbState* owned, LdbComm* comm, int64_t recv_offset, int64_t capacity, LdbError* err);
+/* Repartition the rows of a table across the ranks of `comm` (GrowingBuffer::merge, GrowingBuffer.cpp:100-113, feeding the join build,
+ * LazyJoinHashtable.cpp:12-34, across GPUs; rows partitioned by key hash as the pre-aggregation fragments, PreAggregationHashtable.cpp:
+ * 31-70).  Collective: every rank calls it in the same order, each with its own shard.  Exchange both sides of a join on the join key,
+ * build and probe locally, and finish with ldb_gpu_hashagg_exchange; or broadcast a small build side.
+ *   Owner: n_keys = 1..4: a row goes to rank ((h >> 32) * world) >> 32, h = the key-tuple hash of the aggregation sink over the key
+ *   values as int64 (an integer, date or char(1) cell's value, a decimal cell's low 8 bytes); a NULL component hashes as 0 and sets bit
+ *   k of the hash's seed.  The owner depends on key values only, never on column types (an int32 column and a decimal128 cell holding
+ *   the same number go to the same rank), and is the rank ldb_gpu_hashagg_exchange gives the group with those keys.  n_keys = 0: every
+ *   row goes to every rank (broadcast).
+ *   Sources: any table of comm's context a program can scan: HOST-staged batches (compressed or narrowed staging included; the call
+ *   waits for their staging), DEVICE batches, Arrow validity bitmaps at any bit offset or validity bytes (materialized rows, exported
+ *   groups, earlier exchange results).
+ *   Columns: `columns` names 1..16 fixed-width columns to ship (NULL: all columns of src, at most 16).  *out = a new single-batch
+ *   DEVICE table of this context named `name` (NULL: "received") with those columns: same names, types, precision and scale, cells of
+ *   1 (int8), 2 (int16), 4 (int32, date32, char(1), float32), 8 (int64, float64) or 16 bytes (decimal128; a narrowed 8-byte staged
+ *   cell is sign-extended), one validity byte per value.  Key columns are integer, date32, char(1) or decimal columns and need not be
+ *   shipped.  A utf8 column, shipped or key, or a float key: LDB_ERR_UNSUPPORTED.
+ *   Order: the received rows of source rank 0 in their source row order (the order LDB_OP_ROWID numbers them), then rank 1's, …:
+ *   results do not depend on thread timing.
+ *   Capacity, all or nothing: the receive region is [recv_offset, recv_offset + recv_bytes) of the user heap, the same on every rank,
+ *   recv_offset a multiple of 16.  A rank receiving n rows lays them out column-major: each column's n cells, then each column's n
+ *   validity bytes, every array starting 16-byte aligned.  Every rank learns every rank's row counts before anything is stored; when
+ *   the rows of any rank do not fit its region, EVERY rank fails with LDB_ERR_CAPACITY naming the recv_bytes the largest receiver
+ *   needs, nothing is written into any receive region and the ranks stay in step: a retry with that size succeeds.
+ * Other errors: LDB_ERR_INVALID for null arguments, unknown columns, more than 16 columns, n_keys outside 0..4, a comm of another
+ * context, a region outside the user heap or a misaligned recv_offset.  The call reads the row counts on the host (it synchronises the
+ * compute stream): inside a captured query it fails with LDB_ERR_UNSUPPORTED before enqueueing anything.  Ranks of one process must
+ * call it from one thread each.  On return the receive region is free again; world = 1 is a compacting copy. */
+int ldb_gpu_table_exchange(LdbTable* src, int32_t n_keys, const char* const* key_columns, int32_t n_columns, const char* const* columns /* NULL = all columns of src */,
+                           LdbComm* comm, int64_t recv_offset, int64_t recv_bytes, const char* name, LdbTable** out, LdbError* err);
 /* zero / read back (synchronising) a range of this rank's user heap */
 int ldb_gpu_comm_heap_zero(LdbComm* comm, int64_t user_offset, int64_t bytes, LdbError* err);
 int ldb_gpu_comm_heap_read(LdbComm* comm, int64_t user_offset, int64_t bytes, void* host_dst, LdbError* err);

@@ -295,6 +295,13 @@ struct LdbGraph {
 
 // order the compute stream after the staging of one batch (runtime.cpp)
 void ldb_gpu_wait_batch_internal(LdbContext* ctx, const struct LdbBatch* b);
+namespace ldb {
+// the pointers of column `ci` of batch `b` as a program reads them (validity bitmap or validity bytes included; program_rt.cpp)
+void bindColumn(ProgCol& pc, const LdbBatch& b, int ci);
+// registers a single-batch table this library made: `b` holds nRows and, per column, data / bytes / elemBytes / validBytes; the table
+// takes over the device buffers of `buffers` (program_rt.cpp)
+LdbTable* addResultTable(LdbContext* ctx, std::string name, std::vector<LdbColumn> columns, LdbBatch b, Scratch& buffers);
+} // namespace ldb
 // builds the missing encoded copies of columns cols[0..n) of a borrowed DEVICE batch (encode.cu) for tiles of `tileRows` rows;
 // true when every one of them has a copy.  Runs outside any capture and waits for its work on the host.
 bool ldb_gpu_encode_batch_internal(LdbContext* ctx, LdbTable* t, LdbBatch& b, const int* cols, int n, int tileRows);

@@ -14,7 +14,9 @@
 // never overwritten while a peer still reads it.
 #include "context.h"
 #include "device_utils.cuh"
+#include "keyhash.cuh"
 #include "peer.h"
+#include "progcol.cuh"
 #include "program.h"
 
 #include <algorithm>
@@ -190,6 +192,175 @@ __global__ void peerPublishCountsKernel(PeerView v, size_t cursorsOff, size_t co
    *((unsigned long long*) (v.heap[d] + countsOff) + v.rank) = n; // plain store into the peer; the barrier that follows publishes it
 }
 
+// ---------------------------------------------------------------- table exchange (ldb_gpu_table_exchange, include/ldb_gpu.h)
+// A stable multi-way partition of a table's rows by owner rank, as the radix sort's hist / scan / scatter: the count kernel gives every
+// CTA (a fixed tile of one batch) a per-destination histogram, a scan turns the histograms into each CTA's offset per destination, and
+// the send kernel ranks the rows of each tile per destination (match_any + per-warp counts) and stores their cells straight into the
+// owner's receive region.  Receive region of a rank with n rows (column-major, every array 16-byte aligned):
+//   cells of column 0 (n x outBytes[0]) | … | cells of column m-1 | validity bytes of column 0 (n) | … | validity bytes of column m-1
+// Source s's rows start at row Σ_{s' < s} M[s'][d] of receiver d, M[s][d] = the rows source s sends rank d.
+constexpr int kShipMaxCols = 16;
+constexpr int kShipThreads = 256;
+constexpr int64_t kShipTile = 16 * kShipThreads; // rows per CTA; tiles never span batches
+struct TableShipBatch {
+   ProgCol cols[kShipMaxCols];  // shipped columns of this batch (bindColumn)
+   ProgCol keys[kProgMaxKeys];  // key columns of this batch
+   int32_t outBytes[kShipMaxCols];
+   int32_t nCols, nKeys, world;
+   int32_t broadcast;           // every row to every rank (no keys)
+   int64_t nRows, firstRow;     // this batch's rows and the source row number of its row 0
+   int64_t ctaBase, nCtas;      // this batch's first CTA in the histograms, and the CTAs of all batches
+   uint8_t* owners;             // per source row: its owner (count writes, send reads)
+   unsigned long long* hist;    // [world][nCtas]: count: rows per (destination, CTA); after the scan: the CTA's offset in the destination
+   uint8_t* recv[kMaxPeers];    // every rank's receive region (peer-mapped)
+   unsigned long long rows[kMaxPeers]; // the rows every rank receives (its N_d)
+   unsigned long long base[kMaxPeers]; // the row of receiver d where this source's rows start
+};
+// byte offsets of the arrays of a receive region of n rows; returns its size
+__host__ __device__ inline uint64_t shipLayout(uint64_t n, const int32_t* outBytes, int nCols, uint64_t* colOff, uint64_t* validOff) {
+   uint64_t off = 0;
+   for (int c = 0; c < nCols; c++) {
+      colOff[c] = off;
+      off += (n * (uint64_t) outBytes[c] + 15) & ~uint64_t(15);
+   }
+   for (int c = 0; c < nCols; c++) {
+      validOff[c] = off;
+      off += (n + 15) & ~uint64_t(15);
+   }
+   return off;
+}
+__device__ __forceinline__ int shipOwnerOf(const TableShipBatch& p, int64_t row) {
+   int64_t keys[kProgMaxKeys];
+   uint32_t nulls = 0;
+#pragma unroll
+   for (int k = 0; k < kProgMaxKeys; k++) {
+      if (k >= p.nKeys) break;
+      const Val kv = loadCol(p.keys[k], row); // the value the aggregation sink groups by: int64 of an integer, a decimal's low 8 bytes
+      keys[k] = kv.null ? 0 : (int64_t) kv.v;
+      nulls |= (kv.null ? 1u : 0u) << k;
+   }
+   return keyOwner(keyTupleHash(keys, p.nKeys, nulls), p.world);
+}
+__global__ void __launch_bounds__(kShipThreads) tableShipCountKernel(const __grid_constant__ TableShipBatch p) {
+   __shared__ unsigned int cnt[kMaxPeers];
+   if (threadIdx.x < kMaxPeers) cnt[threadIdx.x] = 0;
+   __syncthreads();
+   const int lane = threadIdx.x & 31;
+   const int64_t begin = (int64_t) blockIdx.x * kShipTile, end = min(begin + kShipTile, p.nRows);
+   for (int64_t t = begin; t < end; t += kShipThreads) {
+      const int64_t i = t + threadIdx.x;
+      const bool valid = i < end;
+      const int d = valid ? shipOwnerOf(p, i) : -1;
+      if (valid) p.owners[p.firstRow + i] = (uint8_t) d;
+      const unsigned same = __match_any_sync(0xffffffffu, d);
+      if (valid && lane == __ffs(same) - 1) atomicAdd(&cnt[d], (unsigned) __popc(same));
+   }
+   __syncthreads();
+   if (threadIdx.x < p.world) p.hist[(size_t) threadIdx.x * p.nCtas + p.ctaBase + blockIdx.x] = cnt[threadIdx.x];
+}
+// CTA d: exclusive scan of destination d's per-CTA counts, in place; totals[d] = the rows this rank sends rank d
+__global__ void __launch_bounds__(1024) tableShipScanKernel(unsigned long long* hist, int64_t nCtas, unsigned long long* totals) {
+   __shared__ unsigned long long warpSums[32];
+   __shared__ unsigned long long carry;
+   unsigned long long* h = hist + (size_t) blockIdx.x * nCtas;
+   if (threadIdx.x == 0) carry = 0;
+   __syncthreads();
+   for (int64_t base = 0; base < nCtas; base += 1024) {
+      const int64_t i = base + threadIdx.x;
+      const unsigned long long v = i < nCtas ? h[i] : 0ull;
+      unsigned long long x = v;
+      for (int o = 1; o < 32; o <<= 1) {
+         const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o);
+         if ((threadIdx.x & 31) >= o) x += y;
+      }
+      if ((threadIdx.x & 31) == 31) warpSums[threadIdx.x >> 5] = x;
+      __syncthreads();
+      if (threadIdx.x < 32) {
+         const unsigned long long w = warpSums[threadIdx.x];
+         unsigned long long ws = w;
+         for (int o = 1; o < 32; o <<= 1) {
+            const unsigned long long y = __shfl_up_sync(0xffffffffu, ws, o);
+            if (threadIdx.x >= o) ws += y;
+         }
+         warpSums[threadIdx.x] = ws - w;
+      }
+      __syncthreads();
+      const unsigned long long excl = carry + warpSums[threadIdx.x >> 5] + (x - v);
+      if (i < nCtas) h[i] = excl;
+      __syncthreads();
+      if (threadIdx.x == 1023) carry = excl + v;
+      __syncthreads();
+   }
+   if (threadIdx.x == 0) totals[blockIdx.x] = carry;
+}
+// one cell into the receive region: the low outBytes bytes of the source cell; a narrowed 8-byte decimal sign-extended to 16
+__device__ __forceinline__ void shipCell(const ProgCol& c, int w, int64_t row, uint8_t* dst) {
+   const uint8_t* s = c.data + (size_t) row * c.elemBytes;
+   switch (w) {
+      case 16:
+         if (c.elemBytes == 16) {
+            *(int4*) dst = *(const int4*) s;
+         } else {
+            const long long v = *(const long long*) s;
+            *(longlong2*) dst = make_longlong2(v, v >> 63);
+         }
+         break;
+      case 8: *(uint64_t*) dst = *(const uint64_t*) s; break;
+      case 4: *(uint32_t*) dst = *(const uint32_t*) s; break;
+      case 2: *(uint16_t*) dst = *(const uint16_t*) s; break;
+      default: *dst = *s;
+   }
+}
+__global__ void __launch_bounds__(kShipThreads) tableShipSendKernel(const __grid_constant__ TableShipBatch p) {
+   __shared__ uint64_t colOff[kMaxPeers][kShipMaxCols], validOff[kMaxPeers][kShipMaxCols];
+   __shared__ unsigned long long running[kMaxPeers];    // the next position of this CTA's rows in receiver d
+   __shared__ unsigned int warpCnt[kShipThreads / 32][kMaxPeers];
+   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+   const int64_t begin = (int64_t) blockIdx.x * kShipTile, end = min(begin + kShipTile, p.nRows);
+   if (threadIdx.x < p.world) {
+      const int d = threadIdx.x;
+      shipLayout(p.rows[d], p.outBytes, p.nCols, colOff[d], validOff[d]);
+      running[d] = p.base[d] + (p.broadcast ? (unsigned long long) (p.firstRow + begin) : p.hist[(size_t) d * p.nCtas + p.ctaBase + blockIdx.x]);
+   }
+   __syncthreads();
+   auto store = [&](int64_t i, int d, unsigned long long pos) {
+      uint8_t* r = p.recv[d];
+      for (int c = 0; c < p.nCols; c++) {
+         const bool null = colIsNull(p.cols[c], i);
+         shipCell(p.cols[c], p.outBytes[c], i, r + colOff[d][c] + pos * (uint64_t) p.outBytes[c]);
+         r[validOff[d][c] + pos] = null ? 0 : 1;
+      }
+   };
+   if (p.broadcast) { // row i of the batch is row base[d] + firstRow + i of every receiver
+      for (int64_t i = begin + threadIdx.x; i < end; i += kShipThreads)
+         for (int d = 0; d < p.world; d++) store(i, d, running[d] + (unsigned long long) (i - begin));
+      return;
+   }
+   for (int64_t t = begin; t < end; t += kShipThreads) {
+      if (threadIdx.x < kShipThreads / 32 * kMaxPeers) (&warpCnt[0][0])[threadIdx.x] = 0;
+      __syncthreads();
+      const int64_t i = t + threadIdx.x;
+      const bool valid = i < end;
+      const int d = valid ? p.owners[p.firstRow + i] : kMaxPeers;
+      const unsigned same = __match_any_sync(0xffffffffu, d);
+      const unsigned rankInWarp = __popc(same & ((1u << lane) - 1));
+      if (valid && rankInWarp == 0) warpCnt[warp][d] = __popc(same);
+      __syncthreads();
+      if (valid) {
+         unsigned before = 0;
+         for (int w = 0; w < warp; w++) before += warpCnt[w][d];
+         store(i, d, running[d] + before + rankInWarp);
+      }
+      __syncthreads();
+      if (threadIdx.x < p.world) {
+         unsigned tot = 0;
+         for (int w = 0; w < kShipThreads / 32; w++) tot += warpCnt[w][threadIdx.x];
+         running[threadIdx.x] += tot;
+      }
+      __syncthreads();
+   }
+}
+
 } // namespace ldb
 
 using namespace ldb;
@@ -238,6 +409,9 @@ int ldb_gpu_comm_create(LdbContext* ctx, int32_t rank, int32_t world, int64_t us
       LDB_CUDA(cudaFuncGetAttributes(&fa, peerGroupAllMergeKernel));
       LDB_CUDA(cudaFuncGetAttributes(&fa, peerOrReduceKernel));
       LDB_CUDA(cudaFuncGetAttributes(&fa, peerPublishCountsKernel));
+      LDB_CUDA(cudaFuncGetAttributes(&fa, tableShipCountKernel));
+      LDB_CUDA(cudaFuncGetAttributes(&fa, tableShipScanKernel));
+      LDB_CUDA(cudaFuncGetAttributes(&fa, tableShipSendKernel));
       loadHashAggExchangeKernels();
       cudaIpcMemHandle_t h;
       LDB_CUDA(cudaIpcGetMemHandle(&h, c->heap));
@@ -325,6 +499,18 @@ int ldb_gpu_comm_barrier(LdbComm* c, LdbError* err) {
    });
 }
 
+// all-gather of `bytes` (multiple of 16, <= kSlotBytes) from DEVICE memory `src`, eagerly on the compute stream (not inside a capture);
+// returns this rank's mailbox half the collective fills: block of rank r at result + r * kSlotBytes, valid until the next-but-one gather
+static uint8_t* allGatherSmall(LdbComm* c, const void* src, size_t bytes) {
+   LdbContext* ctx = c->ctx;
+   const unsigned long long epoch = ++c->gatherEpochHost; // mirror of the device counter (every rank issues the same collectives)
+   ctx->launch("peer_allgather", [&] {
+      peerAllGatherKernel<<<c->world, 256, 0, ctx->compute>>>(c->view(), (const uint8_t*) src, bytes);
+      peerBumpKernel<<<1, 1, 0, ctx->compute>>>(c->view(), EPOCH_GATHER, -1);
+   });
+   return c->heap + kMailboxOff + (size_t) (epoch & 1) * c->world * kSlotBytes;
+}
+
 // all-gather of `bytes` (multiple of 16, <= slot size) from DEVICE memory `src`; returns the device address of the gathered
 // blocks of this collective: block of rank r at result + r * ldb_gpu_comm_slot_bytes().  Valid until the next-but-one gather.
 int64_t ldb_gpu_comm_slot_bytes(void) { return (int64_t) kSlotBytes; }
@@ -335,12 +521,8 @@ int ldb_gpu_comm_allgather_small(LdbComm* c, const void* src, int64_t bytes, voi
       LdbContext* ctx = c->ctx;
       LDB_CUDA(cudaSetDevice(ctx->device));
       if (ctx->capturing) fail(LDB_ERR_UNSUPPORTED, "the small all-gather returns a parity-dependent address and cannot be captured");
-      const unsigned long long epoch = ++c->gatherEpochHost; // mirror of the device counter (every rank issues the same collectives)
-      ctx->launch("peer_allgather", [&] {
-         peerAllGatherKernel<<<c->world, 256, 0, ctx->compute>>>(c->view(), (const uint8_t*) src, (size_t) bytes);
-         peerBumpKernel<<<1, 1, 0, ctx->compute>>>(c->view(), EPOCH_GATHER, -1);
-      });
-      if (result) *result = c->heap + kMailboxOff + (size_t) (epoch & 1) * c->world * kSlotBytes;
+      uint8_t* gathered = allGatherSmall(c, src, (size_t) bytes);
+      if (result) *result = gathered;
    });
 }
 
@@ -519,6 +701,186 @@ int ldb_gpu_hashagg_exchange(LdbState* local, LdbState* owned, LdbComm* c, int64
          fail(LDB_ERR_CAPACITY, "hash aggregation exchange: a source sent this rank " + std::to_string(most) + " groups, more than the receive capacity " +
                                    std::to_string(capacity) + "; retry with capacity " + std::to_string(most));
       ctx->launch("hashagg_merge", [&] { launchHashAggMerge(ot, x, most, ctx->smCount, ctx->compute); });
+   });
+}
+
+// Repartition of a table's rows (include/ldb_gpu.h).  count (per batch) → scan → all-gather of the per-destination totals → host read of
+// the count matrix, capacity decision (identical on every rank) → barrier → send (per batch) → barrier → copy-out of the own region →
+// host wait.  While a rank's collectives wait for its peers nothing here blocks inside the driver: the temporaries and the pinned
+// scratch are taken before the first collective, the output buffers after the last, and host reads go to pinned memory.
+int ldb_gpu_table_exchange(LdbTable* src, int32_t n_keys, const char* const* key_columns, int32_t n_columns, const char* const* columns, LdbComm* c,
+                           int64_t recv_offset, int64_t recv_bytes, const char* name, LdbTable** out, LdbError* err) {
+   return guarded(err, [&] {
+      if (!src || !c || !out || (n_keys > 0 && !key_columns)) fail(LDB_ERR_INVALID, "null argument");
+      if (n_keys < 0 || n_keys > kProgMaxKeys) fail(LDB_ERR_INVALID, "the exchange takes 0..4 key columns");
+      if (src->ctx != c->ctx) fail(LDB_ERR_INVALID, "table and comm belong to different contexts");
+      std::vector<int> ship, key;
+      if (columns) {
+         if (n_columns < 1) fail(LDB_ERR_INVALID, "columns names 1..16 columns (NULL: all columns of the table)");
+         for (int i = 0; i < n_columns; i++) {
+            const int ci = src->colIndex(columns[i]);
+            if (ci < 0) fail(LDB_ERR_INVALID, std::string("unknown column ") + (columns[i] ? columns[i] : "(null)"));
+            ship.push_back(ci);
+         }
+      } else {
+         for (int ci = 0; ci < (int) src->columns.size(); ci++) ship.push_back(ci);
+      }
+      if (ship.size() > (size_t) kShipMaxCols) fail(LDB_ERR_INVALID, "the exchange ships up to 16 columns");
+      for (int ci : ship)
+         if (src->columns[ci].type == LDB_UTF8) fail(LDB_ERR_UNSUPPORTED, "the exchange ships fixed-width columns (utf8 column " + src->columns[ci].name + ")");
+      for (int k = 0; k < n_keys; k++) {
+         const int ci = src->colIndex(key_columns[k]);
+         if (ci < 0) fail(LDB_ERR_INVALID, std::string("unknown key column ") + (key_columns[k] ? key_columns[k] : "(null)"));
+         const int type = src->columns[ci].type;
+         if (type == LDB_UTF8 || type == LDB_FLOAT32 || type == LDB_FLOAT64) fail(LDB_ERR_UNSUPPORTED, "exchange keys are integer, date, char(1) or decimal columns");
+         key.push_back(ci);
+      }
+      wantConnected(c);
+      if (recv_offset < 0 || recv_bytes < 0 || recv_offset % 16 || recv_offset > (int64_t) c->userBytes || recv_bytes > (int64_t) c->userBytes - recv_offset)
+         fail(LDB_ERR_INVALID, "receive region outside the comm's user heap or not 16-byte aligned");
+      LdbContext* ctx = c->ctx;
+      if (ctx->capturing) fail(LDB_ERR_UNSUPPORTED, "the table exchange reads the row counts on the host and cannot be captured");
+      LDB_CUDA(cudaSetDevice(ctx->device));
+      const int world = c->world, nCols = (int) ship.size();
+      int32_t outBytes[kShipMaxCols] = {};
+      for (int j = 0; j < nCols; j++) {
+         switch (src->columns[ship[j]].type) {
+            case LDB_INT8: outBytes[j] = 1; break;
+            case LDB_INT16: outBytes[j] = 2; break;
+            case LDB_INT64:
+            case LDB_FLOAT64: outBytes[j] = 8; break;
+            case LDB_DECIMAL128: outBytes[j] = 16; break;
+            default: outBytes[j] = 4; // int32, date32, fsb4, float32
+         }
+      }
+      // before the first collective: staging waits, temporaries, pinned scratch
+      for (auto& b : src->batches) ldb_gpu_wait_batch_internal(ctx, &b);
+      int64_t nCtas = 0;
+      for (auto& b : src->batches) nCtas += (b.nRows + kShipTile - 1) / kShipTile;
+      Scratch tmp(ctx);
+      const bool broadcast = n_keys == 0;
+      uint8_t* owners = broadcast ? nullptr : tmp.alloc<uint8_t>((size_t) std::max<int64_t>(src->numRows, 1));
+      unsigned long long* hist = broadcast ? nullptr : tmp.alloc<unsigned long long>((size_t) std::max<int64_t>(nCtas, 1) * world * 8);
+      unsigned long long* totals = tmp.alloc<unsigned long long>(8 * kMaxPeers);
+      unsigned long long* matrix = (unsigned long long*) ctx->scratch(); // [world][kMaxPeers] M[s][d]
+      int32_t* timedOut = (int32_t*) (matrix + kMaxPeers * kMaxPeers);
+      unsigned long long* upload = matrix + kMaxPeers * kMaxPeers + 8;
+      TableShipBatch p{};
+      p.nCols = nCols;
+      p.nKeys = n_keys;
+      p.world = world;
+      p.broadcast = broadcast ? 1 : 0;
+      p.nCtas = nCtas;
+      p.owners = owners;
+      p.hist = hist;
+      for (int j = 0; j < nCols; j++) p.outBytes[j] = outBytes[j];
+      auto bindBatch = [&](const LdbBatch& b, int64_t firstRow, int64_t ctaBase) {
+         TableShipBatch q = p;
+         for (int j = 0; j < nCols; j++) {
+            bindColumn(q.cols[j], b, ship[j]);
+            q.cols[j].type = src->columns[ship[j]].type;
+         }
+         for (int k = 0; k < n_keys; k++) {
+            bindColumn(q.keys[k], b, key[k]);
+            q.keys[k].type = src->columns[key[k]].type;
+         }
+         q.nRows = b.nRows;
+         q.firstRow = firstRow;
+         q.ctaBase = ctaBase;
+         return q;
+      };
+      // every non-empty batch with its source row number and first CTA, in source order
+      auto eachBatch = [&](const std::function<void(const TableShipBatch&, int)>& fn) {
+         int64_t first = 0, cta = 0;
+         for (auto& b : src->batches) {
+            if (b.nRows > 0) fn(bindBatch(b, first, cta), (int) ((b.nRows + kShipTile - 1) / kShipTile));
+            first += b.nRows;
+            cta += (b.nRows + kShipTile - 1) / kShipTile;
+         }
+      };
+      if (broadcast) {
+         for (int d = 0; d < kMaxPeers; d++) upload[d] = d < world ? (unsigned long long) src->numRows : 0ull;
+         LDB_CUDA(cudaMemcpyAsync(totals, upload, 8 * kMaxPeers, cudaMemcpyHostToDevice, ctx->compute));
+      } else {
+         ctx->launch("table_exchange_count", [&] {
+            LDB_CUDA(cudaMemsetAsync(totals, 0, 8 * kMaxPeers, ctx->compute));
+            eachBatch([&](const TableShipBatch& q, int grid) { tableShipCountKernel<<<grid, kShipThreads, 0, ctx->compute>>>(q); });
+            tableShipScanKernel<<<world, 1024, 0, ctx->compute>>>(hist, nCtas, totals);
+         });
+      }
+      // the count matrix on every rank
+      if (world == 1) {
+         LDB_CUDA(cudaMemcpyAsync(matrix, totals, 8 * kMaxPeers, cudaMemcpyDeviceToHost, ctx->compute));
+      } else {
+         const uint8_t* gathered = allGatherSmall(c, totals, 8 * kMaxPeers);
+         LDB_CUDA(cudaMemcpy2DAsync(matrix, 8 * kMaxPeers, gathered, kSlotBytes, 8 * kMaxPeers, world, cudaMemcpyDeviceToHost, ctx->compute));
+      }
+      LDB_CUDA(cudaMemcpyAsync(timedOut, c->error, 4, cudaMemcpyDeviceToHost, ctx->compute));
+      ctx->syncStream(ctx->compute);
+      if (*timedOut) fail(LDB_ERR_CUDA, "a peer did not arrive at a collective within the timeout (LDB_PEER_TIMEOUT_MS)");
+      uint64_t colOff[kShipMaxCols], validOff[kShipMaxCols], need = 0;
+      for (int d = 0; d < world; d++) {
+         unsigned long long n = 0;
+         for (int s = 0; s < world; s++) {
+            if (s == c->rank) p.base[d] = n;
+            n += matrix[s * kMaxPeers + d];
+         }
+         p.rows[d] = n;
+         need = std::max(need, shipLayout(n, outBytes, nCols, colOff, validOff));
+      }
+      if (need > (uint64_t) recv_bytes)
+         fail(LDB_ERR_CAPACITY, "table exchange: a rank receives rows that need " + std::to_string(need) + " bytes of receive region, more than recv_bytes " +
+                                   std::to_string(recv_bytes) + "; retry with recv_bytes " + std::to_string(need));
+      const unsigned long long mine = p.rows[c->rank];
+      for (int d = 0; d < world; d++) p.recv[d] = c->peerHeap[d] + kUserOff + recv_offset;
+      auto barrier = [&] {
+         if (world == 1) return;
+         ctx->launch("peer_barrier", [&] {
+            peerBarrierKernel<<<world, 32, 0, ctx->compute>>>(c->view());
+            peerBumpKernel<<<1, 1, 0, ctx->compute>>>(c->view(), EPOCH_BARRIER, -1);
+         });
+      };
+      barrier(); // no peer still copies out of, or otherwise reads, the region it is about to receive into
+      ctx->launch("table_exchange_send", [&] {
+         eachBatch([&](const TableShipBatch& q, int grid) {
+            TableShipBatch r = q;
+            for (int d = 0; d < world; d++) {
+               r.recv[d] = p.recv[d];
+               r.rows[d] = p.rows[d];
+               r.base[d] = p.base[d];
+            }
+            tableShipSendKernel<<<grid, kShipThreads, 0, ctx->compute>>>(r);
+         });
+      });
+      barrier(); // every peer's rows are in this rank's region
+      // copy-out into buffers the new table owns: one device-to-device copy per array
+      shipLayout(mine, outBytes, nCols, colOff, validOff);
+      Scratch cols(ctx);
+      std::vector<LdbColumn> outCols;
+      LdbBatch ob;
+      ob.nRows = (int64_t) mine;
+      const uint8_t* region = c->heap + kUserOff + recv_offset;
+      ctx->launch("table_exchange_copy", [&] {
+         for (int j = 0; j < nCols; j++) {
+            const LdbColumn& sc = src->columns[ship[j]];
+            outCols.push_back({sc.name, sc.type, sc.precision, sc.scale});
+            const size_t bytes = (size_t) mine * outBytes[j];
+            uint8_t* data = cols.alloc<uint8_t>(std::max<size_t>(bytes, 16));
+            uint8_t* valid = cols.alloc<uint8_t>(std::max<size_t>(mine, 16));
+            if (mine) {
+               LDB_CUDA(cudaMemcpyAsync(data, region + colOff[j], bytes, cudaMemcpyDeviceToDevice, ctx->compute));
+               LDB_CUDA(cudaMemcpyAsync(valid, region + validOff[j], (size_t) mine, cudaMemcpyDeviceToDevice, ctx->compute));
+            }
+            ob.data.push_back(data);
+            ob.bytes.push_back(nullptr);
+            ob.elemBytes.push_back(outBytes[j]);
+            ob.validBytes.push_back(valid);
+         }
+      });
+      LDB_CUDA(cudaMemcpyAsync(timedOut, c->error, 4, cudaMemcpyDeviceToHost, ctx->compute));
+      ctx->syncStream(ctx->compute); // the region is free for the next collective, the temporaries for the pool
+      if (*timedOut) fail(LDB_ERR_CUDA, "a peer did not arrive at a collective within the timeout (LDB_PEER_TIMEOUT_MS)");
+      *out = addResultTable(ctx, name ? name : "received", std::move(outCols), std::move(ob), cols);
    });
 }
 

@@ -15,9 +15,7 @@ namespace {
 bool isCountKind(int k) { return k == LDB_AGG_COUNT || k == LDB_AGG_COUNT_STAR; }
 } // namespace
 
-// registers a single-batch table this library made: `b` holds nRows and, per column, data / bytes / elemBytes / validBytes; the table
-// takes over the device buffers of `buffers`
-static LdbTable* addResultTable(LdbContext* ctx, std::string name, std::vector<LdbColumn> columns, LdbBatch b, Scratch& buffers) {
+LdbTable* ldb::addResultTable(LdbContext* ctx, std::string name, std::vector<LdbColumn> columns, LdbBatch b, Scratch& buffers) {
    auto* t = new LdbTable;
    t->ctx = ctx;
    t->name = std::move(name);
@@ -388,8 +386,7 @@ void ldb_gpu_check_keyjoin_error_internal(LdbState* s) {
    }
 }
 
-// the pointers of column `ci` of batch `b` (validity bitmap or validity bytes included)
-static void bindColumn(ProgCol& pc, const LdbBatch& b, int ci) {
+void ldb::bindColumn(ProgCol& pc, const LdbBatch& b, int ci) {
    pc.data = (const uint8_t*) b.data[ci];
    pc.bytes = (const uint8_t*) b.bytes[ci];
    pc.elemBytes = b.elemBytes[ci];

@@ -159,6 +159,29 @@ class Comm:
             capacity = max(self._gather_counts(int(n.value)))
         capi.check(self.L.ldb_gpu_hashagg_exchange(local, owned, self.h, int(recv_offset), int(capacity), C.byref(e)), e)
 
+    def table_exchange(self, table, keys, columns=None, name: str = "received", recv_offset: int = 0, recv_bytes: int = None):
+        """Repartition of a table's rows (ldb_gpu_table_exchange): with 1..4 `keys` every row goes to the rank that owns its key tuple
+        (the rank hashagg_exchange gives the group with those keys); with no keys every row goes to every rank.  `table` is a runtime
+        table, a program.RawTable or a table handle; `columns` the columns to ship (None: all).  Returns this rank's received rows as a
+        program.RawTable, source rank 0's rows first, each source's in its row order.  Collective, and it waits for the peers on the
+        host: the ranks of one process call it from one thread each.  The receive region starts at user-heap offset `recv_offset` and
+        spans `recv_bytes` (None: the rest of the user heap); rows that do not fit fail with LDB_ERR_CAPACITY on every rank.  The
+        received table is named `name` ("received" when None)."""
+        from . import capi
+        from .program import RawTable, _handle
+        keys = list(keys or [])
+        kn = [k.encode() for k in keys]
+        karr = (C.c_char_p * max(1, len(kn)))(*kn)
+        cn = [c.encode() for c in columns] if columns is not None else []
+        carr = (C.c_char_p * max(1, len(cn)))(*cn) if columns is not None else None
+        if recv_bytes is None:
+            recv_bytes = self.heap()[1] - int(recv_offset)
+        out, e = C.c_void_p(), capi.Error()
+        capi.check(self.L.ldb_gpu_table_exchange(C.c_void_p(_handle(table)), len(kn), karr, len(cn), carr, self.h, int(recv_offset), int(recv_bytes),
+                                                 name.encode() if name is not None else None,
+                                                 C.byref(out), C.byref(e)), e)
+        return RawTable(self.ctx, out)
+
     def _gather_counts(self, n: int) -> List[int]:
         """every rank's `n`, in rank order"""
         if self.world == 1:
