@@ -583,7 +583,8 @@ int ldb_gpu_table_gather_strings(LdbTable* t, const char* column, const int64_t*
  * `expected_strings` (a directory of nextPow2(2 x that) slots) and `expected_bytes` of string data.  When the directory or the byte
  * arena overflows, a probe run passes the interpreter's bound or a code would pass INT32_MAX, the program fails with
  * LDB_ERR_CAPACITY; the contents are then unspecified: recreate the dictionary larger.  No string is dropped silently.  Not for
- * captured queries, serialised steps or multi-GPU: codes belong to one context. */
+ * captured queries or serialised steps.  Its codes belong to one context; for codes that agree across the ranks of a comm, unify the
+ * ranks' dictionaries (ldb_gpu_dict_unify). */
 int ldb_gpu_dict_create(LdbContext* ctx, int64_t expected_strings, int64_t expected_bytes, LdbState** out, LdbError* err);
 int ldb_gpu_dict_count(LdbState* s, int64_t* n_strings, LdbError* err);
 /* the dictionary as a single-batch DEVICE table, row i = code i: "str" (utf8) the string, "rank" (int32) its position in bytewise
@@ -681,6 +682,30 @@ int ldb_gpu_hashagg_exchange(LdbState* local, LdbState* owned, LdbComm* comm, in
  * call it from one thread each.  On return the receive region is free again; world = 1 is a compacting copy. */
 int ldb_gpu_table_exchange(LdbTable* src, int32_t n_keys, const char* const* key_columns, int32_t n_columns, const char* const* columns /* NULL = all columns of src */,
                            LdbComm* comm, int64_t recv_offset, int64_t recv_bytes, const char* name, LdbTable** out, LdbError* err);
+/* Unify the string dictionaries of the ranks of `comm` into one dictionary that every rank holds, with codes in bytewise order, so that
+ * string group, join and sort keys work across ranks.  Collective: every rank calls it in the same order, each with a string dictionary
+ * (LDB_STATE_DICT) of comm's context, which may be empty; `local` is only read.
+ *   Result: *out = a new dictionary state on every rank holding the union U of all ranks' strings.  The code of s is the number of
+ *   strings in U that order before s, in bytewise order with unsigned bytes and a proper prefix first: the order of LDB_OP_STRCMP,
+ *   ldb_gpu_table_order_by_keys and the dictionary table's "rank" column.  The strings and their codes are the same, byte for byte, on
+ *   every rank: ldb_gpu_dict_count gives |U|, ldb_gpu_dict_to_table the strings in code order with rank[i] == i.  The empty string is a
+ *   string like any other; NULL is never in a dictionary.  Codes do not depend on thread timing.
+ *   Lookups only: an LDB_OP_STRCODE lookup (b = 0) against a unified dictionary works as against any other (an absent string gives
+ *   NULL); an inserting STRCODE (b = 1) fails the program with LDB_ERR_INVALID before launch, since a rank-local insert would break the
+ *   ranks' agreement.
+ *   Receive region, all or nothing: [recv_offset, recv_offset + recv_bytes) of the user heap, the same on every rank, recv_offset a
+ *   multiple of 16.  Source s's block holds its n_s + 1 int32 offsets rebased to 0, then its B_s bytes, each array 16-byte aligned;
+ *   blocks follow in rank order.  Every rank learns every rank's (n_s, B_s) before anything is stored; when the blocks do not fit, EVERY
+ *   rank fails with LDB_ERR_CAPACITY naming the recv_bytes to retry with, and nothing is written into any receive region.
+ *   Limits, decided identically on every rank: the ranks' strings past 2^31 - 1 bytes in all (int32 utf8 offsets) or |U| past 2^30
+ *   strings (the most a dictionary is made for): LDB_ERR_UNSUPPORTED.  A local dictionary that overflowed earlier (its contents are
+ *   unspecified): LDB_ERR_CAPACITY naming its rank, on every rank.
+ * Other errors, before any collective starts: LDB_ERR_INVALID for null arguments, a state that is not a dictionary, a dictionary or comm
+ * of another context, a region outside the user heap or a misaligned recv_offset; LDB_ERR_UNSUPPORTED inside a captured query (the call
+ * reads the counts on the host and synchronises the compute stream).  Ranks of one process must call it from one thread each.  Every
+ * rank holds the whole union: it suits group keys, flags, names and other columns of moderate cardinality.  On return the receive region
+ * is free again; world = 1 renumbers `local` into bytewise order. */
+int ldb_gpu_dict_unify(LdbState* local, LdbComm* comm, int64_t recv_offset, int64_t recv_bytes, LdbState** out, LdbError* err);
 /* zero / read back (synchronising) a range of this rank's user heap */
 int ldb_gpu_comm_heap_zero(LdbComm* comm, int64_t user_offset, int64_t bytes, LdbError* err);
 int ldb_gpu_comm_heap_read(LdbComm* comm, int64_t user_offset, int64_t bytes, void* host_dst, LdbError* err);

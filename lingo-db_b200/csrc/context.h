@@ -301,6 +301,9 @@ void bindColumn(ProgCol& pc, const LdbBatch& b, int ci);
 // registers a single-batch table this library made: `b` holds nRows and, per column, data / bytes / elemBytes / validBytes; the table
 // takes over the device buffers of `buffers` (program_rt.cpp)
 LdbTable* addResultTable(LdbContext* ctx, std::string name, std::vector<LdbColumn> columns, LdbBatch b, Scratch& buffers);
+// row ids of the single-batch table `t` (n rows, n < 2^32) ordered by the keys (column index, descending), in `scratch`: ORDER BY,
+// dictionary ranks and the union of a unified dictionary (program_rt.cpp)
+uint32_t* sortRows(Scratch& scratch, LdbTable* t, const std::vector<std::pair<int, int>>& keys, int64_t n);
 } // namespace ldb
 // builds the missing encoded copies of columns cols[0..n) of a borrowed DEVICE batch (encode.cu) for tiles of `tileRows` rows;
 // true when every one of them has a copy.  Runs outside any capture and waits for its work on the host.
@@ -323,9 +326,14 @@ struct LdbState {
    uint32_t laneBound = 0;  // aggregates whose width (64 / 128 bits) a pipeline fixed already: a later one must agree
    uint8_t* marks = nullptr; // JOIN_TABLE / KEY_JOIN: one marker byte per directory slot (program.h), from the first program that marks
                              // the table; also in `allocations`
+   bool unified = false;     // DICT made by ldb_gpu_dict_unify: its codes agree across ranks, so programs may only look strings up in it
    std::vector<void*> allocations;
 };
 
+// a new, empty string dictionary with room for `expected_strings` strings of `expected_bytes` bytes (ldb_gpu_dict_create, program_rt.cpp)
+LdbState* ldb_gpu_dict_new_internal(LdbContext* ctx, int64_t expected_strings, int64_t expected_bytes);
+// a dictionary's counters {arena bytes, codes}, after its error word is checked: LDB_ERR_CAPACITY when it overflowed (synchronises)
+std::pair<int64_t, int64_t> ldb_gpu_dict_counters_internal(LdbState* s);
 // reads a join table's error word (synchronises the compute stream) and throws ApiError with the status and message of a
 // non-zero code (runtime.cpp); every caller that reports a join table's failure goes through it
 void ldb_gpu_check_join_error_internal(LdbState* s);

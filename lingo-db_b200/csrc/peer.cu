@@ -361,6 +361,14 @@ __global__ void __launch_bounds__(kShipThreads) tableShipSendKernel(const __grid
    }
 }
 
+// ---------------------------------------------------------------- dictionary unification (ldb_gpu_dict_unify, include/ldb_gpu.h)
+// This rank's exported dictionary into its block of receiver blockIdx.y's region: the offsets array and the bytes array, each padded to
+// 16 bytes, back to back, so the block is one run of 16-byte vectors.  The sources are padded the same way.
+__global__ void __launch_bounds__(256) dictSendKernel(const __grid_constant__ PeerView v, size_t blockOff, const int4* offsets, size_t offVecs, const int4* bytes, size_t byteVecs) {
+   int4* dst = (int4*) (v.heap[blockIdx.y] + blockOff);
+   for (size_t i = (size_t) blockIdx.x * blockDim.x + threadIdx.x; i < offVecs + byteVecs; i += (size_t) gridDim.x * blockDim.x) dst[i] = i < offVecs ? offsets[i] : bytes[i - offVecs];
+}
+
 } // namespace ldb
 
 using namespace ldb;
@@ -412,7 +420,11 @@ int ldb_gpu_comm_create(LdbContext* ctx, int32_t rank, int32_t world, int64_t us
       LDB_CUDA(cudaFuncGetAttributes(&fa, tableShipCountKernel));
       LDB_CUDA(cudaFuncGetAttributes(&fa, tableShipScanKernel));
       LDB_CUDA(cudaFuncGetAttributes(&fa, tableShipSendKernel));
+      LDB_CUDA(cudaFuncGetAttributes(&fa, dictSendKernel));
       loadHashAggExchangeKernels();
+      // the pinned scratch the collectives read counts into: allocating host memory can wait for running kernels, so it is taken now
+      // rather than on a rank's first collective while a peer of the same process may already be waiting for it
+      ctx->scratch();
       cudaIpcMemHandle_t h;
       LDB_CUDA(cudaIpcGetMemHandle(&h, c->heap));
       static_assert(sizeof(h) == LDB_IPC_HANDLE_BYTES, "cudaIpcMemHandle_t is 64 bytes");
@@ -881,6 +893,123 @@ int ldb_gpu_table_exchange(LdbTable* src, int32_t n_keys, const char* const* key
       ctx->syncStream(ctx->compute); // the region is free for the next collective, the temporaries for the pool
       if (*timedOut) fail(LDB_ERR_CUDA, "a peer did not arrive at a collective within the timeout (LDB_PEER_TIMEOUT_MS)");
       *out = addResultTable(ctx, name ? name : "received", std::move(outCols), std::move(ob), cols);
+   });
+}
+
+// Union of every rank's string dictionary (include/ldb_gpu.h).  Local counters → export → all-gather of {status, n, bytes} → host
+// decision from the gathered counts (identical on every rank) → barrier → send → barrier → concatenation of the received blocks → sort →
+// codes → ranked build.  As in the table exchange, the temporaries are taken before the first collective and the rest after the last.
+static uint64_t align16(uint64_t x) { return (x + 15) & ~uint64_t(15); }
+int ldb_gpu_dict_unify(LdbState* local, LdbComm* c, int64_t recv_offset, int64_t recv_bytes, LdbState** out, LdbError* err) {
+   return guarded(err, [&] {
+      if (!local || !c || !out) fail(LDB_ERR_INVALID, "null argument");
+      if (local->kind != LDB_STATE_DICT) fail(LDB_ERR_INVALID, "not a string dictionary");
+      if (local->ctx != c->ctx) fail(LDB_ERR_INVALID, "dictionary and comm belong to different contexts");
+      wantConnected(c);
+      if (recv_offset < 0 || recv_bytes < 0 || recv_offset % 16 || recv_offset > (int64_t) c->userBytes || recv_bytes > (int64_t) c->userBytes - recv_offset)
+         fail(LDB_ERR_INVALID, "receive region outside the comm's user heap or not 16-byte aligned");
+      LdbContext* ctx = c->ctx;
+      if (ctx->capturing) fail(LDB_ERR_UNSUPPORTED, "dictionary unification reads the string counts on the host and cannot be captured");
+      LDB_CUDA(cudaSetDevice(ctx->device));
+      const int world = c->world;
+      // pinned scratch: [0, 4) local counters, [8, 12) this rank's gathered block, [16, 16 + 4 world) every rank's, then the error word
+      unsigned long long* pin = (unsigned long long*) ctx->scratch();
+      unsigned long long* block = pin + 8;
+      unsigned long long* blocks = pin + 16;
+      int32_t* timedOut = (int32_t*) (blocks + 4 * kMaxPeers);
+      LDB_CUDA(cudaMemcpyAsync(pin, local->dict.ctr, 24, cudaMemcpyDeviceToHost, ctx->compute));
+      ctx->syncStream(ctx->compute);
+      // a dictionary that overflowed (its contents are unspecified) or that no block could carry sends no strings, only its status
+      const uint32_t status = (uint32_t) pin[2];
+      const bool sends = status == 0 && pin[0] <= (unsigned long long) INT32_MAX;
+      const int64_t n = sends ? (int64_t) pin[1] : 0, bytes = sends ? (int64_t) pin[0] : 0;
+      block[0] = status;
+      block[1] = (unsigned long long) n;
+      block[2] = status == 0 ? pin[0] : 0;
+      block[3] = 0;
+      Scratch tmp(ctx);
+      uint32_t* offs = tmp.alloc<uint32_t>(align16((uint64_t) (n + 1) * 4));
+      uint8_t* data = tmp.alloc<uint8_t>(std::max<uint64_t>(align16((uint64_t) bytes), 16));
+      ctx->launch("dict_export", [&] { launchDictExport(local->dict, n, offs, data, ctx->smCount, ctx->compute); });
+      const uint8_t* gathered = allGatherSmall(c, block, 32);
+      LDB_CUDA(cudaMemcpy2DAsync(blocks, 32, gathered, kSlotBytes, 32, world, cudaMemcpyDeviceToHost, ctx->compute));
+      LDB_CUDA(cudaMemcpyAsync(timedOut, c->error, 4, cudaMemcpyDeviceToHost, ctx->compute));
+      ctx->syncStream(ctx->compute);
+      if (*timedOut) fail(LDB_ERR_CUDA, "a peer did not arrive at a collective within the timeout (LDB_PEER_TIMEOUT_MS)");
+      // every rank decides from the same gathered counts
+      uint64_t blockOff[kMaxPeers + 1] = {}, byteBase[kMaxPeers + 1] = {}, rowBase[kMaxPeers + 1] = {};
+      for (int s = 0; s < world; s++) {
+         const unsigned long long* b = blocks + 4 * s;
+         if (b[0]) fail(LDB_ERR_CAPACITY, "dictionary unification: the string dictionary of rank " + std::to_string(s) + " overflowed earlier (error word " + std::to_string(b[0]) +
+                                             "; recreate it larger)");
+         blockOff[s + 1] = blockOff[s] + align16((b[1] + 1) * 4) + align16(b[2]);
+         byteBase[s + 1] = byteBase[s] + b[2];
+         rowBase[s + 1] = rowBase[s] + b[1];
+      }
+      if (byteBase[world] > (uint64_t) INT32_MAX) fail(LDB_ERR_UNSUPPORTED, "dictionary unification: the ranks' strings exceed 2^31 - 1 bytes (utf8 offsets are int32)");
+      if (blockOff[world] > (uint64_t) recv_bytes)
+         fail(LDB_ERR_CAPACITY, "dictionary unification: the ranks' strings need " + std::to_string(blockOff[world]) + " bytes of receive region, more than recv_bytes " +
+                                   std::to_string(recv_bytes) + "; retry with recv_bytes " + std::to_string(blockOff[world]));
+      auto barrier = [&] {
+         if (world == 1) return;
+         ctx->launch("peer_barrier", [&] {
+            peerBarrierKernel<<<world, 32, 0, ctx->compute>>>(c->view());
+            peerBumpKernel<<<1, 1, 0, ctx->compute>>>(c->view(), EPOCH_BARRIER, -1);
+         });
+      };
+      barrier(); // no peer still reads the region it is about to receive into
+      const size_t offVecs = align16((uint64_t) (n + 1) * 4) / 16, byteVecs = align16((uint64_t) bytes) / 16;
+      ctx->launch("dict_unify_send", [&] {
+         const dim3 grid((unsigned) std::min<size_t>(std::max<size_t>((offVecs + byteVecs + 255) / 256, 1), (size_t) ctx->smCount * 2), (unsigned) world);
+         dictSendKernel<<<grid, 256, 0, ctx->compute>>>(c->view(), kUserOff + (size_t) recv_offset + blockOff[c->rank], (const int4*) offs, offVecs, (const int4*) data, byteVecs);
+      });
+      barrier(); // every peer's block is in this rank's region
+      LDB_CUDA(cudaMemcpyAsync(timedOut, c->error, 4, cudaMemcpyDeviceToHost, ctx->compute));
+      ctx->syncStream(ctx->compute);
+      if (*timedOut) fail(LDB_ERR_CUDA, "a peer did not arrive at a collective within the timeout (LDB_PEER_TIMEOUT_MS)");
+      // the received blocks as one utf8 column of N strings, in rank order
+      const int64_t N = (int64_t) rowBase[world];
+      Scratch col(ctx);
+      uint32_t* allOffs = col.alloc<uint32_t>((size_t) (N + 1) * 4);
+      uint8_t* allBytes = col.alloc<uint8_t>(std::max<uint64_t>(byteBase[world], 16));
+      const uint8_t* region = c->heap + kUserOff + recv_offset;
+      ctx->launch("dict_unify_concat", [&] {
+         for (int s = 0; s < world; s++) {
+            const uint64_t ns = rowBase[s + 1] - rowBase[s], bs = byteBase[s + 1] - byteBase[s];
+            // n_s + 1 offsets each: the last one of source s equals the first of source s + 1
+            launchDictRebase((const uint32_t*) (region + blockOff[s]), (int64_t) ns + 1, (uint32_t) byteBase[s], allOffs + rowBase[s], ctx->smCount, ctx->compute);
+            if (bs) LDB_CUDA(cudaMemcpyAsync(allBytes + byteBase[s], region + blockOff[s] + align16((ns + 1) * 4), bs, cudaMemcpyDeviceToDevice, ctx->compute));
+         }
+      });
+      LdbTable all{};
+      all.ctx = ctx;
+      all.columns = {{"str", LDB_UTF8, 0, 0}};
+      all.numRows = N;
+      all.batches.resize(1);
+      all.batches[0].nRows = N;
+      all.batches[0].data = {allOffs};
+      all.batches[0].bytes = {allBytes};
+      all.batches[0].elemBytes = {4};
+      uint32_t* ids = sortRows(col, &all, {{0, 0}}, N);
+      uint32_t* codes = col.alloc<uint32_t>((size_t) (N + 1) * 4);
+      uint32_t* arenaOff = col.alloc<uint32_t>((size_t) (N + 1) * 4);
+      ctx->launch("dict_unify_ranks", [&] { launchDictUnionRanks(allOffs, allBytes, ids, N, codes, arenaOff, ctx->smCount, ctx->compute); });
+      uint32_t* totals = (uint32_t*) pin;
+      LDB_CUDA(cudaMemcpyAsync(totals, codes + N, 4, cudaMemcpyDeviceToHost, ctx->compute));
+      LDB_CUDA(cudaMemcpyAsync(totals + 1, arenaOff + N, 4, cudaMemcpyDeviceToHost, ctx->compute));
+      ctx->syncStream(ctx->compute);
+      const int64_t nu = totals[0], bu = totals[1];
+      if (nu > kDictMaxStrings) fail(LDB_ERR_UNSUPPORTED, "dictionary unification: the union holds " + std::to_string(nu) + " strings, more than a dictionary's 2^30");
+      LdbState* u = ldb_gpu_dict_new_internal(ctx, nu, bu);
+      u->unified = true;
+      try {
+         ctx->launch("dict_unify_build", [&] { launchDictRankedBuild(u->dict, allOffs, allBytes, ids, N, codes, arenaOff, ctx->smCount, ctx->compute); });
+         ldb_gpu_dict_counters_internal(u); // synchronises: the region is free again, the temporaries go back to the pool
+      } catch (...) {
+         ldb_gpu_state_destroy(u);
+         throw;
+      }
+      *out = u;
    });
 }
 

@@ -149,6 +149,13 @@ __device__ __forceinline__ uint64_t strHash(const uint8_t* s, int32_t n) {
    }
    return mix64(h);
 }
+// where a string with hash h lives in the directory: its tag (the high 32 bits of h, the upper half of its slot word), its first slot
+// and the linear probe sequence from there, at most dictProbeLimit slots long.  One definition for dictCode and the ranked build of a
+// unified dictionary, so that a lookup finds every string the build placed.
+__device__ __forceinline__ unsigned long long dictTag(uint64_t h) { return (h >> 32) << 32; }
+__device__ __forceinline__ uint64_t dictFirstSlot(uint64_t h, uint64_t mask) { return h & mask; }
+__device__ __forceinline__ uint64_t dictNextSlot(uint64_t slot, uint64_t mask) { return (slot + 1) & mask; }
+__device__ __forceinline__ uint64_t dictProbeLimit(uint64_t mask) { return mask + 1 < 65536 ? mask + 1 : 65536; }
 __device__ __forceinline__ void dictFail(const DictDev& d, int code) { atomicCAS((unsigned int*) (d.ctr + 2), 0u, (unsigned int) code); }
 // the code of string s[0..n) in dictionary d; absent: inserted when `insert`, else -1.  -2: the dictionary failed (its error word
 // is set, the call reports LDB_ERR_CAPACITY).  A slot is claimed by CAS (empty → tag | kDictWriting); its claimer reserves arena
@@ -157,9 +164,9 @@ __device__ __forceinline__ void dictFail(const DictDev& d, int code) { atomicCAS
 // string bytewise (loads through L2: the arena is written by other SMs during the same launch).  A hit takes no atomic.
 __device__ __noinline__ int32_t dictCode(const DictDev& d, const uint8_t* s, int32_t n, int insert) {
    const uint64_t h = strHash(s, n);
-   const unsigned long long tag = (h >> 32) << 32;
-   uint64_t slot = h & d.mask;
-   const uint64_t limit = d.mask + 1 < 65536 ? d.mask + 1 : 65536;
+   const unsigned long long tag = dictTag(h);
+   uint64_t slot = dictFirstSlot(h, d.mask);
+   const uint64_t limit = dictProbeLimit(d.mask);
    for (uint64_t probes = 0; probes < limit; probes++) {
       unsigned long long* sp = d.slots + slot;
       unsigned long long w = *((volatile unsigned long long*) sp);
@@ -204,7 +211,7 @@ __device__ __noinline__ int32_t dictCode(const DictDev& d, const uint8_t* s, int
             if (i == n) return code;
          }
       }
-      slot = (slot + 1) & d.mask;
+      slot = dictNextSlot(slot, d.mask);
    }
    dictFail(d, 1);
    return -2;
@@ -1257,6 +1264,76 @@ void launchDictExport(const DictDev& d, int64_t n, uint32_t* offsets, uint8_t* b
    dictLengthsKernel<<<grid, 256, 0, s>>>(d.entryLen, n, offsets);
    sortScanKernel<<<1, 1024, 0, s>>>(offsets, n + 1); // exclusive: offsets[n] = total bytes
    if (n) dictCopyKernel<<<(int) std::min<int64_t>((n + 7) / 8, (int64_t) smCount * 16), 256, 0, s>>>(d, n, offsets, bytes);
+}
+
+// ---------------------------------------------------------------- unified dictionaries (ldb_gpu_dict_unify, peer.cu)
+__global__ void dictRebaseKernel(const uint32_t* src, int64_t n, uint32_t add, uint32_t* dst) {
+   for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t) gridDim.x * blockDim.x) dst[i] = src[i] + add;
+}
+void launchDictRebase(const uint32_t* src, int64_t n, uint32_t add, uint32_t* dst, int smCount, cudaStream_t s) {
+   int grid = (int) std::min<int64_t>(std::max<int64_t>((n + 255) / 256, 1), (int64_t) smCount * 8);
+   dictRebaseKernel<<<grid, 256, 0, s>>>(src, n, add, dst);
+}
+// sorted position i: isNew[i] = 1 when its string differs from the one at position i - 1 (position 0 always), newLen[i] = its length
+// then, else 0; both get a trailing 0 at position n for the exclusive scans that follow
+__global__ void dictUnionFlagsKernel(const uint32_t* offsets, const uint8_t* bytes, const uint32_t* ids, int64_t n, uint32_t* isNew, uint32_t* newLen) {
+   for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += (int64_t) gridDim.x * blockDim.x) {
+      if (i == n) {
+         isNew[n] = newLen[n] = 0;
+         continue;
+      }
+      const uint32_t r = ids[i], b = offsets[r], len = offsets[r + 1] - b;
+      bool fresh = i == 0;
+      if (!fresh) {
+         const uint32_t q = ids[i - 1], pb = offsets[q], plen = offsets[q + 1] - pb;
+         fresh = plen != len;
+         for (uint32_t j = 0; j < len && !fresh; j++) fresh = bytes[b + j] != bytes[pb + j];
+      }
+      isNew[i] = fresh ? 1u : 0u;
+      newLen[i] = fresh ? len : 0u;
+   }
+}
+void launchDictUnionRanks(const uint32_t* offsets, const uint8_t* bytes, const uint32_t* ids, int64_t n, uint32_t* codes, uint32_t* arenaOff, int smCount, cudaStream_t s) {
+   int grid = (int) std::min<int64_t>(std::max<int64_t>((n + 256) / 256, 1), (int64_t) smCount * 8);
+   dictUnionFlagsKernel<<<grid, 256, 0, s>>>(offsets, bytes, ids, n, codes, arenaOff);
+   sortScanKernel<<<1, 1024, 0, s>>>(codes, n + 1);
+   sortScanKernel<<<1, 1024, 0, s>>>(arenaOff, n + 1);
+}
+// one thread per sorted position that starts a new string: its bytes into the arena at arenaOff[i], its entry at code codes[i], and a slot
+// on its probe sequence claimed and published with code + 1 in one CAS (nothing reads the dictionary during the build).  Which of two
+// strings that share a probe run takes which slot depends on timing; codes, entries and arena do not.
+__global__ void dictRankedBuildKernel(DictDev d, const uint32_t* offsets, const uint8_t* bytes, const uint32_t* ids, int64_t n, const uint32_t* codes,
+                                      const uint32_t* arenaOff) {
+   if (blockIdx.x == 0 && threadIdx.x == 0) {
+      d.ctr[0] = arenaOff[n];
+      d.ctr[1] = codes[n];
+   }
+   for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t) gridDim.x * blockDim.x) {
+      const uint32_t code = codes[i];
+      if (codes[i + 1] == code) continue;
+      const uint32_t r = ids[i], b = offsets[r];
+      const int32_t len = (int32_t) (offsets[r + 1] - b);
+      const uint8_t* s = bytes + b;
+      const uint32_t off = arenaOff[i];
+      for (int32_t j = 0; j < len; j++) d.arena[off + j] = s[j];
+      d.entryOff[code] = off;
+      d.entryLen[code] = len;
+      const uint64_t h = strHash(s, len);
+      const unsigned long long word = dictTag(h) | (unsigned long long) (code + 1);
+      uint64_t slot = dictFirstSlot(h, d.mask);
+      const uint64_t limit = dictProbeLimit(d.mask);
+      uint64_t probes = 0;
+      while (probes < limit && atomicCAS(d.slots + slot, 0ull, word) != 0ull) {
+         slot = dictNextSlot(slot, d.mask);
+         probes++;
+      }
+      if (probes == limit) dictFail(d, 1);
+   }
+}
+void launchDictRankedBuild(const DictDev& d, const uint32_t* offsets, const uint8_t* bytes, const uint32_t* ids, int64_t n, const uint32_t* codes, const uint32_t* arenaOff,
+                           int smCount, cudaStream_t s) {
+   int grid = (int) std::min<int64_t>(std::max<int64_t>((n + 255) / 256, 1), (int64_t) smCount * 8);
+   dictRankedBuildKernel<<<grid, 256, 0, s>>>(d, offsets, bytes, ids, n, codes, arenaOff);
 }
 
 } // namespace ldb

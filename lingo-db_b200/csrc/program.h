@@ -86,6 +86,7 @@ struct DictDev {
    int64_t codeCap; // codes 0..codeCap-1 fit the entry arrays and int32
 };
 constexpr uint32_t kDictWriting = 0xffffffffu, kDictFailed = 0xfffffffeu;
+constexpr int64_t kDictMaxStrings = (int64_t) 1 << 30; // the most strings a dictionary is made for (its codes are int32)
 // key-tuple join table (LDB_STATE_KEY_JOIN): 1..4 int64 keys → int64 payload, open addressing in HBM, cap = nextPow2(2 x expected)
 //   entry = { word:u64 = tag:32 (high 32 bits of the tuple's hash) | state:32 (0 empty: the whole word is 0, kKeyJoinWriting,
 //             kKeyJoinReady), payload:i64, keys[nKeys]:i64 } padded to entryBytes = 32 (1-2 keys: one DRAM sector) or 48 (3-4 keys)
@@ -199,5 +200,14 @@ void launchBuildSortWords(const uint8_t* col, const uint8_t* bytes, int elemByte
 void launchScatterRanks(const uint32_t* ids, int64_t n, int32_t* rank, int smCount, cudaStream_t s);
 // dictionary → table: offsets[0..n] (exclusive scan of the lengths) and the bytes of code i at offsets[i]
 void launchDictExport(const DictDev& d, int64_t n, uint32_t* offsets, uint8_t* bytes, int smCount, cudaStream_t s);
+// unified dictionaries (ldb_gpu_dict_unify): dst[i] = src[i] + add for i < n (a received block's offsets into the concatenated column)
+void launchDictRebase(const uint32_t* src, int64_t n, uint32_t add, uint32_t* dst, int smCount, cudaStream_t s);
+// over the n strings of a utf8 column (offsets, bytes) in sorted order `ids`: codes[i] = the distinct strings before sorted position i,
+// arenaOff[i] = their bytes; codes[n] and arenaOff[n] are the totals (n + 1 entries each)
+void launchDictUnionRanks(const uint32_t* offsets, const uint8_t* bytes, const uint32_t* ids, int64_t n, uint32_t* codes, uint32_t* arenaOff, int smCount, cudaStream_t s);
+// fills a fresh dictionary `d` sized for codes[n] strings of arenaOff[n] bytes: arena and entries in code order, one published slot per
+// string on dictCode's probe sequence, ctr = {bytes, strings}
+void launchDictRankedBuild(const DictDev& d, const uint32_t* offsets, const uint8_t* bytes, const uint32_t* ids, int64_t n, const uint32_t* codes, const uint32_t* arenaOff,
+                           int smCount, cudaStream_t s);
 
 } // namespace ldb

@@ -197,12 +197,13 @@ int ldb_gpu_hashagg_to_table(LdbState* s, const char* name, LdbTable** out, LdbE
 
 static_assert(sizeof(ProgramParams) <= 4096, "ProgramParams exceeds the 4 KB kernel-parameter limit");
 
+} // extern "C"
+
 // ---------------------------------------------------------------- string dictionaries
 static void checkDict(LdbState* s) {
    if (!s || s->kind != LDB_STATE_DICT) fail(LDB_ERR_INVALID, "not a string dictionary");
 }
-// the dictionary's counters {arena bytes, codes}, after its error word is checked (synchronises)
-static std::pair<int64_t, int64_t> checkDictError(LdbState* s) {
+std::pair<int64_t, int64_t> ldb_gpu_dict_counters_internal(LdbState* s) {
    unsigned long long c[3] = {0, 0, 0};
    LDB_CUDA(cudaMemcpyAsync(c, s->dict.ctr, sizeof(c), cudaMemcpyDeviceToHost, s->ctx->compute));
    s->ctx->syncStream(s->ctx->compute);
@@ -218,8 +219,8 @@ static std::pair<int64_t, int64_t> checkDictError(LdbState* s) {
 
 // row ids of the single-batch table `t` (n rows, n < 2^32) ordered by the keys (column index, descending): a device buffer of n
 // uint32 in `scratch`, like the sort's temporaries, so the caller waits for the sort before its scope ends.  The one place that
-// knows the string order: ORDER BY and dictionary ranks.
-static uint32_t* sortRows(Scratch& scratch, LdbTable* t, const std::vector<std::pair<int, int>>& keys, int64_t n) {
+// knows the string order: ORDER BY, dictionary ranks and unified dictionaries.
+uint32_t* ldb::sortRows(Scratch& scratch, LdbTable* t, const std::vector<std::pair<int, int>>& keys, int64_t n) {
    LdbContext* ctx = t->ctx;
    LdbBatch& b = t->batches[0];
    const size_t rows = (size_t) std::max<int64_t>(n, 1);
@@ -265,34 +266,40 @@ static uint32_t* sortRows(Scratch& scratch, LdbTable* t, const std::vector<std::
    return dv;
 }
 
+LdbState* ldb_gpu_dict_new_internal(LdbContext* ctx, int64_t expected_strings, int64_t expected_bytes) {
+   auto* s = new LdbState;
+   s->ctx = ctx;
+   s->kind = LDB_STATE_DICT;
+   ctx->states.push_back(s);
+   auto alloc = [&](size_t bytes) {
+      void* p = ctx->stagingAlloc(std::max<size_t>(bytes, 16));
+      s->allocations.push_back(p);
+      return p;
+   };
+   DictDev& dd = s->dict;
+   const uint64_t cap = nextPow2((uint64_t) std::max<int64_t>(expected_strings, 8) * 2);
+   dd.mask = cap - 1;
+   dd.slots = (unsigned long long*) alloc(cap * 8);
+   dd.entryOff = (int64_t*) alloc(cap * 8);
+   dd.entryLen = (int32_t*) alloc(cap * 4);
+   dd.arenaCap = std::max<int64_t>(expected_bytes, 1);
+   dd.arena = (uint8_t*) alloc((size_t) dd.arenaCap);
+   dd.ctr = (unsigned long long*) alloc(32);
+   dd.codeCap = std::min<int64_t>((int64_t) cap, (int64_t) INT32_MAX + 1);
+   LDB_CUDA(cudaMemsetAsync(dd.slots, 0, cap * 8, ctx->compute));
+   LDB_CUDA(cudaMemsetAsync(dd.ctr, 0, 32, ctx->compute));
+   return s;
+}
+
+extern "C" {
+
 int ldb_gpu_dict_create(LdbContext* ctx, int64_t expected_strings, int64_t expected_bytes, LdbState** out, LdbError* err) {
    return guarded(err, [&] {
       if (!ctx || !out) fail(LDB_ERR_INVALID, "null argument");
       if (expected_strings < 0 || expected_bytes < 0) fail(LDB_ERR_INVALID, "negative dictionary size");
-      if (expected_strings > ((int64_t) 1 << 30)) fail(LDB_ERR_UNSUPPORTED, "a dictionary holds at most 2^30 expected strings (codes are int32)");
+      if (expected_strings > kDictMaxStrings) fail(LDB_ERR_UNSUPPORTED, "a dictionary holds at most 2^30 expected strings (codes are int32)");
       LDB_CUDA(cudaSetDevice(ctx->device));
-      auto* s = new LdbState;
-      s->ctx = ctx;
-      s->kind = LDB_STATE_DICT;
-      ctx->states.push_back(s);
-      auto alloc = [&](size_t bytes) {
-         void* p = ctx->stagingAlloc(std::max<size_t>(bytes, 16));
-         s->allocations.push_back(p);
-         return p;
-      };
-      DictDev& dd = s->dict;
-      const uint64_t cap = nextPow2((uint64_t) std::max<int64_t>(expected_strings, 8) * 2);
-      dd.mask = cap - 1;
-      dd.slots = (unsigned long long*) alloc(cap * 8);
-      dd.entryOff = (int64_t*) alloc(cap * 8);
-      dd.entryLen = (int32_t*) alloc(cap * 4);
-      dd.arenaCap = std::max<int64_t>(expected_bytes, 1);
-      dd.arena = (uint8_t*) alloc((size_t) dd.arenaCap);
-      dd.ctr = (unsigned long long*) alloc(32);
-      dd.codeCap = std::min<int64_t>((int64_t) cap, (int64_t) INT32_MAX + 1);
-      LDB_CUDA(cudaMemsetAsync(dd.slots, 0, cap * 8, ctx->compute));
-      LDB_CUDA(cudaMemsetAsync(dd.ctr, 0, 32, ctx->compute));
-      *out = s;
+      *out = ldb_gpu_dict_new_internal(ctx, expected_strings, expected_bytes);
    });
 }
 int ldb_gpu_dict_count(LdbState* s, int64_t* n_strings, LdbError* err) {
@@ -300,7 +307,7 @@ int ldb_gpu_dict_count(LdbState* s, int64_t* n_strings, LdbError* err) {
       checkDict(s);
       if (!n_strings) fail(LDB_ERR_INVALID, "null argument");
       LDB_CUDA(cudaSetDevice(s->ctx->device));
-      *n_strings = checkDictError(s).second;
+      *n_strings = ldb_gpu_dict_counters_internal(s).second;
    });
 }
 int ldb_gpu_dict_to_table(LdbState* s, const char* name, LdbTable** out, LdbError* err) {
@@ -309,7 +316,7 @@ int ldb_gpu_dict_to_table(LdbState* s, const char* name, LdbTable** out, LdbErro
       if (!out) fail(LDB_ERR_INVALID, "null argument");
       LdbContext* ctx = s->ctx;
       LDB_CUDA(cudaSetDevice(ctx->device));
-      const std::pair<int64_t, int64_t> used = checkDictError(s);
+      const std::pair<int64_t, int64_t> used = ldb_gpu_dict_counters_internal(s);
       const int64_t bytes = used.first, n = used.second;
       if (bytes > (int64_t) INT32_MAX) fail(LDB_ERR_UNSUPPORTED, "dictionary strings exceed 2^31 - 1 bytes (utf8 offsets are int32)");
       Scratch cols(ctx), scratch(ctx);
@@ -409,6 +416,7 @@ struct ProgramPlan {
    bool usesRowid = false;
    int eachTable = -1; // tables[] index PROBE_EACH reads
    bool probed[kProgMaxTables] = {}, coded[kProgMaxTables] = {}; // tables[k] read by PROBE / PROBE_EACH, by STRCODE
+   bool inserted[kProgMaxTables] = {};                           // tables[k] inserted into by STRCODE b = 1
    bool marked[kProgMaxTables] = {};                             // tables[k] marked by MARK
    bool existed[kProgMaxTables] = {};                            // tables[k] read by EXISTS
    // registers written inside an EXISTS block that has ended (they hold whatever its last match left), and the dst registers of ended
@@ -507,6 +515,7 @@ static void validateInstructions(ProgramPlan& p) {
             if (in.arg < 0 || in.arg >= d->n_tables) fail(LDB_ERR_INVALID, "STRCODE: dictionary index out of range");
             if (in.b > 1) fail(LDB_ERR_INVALID, "STRCODE: b is 1 (insert) or 0 (lookup only)");
             p.coded[in.arg] = true;
+            p.inserted[in.arg] |= in.b == 1;
             break;
          case LDB_OP_CONST:
             if (in.arg < 0 || in.arg >= d->n_consts) fail(LDB_ERR_INVALID, "CONST: constant index out of range");
@@ -655,6 +664,7 @@ static void bindTables(ProgramPlan& p) {
          if (p.probed[k]) fail(LDB_ERR_INVALID, "PROBE / PROBE_EACH on a string dictionary (they take join tables)");
          if (js->ctx != ctx) fail(LDB_ERR_INVALID, "string dictionary belongs to another context");
          if (ctx->capturing) fail(LDB_ERR_UNSUPPORTED, "string dictionaries are not part of captured queries");
+         if (js->unified && p.inserted[k]) fail(LDB_ERR_INVALID, "an inserting STRCODE against a unified dictionary (its codes agree across ranks: it takes lookups only)");
          p.base.dicts[k] = js->dict;
          p.dicts.push_back(js);
          continue;
@@ -808,7 +818,7 @@ static void checkErrorWords(const ProgramPlan& p) {
    for (int k = 0; k < d->n_tables; k++)
       if (p.existed[k] && k != p.eachTable && d->tables[k]->kind == LDB_STATE_JOIN_TABLE) ldb_gpu_check_join_error_internal(d->tables[k]);
    for (LdbState* ks : p.tupleTables) ldb_gpu_check_keyjoin_error_internal(ks); // a full build, a probe run at the bound, a key outside int64
-   for (LdbState* ds : p.dicts) checkDictError(ds);
+   for (LdbState* ds : p.dicts) ldb_gpu_dict_counters_internal(ds);
 }
 
 // the materialized rows as a table that takes over the output buffers of `out` (synchronises)

@@ -182,6 +182,19 @@ class Comm:
                                                  C.byref(out), C.byref(e)), e)
         return RawTable(self.ctx, out)
 
+    def dict_unify(self, local, recv_offset: int = 0, recv_bytes: int = None):
+        """Union of every rank's string dictionary (ldb_gpu_dict_unify): returns a new dictionary state, the same on every rank, whose
+        codes are the strings' positions in bytewise order, so ("strcode", unified, column, "lookup") gives codes that agree across ranks
+        and order like the strings.  Programs may only look strings up in it.  Collective, and it waits for the peers on the host: the
+        ranks of one process call it from one thread each.  The receive region starts at user-heap offset `recv_offset` and spans
+        `recv_bytes` (None: the rest of the user heap); strings that do not fit fail with LDB_ERR_CAPACITY on every rank."""
+        from . import capi
+        if recv_bytes is None:
+            recv_bytes = self.heap()[1] - int(recv_offset)
+        out, e = C.c_void_p(), capi.Error()
+        capi.check(self.L.ldb_gpu_dict_unify(local, self.h, int(recv_offset), int(recv_bytes), C.byref(out), C.byref(e)), e)
+        return out
+
     def _gather_counts(self, n: int) -> List[int]:
         """every rank's `n`, in rank order"""
         if self.world == 1:
