@@ -248,6 +248,7 @@ struct LdbBatch {
       uint8_t* data = nullptr;
       int32_t width = 0, tileRows = 0;
       int64_t bytes = 0;
+      int64_t min = 0, max = 0; // of the batch's column, for the factored Q1 scan (kernels.h GroupByParams::encMin)
       bool failed = false; // allocation failed or over the budget: this batch is scanned in Arrow layout
    };
    std::vector<Encoded> enc;

@@ -12,12 +12,15 @@
 
 namespace ldb {
 
+constexpr uint64_t kSign64 = 1ull << 63;
+
 __device__ __forceinline__ int64_t encodeSource(const uint8_t* src, bool isI32, int64_t r) {
    return isI32 ? (int64_t) ((const int32_t*) src)[r] : ((const int64_t*) src)[2 * r]; // decimal128: its low 8 bytes
 }
 
-// one CTA per block: blockMin[b], blockRange[b] = max - min, and the largest range of all blocks
-__global__ void encodeRangeKernel(const uint8_t* src, bool isI32, int64_t n, int64_t* blockMin, int64_t* blockRange, unsigned long long* maxRange) {
+// one CTA per block: blockMin[b], blockRange[b] = max - min, and the column's stats (kEncodeStats words): the largest range of all
+// blocks, and the batch minimum and maximum as order-preserving unsigned keys, so all three reduce with an unsigned atomicMax from zero
+__global__ void encodeRangeKernel(const uint8_t* src, bool isI32, int64_t n, int64_t* blockMin, int64_t* blockRange, unsigned long long* stats) {
    __shared__ int64_t sLo[32], sHi[32];
    const int64_t r0 = (int64_t) blockIdx.x * kEncodeBlockRows, r1 = min(n, r0 + kEncodeBlockRows);
    int64_t lo = LLONG_MAX, hi = LLONG_MIN;
@@ -43,7 +46,9 @@ __global__ void encodeRangeKernel(const uint8_t* src, bool isI32, int64_t n, int
       }
       blockMin[blockIdx.x] = lo;
       blockRange[blockIdx.x] = (int64_t) ((uint64_t) hi - (uint64_t) lo);
-      atomicMax(maxRange, (unsigned long long) ((uint64_t) hi - (uint64_t) lo));
+      atomicMax(&stats[0], (unsigned long long) ((uint64_t) hi - (uint64_t) lo));
+      atomicMax(&stats[1], (unsigned long long) ~((uint64_t) lo ^ kSign64));
+      atomicMax(&stats[2], (unsigned long long) ((uint64_t) hi ^ kSign64));
    }
 }
 
@@ -71,9 +76,9 @@ __global__ void encodePackKernel(const uint8_t* src, bool isI32, int64_t n, cons
    }
 }
 
-void launchEncodeRange(const uint8_t* src, bool isI32, int64_t n, int64_t* blockMin, int64_t* blockRange, unsigned long long* maxRange, cudaStream_t s) {
+void launchEncodeRange(const uint8_t* src, bool isI32, int64_t n, int64_t* blockMin, int64_t* blockRange, unsigned long long* stats, cudaStream_t s) {
    const int64_t blocks = (n + kEncodeBlockRows - 1) / kEncodeBlockRows;
-   encodeRangeKernel<<<(unsigned) blocks, 256, 0, s>>>(src, isI32, n, blockMin, blockRange, maxRange);
+   encodeRangeKernel<<<(unsigned) blocks, 256, 0, s>>>(src, isI32, n, blockMin, blockRange, stats);
 }
 void launchEncodePack(const uint8_t* src, bool isI32, int64_t n, const int64_t* blockMin, const int64_t* blockRange, int width, int tileRows, uint8_t* dst,
                       cudaStream_t s) {
@@ -123,26 +128,27 @@ bool ldb_gpu_encode_batch_internal(LdbContext* ctx, LdbTable* t, LdbBatch& b, co
       LDB_CUDA(cudaStreamWaitEvent(s, ctx->computeDone, 0));
    }
    void* scratch = nullptr;
-   const size_t scratchBytes = (size_t) nTodo * (size_t) blocks * 16 + (size_t) nTodo * 8;
+   const size_t scratchBytes = (size_t) nTodo * (size_t) blocks * 16 + (size_t) nTodo * kEncodeStats * 8;
    if (cudaMalloc(&scratch, scratchBytes) != cudaSuccess) return failAll();
    int64_t* blockMin = (int64_t*) scratch;
    int64_t* blockRange = blockMin + (size_t) nTodo * blocks;
-   unsigned long long* maxRange = (unsigned long long*) (blockRange + (size_t) nTodo * blocks);
-   uint64_t range[kMaxStagedCols];
+   unsigned long long* stats = (unsigned long long*) (blockRange + (size_t) nTodo * blocks);
+   uint64_t st[kMaxStagedCols][kEncodeStats];
    try {
-      LDB_CUDA(cudaMemsetAsync(maxRange, 0, (size_t) nTodo * 8, s));
+      LDB_CUDA(cudaMemsetAsync(stats, 0, (size_t) nTodo * kEncodeStats * 8, s));
       for (int k = 0; k < nTodo; k++) {
          const bool isI32 = t->columns[todo[k]].type != LDB_DECIMAL128;
-         launchEncodeRange((const uint8_t*) b.data[todo[k]], isI32, rows, blockMin + (size_t) k * blocks, blockRange + (size_t) k * blocks, maxRange + k, s);
+         launchEncodeRange((const uint8_t*) b.data[todo[k]], isI32, rows, blockMin + (size_t) k * blocks, blockRange + (size_t) k * blocks,
+                           stats + (size_t) k * kEncodeStats, s);
          LDB_CUDA(cudaGetLastError());
       }
-      LDB_CUDA(cudaMemcpyAsync(range, maxRange, (size_t) nTodo * 8, cudaMemcpyDeviceToHost, s));
+      LDB_CUDA(cudaMemcpyAsync(st, stats, (size_t) nTodo * kEncodeStats * 8, cudaMemcpyDeviceToHost, s));
       LDB_CUDA(cudaStreamSynchronize(s));
       ctx->encodeLaunches += nTodo;
       bool all = true;
       for (int k = 0; k < nTodo; k++) {
          LdbBatch::Encoded& e = b.enc[todo[k]];
-         const int width = encodedWidth(range[k]);
+         const int width = encodedWidth(st[k][0]);
          const int64_t bytes = encodedColumnBytes(rows, width, tileRows);
          void* data = nullptr;
          if (ctx->encodedBytes + bytes > ctx->encodedBudget || cudaMalloc(&data, (size_t) bytes) != cudaSuccess) {
@@ -160,6 +166,8 @@ bool ldb_gpu_encode_batch_internal(LdbContext* ctx, LdbTable* t, LdbBatch& b, co
          e.width = width;
          e.bytes = bytes;
          e.tileRows = tileRows;
+         e.min = (int64_t) (~st[k][1] ^ kSign64);
+         e.max = (int64_t) (st[k][2] ^ kSign64);
          ctx->encodedBytes += bytes;
       }
       LDB_CUDA(cudaStreamSynchronize(s));

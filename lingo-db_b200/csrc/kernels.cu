@@ -823,6 +823,29 @@ extern __shared__ __align__(128) uint8_t dynSmem[];
 constexpr int kEncFrames = 4, kEncStages = 3;
 template <int DB, int FS>
 constexpr bool encodedStages = DB == kDecEncoded && FS == FS_I32_ONE;
+using C0 = Agg<LDB_EXPR_COL, 0>;
+using C1 = Agg<LDB_EXPR_COL, 1>;
+using C2 = Agg<LDB_EXPR_COL, 2>;
+using ONE = Agg<LDB_EXPR_ONE>;
+// Q1: sum(qty) sum(ep) sum(ep*(1-d)) sum(ep*(1-d)*(1+t)) sum(d) count over value columns qty, ep, d, t
+using Q1Aggs = Aggs<C0, C1, Agg<LDB_EXPR_MUL_1MINUS, 1, 2>, Agg<LDB_EXPR_MUL_1MINUS_1PLUS, 1, 2, 3>, C2, ONE>;
+constexpr int kQty = 0, kEp = 1, kDisc = 2, kTax = 3;
+// Factored Q1 stages (FAC).  Discount and tax take few values (TPC-H: 11 and 9), so per register group g
+//   sum(ep*(1-d)*(1+t)) = sum over (d, t) of (1-d)(1+t) * S[g][d][t],   S[g][d][t] = sum of ep over g's rows with that (d, t),
+// and likewise sum(ep*(1-d)), sum(d) = sum of d * count[g][d][t], sum(ep), sum(qty) and count: identities of the integers, so they
+// hold modulo 2^64 and 2^128 too.  A row then costs three 32-bit shared atomics into its cell g*Dd*Dt + (d-min_d)*Dt + (t-min_t)
+// (64-bit shared atomics are CAS loops on sm_90a) and the products run once per cell and CTA at the end.  The summed columns enter
+// as offsets from their batch minimum (ep - min_ep, qty - min_qty; min * count is added back at the end, so negative values stay
+// exact), in three words that cannot overflow in one stage of 2 * kBlock * kEncFrames = 2048 rows when the stage header proves
+// ep_off < 2^28 and qty_off < 2^21:
+//   A = ep_off & 0xfffff  (< 2^20 per row),   B = (ep_off >> 20) << 12 | 1  (< 2^20 per row, the count in the low 12 bits),
+//   C = qty_off  (< 2^21 per row).
+// The words are double-buffered by stage parity: after the barrier that ends a stage, each thread folds the cells it owns (cell mod
+// kBlock) of the previous stage's buffer into 64-bit sums in registers and zeroes them, while the CTA fills the other buffer.  A
+// batch has fewer than 2^36 rows (launchGB), so those sums stay below 2^64.
+constexpr int kCells = 512;
+constexpr int kCellWords = 3;
+static_assert(kEncFrames * kRowsPerThreadScan * kBlock <= 2048 && kCells % kBlock == 0, "factored cell words overflow");
 // the W-byte fields (W = 1 << sh <= 4) of 2 adjacent rows from shared address a (2W-byte aligned), zero-extended: one shared load
 __device__ __forceinline__ void encodedFields2(uint32_t a, int sh, uint32_t (&x)[2]) {
    if (sh == 0) {
@@ -838,11 +861,12 @@ __device__ __forceinline__ void encodedFields2(uint32_t a, int sh, uint32_t (&x)
       ldShared32x2(a, x[0], x[1]);
    }
 }
-template <int DB, bool IN, int FS, int NK, int NV, class... As>
+template <int DB, bool IN, int FS, bool FAC, int NK, int NV, class... As>
 __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_constant__ GroupByParams p) {
    using AL = Aggs<As...>;
    constexpr int N = AL::N;
    constexpr bool kStaged = encodedStages<DB, FS>;
+   static_assert(!FAC || (kStaged && NK == 2 && NV == 4 && std::is_same_v<AL, Q1Aggs>), "the factored stage path is Q1's");
    constexpr int F = kStaged ? kEncFrames : 1;
    constexpr int GREG = NK == 0 ? 1 : 4; // register-resident groups
    constexpr int LG = 16;                // CTA-local groups (registers + shared)
@@ -850,6 +874,7 @@ __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_cons
    __shared__ int32_t sSlot[LG];
    __shared__ int32_t sCount, sLock;
    __shared__ unsigned long long sAcc[LG][N][2];
+   __shared__ uint32_t sCell[FAC ? 2 : 1][kCellWords][FAC ? kCells : 1]; // factored stages: {A, B, C} words per cell, by stage parity
    __shared__ __align__(8) TileBarriers barsStorage;
    TileBarriers* bars = &barsStorage;
 
@@ -862,6 +887,8 @@ __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_cons
       atomicMax(selfTime, ~t0);
    }
    for (int i = threadIdx.x; i < LG * N * 2; i += kBlock) (&sAcc[0][0][0])[i] = 0;
+   if constexpr (FAC)
+      for (int i = threadIdx.x; i < 2 * kCellWords * kCells; i += kBlock) (&sCell[0][0][0])[i] = 0;
    if (threadIdx.x == 0) {
       sCount = NK == 0 ? 1 : 0;
       sLock = 0;
@@ -954,8 +981,9 @@ __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_cons
       }
       return id;
    };
+   // the factored path's register-resident groups sum in their cells; its other rows take the shared and HBM atomics of add()
    auto add = [&](int id, const i128* v, int32_t k0, int32_t k1) {
-      if (id >= 0 && id < GREG) {
+      if (!FAC && id >= 0 && id < GREG) {
 #pragma unroll
          for (int g = 0; g < GREG; g++)
             if (id == g) AL::accumulate(acc[g], v, typename AL::S{});
@@ -982,6 +1010,26 @@ __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_cons
       else AL::template eval<false>(v, vals, one, typename AL::S{});
       if (pass) add(id, v, k0, k1);
    };
+   // factored stages: 64-bit sums of the cells this thread owns (cell j * kBlock + threadIdx.x), and the stages run so far
+   constexpr int kOwned = FAC ? kCells / kBlock : 1;
+   uint64_t cEp[kOwned], cCnt[kOwned], cQty[kOwned];
+#pragma unroll
+   for (int j = 0; j < kOwned; j++) cEp[j] = cCnt[j] = cQty[j] = 0;
+   uint32_t facStages = 0;
+   const uint32_t fDt = FAC ? (uint32_t) p.encRange[kTax] + 1u : 0u, fDdDt = FAC ? ((uint32_t) p.encRange[kDisc] + 1u) * fDt : 0u;
+   auto foldCells = [&](uint32_t buf) {
+#pragma unroll
+      for (int j = 0; j < kOwned; j++) {
+         const int cell = j * kBlock + threadIdx.x;
+         const uint32_t b = sCell[buf][1][cell];
+         if (b != 0) { // B counts the cell's rows
+            cEp[j] += sCell[buf][0][cell] + ((uint64_t) (b >> 12) << 20);
+            cCnt[j] += b & 0xfffu;
+            cQty[j] += sCell[buf][2][cell];
+            sCell[buf][0][cell] = sCell[buf][1][cell] = sCell[buf][2][cell] = 0;
+         }
+      }
+   };
    auto encodedStage = [&](uint32_t stage) {
       const StagedCols& sc = p.src.cols;
       constexpr int FC = NV + NK;                  // staged index of the filter's column
@@ -991,15 +1039,14 @@ __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_cons
       constexpr int kRun = 2;                      // adjacent rows decoded together
       // column c's F tiles lie from stage + F * smemOffset[c]; their headers are equal (kernels.h), tile 0's stands for all
       auto col = [&](int c) { return stage + (uint32_t) (F * sc.smemOffset[c]); };
-      int64_t vb[NV], lo[NV], hi[NV];
+      int64_t vb[NV], lo[NV], hi[NV], range[NV];
 #pragma unroll
       for (int c = 0; c < NV; c++) {
-         int64_t range;
-         ldShared64x2(col(c), vb[c], range);
+         ldShared64x2(col(c), vb[c], range[c]);
          // a column with a wide range or base gets bounds no operand test passes (and no bound arithmetic overflows)
-         const bool small = (uint64_t) range < (1ull << 31) && vb[c] > -(1ll << 40) && vb[c] < (1ll << 40);
+         const bool small = (uint64_t) range[c] < (1ull << 31) && vb[c] > -(1ll << 40) && vb[c] < (1ll << 40);
          lo[c] = small ? vb[c] : -(1ll << 62);
-         hi[c] = small ? vb[c] + range : (1ll << 62);
+         hi[c] = small ? vb[c] + range[c] : (1ll << 62);
       }
       uint32_t kb[2] = {0, 0};
 #pragma unroll
@@ -1014,6 +1061,23 @@ __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_cons
             room = INT64_MAX;
          }
          room -= need;
+      }
+      // factored stage: the previous stage's cells are complete (every thread passed the barrier behind it); this stage fills the other
+      // buffer when its header puts each field's offset from the batch minimum inside its word budget or its cell domain
+      bool fac = false;
+      uint32_t buf = 0, cellOff = 0, offEp = 0, offQty = 0;
+      if constexpr (FAC) {
+         if (facStages > 0) foldCells((facStages - 1) & 1u);
+         buf = facStages++ & 1u;
+         uint64_t off[NV] = {};
+         auto inside = [&](int c, uint64_t top) { // every value of the stage's block in [min, min + top]
+            off[c] = (uint64_t) vb[c] - (uint64_t) p.encMin[c];
+            return (uint64_t) range[c] <= top && off[c] <= top - (uint64_t) range[c];
+         };
+         fac = proven && inside(kQty, (1u << 21) - 1) && inside(kEp, (1u << 28) - 1) && inside(kDisc, p.encRange[kDisc]) && inside(kTax, p.encRange[kTax]);
+         cellOff = (uint32_t) off[kDisc] * fDt + (uint32_t) off[kTax];
+         offEp = (uint32_t) off[kEp];
+         offQty = (uint32_t) off[kQty];
       }
       // `v cmp C` on the raw field x = v - base in [0, 2^32) is `flo <= x <= fhi`, negated for != (mask 5)
       uint32_t flo, fhi;
@@ -1080,11 +1144,26 @@ __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_cons
             int64_t vals[NV];
 #pragma unroll
             for (int c = 0; c < NV; c++) vals[c] = (int64_t) ((uint64_t) vb[c] + xv[c][i]);
-            if (proven) {
+            if (FAC && fac) {
+               if (pass[i] && id[i] >= 0 && id[i] < GREG) {
+                  const uint32_t cell = (uint32_t) id[i] * fDdDt + xv[kDisc][i] * fDt + xv[kTax][i] + cellOff;
+                  const uint32_t ep = xv[kEp][i] + offEp;
+                  atomicAdd(&sCell[buf][0][cell], ep & 0xfffffu);
+                  atomicAdd(&sCell[buf][1][cell], (ep >> 20) << 12 | 1u);
+                  atomicAdd(&sCell[buf][2][cell], xv[kQty][i] + offQty);
+               } else if (pass[i]) {
+                  int64_t q[N];
+                  AL::eval64(q, vals, one, typename AL::S{});
+                  i128 v[N];
+#pragma unroll
+                  for (int a = 0; a < N; a++) v[a] = i128{(uint64_t) q[a], 0};
+                  add(id[i], v, k0, k1);
+               }
+            } else if (proven) {
                int64_t q[N];
                AL::eval64(q, vals, one, typename AL::S{});
                // a one-hot test per group: an `id == g` test here was folded into a dynamically indexed acc[id], which lives in local memory
-               const uint32_t hot = pass[i] && id[i] >= 0 && id[i] < GREG ? 1u << id[i] : 0u;
+               const uint32_t hot = !FAC && pass[i] && id[i] >= 0 && id[i] < GREG ? 1u << id[i] : 0u;
 #pragma unroll
                for (int g = 0; g < GREG; g++)
                   if (hot >> g & 1u) AL::accumulate64(acc[g], acc64[g], q, typename AL::S{});
@@ -1119,11 +1198,42 @@ __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_cons
    });
    // ---- flush: registers → warp sums → shared → one HBM atomic per (CTA, group, aggregate)
    __syncthreads();
+   if constexpr (FAC) {
+      // the last stage's cells, then each owned cell's six aggregates, exact modulo 2^64 / 2^128 like the per-row sums
+      if (facStages > 0) foldCells((facStages - 1) & 1u);
+      // per register group: this thread's owned cells of the group, summed over the warp, one shared atomic per warp and aggregate
+      const int lane = threadIdx.x & 31;
+#pragma unroll 1
+      for (int g = 0; g < GREG; g++) {
+         i128 s[N];
 #pragma unroll
-   for (int g = 0; g < GREG; g++) AL::fold64(acc[g], acc64[g], typename AL::S{});
-   const int lane = threadIdx.x & 31;
+         for (int a = 0; a < N; a++) s[a] = i128{0, 0};
 #pragma unroll
-   for (int g = 0; g < GREG; g++) AL::warpFlush(sAcc[g], acc[g], lane, typename AL::S{});
+         for (int j = 0; j < kOwned; j++) {
+            const uint32_t cell = j * kBlock + threadIdx.x, dt = cell % fDdDt;
+            if (cCnt[j] == 0 || cell / fDdDt != (uint32_t) g) continue;
+            const int64_t d = p.encMin[kDisc] + (int64_t) (dt / fDt), t = p.encMin[kTax] + (int64_t) (dt % fDt);
+            const uint64_t n = cCnt[j];
+            const i128 ep = add128(i128{cEp[j], 0}, mul64x64(p.encMin[kEp], (int64_t) n));
+            const i128 epd = mul128x64(ep, one - d);
+            i128 v[N];
+            v[0] = i128{cQty[j] + (uint64_t) p.encMin[kQty] * n, 0};
+            v[1] = i128{ep.lo, 0};
+            v[2] = epd;
+            v[3] = mul128x64(epd, one + t);
+            v[4] = i128{(uint64_t) d * n, 0};
+            v[5] = i128{n, 0};
+            AL::accumulate(s, v, typename AL::S{});
+         }
+         AL::warpFlush(sAcc[g], s, lane, typename AL::S{});
+      }
+   } else {
+#pragma unroll
+      for (int g = 0; g < GREG; g++) AL::fold64(acc[g], acc64[g], typename AL::S{});
+      const int lane = threadIdx.x & 31;
+#pragma unroll
+      for (int g = 0; g < GREG; g++) AL::warpFlush(sAcc[g], acc[g], lane, typename AL::S{});
+   }
    __syncthreads();
    const int cnt = sCount;
    for (int i = threadIdx.x; i < cnt * N; i += kBlock) {
@@ -1184,11 +1294,18 @@ static bool hasInList(const FilterSet& f) { // "rare" filters: IN lists and LIKE
    return false;
 }
 template <int DB, bool IN, int FS, int NK, int NV, class... As>
-static void launchGBd(const GroupByParams& p, int smCount, cudaStream_t s) {
+static void launchGBd(const GroupByParams& p, int smCount, cudaStream_t s, bool factored = false) {
    size_t dyn;
    constexpr int tiles = encodedStages<DB, FS> ? kEncStages * kEncFrames : kStages; // tiles held in shared memory
-   int grid = persistentGrid(scanGroupByKernel<DB, IN, FS, NK, NV, As...>, p.src.cols, p.src.nRows, smCount, &dyn, kBlock, tiles);
-   scanGroupByKernel<DB, IN, FS, NK, NV, As...><<<grid, kBlock, dyn, s>>>(p);
+   if constexpr (encodedStages<DB, FS> && NK == 2 && NV == 4 && std::is_same_v<Aggs<As...>, Q1Aggs>) {
+      if (factored) {
+         int grid = persistentGrid(scanGroupByKernel<DB, IN, FS, true, NK, NV, As...>, p.src.cols, p.src.nRows, smCount, &dyn, kBlock, tiles);
+         scanGroupByKernel<DB, IN, FS, true, NK, NV, As...><<<grid, kBlock, dyn, s>>>(p);
+         return;
+      }
+   }
+   int grid = persistentGrid(scanGroupByKernel<DB, IN, FS, false, NK, NV, As...>, p.src.cols, p.src.nRows, smCount, &dyn, kBlock, tiles);
+   scanGroupByKernel<DB, IN, FS, false, NK, NV, As...><<<grid, kBlock, dyn, s>>>(p);
 }
 // The stage path reads fields of at most 4 bytes (an 8-byte field is a value column no product proof admits) and must fit its stages in
 // one CTA's shared memory; other encoded batches take the instance with the descriptor-driven filter.
@@ -1202,6 +1319,37 @@ static bool encodedStagesFit(K kernel, const StagedCols& sc) {
    cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
    cudaFuncGetAttributes(&fa, kernel);
    return (int64_t) kEncStages * kEncFrames * sc.stageBytes + (int64_t) fa.sharedSizeBytes <= optin;
+}
+// The factored stage path (Q1Aggs, kCells) runs when the batch's discount and tax domains give every register group its cells, and
+// the batch's own bounds (encMin, encRange) prove what each stage header would: ep - min_ep < 2^28 and qty - min_qty < 2^21 (the
+// word budgets) and the 64-bit product bound of the per-row stage path (aggBound64 on the batch range), so every stage factors and
+// only rows of groups past the register set take the instance's shared-atomic fallback.  The batch must also be short enough for the
+// 64-bit cell sums (2^36 rows of ep_off < 2^28), and its stages and cells must leave two CTAs per SM (one fewer resident CTA costs more
+// than the factoring saves).  Any other batch takes the per-row stage instance, which keeps its sums in registers.
+using Q1FactoredKernel = decltype(&scanGroupByKernel<kDecEncoded, false, FS_I32_ONE, true, 2, 4, C0, C1, Agg<LDB_EXPR_MUL_1MINUS, 1, 2>,
+                                                     Agg<LDB_EXPR_MUL_1MINUS_1PLUS, 1, 2, 3>, C2, ONE>);
+static bool factoredFits(const GroupByParams& p) {
+   const Q1FactoredKernel kernel = scanGroupByKernel<kDecEncoded, false, FS_I32_ONE, true, 2, 4, C0, C1, Agg<LDB_EXPR_MUL_1MINUS, 1, 2>,
+                                                     Agg<LDB_EXPR_MUL_1MINUS_1PLUS, 1, 2, 3>, C2, ONE>;
+   const uint64_t dd = p.encRange[kDisc], dt = p.encRange[kTax];
+   if (dd >= kCells || dt >= kCells || 4 * (dd + 1) * (dt + 1) > (uint64_t) kCells || p.src.nRows >= (1ll << 36)) return false;
+   if (p.encRange[kEp] >= (1ull << 28) || p.encRange[kQty] >= (1ull << 21)) return false;
+   // aggBound64 of ep * (1 - d) * (1 + t) over the batch: operands in [0, 2^31), largest product below 2^63 / (2 * kEncFrames)
+   const int64_t one = 100, k31 = 1ll << 31;
+   const int64_t epLo = p.encMin[kEp], epHi = epLo + (int64_t) p.encRange[kEp];
+   const int64_t dLo = one - (p.encMin[kDisc] + (int64_t) dd), dHi = one - p.encMin[kDisc];
+   const int64_t tLo = one + p.encMin[kTax], tHi = one + p.encMin[kTax] + (int64_t) dt;
+   if (p.encMin[kDisc] < -k31 || p.encMin[kDisc] > k31 || p.encMin[kTax] < -k31 || p.encMin[kTax] > k31) return false;
+   if (epLo < 0 || epHi >= k31 || dLo < 0 || dHi >= k31 || tLo < 0 || tHi >= k31) return false;
+   if ((unsigned __int128) epHi * (uint64_t) dHi * (uint64_t) tHi >= (unsigned __int128) ((1ull << 63) / (kRowsPerThreadScan * kEncFrames))) return false;
+   if (!encodedStagesFit(kernel, p.src.cols)) return false;
+   int dev = 0, perSm = 0, reserved = 0;
+   cudaFuncAttributes fa{};
+   cudaGetDevice(&dev);
+   cudaDeviceGetAttribute(&perSm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev);
+   cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev);
+   cudaFuncGetAttributes(&fa, (const void*) kernel);
+   return 2 * ((int64_t) kEncStages * kEncFrames * p.src.cols.stageBytes + (int64_t) fa.sharedSizeBytes + reserved) <= perSm;
 }
 // The encoded instance reads its columns' layout at constant indices: value column c is staged column c, key k is NV + k, and a
 // shaped filter's column is NV + NK.  Permutes the staged columns (and every index into them) into that order; returns the filter
@@ -1245,9 +1393,17 @@ static void launchGB(const GroupByParams& p, int smCount, cudaStream_t s) {
          GroupByParams q = p;
          const int fs = toSignatureOrder(q);
          if constexpr (ENC_ONE) {
-            if (fs == FS_I32_ONE && encodedStagesFit(scanGroupByKernel<kDecEncoded, false, FS_I32_ONE, NK, NV, As...>, q.src.cols)) {
-               launchGBd<kDecEncoded, false, FS_I32_ONE, NK, NV, As...>(q, smCount, s);
-               return;
+            if (fs == FS_I32_ONE) {
+               if constexpr (NK == 2 && NV == 4 && std::is_same_v<Aggs<As...>, Q1Aggs>) {
+                  if (factoredFits(q)) {
+                     launchGBd<kDecEncoded, false, FS_I32_ONE, NK, NV, As...>(q, smCount, s, true);
+                     return;
+                  }
+               }
+               if (encodedStagesFit(scanGroupByKernel<kDecEncoded, false, FS_I32_ONE, false, NK, NV, As...>, q.src.cols)) {
+                  launchGBd<kDecEncoded, false, FS_I32_ONE, NK, NV, As...>(q, smCount, s);
+                  return;
+               }
             }
          }
          launchGBd<kDecEncoded, false, FS_GENERIC, NK, NV, As...>(q, smCount, s);
@@ -1262,10 +1418,6 @@ static void launchGB(const GroupByParams& p, int smCount, cudaStream_t s) {
       else launchGBd<16, false, FS_GENERIC, NK, NV, As...>(p, smCount, s);
    }
 }
-using C0 = Agg<LDB_EXPR_COL, 0>;
-using C1 = Agg<LDB_EXPR_COL, 1>;
-using C2 = Agg<LDB_EXPR_COL, 2>;
-using ONE = Agg<LDB_EXPR_ONE>;
 // the signatures compiled for the encoded layout as well: Q1 and Q6, the two the encoded column copy exists for
 static const char* const kSigQ1 = "k2v4|0:0|0:1|2:1,2|3:1,2,3|0:2|4";
 static const char* const kSigQ6 = "k0v2|1:0,1";
@@ -1280,6 +1432,11 @@ bool scanGroupByEncodable(const GroupByParams& p) {
       for (int j = 0; j < i; j++)
          if (stage[i] == stage[j]) return false;
    return true;
+}
+bool scanGroupByFactored(const GroupByParams& p) {
+   if (p.src.cols.decBytes != kDecEncoded || signature(p) != kSigQ1 || hasInList(p.src.filters)) return false;
+   GroupByParams q = p;
+   return toSignatureOrder(q) == FS_I32_ONE && factoredFits(q);
 }
 bool launchScanGroupBy(const GroupByParams& p, int smCount, cudaStream_t s, const char** why) {
    std::string sig = signature(p);

@@ -159,6 +159,10 @@ struct GroupByParams {
    int32_t nAggs;
    AggSpec aggs[kMaxAggs];
    GroupTableDev table;
+   // encoded layout: the batch's minimum and max - min of value column v (LdbBatch::Encoded), which bound every stage header's
+   // block; the factored Q1 scan indexes its per-cell sums by them
+   int64_t encMin[kMaxValueCols];
+   uint64_t encRange[kMaxValueCols];
 };
 
 enum PayloadKind : int32_t { PAYLOAD_I32 = 0, PAYLOAD_YEAR_OF_DATE32 = 1, PAYLOAD_DEC_LO64 = 2 };
@@ -271,12 +275,15 @@ void launchProbeReceivedGroupBy(const JoinTableDev& tableA, const JoinTableDev& 
 
 // signature → instantiation registry for the group-by kernel; returns false when no compiled shape matches
 bool launchScanGroupBy(const GroupByParams& p, int smCount, cudaStream_t s, const char** why);
+// true when launchScanGroupBy runs p (bound to the encoded layout) on the factored Q1 instance (kernels.cu factoredFits)
+bool scanGroupByFactored(const GroupByParams& p);
 // true when launchScanGroupBy has an instantiation of p's signature for the encoded layout (p.src.cols need not be bound yet)
 bool scanGroupByEncodable(const GroupByParams& p);
 // encoder (encode.cu).  A source column is `n` int32 cells (isI32) or decimal128 cells of which the low 8 bytes are taken.
-// Range pass: blockMin[b] = minimum of block b, blockRange[b] = its max - min, *maxRange = max over blocks of (max - min) as unsigned
-// (caller zeroes it).
-void launchEncodeRange(const uint8_t* src, bool isI32, int64_t n, int64_t* blockMin, int64_t* blockRange, unsigned long long* maxRange, cudaStream_t s);
+// Range pass: blockMin[b] = minimum of block b, blockRange[b] = its max - min; stats[kEncodeStats] (caller zeroes them) = {max over
+// blocks of (max - min) as unsigned, ~(min ^ 2^63), max ^ 2^63} of the column.
+constexpr int kEncodeStats = 3;
+void launchEncodeRange(const uint8_t* src, bool isI32, int64_t n, int64_t* blockMin, int64_t* blockRange, unsigned long long* stats, cudaStream_t s);
 // Pack pass: writes the tile-framed copy (kernels.h, kEncodeTileHeader) of width `width` for tiles of `tileRows` rows
 void launchEncodePack(const uint8_t* src, bool isI32, int64_t n, const int64_t* blockMin, const int64_t* blockRange, int width, int tileRows, uint8_t* dst,
                       cudaStream_t s);

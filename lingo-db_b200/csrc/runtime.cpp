@@ -1274,12 +1274,22 @@ int ldb_gpu_run_pipeline(LdbContext* ctx, const LdbPipelineDesc* d, LdbError* er
                // batches, signatures without an encoded instantiation and copies that could not be allocated use the Arrow cells
                const bool encoded = tuning().encodedScan && b.borrowed && scanGroupByEncodable(p) &&
                                     ldb_gpu_encode_batch_internal(ctx, t, b, sp.colIdx, sp.n, kBlockThreads * kRowsPerThreadScan);
-               if (encoded) sp.bindEncoded(t, b, p.src.cols, kRowsPerThreadScan);
-               else sp.bind(t, b, p.src.cols, kRowsPerThreadScan);
+               if (encoded) {
+                  sp.bindEncoded(t, b, p.src.cols, kRowsPerThreadScan);
+                  for (int v = 0; v < ap.nValueCols; v++) {
+                     const LdbBatch::Encoded& e = b.enc[ap.valueCol[v]];
+                     p.encMin[v] = e.min;
+                     p.encRange[v] = (uint64_t) e.max - (uint64_t) e.min;
+                  }
+               } else {
+                  sp.bind(t, b, p.src.cols, kRowsPerThreadScan);
+               }
                waitBatch(ctx, b);
                bool ok = true;
                ctx->launch(keyless ? "scan_reduce" : "scan_groupby", [&] { ok = launchScanGroupBy(p, ctx->smCount, ctx->compute, &why); });
                if (!ok) fail(LDB_ERR_UNSUPPORTED, why);
+               // which Q1 instance ran: the factored one's eager launches also count (without a time) as family "scan_groupby_factored"
+               if (encoded && ctx->timing && !ctx->capturing && scanGroupByFactored(p)) ctx->timers["scan_groupby_factored"].launches++;
             }
             break;
          }
