@@ -682,6 +682,26 @@ int ldb_gpu_hashagg_exchange(LdbState* local, LdbState* owned, LdbComm* comm, in
  * call it from one thread each.  On return the receive region is free again; world = 1 is a compacting copy. */
 int ldb_gpu_table_exchange(LdbTable* src, int32_t n_keys, const char* const* key_columns, int32_t n_columns, const char* const* columns /* NULL = all columns of src */,
                            LdbComm* comm, int64_t recv_offset, int64_t recv_bytes, const char* name, LdbTable** out, LdbError* err);
+/* ldb_gpu_table_exchange whose shipped columns may also be utf8, so string columns travel with their rows (names, comments, any string
+ * that is output or of high cardinality) without a dictionary.  Signature, owners, order, sources, errors, capture refusal and threading
+ * are those of ldb_gpu_table_exchange; both run one implementation, and without a utf8 column shipped they give byte-identical received
+ * tables and receive regions.  Every rank names the same columns.
+ *   Columns: 1..16 columns of any physical type a table holds, utf8 included (NULL: all columns of src, at most 16).  A received utf8
+ *   column is an ordinary single-batch utf8 column: n + 1 int32 offsets starting at 0, the bytes, one validity byte per row.  A source
+ *   cell's string is bytes[off[i] .. off[i+1]) as LDB_OP_STRCMP reads it (HOST slices, DEVICE batches whose offsets do not start at 0 and
+ *   library-made tables alike); a NULL string ships no bytes, so its two offsets are equal.
+ *   Keys: as ldb_gpu_table_exchange (integer, date32, char(1) or decimal columns; a utf8 or float key: LDB_ERR_UNSUPPORTED).  String
+ *   keys go through unified dictionary codes (ldb_gpu_dict_unify).
+ *   Receive region of a rank receiving n rows, utf8 column j receiving B_j bytes, every array 16-byte aligned: per shipped column in
+ *   order its n cells (fixed-width) or its n + 1 int32 offsets (utf8); then per utf8 column in order its B_j bytes; then the validity
+ *   bytes of every column.  Without utf8 columns this is ldb_gpu_table_exchange's layout.  Source s's rows start at row
+ *   Σ_{s' < s} M[s'][d], its bytes of column j at byte Σ_{s' < s} Bytes[s'][d][j].
+ *   Decisions, identical on every rank and made before anything is stored: (1) when a receiver's B_j exceeds 2^31 - 1 (utf8 offsets
+ *   are int32), EVERY rank fails with LDB_ERR_UNSUPPORTED naming the column and the byte count; (2) otherwise, when the region of any
+ *   rank does not fit recv_bytes, EVERY rank fails with LDB_ERR_CAPACITY naming the recv_bytes to retry with.  Either way nothing is
+ *   written into any receive region and the ranks stay in step. */
+int ldb_gpu_table_exchange_varlen(LdbTable* src, int32_t n_keys, const char* const* key_columns, int32_t n_columns, const char* const* columns /* NULL = all columns of src */,
+                                  LdbComm* comm, int64_t recv_offset, int64_t recv_bytes, const char* name, LdbTable** out, LdbError* err);
 /* Unify the string dictionaries of the ranks of `comm` into one dictionary that every rank holds, with codes in bytewise order, so that
  * string group, join and sort keys work across ranks.  Collective: every rank calls it in the same order, each with a string dictionary
  * (LDB_STATE_DICT) of comm's context, which may be empty; `local` is only read.

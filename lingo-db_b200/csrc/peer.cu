@@ -199,6 +199,9 @@ __global__ void peerPublishCountsKernel(PeerView v, size_t cursorsOff, size_t co
 // owner's receive region.  Receive region of a rank with n rows (column-major, every array 16-byte aligned):
 //   cells of column 0 (n x outBytes[0]) | … | cells of column m-1 | validity bytes of column 0 (n) | … | validity bytes of column m-1
 // Source s's rows start at row Σ_{s' < s} M[s'][d] of receiver d, M[s][d] = the rows source s sends rank d.
+// With utf8 columns (ldb_gpu_table_exchange_varlen) a utf8 column's "cells" are its n + 1 int32 offsets, and its bytes follow every
+// column's cells: … cells / offsets of column m-1 | bytes of utf8 column 0 (B_0) | … | validity bytes …; source s's bytes of utf8 column
+// j start at byte Σ_{s' < s} Bytes[s'][d][j].  The count kernel then also histograms the bytes per (destination, utf8 column, CTA).
 constexpr int kShipMaxCols = 16;
 constexpr int kShipThreads = 256;
 constexpr int64_t kShipTile = 16 * kShipThreads; // rows per CTA; tiles never span batches
@@ -215,13 +218,42 @@ struct TableShipBatch {
    uint8_t* recv[kMaxPeers];    // every rank's receive region (peer-mapped)
    unsigned long long rows[kMaxPeers]; // the rows every rank receives (its N_d)
    unsigned long long base[kMaxPeers]; // the row of receiver d where this source's rows start
+   // utf8 columns (the string kernels only; the fixed-width kernels never read these)
+   int32_t nStr;                       // shipped utf8 columns
+   int8_t strCol[kShipMaxCols];        // utf8 column j: its index among the shipped columns
+   int8_t strOf[kShipMaxCols];         // shipped column c: its utf8 index j, or -1
+   uint32_t strBytes[kMaxPeers][kShipMaxCols]; // B_j of every receiver (<= 2^31 - 1: decided before the send)
+   uint32_t byteBase[kMaxPeers][kShipMaxCols]; // the byte of receiver d's column j where this source's bytes start
 };
+static_assert(sizeof(TableShipBatch) <= 4096, "TableShipBatch is a __grid_constant__ kernel parameter (4 KiB at most)");
+// hist rows of the string count kernel: rows of destination d at row d, bytes of (destination d, utf8 column j) at row world + d nStr + j;
+// the scan turns row r into totals[r], which the matrix all-gather carries (kShipBlockU64 u64 per rank at most)
+constexpr int kShipBlockU64 = kMaxPeers * (1 + kShipMaxCols);
 // byte offsets of the arrays of a receive region of n rows; returns its size
 __host__ __device__ inline uint64_t shipLayout(uint64_t n, const int32_t* outBytes, int nCols, uint64_t* colOff, uint64_t* validOff) {
    uint64_t off = 0;
    for (int c = 0; c < nCols; c++) {
       colOff[c] = off;
       off += (n * (uint64_t) outBytes[c] + 15) & ~uint64_t(15);
+   }
+   for (int c = 0; c < nCols; c++) {
+      validOff[c] = off;
+      off += (n + 15) & ~uint64_t(15);
+   }
+   return off;
+}
+// the same with utf8 columns: strOf[c] >= 0 marks a utf8 column (n + 1 int32 offsets) whose bytes, strBytes[strOf[c]], follow the cells
+// of every column; bytesOff[j] = where utf8 column j's bytes start.  Without utf8 columns this is shipLayout.
+__host__ __device__ inline uint64_t shipLayoutVar(uint64_t n, const int32_t* outBytes, int nCols, const int8_t* strOf, int nStr, const uint32_t* strBytes,
+                                                  uint64_t* colOff, uint64_t* validOff, uint64_t* bytesOff) {
+   uint64_t off = 0;
+   for (int c = 0; c < nCols; c++) {
+      colOff[c] = off;
+      off += ((strOf[c] >= 0 ? (n + 1) * 4 : n * (uint64_t) outBytes[c]) + 15) & ~uint64_t(15);
+   }
+   for (int j = 0; j < nStr; j++) {
+      bytesOff[j] = off;
+      off += ((uint64_t) strBytes[j] + 15) & ~uint64_t(15);
    }
    for (int c = 0; c < nCols; c++) {
       validOff[c] = off;
@@ -257,6 +289,41 @@ __global__ void __launch_bounds__(kShipThreads) tableShipCountKernel(const __gri
    }
    __syncthreads();
    if (threadIdx.x < p.world) p.hist[(size_t) threadIdx.x * p.nCtas + p.ctaBase + blockIdx.x] = cnt[threadIdx.x];
+}
+// a utf8 cell's byte count: bytes[off[i] .. off[i+1]) as strCompare (program.cu) reads them; a NULL string ships none.  A warp's 32 cells
+// come from one batch, whose offsets are int32, so their sum fits 32 bits.
+__device__ __forceinline__ uint32_t shipStrLen(const ProgCol& c, int64_t row) {
+   if (colIsNull(c, row)) return 0;
+   const int32_t* off = (const int32_t*) c.data + row;
+   return (uint32_t) (off[1] - off[0]);
+}
+// tableShipCountKernel with utf8 columns: also the bytes per (destination, utf8 column, CTA), in hist row world + d nStr + j.  A broadcast
+// counts every row for destination 0 (the other destinations' rows stay 0) and writes no owners.
+__global__ void __launch_bounds__(kShipThreads) tableShipCountStrKernel(const __grid_constant__ TableShipBatch p) {
+   __shared__ unsigned int cnt[kMaxPeers];
+   __shared__ unsigned long long bytes[kMaxPeers * kShipMaxCols];
+   if (threadIdx.x < kMaxPeers) cnt[threadIdx.x] = 0;
+   for (int x = threadIdx.x; x < kMaxPeers * kShipMaxCols; x += kShipThreads) bytes[x] = 0;
+   __syncthreads();
+   const int lane = threadIdx.x & 31;
+   const int64_t begin = (int64_t) blockIdx.x * kShipTile, end = min(begin + kShipTile, p.nRows);
+   for (int64_t t = begin; t < end; t += kShipThreads) {
+      const int64_t i = t + threadIdx.x;
+      const bool valid = i < end;
+      const int d = !valid ? -1 : p.broadcast ? 0 : shipOwnerOf(p, i);
+      if (valid && !p.broadcast) p.owners[p.firstRow + i] = (uint8_t) d;
+      const unsigned same = __match_any_sync(0xffffffffu, d);
+      const bool leader = valid && lane == __ffs(same) - 1;
+      if (leader) atomicAdd(&cnt[d], (unsigned) __popc(same));
+      for (int j = 0; j < p.nStr; j++) {
+         const unsigned sum = __reduce_add_sync(same, valid ? shipStrLen(p.cols[p.strCol[j]], i) : 0u);
+         if (leader) atomicAdd(&bytes[d * p.nStr + j], (unsigned long long) sum);
+      }
+   }
+   __syncthreads();
+   const size_t at = (size_t) p.ctaBase + blockIdx.x;
+   if (threadIdx.x < p.world) p.hist[(size_t) threadIdx.x * p.nCtas + at] = cnt[threadIdx.x];
+   for (int x = threadIdx.x; x < p.world * p.nStr; x += kShipThreads) p.hist[(size_t) (p.world + x) * p.nCtas + at] = bytes[x];
 }
 // CTA d: exclusive scan of destination d's per-CTA counts, in place; totals[d] = the rows this rank sends rank d
 __global__ void __launch_bounds__(1024) tableShipScanKernel(unsigned long long* hist, int64_t nCtas, unsigned long long* totals) {
@@ -360,6 +427,126 @@ __global__ void __launch_bounds__(kShipThreads) tableShipSendKernel(const __grid
       __syncthreads();
    }
 }
+// tableShipSendKernel with utf8 columns.  Rows are ranked as there; a row's thread stores its fixed-width cells, its validity bytes and,
+// per utf8 column, the offset of its string in the receiver: this source's byte base + the CTA's scanned bytes + the bytes of earlier
+// passes, of earlier warps and of the earlier lanes of its warp with the same destination.  So the strings of one warp's rows for one
+// destination are adjacent in the receiver, and the whole warp copies that range: lanes take consecutive bytes, each walking the
+// warp's rows in (destination, lane) order.  A broadcast ranks every row for destination 0 and stores it into every rank.
+constexpr int kShipWarps = kShipThreads / 32;
+__global__ void __launch_bounds__(kShipThreads) tableShipSendStrKernel(const __grid_constant__ TableShipBatch p) {
+   __shared__ uint64_t colOff[kMaxPeers][kShipMaxCols], validOff[kMaxPeers][kShipMaxCols], bytesOff[kMaxPeers][kShipMaxCols];
+   __shared__ unsigned long long running[kMaxPeers];                   // this CTA's rows for destination d before the pass (from base[d])
+   __shared__ unsigned long long byteRunning[kMaxPeers][kShipMaxCols]; // its bytes of utf8 column j for d before the pass (from byteBase)
+   __shared__ unsigned int warpCnt[kShipWarps][kMaxPeers];
+   __shared__ unsigned int warpBytes[kShipWarps][kMaxPeers][kShipMaxCols];
+   __shared__ uint32_t slotEnd[kShipWarps][33]; // the warp's lanes in (destination, lane) order: slot k's string is [slotEnd[k], slotEnd[k+1])
+   __shared__ int32_t slotSrc[kShipWarps][32];  // and starts at source byte slotSrc[k]
+   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+   const int world = p.world, nStr = p.nStr;
+   const int64_t begin = (int64_t) blockIdx.x * kShipTile, end = min(begin + kShipTile, p.nRows);
+   const size_t at = (size_t) p.ctaBase + blockIdx.x;
+   if (threadIdx.x < world) {
+      const int d = threadIdx.x;
+      shipLayoutVar(p.rows[d], p.outBytes, p.nCols, p.strOf, nStr, p.strBytes[d], colOff[d], validOff[d], bytesOff[d]);
+      running[d] = p.hist[(size_t) d * p.nCtas + at];
+   }
+   for (int x = threadIdx.x; x < world * nStr; x += kShipThreads) byteRunning[x / nStr][x % nStr] = p.hist[(size_t) (world + x) * p.nCtas + at];
+   __syncthreads();
+   for (int64_t t = begin; t < end; t += kShipThreads) {
+      for (int x = threadIdx.x; x < kShipWarps * kMaxPeers; x += kShipThreads) (&warpCnt[0][0])[x] = 0;
+      for (int x = threadIdx.x; x < kShipWarps * kMaxPeers * kShipMaxCols; x += kShipThreads) (&warpBytes[0][0][0])[x] = 0;
+      __syncthreads();
+      const int64_t i = t + threadIdx.x;
+      const bool valid = i < end;
+      const int d = !valid ? kMaxPeers : p.broadcast ? 0 : p.owners[p.firstRow + i];
+      const unsigned same = __match_any_sync(0xffffffffu, d);
+      const unsigned rankInWarp = __popc(same & ((1u << lane) - 1));
+      const bool leader = valid && rankInWarp == 0;
+      if (leader) warpCnt[warp][d] = __popc(same);
+      for (int j = 0; j < nStr; j++) {
+         const unsigned sum = __reduce_add_sync(same, valid ? shipStrLen(p.cols[p.strCol[j]], i) : 0u);
+         if (leader) warpBytes[warp][d][j] = sum;
+      }
+      __syncthreads();
+      // the row's slot (invalid lanes take the last ones) and its position relative to the source's first row in a receiver
+      unsigned slot = __popc(__ballot_sync(0xffffffffu, valid)) + rankInWarp, first = 0;
+      unsigned long long rel = 0;
+      if (valid) {
+         unsigned before = 0;
+         for (int w = 0; w < warp; w++) before += warpCnt[w][d];
+         for (int e = 0; e < d; e++) first += warpCnt[warp][e];
+         slot = first + rankInWarp;
+         rel = running[d] + before + rankInWarp;
+         for (int r = p.broadcast ? 0 : d; r < (p.broadcast ? world : d + 1); r++) {
+            uint8_t* dst = p.recv[r];
+            const unsigned long long pos = p.base[r] + rel;
+            for (int c = 0; c < p.nCols; c++) {
+               const bool null = colIsNull(p.cols[c], i);
+               if (p.strOf[c] < 0) shipCell(p.cols[c], p.outBytes[c], i, dst + colOff[r][c] + pos * (uint64_t) p.outBytes[c]);
+               dst[validOff[r][c] + pos] = null ? 0 : 1;
+            }
+         }
+      }
+      for (int j = 0; j < nStr; j++) {
+         const int c = p.strCol[j];
+         const ProgCol& sc = p.cols[c];
+         uint32_t len = 0;
+         int32_t from = 0;
+         if (valid && !colIsNull(sc, i)) {
+            const int32_t* o = (const int32_t*) sc.data + i;
+            from = o[0];
+            len = (uint32_t) (o[1] - o[0]);
+         }
+         __syncwarp(); // the previous column's copy is done with the slots
+         slotSrc[warp][slot] = from;
+         slotEnd[warp][slot + 1] = len;
+         __syncwarp();
+         uint32_t x = slotEnd[warp][lane + 1]; // inclusive scan of the lengths in slot order
+         for (int o = 1; o < 32; o <<= 1) {
+            const uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
+            if (lane >= o) x += y;
+         }
+         slotEnd[warp][lane + 1] = x;
+         if (lane == 0) slotEnd[warp][0] = 0;
+         __syncwarp();
+         if (valid) { // the row's offset: where its string starts in the receiver's column
+            unsigned long long relB = byteRunning[d][j] + (slotEnd[warp][slot] - slotEnd[warp][first]);
+            for (int w = 0; w < warp; w++) relB += warpBytes[w][d][j];
+            for (int r = p.broadcast ? 0 : d; r < (p.broadcast ? world : d + 1); r++)
+               *(int32_t*) (p.recv[r] + colOff[r][c] + (p.base[r] + rel) * 4) = (int32_t) (p.byteBase[r][j] + relB);
+         }
+         // the strings: per destination of the warp, one contiguous range of the receiver's bytes
+         unsigned gs = 0;
+         for (int g = 0; g < world; g++) {
+            const unsigned n = warpCnt[warp][g];
+            if (n == 0) continue;
+            const uint32_t e0 = slotEnd[warp][gs], total = slotEnd[warp][gs + n] - e0;
+            unsigned long long relB = byteRunning[g][j];
+            for (int w = 0; w < warp; w++) relB += warpBytes[w][g][j];
+            unsigned k = gs;
+            for (uint32_t b = lane; b < total; b += 32) {
+               const uint32_t a = e0 + b;
+               while (slotEnd[warp][k + 1] <= a) k++;
+               const uint8_t v = sc.bytes[(int64_t) slotSrc[warp][k] + (a - slotEnd[warp][k])];
+               for (int r = p.broadcast ? 0 : g; r < (p.broadcast ? world : g + 1); r++) p.recv[r][bytesOff[r][j] + p.byteBase[r][j] + relB + b] = v;
+            }
+            gs += n;
+         }
+      }
+      __syncthreads();
+      if (threadIdx.x < world) {
+         unsigned tot = 0;
+         for (int w = 0; w < kShipWarps; w++) tot += warpCnt[w][threadIdx.x];
+         running[threadIdx.x] += tot;
+      }
+      for (int x = threadIdx.x; x < world * nStr; x += kShipThreads) {
+         unsigned long long tot = 0;
+         for (int w = 0; w < kShipWarps; w++) tot += warpBytes[w][x / nStr][x % nStr];
+         byteRunning[x / nStr][x % nStr] += tot;
+      }
+      __syncthreads();
+   }
+}
 
 // ---------------------------------------------------------------- dictionary unification (ldb_gpu_dict_unify, include/ldb_gpu.h)
 // This rank's exported dictionary into its block of receiver blockIdx.y's region: the offsets array and the bytes array, each padded to
@@ -420,6 +607,8 @@ int ldb_gpu_comm_create(LdbContext* ctx, int32_t rank, int32_t world, int64_t us
       LDB_CUDA(cudaFuncGetAttributes(&fa, tableShipCountKernel));
       LDB_CUDA(cudaFuncGetAttributes(&fa, tableShipScanKernel));
       LDB_CUDA(cudaFuncGetAttributes(&fa, tableShipSendKernel));
+      LDB_CUDA(cudaFuncGetAttributes(&fa, tableShipCountStrKernel));
+      LDB_CUDA(cudaFuncGetAttributes(&fa, tableShipSendStrKernel));
       LDB_CUDA(cudaFuncGetAttributes(&fa, dictSendKernel));
       loadHashAggExchangeKernels();
       // the pinned scratch the collectives read counts into: allocating host memory can wait for running kernels, so it is taken now
@@ -720,9 +909,13 @@ int ldb_gpu_hashagg_exchange(LdbState* local, LdbState* owned, LdbComm* c, int64
 // the count matrix, capacity decision (identical on every rank) → barrier → send (per batch) → barrier → copy-out of the own region →
 // host wait.  While a rank's collectives wait for its peers nothing here blocks inside the driver: the temporaries and the pinned
 // scratch are taken before the first collective, the output buffers after the last, and host reads go to pinned memory.
-int ldb_gpu_table_exchange(LdbTable* src, int32_t n_keys, const char* const* key_columns, int32_t n_columns, const char* const* columns, LdbComm* c,
-                           int64_t recv_offset, int64_t recv_bytes, const char* name, LdbTable** out, LdbError* err) {
-   return guarded(err, [&] {
+// With utf8 columns (ldb_gpu_table_exchange_varlen) the string kernels run instead, the matrix also carries every rank's bytes per
+// (destination, utf8 column), and the host decides the int32 limit of the receivers' offsets before the capacity.
+static_assert((size_t) kMaxPeers * kShipBlockU64 * 8 + 64 + 8 * kMaxPeers + 4 * kShipMaxCols <= LdbContext::kPinnedScratchBytes,
+              "the table exchange's matrix, error word and offset ends fit the pinned scratch");
+static void tableExchange(bool varlen, LdbTable* src, int32_t n_keys, const char* const* key_columns, int32_t n_columns, const char* const* columns, LdbComm* c,
+                          int64_t recv_offset, int64_t recv_bytes, const char* name, LdbTable** out) {
+   {
       if (!src || !c || !out || (n_keys > 0 && !key_columns)) fail(LDB_ERR_INVALID, "null argument");
       if (n_keys < 0 || n_keys > kProgMaxKeys) fail(LDB_ERR_INVALID, "the exchange takes 0..4 key columns");
       if (src->ctx != c->ctx) fail(LDB_ERR_INVALID, "table and comm belong to different contexts");
@@ -739,7 +932,7 @@ int ldb_gpu_table_exchange(LdbTable* src, int32_t n_keys, const char* const* key
       }
       if (ship.size() > (size_t) kShipMaxCols) fail(LDB_ERR_INVALID, "the exchange ships up to 16 columns");
       for (int ci : ship)
-         if (src->columns[ci].type == LDB_UTF8) fail(LDB_ERR_UNSUPPORTED, "the exchange ships fixed-width columns (utf8 column " + src->columns[ci].name + ")");
+         if (!varlen && src->columns[ci].type == LDB_UTF8) fail(LDB_ERR_UNSUPPORTED, "the exchange ships fixed-width columns (utf8 column " + src->columns[ci].name + ")");
       for (int k = 0; k < n_keys; k++) {
          const int ci = src->colIndex(key_columns[k]);
          if (ci < 0) fail(LDB_ERR_INVALID, std::string("unknown key column ") + (key_columns[k] ? key_columns[k] : "(null)"));
@@ -769,14 +962,27 @@ int ldb_gpu_table_exchange(LdbTable* src, int32_t n_keys, const char* const* key
       for (auto& b : src->batches) ldb_gpu_wait_batch_internal(ctx, &b);
       int64_t nCtas = 0;
       for (auto& b : src->batches) nCtas += (b.nRows + kShipTile - 1) / kShipTile;
+      // the utf8 columns among the shipped ones: they select the string kernels, whose histograms have world (1 + nStr) rows
+      int nStr = 0;
+      int8_t strCol[kShipMaxCols], strOf[kShipMaxCols];
+      for (int j = 0; j < nCols; j++) {
+         strOf[j] = -1;
+         if (src->columns[ship[j]].type == LDB_UTF8) {
+            strOf[j] = (int8_t) nStr;
+            strCol[nStr++] = (int8_t) j;
+         }
+      }
+      const bool strings = nStr > 0;
+      const size_t blockU64 = (size_t) kMaxPeers * (1 + nStr); // this rank's totals in the all-gather: rows, then bytes per (d, column)
       Scratch tmp(ctx);
       const bool broadcast = n_keys == 0;
       uint8_t* owners = broadcast ? nullptr : tmp.alloc<uint8_t>((size_t) std::max<int64_t>(src->numRows, 1));
-      unsigned long long* hist = broadcast ? nullptr : tmp.alloc<unsigned long long>((size_t) std::max<int64_t>(nCtas, 1) * world * 8);
-      unsigned long long* totals = tmp.alloc<unsigned long long>(8 * kMaxPeers);
-      unsigned long long* matrix = (unsigned long long*) ctx->scratch(); // [world][kMaxPeers] M[s][d]
-      int32_t* timedOut = (int32_t*) (matrix + kMaxPeers * kMaxPeers);
-      unsigned long long* upload = matrix + kMaxPeers * kMaxPeers + 8;
+      unsigned long long* hist = broadcast && !strings ? nullptr : tmp.alloc<unsigned long long>((size_t) std::max<int64_t>(nCtas, 1) * world * (1 + nStr) * 8);
+      unsigned long long* totals = tmp.alloc<unsigned long long>(8 * blockU64);
+      unsigned long long* matrix = (unsigned long long*) ctx->scratch(); // [world][blockU64]: M[s][d] at [s][d], Bytes[s][d][j] at [s][world + d nStr + j]
+      int32_t* timedOut = (int32_t*) (matrix + kMaxPeers * kShipBlockU64);
+      unsigned long long* upload = matrix + kMaxPeers * kShipBlockU64 + 8;
+      uint32_t* offEnds = (uint32_t*) (upload + kMaxPeers); // B_j of this rank: the last offset of each received utf8 column
       TableShipBatch p{};
       p.nCols = nCols;
       p.nKeys = n_keys;
@@ -786,6 +992,9 @@ int ldb_gpu_table_exchange(LdbTable* src, int32_t n_keys, const char* const* key
       p.owners = owners;
       p.hist = hist;
       for (int j = 0; j < nCols; j++) p.outBytes[j] = outBytes[j];
+      p.nStr = nStr;
+      for (int j = 0; j < nCols; j++) p.strOf[j] = strOf[j];
+      for (int j = 0; j < nStr; j++) p.strCol[j] = strCol[j];
       auto bindBatch = [&](const LdbBatch& b, int64_t firstRow, int64_t ctaBase) {
          TableShipBatch q = p;
          for (int j = 0; j < nCols; j++) {
@@ -810,35 +1019,57 @@ int ldb_gpu_table_exchange(LdbTable* src, int32_t n_keys, const char* const* key
             cta += (b.nRows + kShipTile - 1) / kShipTile;
          }
       };
-      if (broadcast) {
+      if (broadcast && !strings) {
          for (int d = 0; d < kMaxPeers; d++) upload[d] = d < world ? (unsigned long long) src->numRows : 0ull;
          LDB_CUDA(cudaMemcpyAsync(totals, upload, 8 * kMaxPeers, cudaMemcpyHostToDevice, ctx->compute));
       } else {
          ctx->launch("table_exchange_count", [&] {
-            LDB_CUDA(cudaMemsetAsync(totals, 0, 8 * kMaxPeers, ctx->compute));
-            eachBatch([&](const TableShipBatch& q, int grid) { tableShipCountKernel<<<grid, kShipThreads, 0, ctx->compute>>>(q); });
-            tableShipScanKernel<<<world, 1024, 0, ctx->compute>>>(hist, nCtas, totals);
+            LDB_CUDA(cudaMemsetAsync(totals, 0, 8 * blockU64, ctx->compute));
+            eachBatch([&](const TableShipBatch& q, int grid) {
+               if (strings) tableShipCountStrKernel<<<grid, kShipThreads, 0, ctx->compute>>>(q);
+               else tableShipCountKernel<<<grid, kShipThreads, 0, ctx->compute>>>(q);
+            });
+            tableShipScanKernel<<<world * (1 + nStr), 1024, 0, ctx->compute>>>(hist, nCtas, totals);
          });
       }
       // the count matrix on every rank
       if (world == 1) {
-         LDB_CUDA(cudaMemcpyAsync(matrix, totals, 8 * kMaxPeers, cudaMemcpyDeviceToHost, ctx->compute));
+         LDB_CUDA(cudaMemcpyAsync(matrix, totals, 8 * blockU64, cudaMemcpyDeviceToHost, ctx->compute));
       } else {
-         const uint8_t* gathered = allGatherSmall(c, totals, 8 * kMaxPeers);
-         LDB_CUDA(cudaMemcpy2DAsync(matrix, 8 * kMaxPeers, gathered, kSlotBytes, 8 * kMaxPeers, world, cudaMemcpyDeviceToHost, ctx->compute));
+         const uint8_t* gathered = allGatherSmall(c, totals, 8 * blockU64);
+         LDB_CUDA(cudaMemcpy2DAsync(matrix, 8 * blockU64, gathered, kSlotBytes, 8 * blockU64, world, cudaMemcpyDeviceToHost, ctx->compute));
       }
       LDB_CUDA(cudaMemcpyAsync(timedOut, c->error, 4, cudaMemcpyDeviceToHost, ctx->compute));
       ctx->syncStream(ctx->compute);
       if (*timedOut) fail(LDB_ERR_CUDA, "a peer did not arrive at a collective within the timeout (LDB_PEER_TIMEOUT_MS)");
-      uint64_t colOff[kShipMaxCols], validOff[kShipMaxCols], need = 0;
+      // per receiver, from the same matrix on every rank: its rows and bytes, this source's bases in them, then the two decisions.  A
+      // broadcast counted every row for destination 0, and every rank receives what destination 0 would.
+      auto rowsOf = [&](int s, int d) { return matrix[s * blockU64 + (broadcast ? 0 : d)]; };
+      auto bytesOf = [&](int s, int d, int j) { return matrix[s * blockU64 + world + (broadcast ? 0 : d) * nStr + j]; };
+      uint64_t recvBytes[kMaxPeers][kShipMaxCols] = {};
       for (int d = 0; d < world; d++) {
          unsigned long long n = 0;
          for (int s = 0; s < world; s++) {
             if (s == c->rank) p.base[d] = n;
-            n += matrix[s * kMaxPeers + d];
+            n += rowsOf(s, d);
          }
          p.rows[d] = n;
-         need = std::max(need, shipLayout(n, outBytes, nCols, colOff, validOff));
+         for (int j = 0; j < nStr; j++) {
+            for (int s = 0; s < world; s++) {
+               if (s == c->rank) p.byteBase[d][j] = (uint32_t) std::min<uint64_t>(recvBytes[d][j], INT32_MAX); // exact once the limit holds
+               recvBytes[d][j] += bytesOf(s, d, j);
+            }
+         }
+      }
+      for (int d = 0; d < world; d++)
+         for (int j = 0; j < nStr; j++)
+            if (recvBytes[d][j] > (uint64_t) INT32_MAX)
+               fail(LDB_ERR_UNSUPPORTED, "table exchange: rank " + std::to_string(d) + " would receive " + std::to_string(recvBytes[d][j]) + " bytes of utf8 column " +
+                                            src->columns[ship[strCol[j]]].name + ", more than 2^31 - 1 (utf8 offsets are int32)");
+      uint64_t colOff[kShipMaxCols], validOff[kShipMaxCols], bytesOff[kShipMaxCols], need = 0;
+      for (int d = 0; d < world; d++) {
+         for (int j = 0; j < nStr; j++) p.strBytes[d][j] = (uint32_t) recvBytes[d][j];
+         need = std::max(need, shipLayoutVar(p.rows[d], outBytes, nCols, strOf, nStr, p.strBytes[d], colOff, validOff, bytesOff));
       }
       if (need > (uint64_t) recv_bytes)
          fail(LDB_ERR_CAPACITY, "table exchange: a rank receives rows that need " + std::to_string(need) + " bytes of receive region, more than recv_bytes " +
@@ -860,31 +1091,47 @@ int ldb_gpu_table_exchange(LdbTable* src, int32_t n_keys, const char* const* key
                r.recv[d] = p.recv[d];
                r.rows[d] = p.rows[d];
                r.base[d] = p.base[d];
+               for (int j = 0; j < nStr; j++) {
+                  r.strBytes[d][j] = p.strBytes[d][j];
+                  r.byteBase[d][j] = p.byteBase[d][j];
+               }
             }
-            tableShipSendKernel<<<grid, kShipThreads, 0, ctx->compute>>>(r);
+            if (strings) tableShipSendStrKernel<<<grid, kShipThreads, 0, ctx->compute>>>(r);
+            else tableShipSendKernel<<<grid, kShipThreads, 0, ctx->compute>>>(r);
          });
       });
       barrier(); // every peer's rows are in this rank's region
-      // copy-out into buffers the new table owns: one device-to-device copy per array
-      shipLayout(mine, outBytes, nCols, colOff, validOff);
+      // copy-out into buffers the new table owns: one device-to-device copy per array.  A utf8 column's last offset is B_j, which the
+      // matrix gave: it is written into the region first, so the n + 1 offsets are one copy too.
+      shipLayoutVar(mine, outBytes, nCols, strOf, nStr, p.strBytes[c->rank], colOff, validOff, bytesOff);
       Scratch cols(ctx);
       std::vector<LdbColumn> outCols;
       LdbBatch ob;
       ob.nRows = (int64_t) mine;
-      const uint8_t* region = c->heap + kUserOff + recv_offset;
+      uint8_t* region = c->heap + kUserOff + recv_offset;
       ctx->launch("table_exchange_copy", [&] {
          for (int j = 0; j < nCols; j++) {
             const LdbColumn& sc = src->columns[ship[j]];
             outCols.push_back({sc.name, sc.type, sc.precision, sc.scale});
-            const size_t bytes = (size_t) mine * outBytes[j];
+            const int sj = strOf[j];
+            const size_t bytes = sj >= 0 ? ((size_t) mine + 1) * 4 : (size_t) mine * outBytes[j];
             uint8_t* data = cols.alloc<uint8_t>(std::max<size_t>(bytes, 16));
             uint8_t* valid = cols.alloc<uint8_t>(std::max<size_t>(mine, 16));
-            if (mine) {
+            uint8_t* chars = nullptr;
+            if (sj >= 0) {
+               const size_t nb = p.strBytes[c->rank][sj];
+               chars = cols.alloc<uint8_t>(std::max<size_t>(nb, 16));
+               offEnds[sj] = (uint32_t) nb;
+               LDB_CUDA(cudaMemcpyAsync(region + colOff[j] + mine * 4, &offEnds[sj], 4, cudaMemcpyHostToDevice, ctx->compute));
                LDB_CUDA(cudaMemcpyAsync(data, region + colOff[j], bytes, cudaMemcpyDeviceToDevice, ctx->compute));
+               if (nb) LDB_CUDA(cudaMemcpyAsync(chars, region + bytesOff[sj], nb, cudaMemcpyDeviceToDevice, ctx->compute));
+            }
+            if (mine) {
+               if (sj < 0) LDB_CUDA(cudaMemcpyAsync(data, region + colOff[j], bytes, cudaMemcpyDeviceToDevice, ctx->compute));
                LDB_CUDA(cudaMemcpyAsync(valid, region + validOff[j], (size_t) mine, cudaMemcpyDeviceToDevice, ctx->compute));
             }
             ob.data.push_back(data);
-            ob.bytes.push_back(nullptr);
+            ob.bytes.push_back(chars);
             ob.elemBytes.push_back(outBytes[j]);
             ob.validBytes.push_back(valid);
          }
@@ -893,7 +1140,15 @@ int ldb_gpu_table_exchange(LdbTable* src, int32_t n_keys, const char* const* key
       ctx->syncStream(ctx->compute); // the region is free for the next collective, the temporaries for the pool
       if (*timedOut) fail(LDB_ERR_CUDA, "a peer did not arrive at a collective within the timeout (LDB_PEER_TIMEOUT_MS)");
       *out = addResultTable(ctx, name ? name : "received", std::move(outCols), std::move(ob), cols);
-   });
+   }
+}
+int ldb_gpu_table_exchange(LdbTable* src, int32_t n_keys, const char* const* key_columns, int32_t n_columns, const char* const* columns, LdbComm* c,
+                           int64_t recv_offset, int64_t recv_bytes, const char* name, LdbTable** out, LdbError* err) {
+   return guarded(err, [&] { tableExchange(false, src, n_keys, key_columns, n_columns, columns, c, recv_offset, recv_bytes, name, out); });
+}
+int ldb_gpu_table_exchange_varlen(LdbTable* src, int32_t n_keys, const char* const* key_columns, int32_t n_columns, const char* const* columns, LdbComm* c,
+                                  int64_t recv_offset, int64_t recv_bytes, const char* name, LdbTable** out, LdbError* err) {
+   return guarded(err, [&] { tableExchange(true, src, n_keys, key_columns, n_columns, columns, c, recv_offset, recv_bytes, name, out); });
 }
 
 // Union of every rank's string dictionary (include/ldb_gpu.h).  Local counters → export → all-gather of {status, n, bytes} → host

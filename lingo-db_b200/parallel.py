@@ -167,6 +167,17 @@ class Comm:
         host: the ranks of one process call it from one thread each.  The receive region starts at user-heap offset `recv_offset` and
         spans `recv_bytes` (None: the rest of the user heap); rows that do not fit fail with LDB_ERR_CAPACITY on every rank.  The
         received table is named `name` ("received" when None)."""
+        return self._exchange(self.L.ldb_gpu_table_exchange, table, keys, columns, name, recv_offset, recv_bytes)
+
+    def table_exchange_varlen(self, table, keys, columns=None, name: str = "received", recv_offset: int = 0, recv_bytes: int = None):
+        """table_exchange whose shipped columns may also be utf8 (ldb_gpu_table_exchange_varlen): string columns travel with their rows,
+        without a dictionary, and arrive as ordinary utf8 columns (offsets from 0, the bytes, validity bytes).  Keys, owners, order and
+        errors are those of table_exchange, and without utf8 columns the received table is the same.  The receive region also holds the
+        received strings' bytes; a receiver whose bytes of one utf8 column pass 2^31 - 1 fails with LDB_ERR_UNSUPPORTED on every rank, rows
+        and bytes that do not fit `recv_bytes` with LDB_ERR_CAPACITY on every rank."""
+        return self._exchange(self.L.ldb_gpu_table_exchange_varlen, table, keys, columns, name, recv_offset, recv_bytes)
+
+    def _exchange(self, entry, table, keys, columns, name, recv_offset, recv_bytes):
         from . import capi
         from .program import RawTable, _handle
         keys = list(keys or [])
@@ -177,9 +188,8 @@ class Comm:
         if recv_bytes is None:
             recv_bytes = self.heap()[1] - int(recv_offset)
         out, e = C.c_void_p(), capi.Error()
-        capi.check(self.L.ldb_gpu_table_exchange(C.c_void_p(_handle(table)), len(kn), karr, len(cn), carr, self.h, int(recv_offset), int(recv_bytes),
-                                                 name.encode() if name is not None else None,
-                                                 C.byref(out), C.byref(e)), e)
+        capi.check(entry(C.c_void_p(_handle(table)), len(kn), karr, len(cn), carr, self.h, int(recv_offset), int(recv_bytes),
+                         name.encode() if name is not None else None, C.byref(out), C.byref(e)), e)
         return RawTable(self.ctx, out)
 
     def dict_unify(self, local, recv_offset: int = 0, recv_bytes: int = None):
