@@ -702,6 +702,34 @@ int ldb_gpu_table_exchange(LdbTable* src, int32_t n_keys, const char* const* key
  *   written into any receive region and the ranks stay in step. */
 int ldb_gpu_table_exchange_varlen(LdbTable* src, int32_t n_keys, const char* const* key_columns, int32_t n_columns, const char* const* columns /* NULL = all columns of src */,
                                   LdbComm* comm, int64_t recv_offset, int64_t recv_bytes, const char* name, LdbTable** out, LdbError* err);
+/* ORDER BY (… LIMIT) over the rows of every rank of `comm`: collective, every rank calls it in the same order with the same keys, columns
+ * and limit.
+ *   Result: *out = a new single-batch DEVICE table of this context named `name` (NULL: "sorted") with the shipped columns, whose names,
+ *   types and cells are those of ldb_gpu_table_exchange_varlen; its rows are already in order.  Reading rank 0's table, then rank 1's,
+ *   … gives ORDER BY over the union of all ranks' rows.  *first_row = the result rows on lower ranks, *total_rows = the result rows of
+ *   all ranks.
+ *   Order: the order of ldb_gpu_table_order_by_keys: 1..4 keys, each ascending (descending[k] = 0) or descending; a NULL compares greater
+ *   than any value and equal to another NULL, DESC swaps the operands; decimals compare by their full 128-bit value, whatever width a
+ *   shard staged them at.  Rows that tie on every key are ordered by (source rank, source row number as LDB_OP_ROWID gives it), so the
+ *   result equals ldb_gpu_table_order_by_keys over the concatenation of the shards in rank order and does not depend on thread timing.
+ *   Without LIMIT (limit < 0): every rank samples 1024 key tuples (key values, rank, row) at hashed positions, the samples go through the
+ *   small all-gather, and every rank picks the same world - 1 splitters, each sample weighted by the rows it stands for; rank d receives
+ *   the rows between splitters d - 1 and d, sorts and permutes them.  With LIMIT (limit >= 0): the first `limit` rows of the global order,
+ *   all on rank 0 (the other ranks get empty tables); each rank ships only its own first `limit` rows, so a region for world * limit rows
+ *   is enough however large the shards are.
+ *   Keys: int32, date32, char(1), int64 or decimal columns (narrowed 8-byte or 16-byte cells; exported group keys and aggregates).  A
+ *   utf8, float, int8 or int16 key: LDB_ERR_UNSUPPORTED naming the column; strings sort across ranks as unified dictionary codes
+ *   (ldb_gpu_dict_unify).  Keys need not be shipped: a key outside `columns` travels as a hidden column, and the shipped columns and such
+ *   keys are at most 16.
+ *   Columns and sources: as ldb_gpu_table_exchange_varlen (1..16 columns of any type, utf8 included; every table the exchange takes).
+ *   Receive region, capacity (all or nothing, LDB_ERR_CAPACITY on every rank naming the recv_bytes to retry with), the 2^31 - 1 byte
+ *   limit of a received utf8 column, the capture refusal (LDB_ERR_UNSUPPORTED), threading and the free region on return: as
+ *   ldb_gpu_table_exchange_varlen, over the shipped and hidden key columns.  n_keys outside 1..4 or an unknown column: LDB_ERR_INVALID.
+ *   Up to 2^32 - 1 rows per rank.  With LIMIT, a rank whose own first `limit` rows hold more than 2^31 - 1 bytes of one utf8 column
+ *   fails with LDB_ERR_UNSUPPORTED before its first collective.  world = 1 is a local ORDER BY into a new table. */
+int ldb_gpu_table_sort_exchange(LdbTable* src, int32_t n_keys, const char* const* key_columns, const int32_t* descending, int32_t n_columns,
+                                const char* const* columns /* NULL = all columns of src */, int64_t limit, LdbComm* comm, int64_t recv_offset, int64_t recv_bytes,
+                                const char* name, LdbTable** out, int64_t* first_row, int64_t* total_rows, LdbError* err);
 /* Unify the string dictionaries of the ranks of `comm` into one dictionary that every rank holds, with codes in bytewise order, so that
  * string group, join and sort keys work across ranks.  Collective: every rank calls it in the same order, each with a string dictionary
  * (LDB_STATE_DICT) of comm's context, which may be empty; `local` is only read.

@@ -225,6 +225,8 @@ SIGNATURES = {
     "ldb_gpu_hashagg_exchange": (C.c_int, [_P, _P, _P, C.c_int64, C.c_int64, _E]),
     "ldb_gpu_table_exchange": (C.c_int, [_P, C.c_int32, C.POINTER(C.c_char_p), C.c_int32, C.POINTER(C.c_char_p), _P, C.c_int64, C.c_int64, C.c_char_p, C.POINTER(_P), _E]),
     "ldb_gpu_table_exchange_varlen": (C.c_int, [_P, C.c_int32, C.POINTER(C.c_char_p), C.c_int32, C.POINTER(C.c_char_p), _P, C.c_int64, C.c_int64, C.c_char_p, C.POINTER(_P), _E]),
+    "ldb_gpu_table_sort_exchange": (C.c_int, [_P, C.c_int32, C.POINTER(C.c_char_p), C.POINTER(C.c_int32), C.c_int32, C.POINTER(C.c_char_p), C.c_int64, _P, C.c_int64,
+                                              C.c_int64, C.c_char_p, C.POINTER(_P), C.POINTER(C.c_int64), C.POINTER(C.c_int64), _E]),
     "ldb_gpu_dict_unify": (C.c_int, [_P, _P, C.c_int64, C.c_int64, C.POINTER(_P), _E]),
     "ldb_gpu_comm_heap_zero": (C.c_int, [_P, C.c_int64, C.c_int64, _E]),
     "ldb_gpu_comm_heap_read": (C.c_int, [_P, C.c_int64, C.c_int64, _P, _E]),

@@ -158,7 +158,7 @@ struct LdbContext {
    }
    // pinned scratch for small result reads: a copy into pageable memory would be staged by the driver and serialise with the host
    void* pinnedScratch = nullptr;
-   static constexpr size_t kPinnedScratchBytes = 512u << 10;
+   static constexpr size_t kPinnedScratchBytes = 1u << 20; // the sort exchange reads every rank's samples into it
    void* scratch() {
       if (!pinnedScratch) LDB_CUDA(cudaMallocHost(&pinnedScratch, kPinnedScratchBytes));
       return pinnedScratch;

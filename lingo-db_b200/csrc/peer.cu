@@ -18,6 +18,7 @@
 #include "peer.h"
 #include "progcol.cuh"
 #include "program.h"
+#include "sortkey.cuh"
 
 #include <algorithm>
 #include <cstring>
@@ -273,7 +274,9 @@ __device__ __forceinline__ int shipOwnerOf(const TableShipBatch& p, int64_t row)
    }
    return keyOwner(keyTupleHash(keys, p.nKeys, nulls), p.world);
 }
-__global__ void __launch_bounds__(kShipThreads) tableShipCountKernel(const __grid_constant__ TableShipBatch p) {
+// the count kernel's body for an owner rule ownerOf(row): tableShipCountKernel (key hash) and tableShipCountRangeKernel (sort splitters)
+template <class OwnerOf>
+__device__ __forceinline__ void shipCountRows(const TableShipBatch& p, const OwnerOf& ownerOf) {
    __shared__ unsigned int cnt[kMaxPeers];
    if (threadIdx.x < kMaxPeers) cnt[threadIdx.x] = 0;
    __syncthreads();
@@ -282,13 +285,16 @@ __global__ void __launch_bounds__(kShipThreads) tableShipCountKernel(const __gri
    for (int64_t t = begin; t < end; t += kShipThreads) {
       const int64_t i = t + threadIdx.x;
       const bool valid = i < end;
-      const int d = valid ? shipOwnerOf(p, i) : -1;
+      const int d = valid ? ownerOf(i) : -1;
       if (valid) p.owners[p.firstRow + i] = (uint8_t) d;
       const unsigned same = __match_any_sync(0xffffffffu, d);
       if (valid && lane == __ffs(same) - 1) atomicAdd(&cnt[d], (unsigned) __popc(same));
    }
    __syncthreads();
    if (threadIdx.x < p.world) p.hist[(size_t) threadIdx.x * p.nCtas + p.ctaBase + blockIdx.x] = cnt[threadIdx.x];
+}
+__global__ void __launch_bounds__(kShipThreads) tableShipCountKernel(const __grid_constant__ TableShipBatch p) {
+   shipCountRows(p, [&](int64_t i) { return shipOwnerOf(p, i); });
 }
 // a utf8 cell's byte count: bytes[off[i] .. off[i+1]) as strCompare (program.cu) reads them; a NULL string ships none.  A warp's 32 cells
 // come from one batch, whose offsets are int32, so their sum fits 32 bits.
@@ -299,7 +305,8 @@ __device__ __forceinline__ uint32_t shipStrLen(const ProgCol& c, int64_t row) {
 }
 // tableShipCountKernel with utf8 columns: also the bytes per (destination, utf8 column, CTA), in hist row world + d nStr + j.  A broadcast
 // counts every row for destination 0 (the other destinations' rows stay 0) and writes no owners.
-__global__ void __launch_bounds__(kShipThreads) tableShipCountStrKernel(const __grid_constant__ TableShipBatch p) {
+template <class OwnerOf>
+__device__ __forceinline__ void shipCountStrRows(const TableShipBatch& p, const OwnerOf& ownerOf) {
    __shared__ unsigned int cnt[kMaxPeers];
    __shared__ unsigned long long bytes[kMaxPeers * kShipMaxCols];
    if (threadIdx.x < kMaxPeers) cnt[threadIdx.x] = 0;
@@ -310,7 +317,7 @@ __global__ void __launch_bounds__(kShipThreads) tableShipCountStrKernel(const __
    for (int64_t t = begin; t < end; t += kShipThreads) {
       const int64_t i = t + threadIdx.x;
       const bool valid = i < end;
-      const int d = !valid ? -1 : p.broadcast ? 0 : shipOwnerOf(p, i);
+      const int d = !valid ? -1 : p.broadcast ? 0 : ownerOf(i);
       if (valid && !p.broadcast) p.owners[p.firstRow + i] = (uint8_t) d;
       const unsigned same = __match_any_sync(0xffffffffu, d);
       const bool leader = valid && lane == __ffs(same) - 1;
@@ -324,6 +331,9 @@ __global__ void __launch_bounds__(kShipThreads) tableShipCountStrKernel(const __
    const size_t at = (size_t) p.ctaBase + blockIdx.x;
    if (threadIdx.x < p.world) p.hist[(size_t) threadIdx.x * p.nCtas + at] = cnt[threadIdx.x];
    for (int x = threadIdx.x; x < p.world * p.nStr; x += kShipThreads) p.hist[(size_t) (p.world + x) * p.nCtas + at] = bytes[x];
+}
+__global__ void __launch_bounds__(kShipThreads) tableShipCountStrKernel(const __grid_constant__ TableShipBatch p) {
+   shipCountStrRows(p, [&](int64_t i) { return shipOwnerOf(p, i); });
 }
 // CTA d: exclusive scan of destination d's per-CTA counts, in place; totals[d] = the rows this rank sends rank d
 __global__ void __launch_bounds__(1024) tableShipScanKernel(unsigned long long* hist, int64_t nCtas, unsigned long long* totals) {
@@ -548,6 +558,198 @@ __global__ void __launch_bounds__(kShipThreads) tableShipSendStrKernel(const __g
    }
 }
 
+// ---------------------------------------------------------------- sort exchange (ldb_gpu_table_sort_exchange, include/ldb_gpu.h)
+// A row's place in the global order is its canonical tuple: per key its NULL flag and its value sign-extended to 128 bits (sortCell,
+// sortkey.cuh: the cell read buildSortWordsKernel makes), both inverted for DESC, then (source rank, source row).  Word 0 holds the NULL
+// flags in bits 56.. and rank << 48 | row below them; words 1 + 2k and 2 + 2k the high word (sign bit flipped) and the low word of key k,
+// so unsigned word comparisons give the order of ldb_gpu_table_order_by_keys whatever width a shard staged a decimal key at.  Every tuple
+// is distinct, so splitters taken from samples cut even a table of equal keys into balanced ranges.
+constexpr int kSortSamples = 1024;                     // samples per rank (S)
+constexpr int kSortTupleWords = 1 + 2 * kProgMaxKeys;  // 72 bytes
+constexpr size_t kSortBlockBytes = 16 + (size_t) kSortSamples * kSortTupleWords * 8; // {n_r, S_r}, then S_r tuples
+static_assert(kSortBlockBytes % 16 == 0 && kSortBlockBytes <= kSlotBytes, "a rank's samples are one all-gather block");
+constexpr unsigned long long kSortRowMask = (1ull << 56) - 1; // (rank, row) of word 0
+struct SortSplit {
+   int32_t nKeys, nSplit, rank, pad;
+   int32_t desc[kProgMaxKeys];
+   unsigned long long split[kMaxPeers - 1][kSortTupleWords]; // ascending; rank d owns the tuples t with split[d-1] < t <= split[d]
+};
+__host__ __device__ __forceinline__ bool sortTupleLess(const unsigned long long* a, const unsigned long long* b, int nKeys) {
+#pragma unroll
+   for (int k = 0; k < kProgMaxKeys; k++) {
+      if (k >= nKeys) break;
+      const unsigned long long na = (a[0] >> (56 + k)) & 1, nb = (b[0] >> (56 + k)) & 1;
+      if (na != nb) return na < nb;
+      if (a[1 + 2 * k] != b[1 + 2 * k]) return a[1 + 2 * k] < b[1 + 2 * k];
+      if (a[2 + 2 * k] != b[2 + 2 * k]) return a[2 + 2 * k] < b[2 + 2 * k];
+   }
+   return (a[0] & kSortRowMask) < (b[0] & kSortRowMask);
+}
+__device__ __forceinline__ void sortTupleOf(const TableShipBatch& p, const SortSplit& s, int64_t i, unsigned long long (&w)[kSortTupleWords]) {
+   unsigned long long nulls = 0;
+#pragma unroll
+   for (int k = 0; k < kProgMaxKeys; k++) {
+      w[1 + 2 * k] = w[2 + 2 * k] = 0;
+      if (k >= s.nKeys) continue;
+      const ProgCol& c = p.keys[k];
+      const bool null = colIsNull(c, i);
+      const SortCell v = null ? SortCell{0, 0} : sortCell(c.data, c.elemBytes, i);
+      const unsigned long long inv = s.desc[k] ? ~0ull : 0ull;
+      w[1 + 2 * k] = v.hi ^ 0x8000000000000000ull ^ inv;
+      w[2 + 2 * k] = v.lo ^ inv;
+      nulls |= (unsigned long long) ((null ? 1 : 0) ^ (s.desc[k] ? 1 : 0)) << k;
+   }
+   w[0] = nulls << 56 | (unsigned long long) s.rank << 48 | (unsigned long long) (p.firstRow + i);
+}
+// the range owner: the number of splitters below the row's tuple (binary search over <= 7 splitters in the parameter space)
+__device__ __forceinline__ int sortRangeOwner(const TableShipBatch& p, const SortSplit& s, int64_t i) {
+   unsigned long long w[kSortTupleWords];
+   sortTupleOf(p, s, i, w);
+   int lo = 0, hi = s.nSplit;
+   while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (sortTupleLess(s.split[mid], w, s.nKeys)) lo = mid + 1;
+      else hi = mid;
+   }
+   return lo;
+}
+__global__ void __launch_bounds__(kShipThreads) tableShipCountRangeKernel(const __grid_constant__ TableShipBatch p, const __grid_constant__ SortSplit s) {
+   shipCountRows(p, [&](int64_t i) { return sortRangeOwner(p, s, i); });
+}
+__global__ void __launch_bounds__(kShipThreads) tableShipCountRangeStrKernel(const __grid_constant__ TableShipBatch p, const __grid_constant__ SortSplit s) {
+   shipCountStrRows(p, [&](int64_t i) { return sortRangeOwner(p, s, i); });
+}
+// sample j of a table of `total` rows is row mix64(j + c) mod total (a hash of the index, not a stride: a periodic input cannot alias
+// it); the launch over one batch writes the samples that fall into it, as tuples at out[j]
+__global__ void __launch_bounds__(256) sortSampleKernel(const __grid_constant__ TableShipBatch p, const __grid_constant__ SortSplit s, int64_t total, unsigned long long* out) {
+   const int j = blockIdx.x * blockDim.x + threadIdx.x;
+   if (j >= kSortSamples) return;
+   const int64_t row = (int64_t) (mix64(0x9E3779B97F4A7C15ull + (unsigned long long) j) % (unsigned long long) total) - p.firstRow;
+   if (row < 0 || row >= p.nRows) return;
+   unsigned long long w[kSortTupleWords];
+   sortTupleOf(p, s, row, w);
+#pragma unroll
+   for (int x = 0; x < kSortTupleWords; x++) out[(size_t) j * kSortTupleWords + x] = w[x];
+}
+
+// Permute: rows ids[0..n) (ids null: rows 0..n-1) of a table of one or more batches into new single-batch columns: fixed-width cells at
+// outBytes (a narrowed decimal sign-extended, as the exchange ships it) and validity bytes by row id; a utf8 column's lengths by row id
+// (permuteCellsKernel, which also sums each CTA's bytes), the exclusive scan of the CTA sums (tableShipScanKernel), then its offsets and
+// bytes (permuteStringsKernel: each warp copies its 32 rows' strings, one contiguous range of the output, together).
+struct PermuteBatch {
+   ProgCol cols[kShipMaxCols];
+   int64_t firstRow, nRows;
+};
+struct PermuteParams {
+   const PermuteBatch* dir; // device, sorted by firstRow
+   int32_t nBatches, nCols, nStr, pad;
+   int32_t outBytes[kShipMaxCols];
+   int8_t strOf[kShipMaxCols], strCol[kShipMaxCols];
+   const uint32_t* ids;
+   int64_t n, nCtas;
+   uint8_t* data[kShipMaxCols]; // cells, or n + 1 int32 offsets (lengths until permuteStringsKernel)
+   uint8_t* valid[kShipMaxCols];
+   uint8_t* chars[kShipMaxCols];
+   unsigned long long* hist; // [nStr][nCtas]: a CTA's bytes, then (scanned) where they start
+};
+// the batch holding row `row`, as the program kernel's side-column directory is searched
+__device__ __forceinline__ const PermuteBatch& permuteBatchOf(const PermuteParams& q, int64_t row) {
+   int lo = 0, hi = q.nBatches - 1;
+   while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (q.dir[mid].firstRow <= row) lo = mid;
+      else hi = mid - 1;
+   }
+   return q.dir[lo];
+}
+__global__ void __launch_bounds__(kShipThreads) permuteCellsKernel(const __grid_constant__ PermuteParams q) {
+   __shared__ unsigned long long bytes[kShipMaxCols];
+   for (int j = threadIdx.x; j < kShipMaxCols; j += kShipThreads) bytes[j] = 0;
+   __syncthreads();
+   const int64_t begin = (int64_t) blockIdx.x * kShipTile, end = min(begin + kShipTile, q.n);
+   for (int64_t t = begin; t < end; t += kShipThreads) {
+      const int64_t i = t + threadIdx.x;
+      const bool ok = i < end;
+      const int64_t row = !ok ? 0 : q.ids ? (int64_t) q.ids[i] : i;
+      const PermuteBatch& b = permuteBatchOf(q, row);
+      const int64_t r = row - b.firstRow;
+      for (int c = 0; c < q.nCols; c++) {
+         const ProgCol& col = b.cols[c];
+         uint32_t len = 0;
+         if (ok) {
+            const bool null = colIsNull(col, r);
+            q.valid[c][i] = null ? 0 : 1;
+            if (q.strOf[c] < 0) {
+               shipCell(col, q.outBytes[c], r, q.data[c] + (size_t) i * q.outBytes[c]);
+            } else {
+               if (!null) len = (uint32_t) (((const int32_t*) col.data)[r + 1] - ((const int32_t*) col.data)[r]);
+               ((uint32_t*) q.data[c])[i] = len;
+            }
+         }
+         if (q.strOf[c] >= 0) {
+            const unsigned sum = __reduce_add_sync(0xffffffffu, len);
+            if ((threadIdx.x & 31) == 0 && sum) atomicAdd(&bytes[q.strOf[c]], (unsigned long long) sum);
+         }
+      }
+   }
+   __syncthreads();
+   for (int j = threadIdx.x; j < q.nStr; j += kShipThreads) q.hist[(size_t) j * q.nCtas + blockIdx.x] = bytes[j];
+}
+__global__ void __launch_bounds__(kShipThreads) permuteStringsKernel(const __grid_constant__ PermuteParams q) {
+   __shared__ unsigned long long warpSums[kShipWarps];
+   __shared__ unsigned long long running;
+   __shared__ uint32_t slotEnd[kShipWarps][33]; // the warp's strings: slot k at [slotEnd[k], slotEnd[k+1]) of the warp's range
+   __shared__ const uint8_t* slotSrc[kShipWarps][32];
+   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+   const int64_t begin = (int64_t) blockIdx.x * kShipTile, end = min(begin + kShipTile, q.n);
+   for (int j = 0; j < q.nStr; j++) {
+      const int c = q.strCol[j];
+      int32_t* off = (int32_t*) q.data[c];
+      uint8_t* out = q.chars[c];
+      if (threadIdx.x == 0) running = q.hist[(size_t) j * q.nCtas + blockIdx.x];
+      __syncthreads();
+      for (int64_t t = begin; t < end; t += kShipThreads) {
+         const int64_t i = t + threadIdx.x;
+         const bool ok = i < end;
+         const uint32_t len = ok ? (uint32_t) off[i] : 0u;
+         const uint8_t* src = nullptr;
+         if (ok && len) {
+            const int64_t row = q.ids ? (int64_t) q.ids[i] : i;
+            const PermuteBatch& b = permuteBatchOf(q, row);
+            const ProgCol& col = b.cols[c];
+            src = col.bytes + ((const int32_t*) col.data)[row - b.firstRow];
+         }
+         uint32_t x = len; // inclusive scan of the warp's lengths
+         for (int o = 1; o < 32; o <<= 1) {
+            const uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
+            if (lane >= o) x += y;
+         }
+         if (lane == 31) warpSums[warp] = x;
+         slotEnd[warp][lane + 1] = x;
+         if (lane == 0) slotEnd[warp][0] = 0;
+         slotSrc[warp][lane] = src;
+         __syncthreads();
+         unsigned long long warpBase = running;
+         for (int w = 0; w < warp; w++) warpBase += warpSums[w];
+         if (ok) {
+            off[i] = (int32_t) (warpBase + x - len);
+            if (i == q.n - 1) off[q.n] = (int32_t) (warpBase + x);
+         }
+         __syncwarp();
+         const uint32_t total = slotEnd[warp][32];
+         unsigned k = 0;
+         for (uint32_t a = lane; a < total; a += 32) {
+            while (slotEnd[warp][k + 1] <= a) k++;
+            out[warpBase + a] = slotSrc[warp][k][a - slotEnd[warp][k]];
+         }
+         __syncthreads();
+         if (threadIdx.x == 0)
+            for (int w = 0; w < kShipWarps; w++) running += warpSums[w];
+         __syncthreads();
+      }
+   }
+}
+
 // ---------------------------------------------------------------- dictionary unification (ldb_gpu_dict_unify, include/ldb_gpu.h)
 // This rank's exported dictionary into its block of receiver blockIdx.y's region: the offsets array and the bytes array, each padded to
 // 16 bytes, back to back, so the block is one run of 16-byte vectors.  The sources are padded the same way.
@@ -609,6 +811,11 @@ int ldb_gpu_comm_create(LdbContext* ctx, int32_t rank, int32_t world, int64_t us
       LDB_CUDA(cudaFuncGetAttributes(&fa, tableShipSendKernel));
       LDB_CUDA(cudaFuncGetAttributes(&fa, tableShipCountStrKernel));
       LDB_CUDA(cudaFuncGetAttributes(&fa, tableShipSendStrKernel));
+      LDB_CUDA(cudaFuncGetAttributes(&fa, tableShipCountRangeKernel));
+      LDB_CUDA(cudaFuncGetAttributes(&fa, tableShipCountRangeStrKernel));
+      LDB_CUDA(cudaFuncGetAttributes(&fa, sortSampleKernel));
+      LDB_CUDA(cudaFuncGetAttributes(&fa, permuteCellsKernel));
+      LDB_CUDA(cudaFuncGetAttributes(&fa, permuteStringsKernel));
       LDB_CUDA(cudaFuncGetAttributes(&fa, dictSendKernel));
       loadHashAggExchangeKernels();
       // the pinned scratch the collectives read counts into: allocating host memory can wait for running kernels, so it is taken now
@@ -911,60 +1118,78 @@ int ldb_gpu_hashagg_exchange(LdbState* local, LdbState* owned, LdbComm* c, int64
 // scratch are taken before the first collective, the output buffers after the last, and host reads go to pinned memory.
 // With utf8 columns (ldb_gpu_table_exchange_varlen) the string kernels run instead, the matrix also carries every rank's bytes per
 // (destination, utf8 column), and the host decides the int32 limit of the receivers' offsets before the capacity.
+// The sort exchange (ldb_gpu_table_sort_exchange) runs the same shipment with the range owner rule of its splitters; only the count
+// kernel differs, and what it does with the received region (sort and permute instead of copy-out).
 static_assert((size_t) kMaxPeers * kShipBlockU64 * 8 + 64 + 8 * kMaxPeers + 4 * kShipMaxCols <= LdbContext::kPinnedScratchBytes,
               "the table exchange's matrix, error word and offset ends fit the pinned scratch");
-static void tableExchange(bool varlen, LdbTable* src, int32_t n_keys, const char* const* key_columns, int32_t n_columns, const char* const* columns, LdbComm* c,
-                          int64_t recv_offset, int64_t recv_bytes, const char* name, LdbTable** out) {
-   {
-      if (!src || !c || !out || (n_keys > 0 && !key_columns)) fail(LDB_ERR_INVALID, "null argument");
-      if (n_keys < 0 || n_keys > kProgMaxKeys) fail(LDB_ERR_INVALID, "the exchange takes 0..4 key columns");
-      if (src->ctx != c->ctx) fail(LDB_ERR_INVALID, "table and comm belong to different contexts");
-      std::vector<int> ship, key;
-      if (columns) {
-         if (n_columns < 1) fail(LDB_ERR_INVALID, "columns names 1..16 columns (NULL: all columns of the table)");
-         for (int i = 0; i < n_columns; i++) {
-            const int ci = src->colIndex(columns[i]);
-            if (ci < 0) fail(LDB_ERR_INVALID, std::string("unknown column ") + (columns[i] ? columns[i] : "(null)"));
-            ship.push_back(ci);
-         }
-      } else {
-         for (int ci = 0; ci < (int) src->columns.size(); ci++) ship.push_back(ci);
+// the columns `columns` names (NULL: every column of src) as column indices of src
+static std::vector<int> shipColumns(bool varlen, LdbTable* src, int32_t n_columns, const char* const* columns) {
+   std::vector<int> ship;
+   if (columns) {
+      if (n_columns < 1) fail(LDB_ERR_INVALID, "columns names 1..16 columns (NULL: all columns of the table)");
+      for (int i = 0; i < n_columns; i++) {
+         const int ci = src->colIndex(columns[i]);
+         if (ci < 0) fail(LDB_ERR_INVALID, std::string("unknown column ") + (columns[i] ? columns[i] : "(null)"));
+         ship.push_back(ci);
       }
-      if (ship.size() > (size_t) kShipMaxCols) fail(LDB_ERR_INVALID, "the exchange ships up to 16 columns");
-      for (int ci : ship)
-         if (!varlen && src->columns[ci].type == LDB_UTF8) fail(LDB_ERR_UNSUPPORTED, "the exchange ships fixed-width columns (utf8 column " + src->columns[ci].name + ")");
-      for (int k = 0; k < n_keys; k++) {
-         const int ci = src->colIndex(key_columns[k]);
-         if (ci < 0) fail(LDB_ERR_INVALID, std::string("unknown key column ") + (key_columns[k] ? key_columns[k] : "(null)"));
-         const int type = src->columns[ci].type;
-         if (type == LDB_UTF8 || type == LDB_FLOAT32 || type == LDB_FLOAT64) fail(LDB_ERR_UNSUPPORTED, "exchange keys are integer, date, char(1) or decimal columns");
-         key.push_back(ci);
-      }
-      wantConnected(c);
-      if (recv_offset < 0 || recv_bytes < 0 || recv_offset % 16 || recv_offset > (int64_t) c->userBytes || recv_bytes > (int64_t) c->userBytes - recv_offset)
-         fail(LDB_ERR_INVALID, "receive region outside the comm's user heap or not 16-byte aligned");
-      LdbContext* ctx = c->ctx;
-      if (ctx->capturing) fail(LDB_ERR_UNSUPPORTED, "the table exchange reads the row counts on the host and cannot be captured");
+   } else {
+      for (int ci = 0; ci < (int) src->columns.size(); ci++) ship.push_back(ci);
+   }
+   if (ship.size() > (size_t) kShipMaxCols) fail(LDB_ERR_INVALID, "the exchange ships up to 16 columns");
+   for (int ci : ship)
+      if (!varlen && src->columns[ci].type == LDB_UTF8) fail(LDB_ERR_UNSUPPORTED, "the exchange ships fixed-width columns (utf8 column " + src->columns[ci].name + ")");
+   return ship;
+}
+static void wantRegion(LdbComm* c, int64_t recv_offset, int64_t recv_bytes) {
+   if (recv_offset < 0 || recv_bytes < 0 || recv_offset % 16 || recv_offset > (int64_t) c->userBytes || recv_bytes > (int64_t) c->userBytes - recv_offset)
+      fail(LDB_ERR_INVALID, "receive region outside the comm's user heap or not 16-byte aligned");
+}
+static int32_t shipCellBytes(int type) {
+   switch (type) {
+      case LDB_INT8: return 1;
+      case LDB_INT16: return 2;
+      case LDB_INT64:
+      case LDB_FLOAT64: return 8;
+      case LDB_DECIMAL128: return 16;
+      default: return 4; // int32, date32, fsb4, float32
+   }
+}
+
+// One shipment of a table's rows, for arguments the caller checked.  The constructor takes what a rank needs before its first collective
+// (staging waits, temporaries, pinned scratch); ship() counts under an owner rule (the key hash, or the splitters of a sort) and runs the
+// protocol up to the second barrier, after which this rank's region holds its `mine` received rows at colOff / bytesOff / validOff;
+// finish() waits for the work queued after it and reports a peer that timed out.
+struct TableShipment {
+   LdbTable* src;
+   LdbComm* c;
+   LdbContext* ctx;
+   int world;
+   std::vector<int> ship, key;
+   int nCols, nStr = 0;
+   int32_t outBytes[kShipMaxCols] = {};
+   int8_t strCol[kShipMaxCols] = {}, strOf[kShipMaxCols] = {};
+   bool broadcast, strings;
+   size_t blockU64;
+   int64_t nCtas = 0;
+   Scratch tmp;
+   unsigned long long *hist, *totals, *matrix, *upload;
+   int32_t* timedOut;
+   uint32_t* offEnds;
+   TableShipBatch p{};
+   int64_t recvOffset, regionBytes;
+   unsigned long long mine = 0;
+   uint64_t colOff[kShipMaxCols], validOff[kShipMaxCols], bytesOff[kShipMaxCols];
+   uint8_t* region = nullptr;
+
+   TableShipment(LdbTable* s, std::vector<int> shipped, std::vector<int> keys, LdbComm* comm, int64_t recv_offset, int64_t recv_bytes)
+       : src(s), c(comm), ctx(comm->ctx), world(comm->world), ship(std::move(shipped)), key(std::move(keys)), nCols((int) ship.size()), tmp(comm->ctx),
+         recvOffset(recv_offset), regionBytes(recv_bytes) {
       LDB_CUDA(cudaSetDevice(ctx->device));
-      const int world = c->world, nCols = (int) ship.size();
-      int32_t outBytes[kShipMaxCols] = {};
-      for (int j = 0; j < nCols; j++) {
-         switch (src->columns[ship[j]].type) {
-            case LDB_INT8: outBytes[j] = 1; break;
-            case LDB_INT16: outBytes[j] = 2; break;
-            case LDB_INT64:
-            case LDB_FLOAT64: outBytes[j] = 8; break;
-            case LDB_DECIMAL128: outBytes[j] = 16; break;
-            default: outBytes[j] = 4; // int32, date32, fsb4, float32
-         }
-      }
+      for (int j = 0; j < nCols; j++) outBytes[j] = shipCellBytes(src->columns[ship[j]].type);
       // before the first collective: staging waits, temporaries, pinned scratch
       for (auto& b : src->batches) ldb_gpu_wait_batch_internal(ctx, &b);
-      int64_t nCtas = 0;
       for (auto& b : src->batches) nCtas += (b.nRows + kShipTile - 1) / kShipTile;
       // the utf8 columns among the shipped ones: they select the string kernels, whose histograms have world (1 + nStr) rows
-      int nStr = 0;
-      int8_t strCol[kShipMaxCols], strOf[kShipMaxCols];
       for (int j = 0; j < nCols; j++) {
          strOf[j] = -1;
          if (src->columns[ship[j]].type == LDB_UTF8) {
@@ -972,20 +1197,18 @@ static void tableExchange(bool varlen, LdbTable* src, int32_t n_keys, const char
             strCol[nStr++] = (int8_t) j;
          }
       }
-      const bool strings = nStr > 0;
-      const size_t blockU64 = (size_t) kMaxPeers * (1 + nStr); // this rank's totals in the all-gather: rows, then bytes per (d, column)
-      Scratch tmp(ctx);
-      const bool broadcast = n_keys == 0;
+      strings = nStr > 0;
+      blockU64 = (size_t) kMaxPeers * (1 + nStr); // this rank's totals in the all-gather: rows, then bytes per (d, column)
+      broadcast = key.empty();
       uint8_t* owners = broadcast ? nullptr : tmp.alloc<uint8_t>((size_t) std::max<int64_t>(src->numRows, 1));
-      unsigned long long* hist = broadcast && !strings ? nullptr : tmp.alloc<unsigned long long>((size_t) std::max<int64_t>(nCtas, 1) * world * (1 + nStr) * 8);
-      unsigned long long* totals = tmp.alloc<unsigned long long>(8 * blockU64);
-      unsigned long long* matrix = (unsigned long long*) ctx->scratch(); // [world][blockU64]: M[s][d] at [s][d], Bytes[s][d][j] at [s][world + d nStr + j]
-      int32_t* timedOut = (int32_t*) (matrix + kMaxPeers * kShipBlockU64);
-      unsigned long long* upload = matrix + kMaxPeers * kShipBlockU64 + 8;
-      uint32_t* offEnds = (uint32_t*) (upload + kMaxPeers); // B_j of this rank: the last offset of each received utf8 column
-      TableShipBatch p{};
+      hist = broadcast && !strings ? nullptr : tmp.alloc<unsigned long long>((size_t) std::max<int64_t>(nCtas, 1) * world * (1 + nStr) * 8);
+      totals = tmp.alloc<unsigned long long>(8 * blockU64);
+      matrix = (unsigned long long*) ctx->scratch(); // [world][blockU64]: M[s][d] at [s][d], Bytes[s][d][j] at [s][world + d nStr + j]
+      timedOut = (int32_t*) (matrix + kMaxPeers * kShipBlockU64);
+      upload = matrix + kMaxPeers * kShipBlockU64 + 8;
+      offEnds = (uint32_t*) (upload + kMaxPeers); // B_j of this rank: the last offset of each received utf8 column
       p.nCols = nCols;
-      p.nKeys = n_keys;
+      p.nKeys = (int32_t) key.size();
       p.world = world;
       p.broadcast = broadcast ? 1 : 0;
       p.nCtas = nCtas;
@@ -995,30 +1218,45 @@ static void tableExchange(bool varlen, LdbTable* src, int32_t n_keys, const char
       p.nStr = nStr;
       for (int j = 0; j < nCols; j++) p.strOf[j] = strOf[j];
       for (int j = 0; j < nStr; j++) p.strCol[j] = strCol[j];
-      auto bindBatch = [&](const LdbBatch& b, int64_t firstRow, int64_t ctaBase) {
-         TableShipBatch q = p;
-         for (int j = 0; j < nCols; j++) {
-            bindColumn(q.cols[j], b, ship[j]);
-            q.cols[j].type = src->columns[ship[j]].type;
-         }
-         for (int k = 0; k < n_keys; k++) {
-            bindColumn(q.keys[k], b, key[k]);
-            q.keys[k].type = src->columns[key[k]].type;
-         }
-         q.nRows = b.nRows;
-         q.firstRow = firstRow;
-         q.ctaBase = ctaBase;
-         return q;
-      };
-      // every non-empty batch with its source row number and first CTA, in source order
-      auto eachBatch = [&](const std::function<void(const TableShipBatch&, int)>& fn) {
-         int64_t first = 0, cta = 0;
-         for (auto& b : src->batches) {
-            if (b.nRows > 0) fn(bindBatch(b, first, cta), (int) ((b.nRows + kShipTile - 1) / kShipTile));
-            first += b.nRows;
-            cta += (b.nRows + kShipTile - 1) / kShipTile;
-         }
-      };
+   }
+   TableShipBatch bindBatch(const LdbBatch& b, int64_t firstRow, int64_t ctaBase) const {
+      TableShipBatch q = p;
+      for (int j = 0; j < nCols; j++) {
+         bindColumn(q.cols[j], b, ship[j]);
+         q.cols[j].type = src->columns[ship[j]].type;
+      }
+      for (int k = 0; k < (int) key.size(); k++) {
+         bindColumn(q.keys[k], b, key[k]);
+         q.keys[k].type = src->columns[key[k]].type;
+      }
+      q.nRows = b.nRows;
+      q.firstRow = firstRow;
+      q.ctaBase = ctaBase;
+      return q;
+   }
+   // every non-empty batch with its source row number and first CTA, in source order
+   void eachBatch(const std::function<void(const TableShipBatch&, int)>& fn) const {
+      int64_t first = 0, cta = 0;
+      for (auto& b : src->batches) {
+         if (b.nRows > 0) fn(bindBatch(b, first, cta), (int) ((b.nRows + kShipTile - 1) / kShipTile));
+         first += b.nRows;
+         cta += (b.nRows + kShipTile - 1) / kShipTile;
+      }
+   }
+   void barrier() {
+      if (world == 1) return;
+      ctx->launch("peer_barrier", [&] {
+         peerBarrierKernel<<<world, 32, 0, ctx->compute>>>(c->view());
+         peerBumpKernel<<<1, 1, 0, ctx->compute>>>(c->view(), EPOCH_BARRIER, -1);
+      });
+   }
+   void checkPeers() {
+      LDB_CUDA(cudaMemcpyAsync(timedOut, c->error, 4, cudaMemcpyDeviceToHost, ctx->compute));
+      ctx->syncStream(ctx->compute);
+      if (*timedOut) fail(LDB_ERR_CUDA, "a peer did not arrive at a collective within the timeout (LDB_PEER_TIMEOUT_MS)");
+   }
+   // range: the owner rule of the sort exchange's splitters (null: the key hash, or every rank without keys)
+   void run(const SortSplit* range) {
       if (broadcast && !strings) {
          for (int d = 0; d < kMaxPeers; d++) upload[d] = d < world ? (unsigned long long) src->numRows : 0ull;
          LDB_CUDA(cudaMemcpyAsync(totals, upload, 8 * kMaxPeers, cudaMemcpyHostToDevice, ctx->compute));
@@ -1026,7 +1264,9 @@ static void tableExchange(bool varlen, LdbTable* src, int32_t n_keys, const char
          ctx->launch("table_exchange_count", [&] {
             LDB_CUDA(cudaMemsetAsync(totals, 0, 8 * blockU64, ctx->compute));
             eachBatch([&](const TableShipBatch& q, int grid) {
-               if (strings) tableShipCountStrKernel<<<grid, kShipThreads, 0, ctx->compute>>>(q);
+               if (range && strings) tableShipCountRangeStrKernel<<<grid, kShipThreads, 0, ctx->compute>>>(q, *range);
+               else if (range) tableShipCountRangeKernel<<<grid, kShipThreads, 0, ctx->compute>>>(q, *range);
+               else if (strings) tableShipCountStrKernel<<<grid, kShipThreads, 0, ctx->compute>>>(q);
                else tableShipCountKernel<<<grid, kShipThreads, 0, ctx->compute>>>(q);
             });
             tableShipScanKernel<<<world * (1 + nStr), 1024, 0, ctx->compute>>>(hist, nCtas, totals);
@@ -1039,9 +1279,7 @@ static void tableExchange(bool varlen, LdbTable* src, int32_t n_keys, const char
          const uint8_t* gathered = allGatherSmall(c, totals, 8 * blockU64);
          LDB_CUDA(cudaMemcpy2DAsync(matrix, 8 * blockU64, gathered, kSlotBytes, 8 * blockU64, world, cudaMemcpyDeviceToHost, ctx->compute));
       }
-      LDB_CUDA(cudaMemcpyAsync(timedOut, c->error, 4, cudaMemcpyDeviceToHost, ctx->compute));
-      ctx->syncStream(ctx->compute);
-      if (*timedOut) fail(LDB_ERR_CUDA, "a peer did not arrive at a collective within the timeout (LDB_PEER_TIMEOUT_MS)");
+      checkPeers();
       // per receiver, from the same matrix on every rank: its rows and bytes, this source's bases in them, then the two decisions.  A
       // broadcast counted every row for destination 0, and every rank receives what destination 0 would.
       auto rowsOf = [&](int s, int d) { return matrix[s * blockU64 + (broadcast ? 0 : d)]; };
@@ -1066,23 +1304,16 @@ static void tableExchange(bool varlen, LdbTable* src, int32_t n_keys, const char
             if (recvBytes[d][j] > (uint64_t) INT32_MAX)
                fail(LDB_ERR_UNSUPPORTED, "table exchange: rank " + std::to_string(d) + " would receive " + std::to_string(recvBytes[d][j]) + " bytes of utf8 column " +
                                             src->columns[ship[strCol[j]]].name + ", more than 2^31 - 1 (utf8 offsets are int32)");
-      uint64_t colOff[kShipMaxCols], validOff[kShipMaxCols], bytesOff[kShipMaxCols], need = 0;
+      uint64_t need = 0;
       for (int d = 0; d < world; d++) {
          for (int j = 0; j < nStr; j++) p.strBytes[d][j] = (uint32_t) recvBytes[d][j];
          need = std::max(need, shipLayoutVar(p.rows[d], outBytes, nCols, strOf, nStr, p.strBytes[d], colOff, validOff, bytesOff));
       }
-      if (need > (uint64_t) recv_bytes)
+      if (need > (uint64_t) regionBytes)
          fail(LDB_ERR_CAPACITY, "table exchange: a rank receives rows that need " + std::to_string(need) + " bytes of receive region, more than recv_bytes " +
-                                   std::to_string(recv_bytes) + "; retry with recv_bytes " + std::to_string(need));
-      const unsigned long long mine = p.rows[c->rank];
-      for (int d = 0; d < world; d++) p.recv[d] = c->peerHeap[d] + kUserOff + recv_offset;
-      auto barrier = [&] {
-         if (world == 1) return;
-         ctx->launch("peer_barrier", [&] {
-            peerBarrierKernel<<<world, 32, 0, ctx->compute>>>(c->view());
-            peerBumpKernel<<<1, 1, 0, ctx->compute>>>(c->view(), EPOCH_BARRIER, -1);
-         });
-      };
+                                   std::to_string(regionBytes) + "; retry with recv_bytes " + std::to_string(need));
+      mine = p.rows[c->rank];
+      for (int d = 0; d < world; d++) p.recv[d] = c->peerHeap[d] + kUserOff + recvOffset;
       barrier(); // no peer still copies out of, or otherwise reads, the region it is about to receive into
       ctx->launch("table_exchange_send", [&] {
          eachBatch([&](const TableShipBatch& q, int grid) {
@@ -1101,46 +1332,84 @@ static void tableExchange(bool varlen, LdbTable* src, int32_t n_keys, const char
          });
       });
       barrier(); // every peer's rows are in this rank's region
-      // copy-out into buffers the new table owns: one device-to-device copy per array.  A utf8 column's last offset is B_j, which the
-      // matrix gave: it is written into the region first, so the n + 1 offsets are one copy too.
       shipLayoutVar(mine, outBytes, nCols, strOf, nStr, p.strBytes[c->rank], colOff, validOff, bytesOff);
-      Scratch cols(ctx);
-      std::vector<LdbColumn> outCols;
-      LdbBatch ob;
-      ob.nRows = (int64_t) mine;
-      uint8_t* region = c->heap + kUserOff + recv_offset;
-      ctx->launch("table_exchange_copy", [&] {
-         for (int j = 0; j < nCols; j++) {
-            const LdbColumn& sc = src->columns[ship[j]];
-            outCols.push_back({sc.name, sc.type, sc.precision, sc.scale});
-            const int sj = strOf[j];
-            const size_t bytes = sj >= 0 ? ((size_t) mine + 1) * 4 : (size_t) mine * outBytes[j];
-            uint8_t* data = cols.alloc<uint8_t>(std::max<size_t>(bytes, 16));
-            uint8_t* valid = cols.alloc<uint8_t>(std::max<size_t>(mine, 16));
-            uint8_t* chars = nullptr;
-            if (sj >= 0) {
-               const size_t nb = p.strBytes[c->rank][sj];
-               chars = cols.alloc<uint8_t>(std::max<size_t>(nb, 16));
-               offEnds[sj] = (uint32_t) nb;
-               LDB_CUDA(cudaMemcpyAsync(region + colOff[j] + mine * 4, &offEnds[sj], 4, cudaMemcpyHostToDevice, ctx->compute));
-               LDB_CUDA(cudaMemcpyAsync(data, region + colOff[j], bytes, cudaMemcpyDeviceToDevice, ctx->compute));
-               if (nb) LDB_CUDA(cudaMemcpyAsync(chars, region + bytesOff[sj], nb, cudaMemcpyDeviceToDevice, ctx->compute));
-            }
-            if (mine) {
-               if (sj < 0) LDB_CUDA(cudaMemcpyAsync(data, region + colOff[j], bytes, cudaMemcpyDeviceToDevice, ctx->compute));
-               LDB_CUDA(cudaMemcpyAsync(valid, region + validOff[j], (size_t) mine, cudaMemcpyDeviceToDevice, ctx->compute));
-            }
-            ob.data.push_back(data);
-            ob.bytes.push_back(chars);
-            ob.elemBytes.push_back(outBytes[j]);
-            ob.validBytes.push_back(valid);
-         }
-      });
-      LDB_CUDA(cudaMemcpyAsync(timedOut, c->error, 4, cudaMemcpyDeviceToHost, ctx->compute));
-      ctx->syncStream(ctx->compute); // the region is free for the next collective, the temporaries for the pool
-      if (*timedOut) fail(LDB_ERR_CUDA, "a peer did not arrive at a collective within the timeout (LDB_PEER_TIMEOUT_MS)");
-      *out = addResultTable(ctx, name ? name : "received", std::move(outCols), std::move(ob), cols);
+      region = c->heap + kUserOff + recvOffset;
+      // a utf8 column's last offset is B_j, which the matrix gave: written into the region, its n + 1 offsets are one array
+      for (int j = 0; j < nStr; j++) {
+         offEnds[j] = p.strBytes[c->rank][j];
+         LDB_CUDA(cudaMemcpyAsync(region + colOff[strCol[j]] + mine * 4, &offEnds[j], 4, cudaMemcpyHostToDevice, ctx->compute));
+      }
    }
+   // the received rows as a single-batch table over the region (valid until finish())
+   void receivedView(LdbTable& v) const {
+      v.ctx = ctx;
+      v.numRows = (int64_t) mine;
+      v.batches.resize(1);
+      LdbBatch& b = v.batches[0];
+      b.nRows = (int64_t) mine;
+      for (int j = 0; j < nCols; j++) {
+         v.columns.push_back(src->columns[ship[j]]);
+         b.data.push_back(region + colOff[j]);
+         b.bytes.push_back(strOf[j] >= 0 ? region + bytesOff[strOf[j]] : nullptr);
+         b.elemBytes.push_back(outBytes[j]);
+         b.validBytes.push_back(region + validOff[j]);
+      }
+   }
+   void finish() { checkPeers(); } // the region is free for the next collective, the temporaries for the pool
+};
+
+static void tableExchange(bool varlen, LdbTable* src, int32_t n_keys, const char* const* key_columns, int32_t n_columns, const char* const* columns, LdbComm* c,
+                          int64_t recv_offset, int64_t recv_bytes, const char* name, LdbTable** out) {
+   if (!src || !c || !out || (n_keys > 0 && !key_columns)) fail(LDB_ERR_INVALID, "null argument");
+   if (n_keys < 0 || n_keys > kProgMaxKeys) fail(LDB_ERR_INVALID, "the exchange takes 0..4 key columns");
+   if (src->ctx != c->ctx) fail(LDB_ERR_INVALID, "table and comm belong to different contexts");
+   std::vector<int> ship = shipColumns(varlen, src, n_columns, columns), key;
+   for (int k = 0; k < n_keys; k++) {
+      const int ci = src->colIndex(key_columns[k]);
+      if (ci < 0) fail(LDB_ERR_INVALID, std::string("unknown key column ") + (key_columns[k] ? key_columns[k] : "(null)"));
+      const int type = src->columns[ci].type;
+      if (type == LDB_UTF8 || type == LDB_FLOAT32 || type == LDB_FLOAT64) fail(LDB_ERR_UNSUPPORTED, "exchange keys are integer, date, char(1) or decimal columns");
+      key.push_back(ci);
+   }
+   wantConnected(c);
+   wantRegion(c, recv_offset, recv_bytes);
+   LdbContext* ctx = c->ctx;
+   if (ctx->capturing) fail(LDB_ERR_UNSUPPORTED, "the table exchange reads the row counts on the host and cannot be captured");
+   TableShipment s(src, std::move(ship), std::move(key), c, recv_offset, recv_bytes);
+   s.run(nullptr);
+   // copy-out into buffers the new table owns: one device-to-device copy per array
+   const unsigned long long mine = s.mine;
+   Scratch cols(ctx);
+   std::vector<LdbColumn> outCols;
+   LdbBatch ob;
+   ob.nRows = (int64_t) mine;
+   ctx->launch("table_exchange_copy", [&] {
+      for (int j = 0; j < s.nCols; j++) {
+         const LdbColumn& sc = src->columns[s.ship[j]];
+         outCols.push_back({sc.name, sc.type, sc.precision, sc.scale});
+         const int sj = s.strOf[j];
+         const size_t bytes = sj >= 0 ? ((size_t) mine + 1) * 4 : (size_t) mine * s.outBytes[j];
+         uint8_t* data = cols.alloc<uint8_t>(std::max<size_t>(bytes, 16));
+         uint8_t* valid = cols.alloc<uint8_t>(std::max<size_t>(mine, 16));
+         uint8_t* chars = nullptr;
+         if (sj >= 0) {
+            const size_t nb = s.p.strBytes[c->rank][sj];
+            chars = cols.alloc<uint8_t>(std::max<size_t>(nb, 16));
+            LDB_CUDA(cudaMemcpyAsync(data, s.region + s.colOff[j], bytes, cudaMemcpyDeviceToDevice, ctx->compute));
+            if (nb) LDB_CUDA(cudaMemcpyAsync(chars, s.region + s.bytesOff[sj], nb, cudaMemcpyDeviceToDevice, ctx->compute));
+         }
+         if (mine) {
+            if (sj < 0) LDB_CUDA(cudaMemcpyAsync(data, s.region + s.colOff[j], bytes, cudaMemcpyDeviceToDevice, ctx->compute));
+            LDB_CUDA(cudaMemcpyAsync(valid, s.region + s.validOff[j], (size_t) mine, cudaMemcpyDeviceToDevice, ctx->compute));
+         }
+         ob.data.push_back(data);
+         ob.bytes.push_back(chars);
+         ob.elemBytes.push_back(s.outBytes[j]);
+         ob.validBytes.push_back(valid);
+      }
+   });
+   s.finish();
+   *out = addResultTable(ctx, name ? name : "received", std::move(outCols), std::move(ob), cols);
 }
 int ldb_gpu_table_exchange(LdbTable* src, int32_t n_keys, const char* const* key_columns, int32_t n_columns, const char* const* columns, LdbComm* c,
                            int64_t recv_offset, int64_t recv_bytes, const char* name, LdbTable** out, LdbError* err) {
@@ -1149,6 +1418,235 @@ int ldb_gpu_table_exchange(LdbTable* src, int32_t n_keys, const char* const* key
 int ldb_gpu_table_exchange_varlen(LdbTable* src, int32_t n_keys, const char* const* key_columns, int32_t n_columns, const char* const* columns, LdbComm* c,
                                   int64_t recv_offset, int64_t recv_bytes, const char* name, LdbTable** out, LdbError* err) {
    return guarded(err, [&] { tableExchange(true, src, n_keys, key_columns, n_columns, columns, c, recv_offset, recv_bytes, name, out); });
+}
+
+// Rows ids[0..n) (null: 0..n-1) of columns `cols` of `t` (any number of batches) into new single-batch buffers of `bufs`, cells at
+// outBytes: the permute kernels, with a host read of each utf8 column's byte total in between (it sizes the bytes array).  Returns the
+// batch (nRows, data, bytes, elemBytes, validBytes); synchronises.
+static LdbBatch permuteRows(LdbTable* t, const std::vector<int>& cols, const int32_t* outBytes, const uint32_t* ids, int64_t n, Scratch& bufs) {
+   LdbContext* ctx = t->ctx;
+   Scratch tmp(ctx);
+   PermuteParams q{};
+   q.nCols = (int32_t) cols.size();
+   q.ids = ids;
+   q.n = n;
+   q.nCtas = (n + kShipTile - 1) / kShipTile;
+   std::vector<PermuteBatch> dir;
+   int64_t first = 0;
+   for (auto& b : t->batches) {
+      if (b.nRows > 0) {
+         PermuteBatch pb{};
+         for (int j = 0; j < q.nCols; j++) {
+            bindColumn(pb.cols[j], b, cols[j]);
+            pb.cols[j].type = t->columns[cols[j]].type;
+         }
+         pb.firstRow = first;
+         pb.nRows = b.nRows;
+         dir.push_back(pb);
+      }
+      first += b.nRows;
+   }
+   q.nBatches = (int32_t) dir.size();
+   LdbBatch ob;
+   ob.nRows = n;
+   for (int j = 0; j < q.nCols; j++) {
+      const bool str = t->columns[cols[j]].type == LDB_UTF8;
+      q.outBytes[j] = outBytes[j];
+      q.strOf[j] = (int8_t) (str ? q.nStr : -1);
+      if (str) q.strCol[q.nStr++] = (int8_t) j;
+      q.data[j] = bufs.alloc<uint8_t>(std::max<size_t>(str ? ((size_t) n + 1) * 4 : (size_t) n * outBytes[j], 16));
+      q.valid[j] = bufs.alloc<uint8_t>(std::max<size_t>((size_t) n, 16));
+      if (str && n == 0) LDB_CUDA(cudaMemsetAsync(q.data[j], 0, 4, ctx->compute));
+   }
+   unsigned long long* totals = (unsigned long long*) ((uint8_t*) ctx->scratch() + LdbContext::kPinnedScratchBytes) - kShipMaxCols;
+   if (n > 0) {
+      PermuteBatch* dd = tmp.alloc<PermuteBatch>(dir.size() * sizeof(PermuteBatch));
+      LDB_CUDA(cudaMemcpyAsync(dd, dir.data(), dir.size() * sizeof(PermuteBatch), cudaMemcpyHostToDevice, ctx->compute));
+      q.dir = dd;
+      q.hist = tmp.alloc<unsigned long long>((size_t) std::max(q.nStr, 1) * (size_t) q.nCtas * 8);
+      unsigned long long* devTotals = tmp.alloc<unsigned long long>(kShipMaxCols * 8);
+      ctx->launch("sort_exchange_permute", [&] {
+         permuteCellsKernel<<<(unsigned) q.nCtas, kShipThreads, 0, ctx->compute>>>(q);
+         if (q.nStr) {
+            tableShipScanKernel<<<q.nStr, 1024, 0, ctx->compute>>>(q.hist, q.nCtas, devTotals);
+            LDB_CUDA(cudaMemcpyAsync(totals, devTotals, 8 * (size_t) q.nStr, cudaMemcpyDeviceToHost, ctx->compute));
+         }
+      });
+      ctx->syncStream(ctx->compute);
+   }
+   for (int j = 0; j < q.nCols; j++) {
+      const int sj = q.strOf[j];
+      const uint64_t nb = sj >= 0 && n > 0 ? totals[sj] : 0;
+      if (nb > (uint64_t) INT32_MAX)
+         fail(LDB_ERR_UNSUPPORTED, "sort exchange: " + std::to_string(nb) + " bytes of utf8 column " + t->columns[cols[j]].name + " in one table, more than 2^31 - 1 (utf8 offsets are int32)");
+      q.chars[j] = sj >= 0 ? bufs.alloc<uint8_t>(std::max<size_t>(nb, 16)) : nullptr;
+      ob.data.push_back(q.data[j]);
+      ob.bytes.push_back(q.chars[j]);
+      ob.elemBytes.push_back(outBytes[j]);
+      ob.validBytes.push_back(q.valid[j]);
+   }
+   if (n > 0 && q.nStr) ctx->launch("sort_exchange_permute", [&] { permuteStringsKernel<<<(unsigned) q.nCtas, kShipThreads, 0, ctx->compute>>>(q); });
+   ctx->syncStream(ctx->compute); // the directory and the CTA sums go back to the pool
+   return ob;
+}
+// the stable sort of a table of any number of batches by its key columns (index, descending): row ids global to the table, in `scratch`.
+// A single batch is sorted where it is; otherwise the keys are first permuted into one batch (16-byte decimal cells), whose order is the
+// same: sortRows composes a key's words from its canonical value (sortCell).
+static uint32_t* sortTableRows(Scratch& scratch, LdbTable* t, const std::vector<std::pair<int, int>>& keys) {
+   if (t->batches.size() == 1) return sortRows(scratch, t, keys, t->numRows);
+   std::vector<int> cols;
+   std::vector<int32_t> widths;
+   std::vector<std::pair<int, int>> at;
+   LdbTable k{};
+   k.ctx = t->ctx;
+   k.numRows = t->numRows;
+   for (auto& kc : keys) {
+      at.push_back({(int) cols.size(), kc.second});
+      cols.push_back(kc.first);
+      widths.push_back(shipCellBytes(t->columns[kc.first].type));
+      k.columns.push_back(t->columns[kc.first]);
+   }
+   k.batches.push_back(permuteRows(t, cols, widths.data(), nullptr, t->numRows, scratch));
+   return sortRows(scratch, &k, at, t->numRows);
+}
+
+// Rows in global order (include/ldb_gpu.h).  Without LIMIT: samples of every rank's canonical tuples → all-gather → the same splitters
+// on every rank (host) → the table shipment with the range owner rule → sort of the received rows by the keys (the received order,
+// source rank then source row, breaks ties) → permute from the region into the new table.  With LIMIT: a local sort and permute of
+// the rank's first `limit` rows → the shipment of those rows to rank 0 (every splitter above every tuple) → rank 0 sorts them and
+// keeps the first `limit`.
+static_assert((size_t) kMaxPeers * kSortBlockBytes + 8 * kShipMaxCols + 64 <= LdbContext::kPinnedScratchBytes, "every rank's samples fit the pinned scratch");
+static_assert(sizeof(TableShipBatch) + sizeof(SortSplit) <= 4096, "the range count kernels' parameters");
+static void sortExchange(LdbTable* src, int32_t n_keys, const char* const* key_columns, const int32_t* descending, int32_t n_columns, const char* const* columns,
+                         int64_t limit, LdbComm* c, int64_t recv_offset, int64_t recv_bytes, const char* name, LdbTable** out, int64_t* first_row,
+                         int64_t* total_rows) {
+   int devices = 0;
+   if (cudaGetDeviceCount(&devices) != cudaSuccess || devices == 0) {
+      cudaGetLastError();
+      fail(LDB_ERR_NO_DEVICE, "no CUDA device available: the GPU operator runtime has no CPU fallback");
+   }
+   if (!src || !c || !out || !key_columns || !descending || !first_row || !total_rows) fail(LDB_ERR_INVALID, "null argument");
+   if (n_keys < 1 || n_keys > kProgMaxKeys) fail(LDB_ERR_INVALID, "the sort exchange takes 1..4 key columns");
+   if (src->ctx != c->ctx) fail(LDB_ERR_INVALID, "table and comm belong to different contexts");
+   std::vector<int> ship = shipColumns(true, src, n_columns, columns), key, keyAt;
+   const int nUser = (int) ship.size();
+   for (int k = 0; k < n_keys; k++) {
+      const int ci = src->colIndex(key_columns[k]);
+      if (ci < 0) fail(LDB_ERR_INVALID, std::string("unknown key column ") + (key_columns[k] ? key_columns[k] : "(null)"));
+      const int type = src->columns[ci].type;
+      if (type != LDB_INT32 && type != LDB_DATE32 && type != LDB_FSB4 && type != LDB_INT64 && type != LDB_DECIMAL128)
+         fail(LDB_ERR_UNSUPPORTED, "sort exchange keys are int32, date32, char(1), int64 or decimal columns (column " + src->columns[ci].name + ")");
+      key.push_back(ci);
+      const int at = (int) (std::find(ship.begin(), ship.end(), ci) - ship.begin());
+      if (at == (int) ship.size()) ship.push_back(ci); // a key that is not shipped travels as a hidden column
+      keyAt.push_back(at);
+   }
+   if (ship.size() > (size_t) kShipMaxCols) fail(LDB_ERR_INVALID, "the sort exchange ships up to 16 columns, key columns not among them included");
+   wantConnected(c);
+   wantRegion(c, recv_offset, recv_bytes);
+   LdbContext* ctx = c->ctx;
+   if (ctx->capturing) fail(LDB_ERR_UNSUPPORTED, "the sort exchange reads row counts and samples on the host and cannot be captured");
+   LDB_CUDA(cudaSetDevice(ctx->device));
+   if (src->numRows >= (int64_t) 1 << 32) fail(LDB_ERR_UNSUPPORTED, "the sort exchange sorts up to 2^32 - 1 rows per rank");
+   for (auto& b : src->batches) ldb_gpu_wait_batch_internal(ctx, &b);
+   const int world = c->world;
+   std::vector<std::pair<int, int>> order; // (column of the received rows, descending)
+   for (int k = 0; k < n_keys; k++) order.push_back({keyAt[k], descending[k] ? 1 : 0});
+   SortSplit split{};
+   split.nKeys = n_keys;
+   split.nSplit = world - 1;
+   split.rank = c->rank;
+   for (int k = 0; k < n_keys; k++) split.desc[k] = descending[k] ? 1 : 0;
+   Scratch local(ctx);
+   LdbTable top{}; // LIMIT: this rank's first `limit` rows in order, the shipped columns
+   LdbTable* from = src;
+   std::vector<int> fromCols = ship, fromKeys = key;
+   if (limit >= 0) {
+      const int64_t m = std::min<int64_t>(limit, src->numRows);
+      std::vector<std::pair<int, int>> keys;
+      for (int k = 0; k < n_keys; k++) keys.push_back({key[k], split.desc[k]});
+      const uint32_t* ids = m ? sortTableRows(local, src, keys) : nullptr;
+      int32_t widths[kShipMaxCols];
+      for (size_t j = 0; j < ship.size(); j++) widths[j] = shipCellBytes(src->columns[ship[j]].type);
+      top.ctx = ctx;
+      top.numRows = m;
+      for (int ci : ship) top.columns.push_back(src->columns[ci]);
+      top.batches.push_back(permuteRows(src, ship, widths, ids, m, local));
+      from = &top;
+      for (size_t j = 0; j < ship.size(); j++) fromCols[j] = (int) j;
+      for (int k = 0; k < n_keys; k++) fromKeys[k] = keyAt[k];
+      for (auto& w : split.split) // every tuple goes below every splitter: to rank 0
+         for (auto& x : w) x = ~0ull;
+   }
+   TableShipment s(from, fromCols, fromKeys, c, recv_offset, recv_bytes);
+   if (limit < 0) {
+      unsigned long long* block = s.tmp.alloc<unsigned long long>(kSortBlockBytes);
+      unsigned long long* pin = (unsigned long long*) ctx->scratch();
+      unsigned long long* hdr = (unsigned long long*) ((uint8_t*) pin + LdbContext::kPinnedScratchBytes) - kShipMaxCols - 8;
+      const int64_t n = src->numRows;
+      hdr[0] = (unsigned long long) n;
+      hdr[1] = n > 0 ? kSortSamples : 0;
+      ctx->launch("sort_exchange_sample", [&] {
+         LDB_CUDA(cudaMemcpyAsync(block, hdr, 16, cudaMemcpyHostToDevice, ctx->compute));
+         s.eachBatch([&](const TableShipBatch& q, int) { sortSampleKernel<<<kSortSamples / 256, 256, 0, ctx->compute>>>(q, split, n, block + 2); });
+      });
+      if (world == 1) {
+         LDB_CUDA(cudaMemcpyAsync(pin, block, kSortBlockBytes, cudaMemcpyDeviceToHost, ctx->compute));
+      } else {
+         const uint8_t* gathered = allGatherSmall(c, block, kSortBlockBytes);
+         LDB_CUDA(cudaMemcpy2DAsync(pin, kSortBlockBytes, gathered, kSlotBytes, kSortBlockBytes, world, cudaMemcpyDeviceToHost, ctx->compute));
+      }
+      s.checkPeers();
+      // the splitters, the same on every rank: sample j of rank r stands for n_r / S_r rows; splitter d - 1 is the sample at which the
+      // rows it and the smaller samples stand for first reach d N / world
+      struct Sample {
+         const unsigned long long* w;
+         double rows;
+      };
+      std::vector<Sample> all;
+      double total = 0;
+      for (int r = 0; r < world; r++) {
+         const unsigned long long* b = pin + r * (kSortBlockBytes / 8);
+         total += (double) b[0];
+         for (unsigned long long j = 0; j < b[1]; j++) all.push_back({b + 2 + j * kSortTupleWords, (double) b[0] / (double) b[1]});
+      }
+      std::sort(all.begin(), all.end(), [&](const Sample& a, const Sample& b) { return sortTupleLess(a.w, b.w, n_keys); });
+      size_t i = 0;
+      double below = 0;
+      for (int d = 1; d < world; d++) {
+         while (i < all.size() && below + all[i].rows < total * d / world) below += all[i++].rows;
+         for (int x = 0; x < kSortTupleWords; x++) split.split[d - 1][x] = i < all.size() ? all[i].w[x] : ~0ull;
+      }
+   }
+   s.run(&split);
+   // the received rows (source rank, then source row: the tie order) sorted by the keys, permuted from the region into the new table
+   LdbTable view{};
+   s.receivedView(view);
+   const int64_t got = (int64_t) s.mine;
+   if (got >= (int64_t) 1 << 32) fail(LDB_ERR_UNSUPPORTED, "the sort exchange sorts up to 2^32 - 1 received rows per rank");
+   const int64_t keep = limit >= 0 ? std::min<int64_t>(got, limit) : got;
+   Scratch sorted(ctx), cols(ctx);
+   const uint32_t* ids = keep ? sortRows(sorted, &view, order, got) : nullptr;
+   std::vector<int> outCols;
+   for (int j = 0; j < nUser; j++) outCols.push_back(j);
+   LdbBatch ob = permuteRows(&view, outCols, s.outBytes, ids, keep, cols);
+   s.finish();
+   int64_t before = 0, all = 0;
+   for (int d = 0; d < world; d++) {
+      const int64_t rows = limit >= 0 ? (d == 0 ? std::min<int64_t>((int64_t) s.p.rows[0], limit) : 0) : (int64_t) s.p.rows[d];
+      if (d < c->rank) before += rows;
+      all += rows;
+   }
+   std::vector<LdbColumn> outDesc;
+   for (int j = 0; j < nUser; j++) outDesc.push_back(src->columns[ship[j]]);
+   *out = addResultTable(ctx, name ? name : "sorted", std::move(outDesc), std::move(ob), cols);
+   *first_row = before;
+   *total_rows = all;
+}
+int ldb_gpu_table_sort_exchange(LdbTable* src, int32_t n_keys, const char* const* key_columns, const int32_t* descending, int32_t n_columns, const char* const* columns,
+                                int64_t limit, LdbComm* c, int64_t recv_offset, int64_t recv_bytes, const char* name, LdbTable** out, int64_t* first_row,
+                                int64_t* total_rows, LdbError* err) {
+   return guarded(err, [&] { sortExchange(src, n_keys, key_columns, descending, n_columns, columns, limit, c, recv_offset, recv_bytes, name, out, first_row, total_rows); });
 }
 
 // Union of every rank's string dictionary (include/ldb_gpu.h).  Local counters → export → all-gather of {status, n, bytes} → host

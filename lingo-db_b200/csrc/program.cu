@@ -4,6 +4,7 @@
 #include "keyhash.cuh"
 #include "progcol.cuh"
 #include "program.h"
+#include "sortkey.cuh"
 #include "../../include/ldb_gpu.h"
 
 #include <algorithm>
@@ -1209,12 +1210,10 @@ __global__ void buildSortWordsKernel(const uint8_t* col, const uint8_t* bytes, i
          k = isNull;
       } else if (isNull) {
          // k = 0: every NULL gets the same value word
-      } else if (kind == 0 && elemBytes == 16) {
-         const unsigned long long* w = (const unsigned long long*) (col + (size_t) row * 16);
-         k = chunk ? w[1] ^ 0x8000000000000000ull : w[0];
+      } else if (kind == 0 && elemBytes == 16) { // the value of sortCell (sortkey.cuh), a word at a time
+         k = chunk ? sortWideWord(col, row, 1) ^ 0x8000000000000000ull : sortWideWord(col, row, 0);
       } else if (kind == 0) {
-         const int64_t v = elemBytes == 4 ? (int64_t) ((const int32_t*) col)[row] : *(const int64_t*) (col + (size_t) row * elemBytes);
-         k = (unsigned long long) v ^ 0x8000000000000000ull;
+         k = (unsigned long long) sortNarrowValue(col, elemBytes, row) ^ 0x8000000000000000ull;
       } else {
          const int32_t* off = (const int32_t*) col + row;
          const int32_t b = off[0], len = off[1] - off[0];

@@ -177,6 +177,31 @@ class Comm:
         and bytes that do not fit `recv_bytes` with LDB_ERR_CAPACITY on every rank."""
         return self._exchange(self.L.ldb_gpu_table_exchange_varlen, table, keys, columns, name, recv_offset, recv_bytes)
 
+    def sort_exchange(self, table, keys, columns=None, limit=None, name: str = "sorted", recv_offset: int = 0, recv_bytes: int = None):
+        """ORDER BY (… LIMIT) across ranks (ldb_gpu_table_sort_exchange): `keys` are 1..4 (column, descending) pairs (a bare column name
+        is ascending), in the order of order_by_keys, with ties broken by (source rank, source row).  Without a `limit` every rank gets one
+        range of the global order, cut by splitters sampled from every rank; with one, rank 0 gets the first `limit` rows and the other
+        ranks empty tables.  `columns` are the columns to ship (None: all, utf8 included); keys need not be among them.  Returns
+        (program.RawTable, first_row, total_rows): this rank's rows already in order, the result rows on lower ranks and on all ranks.
+        Collective, and it waits for the peers on the host: the ranks of one process call it from one thread each.  The receive region
+        starts at user-heap offset `recv_offset` and spans `recv_bytes` (None: the rest of the user heap); rows that do not fit fail with
+        LDB_ERR_CAPACITY on every rank."""
+        from . import capi
+        from .program import RawTable, _handle
+        keys = [(k, False) if isinstance(k, str) else (k[0], bool(k[1])) for k in keys or []]
+        kn = [k.encode() for k, _ in keys]
+        karr = (C.c_char_p * max(1, len(kn)))(*kn)
+        darr = (C.c_int32 * max(1, len(kn)))(*[int(d) for _, d in keys])
+        cn = [c.encode() for c in columns] if columns is not None else []
+        carr = (C.c_char_p * max(1, len(cn)))(*cn) if columns is not None else None
+        if recv_bytes is None:
+            recv_bytes = self.heap()[1] - int(recv_offset)
+        out, first, total, e = C.c_void_p(), C.c_int64(), C.c_int64(), capi.Error()
+        capi.check(self.L.ldb_gpu_table_sort_exchange(C.c_void_p(_handle(table)), len(kn), karr, darr, len(cn), carr, -1 if limit is None else int(limit), self.h,
+                                                      int(recv_offset), int(recv_bytes), name.encode() if name is not None else None, C.byref(out),
+                                                      C.byref(first), C.byref(total), C.byref(e)), e)
+        return RawTable(self.ctx, out), int(first.value), int(total.value)
+
     def _exchange(self, entry, table, keys, columns, name, recv_offset, recv_bytes):
         from . import capi
         from .program import RawTable, _handle
