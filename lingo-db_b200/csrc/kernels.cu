@@ -830,19 +830,18 @@ using ONE = Agg<LDB_EXPR_ONE>;
 // Q1: sum(qty) sum(ep) sum(ep*(1-d)) sum(ep*(1-d)*(1+t)) sum(d) count over value columns qty, ep, d, t
 using Q1Aggs = Aggs<C0, C1, Agg<LDB_EXPR_MUL_1MINUS, 1, 2>, Agg<LDB_EXPR_MUL_1MINUS_1PLUS, 1, 2, 3>, C2, ONE>;
 constexpr int kQty = 0, kEp = 1, kDisc = 2, kTax = 3;
-// Factored Q1 stages (FAC).  Discount and tax take few values (TPC-H: 11 and 9), so per register group g
+// Factored Q1 (scanQ1FactoredKernel).  Discount and tax take few values (TPC-H: 11 and 9), so per register group g
 //   sum(ep*(1-d)*(1+t)) = sum over (d, t) of (1-d)(1+t) * S[g][d][t],   S[g][d][t] = sum of ep over g's rows with that (d, t),
 // and likewise sum(ep*(1-d)), sum(d) = sum of d * count[g][d][t], sum(ep), sum(qty) and count: identities of the integers, so they
 // hold modulo 2^64 and 2^128 too.  A row then costs three 32-bit shared atomics into its cell g*Dd*Dt + (d-min_d)*Dt + (t-min_t)
 // (64-bit shared atomics are CAS loops on sm_90a) and the products run once per cell and CTA at the end.  The summed columns enter
 // as offsets from their batch minimum (ep - min_ep, qty - min_qty; min * count is added back at the end, so negative values stay
-// exact), in three words that cannot overflow in one stage of 2 * kBlock * kEncFrames = 2048 rows when the stage header proves
-// ep_off < 2^28 and qty_off < 2^21:
+// exact), in three words that cannot overflow in one stage of 2 * kBlock * kEncFrames = 2048 rows when ep_off < 2^28 and
+// qty_off < 2^21 (the batch bounds, factoredFits):
 //   A = ep_off & 0xfffff  (< 2^20 per row),   B = (ep_off >> 20) << 12 | 1  (< 2^20 per row, the count in the low 12 bits),
 //   C = qty_off  (< 2^21 per row).
-// The words are double-buffered by stage parity: after the barrier that ends a stage, each thread folds the cells it owns (cell mod
-// kBlock) of the previous stage's buffer into 64-bit sums in registers and zeroes them, while the CTA fills the other buffer.  A
-// batch has fewer than 2^36 rows (launchGB), so those sums stay below 2^64.
+// After each stage every thread folds the cells it owns (cell mod kBlock) into 64-bit sums in registers and zeroes them.  A batch has
+// fewer than 2^36 rows (factoredFits), so those sums stay below 2^64.
 constexpr int kCells = 512;
 constexpr int kCellWords = 3;
 static_assert(kEncFrames * kRowsPerThreadScan * kBlock <= 2048 && kCells % kBlock == 0, "factored cell words overflow");
@@ -861,12 +860,88 @@ __device__ __forceinline__ void encodedFields2(uint32_t a, int sh, uint32_t (&x)
       ldShared32x2(a, x[0], x[1]);
    }
 }
-template <int DB, bool IN, int FS, bool FAC, int NK, int NV, class... As>
+// CTA-local id of the keys of the lanes that `need` one (their register keys did not hold them; warp-collective: every lane calls it):
+// the CTA's shared key list first, then at the first sight of a key one elected lane registers it under the CTA lock (with its HBM
+// slot).  Keys are append-only, so ids never change.  A lane gets -1 when the CTA tracks LG groups already (its row goes straight to
+// HBM); lanes without `need` keep `id`.
+template <int LG>
+__device__ __forceinline__ int ctaGroupLookup(const GroupTableDev& table, int32_t (*sKeys)[kMaxKeys], int32_t* sSlot, int32_t* sCount, int32_t* sLock,
+                                              int32_t k0, int32_t k1, bool need, int id) {
+   if (need) {
+      const int cnt = *((volatile int32_t*) sCount);
+      for (int g = 0; g < cnt; g++)
+         if (sKeys[g][0] == k0 && sKeys[g][1] == k1) id = g;
+      need = id < 0;
+   }
+   unsigned pending = __ballot_sync(0xffffffffu, need);
+   while (pending) {
+      const int leader = __ffs(pending) - 1;
+      const int32_t lk0 = __shfl_sync(0xffffffffu, k0, leader), lk1 = __shfl_sync(0xffffffffu, k1, leader);
+      int newId = -1;
+      if ((threadIdx.x & 31) == leader) {
+         while (atomicCAS(sLock, 0, 1) != 0) {}
+         __threadfence_block();
+         const int c2 = *((volatile int32_t*) sCount);
+         for (int g = 0; g < c2; g++)
+            if (((volatile int32_t*) sKeys[g])[0] == lk0 && ((volatile int32_t*) sKeys[g])[1] == lk1) newId = g;
+         if (newId < 0 && c2 < LG) {
+            int32_t kk[2] = {lk0, lk1};
+            sSlot[c2] = groupLookupOrInsert(table, kk);
+            sKeys[c2][0] = lk0;
+            sKeys[c2][1] = lk1;
+            __threadfence_block();
+            *((volatile int32_t*) sCount) = c2 + 1;
+            newId = c2;
+         }
+         __threadfence_block();
+         atomicExch(sLock, 0);
+      }
+      newId = __shfl_sync(0xffffffffu, newId, leader);
+      if (need && k0 == lk0 && k1 == lk1) {
+         id = newId;
+         need = false;
+      }
+      pending = __ballot_sync(0xffffffffu, need);
+   }
+   return id;
+}
+// self-timing (two words behind the table's error word): max(~start), max(end) of %globaltimer over the CTAs — the kernel's
+// duration without event nodes, so that a captured query (CUDA graph) still reports its kernel time (runtime.cpp groupby_read)
+__device__ __forceinline__ unsigned long long* selfTimeStart(const GroupTableDev& t) {
+   unsigned long long* const selfTime = (unsigned long long*) (t.error) + 1;
+   if (threadIdx.x == 0) {
+      unsigned long long t0;
+      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
+      atomicMax(selfTime, ~t0);
+   }
+   return selfTime;
+}
+// the CTA's shared sums → one HBM atomic per (group, aggregate), then the end of the self-timing (after a barrier behind every sum)
+template <int N>
+__device__ __forceinline__ void flushCtaGroups(const GroupTableDev& t, const unsigned long long (*sAcc)[N][2], const int32_t* sSlot, int cnt,
+                                               unsigned long long* selfTime) {
+   for (int i = threadIdx.x; i < cnt * N; i += kBlock) {
+      int g = i / N, a = i % N;
+      int slot = sSlot[g];
+      if (slot < 0) continue;
+      i128 s{sAcc[g][a][0], (int64_t) sAcc[g][a][1]};
+      if (s.lo | (uint64_t) s.hi) {
+         unsigned long long* dst = t.acc + ((size_t) slot * kMaxAggs + a) * 2;
+         atomicAdd128(dst, dst + 1, s); // 64-bit aggregates keep hi == 0 and are read back as i64
+      }
+   }
+   __syncthreads();
+   if (threadIdx.x == 0) {
+      unsigned long long t1;
+      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
+      atomicMax(selfTime + 1, t1);
+   }
+}
+template <int DB, bool IN, int FS, int NK, int NV, class... As>
 __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_constant__ GroupByParams p) {
    using AL = Aggs<As...>;
    constexpr int N = AL::N;
    constexpr bool kStaged = encodedStages<DB, FS>;
-   static_assert(!FAC || (kStaged && NK == 2 && NV == 4 && std::is_same_v<AL, Q1Aggs>), "the factored stage path is Q1's");
    constexpr int F = kStaged ? kEncFrames : 1;
    constexpr int GREG = NK == 0 ? 1 : 4; // register-resident groups
    constexpr int LG = 16;                // CTA-local groups (registers + shared)
@@ -874,21 +949,11 @@ __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_cons
    __shared__ int32_t sSlot[LG];
    __shared__ int32_t sCount, sLock;
    __shared__ unsigned long long sAcc[LG][N][2];
-   __shared__ uint32_t sCell[FAC ? 2 : 1][kCellWords][FAC ? kCells : 1]; // factored stages: {A, B, C} words per cell, by stage parity
    __shared__ __align__(8) TileBarriers barsStorage;
    TileBarriers* bars = &barsStorage;
 
-   // self-timing (two words behind the table's error word): max(~start), max(end) of %globaltimer over the CTAs — the kernel's
-   // duration without event nodes, so that a captured query (CUDA graph) still reports its kernel time (runtime.cpp groupby_read)
-   unsigned long long* const selfTime = (unsigned long long*) (p.table.error) + 1;
-   if (threadIdx.x == 0) {
-      unsigned long long t0;
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
-      atomicMax(selfTime, ~t0);
-   }
+   unsigned long long* const selfTime = selfTimeStart(p.table);
    for (int i = threadIdx.x; i < LG * N * 2; i += kBlock) (&sAcc[0][0][0])[i] = 0;
-   if constexpr (FAC)
-      for (int i = threadIdx.x; i < 2 * kCellWords * kCells; i += kBlock) (&sCell[0][0][0])[i] = 0;
    if (threadIdx.x == 0) {
       sCount = NK == 0 ? 1 : 0;
       sLock = 0;
@@ -927,46 +992,9 @@ __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_cons
 #pragma unroll
          for (int g = 0; g < GREG; g++)
             if (g < rcnt && k0 == rk0[g] && k1 == rk1[g]) id = g;
-         bool need = pass && id < 0;
-         unsigned pending = __ballot_sync(0xffffffffu, need);
-         if (pending) { // rare after the first tiles: a key outside the register-resident set
-            if (need) {
-               const int cnt = *((volatile int32_t*) &sCount);
-               for (int g = 0; g < cnt; g++)
-                  if (sKeys[g][0] == k0 && sKeys[g][1] == k1) id = g;
-               need = id < 0;
-            }
-            pending = __ballot_sync(0xffffffffu, need);
-            // first sight of a key in this CTA: one elected lane registers it under the CTA lock
-            while (pending) {
-               const int leader = __ffs(pending) - 1;
-               const int32_t lk0 = __shfl_sync(0xffffffffu, k0, leader), lk1 = __shfl_sync(0xffffffffu, k1, leader);
-               int newId = -1;
-               if ((threadIdx.x & 31) == leader) {
-                  while (atomicCAS(&sLock, 0, 1) != 0) {}
-                  __threadfence_block();
-                  const int c2 = *((volatile int32_t*) &sCount);
-                  for (int g = 0; g < c2; g++)
-                     if (((volatile int32_t*) sKeys[g])[0] == lk0 && ((volatile int32_t*) sKeys[g])[1] == lk1) newId = g;
-                  if (newId < 0 && c2 < LG) {
-                     int32_t kk[2] = {lk0, lk1};
-                     sSlot[c2] = groupLookupOrInsert(p.table, kk);
-                     sKeys[c2][0] = lk0;
-                     sKeys[c2][1] = lk1;
-                     __threadfence_block();
-                     *((volatile int32_t*) &sCount) = c2 + 1;
-                     newId = c2;
-                  }
-                  __threadfence_block();
-                  atomicExch(&sLock, 0);
-               }
-               newId = __shfl_sync(0xffffffffu, newId, leader);
-               if (need && k0 == lk0 && k1 == lk1) {
-                  id = newId; // -1: the CTA tracks LG groups already → this row goes straight to HBM
-                  need = false;
-               }
-               pending = __ballot_sync(0xffffffffu, need);
-            }
+         const bool need = pass && id < 0;
+         if (__ballot_sync(0xffffffffu, need)) { // rare after the first tiles: a key outside the register-resident set
+            id = ctaGroupLookup<LG>(p.table, sKeys, sSlot, &sCount, &sLock, k0, k1, need, id);
             // refresh the register copies (keys are append-only, so ids never change)
             const int cnt = *((volatile int32_t*) &sCount);
             rcnt = cnt < GREG ? cnt : GREG;
@@ -981,9 +1009,8 @@ __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_cons
       }
       return id;
    };
-   // the factored path's register-resident groups sum in their cells; its other rows take the shared and HBM atomics of add()
    auto add = [&](int id, const i128* v, int32_t k0, int32_t k1) {
-      if (!FAC && id >= 0 && id < GREG) {
+      if (id >= 0 && id < GREG) {
 #pragma unroll
          for (int g = 0; g < GREG; g++)
             if (id == g) AL::accumulate(acc[g], v, typename AL::S{});
@@ -1009,26 +1036,6 @@ __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_cons
       if (__all_sync(0xffffffffu, !pass || AL::fits32(vals, one))) AL::template eval<true>(v, vals, one, typename AL::S{});
       else AL::template eval<false>(v, vals, one, typename AL::S{});
       if (pass) add(id, v, k0, k1);
-   };
-   // factored stages: 64-bit sums of the cells this thread owns (cell j * kBlock + threadIdx.x), and the stages run so far
-   constexpr int kOwned = FAC ? kCells / kBlock : 1;
-   uint64_t cEp[kOwned], cCnt[kOwned], cQty[kOwned];
-#pragma unroll
-   for (int j = 0; j < kOwned; j++) cEp[j] = cCnt[j] = cQty[j] = 0;
-   uint32_t facStages = 0;
-   const uint32_t fDt = FAC ? (uint32_t) p.encRange[kTax] + 1u : 0u, fDdDt = FAC ? ((uint32_t) p.encRange[kDisc] + 1u) * fDt : 0u;
-   auto foldCells = [&](uint32_t buf) {
-#pragma unroll
-      for (int j = 0; j < kOwned; j++) {
-         const int cell = j * kBlock + threadIdx.x;
-         const uint32_t b = sCell[buf][1][cell];
-         if (b != 0) { // B counts the cell's rows
-            cEp[j] += sCell[buf][0][cell] + ((uint64_t) (b >> 12) << 20);
-            cCnt[j] += b & 0xfffu;
-            cQty[j] += sCell[buf][2][cell];
-            sCell[buf][0][cell] = sCell[buf][1][cell] = sCell[buf][2][cell] = 0;
-         }
-      }
    };
    auto encodedStage = [&](uint32_t stage) {
       const StagedCols& sc = p.src.cols;
@@ -1061,23 +1068,6 @@ __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_cons
             room = INT64_MAX;
          }
          room -= need;
-      }
-      // factored stage: the previous stage's cells are complete (every thread passed the barrier behind it); this stage fills the other
-      // buffer when its header puts each field's offset from the batch minimum inside its word budget or its cell domain
-      bool fac = false;
-      uint32_t buf = 0, cellOff = 0, offEp = 0, offQty = 0;
-      if constexpr (FAC) {
-         if (facStages > 0) foldCells((facStages - 1) & 1u);
-         buf = facStages++ & 1u;
-         uint64_t off[NV] = {};
-         auto inside = [&](int c, uint64_t top) { // every value of the stage's block in [min, min + top]
-            off[c] = (uint64_t) vb[c] - (uint64_t) p.encMin[c];
-            return (uint64_t) range[c] <= top && off[c] <= top - (uint64_t) range[c];
-         };
-         fac = proven && inside(kQty, (1u << 21) - 1) && inside(kEp, (1u << 28) - 1) && inside(kDisc, p.encRange[kDisc]) && inside(kTax, p.encRange[kTax]);
-         cellOff = (uint32_t) off[kDisc] * fDt + (uint32_t) off[kTax];
-         offEp = (uint32_t) off[kEp];
-         offQty = (uint32_t) off[kQty];
       }
       // `v cmp C` on the raw field x = v - base in [0, 2^32) is `flo <= x <= fhi`, negated for != (mask 5)
       uint32_t flo, fhi;
@@ -1144,26 +1134,11 @@ __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_cons
             int64_t vals[NV];
 #pragma unroll
             for (int c = 0; c < NV; c++) vals[c] = (int64_t) ((uint64_t) vb[c] + xv[c][i]);
-            if (FAC && fac) {
-               if (pass[i] && id[i] >= 0 && id[i] < GREG) {
-                  const uint32_t cell = (uint32_t) id[i] * fDdDt + xv[kDisc][i] * fDt + xv[kTax][i] + cellOff;
-                  const uint32_t ep = xv[kEp][i] + offEp;
-                  atomicAdd(&sCell[buf][0][cell], ep & 0xfffffu);
-                  atomicAdd(&sCell[buf][1][cell], (ep >> 20) << 12 | 1u);
-                  atomicAdd(&sCell[buf][2][cell], xv[kQty][i] + offQty);
-               } else if (pass[i]) {
-                  int64_t q[N];
-                  AL::eval64(q, vals, one, typename AL::S{});
-                  i128 v[N];
-#pragma unroll
-                  for (int a = 0; a < N; a++) v[a] = i128{(uint64_t) q[a], 0};
-                  add(id[i], v, k0, k1);
-               }
-            } else if (proven) {
+            if (proven) {
                int64_t q[N];
                AL::eval64(q, vals, one, typename AL::S{});
                // a one-hot test per group: an `id == g` test here was folded into a dynamically indexed acc[id], which lives in local memory
-               const uint32_t hot = !FAC && pass[i] && id[i] >= 0 && id[i] < GREG ? 1u << id[i] : 0u;
+               const uint32_t hot = pass[i] && id[i] >= 0 && id[i] < GREG ? 1u << id[i] : 0u;
 #pragma unroll
                for (int g = 0; g < GREG; g++)
                   if (hot >> g & 1u) AL::accumulate64(acc[g], acc64[g], q, typename AL::S{});
@@ -1198,60 +1173,244 @@ __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_cons
    });
    // ---- flush: registers → warp sums → shared → one HBM atomic per (CTA, group, aggregate)
    __syncthreads();
-   if constexpr (FAC) {
-      // the last stage's cells, then each owned cell's six aggregates, exact modulo 2^64 / 2^128 like the per-row sums
-      if (facStages > 0) foldCells((facStages - 1) & 1u);
-      // per register group: this thread's owned cells of the group, summed over the warp, one shared atomic per warp and aggregate
-      const int lane = threadIdx.x & 31;
-#pragma unroll 1
-      for (int g = 0; g < GREG; g++) {
-         i128 s[N];
 #pragma unroll
-         for (int a = 0; a < N; a++) s[a] = i128{0, 0};
+   for (int g = 0; g < GREG; g++) AL::fold64(acc[g], acc64[g], typename AL::S{});
+   const int lane = threadIdx.x & 31;
 #pragma unroll
-         for (int j = 0; j < kOwned; j++) {
-            const uint32_t cell = j * kBlock + threadIdx.x, dt = cell % fDdDt;
-            if (cCnt[j] == 0 || cell / fDdDt != (uint32_t) g) continue;
-            const int64_t d = p.encMin[kDisc] + (int64_t) (dt / fDt), t = p.encMin[kTax] + (int64_t) (dt % fDt);
-            const uint64_t n = cCnt[j];
-            const i128 ep = add128(i128{cEp[j], 0}, mul64x64(p.encMin[kEp], (int64_t) n));
-            const i128 epd = mul128x64(ep, one - d);
-            i128 v[N];
-            v[0] = i128{cQty[j] + (uint64_t) p.encMin[kQty] * n, 0};
-            v[1] = i128{ep.lo, 0};
-            v[2] = epd;
-            v[3] = mul128x64(epd, one + t);
-            v[4] = i128{(uint64_t) d * n, 0};
-            v[5] = i128{n, 0};
-            AL::accumulate(s, v, typename AL::S{});
+   for (int g = 0; g < GREG; g++) AL::warpFlush(sAcc[g], acc[g], lane, typename AL::S{});
+   __syncthreads();
+   flushCtaGroups<N>(p.table, sAcc, sSlot, sCount, selfTime);
+}
+
+// The factored Q1 kernel: Q1's signature over an encoded batch with the one-int32-constant filter, when factoredFits admits the batch.  Its
+// columns are in signature order (qty, ep, d, t, the two keys, the filter's column; toSignatureOrder).  Invariant: factoredFits proves
+// on the host, from the batch's minima and ranges, that every value lies in [encMin, encMin + encRange] with ep - min_ep < 2^28,
+// qty - min_qty < 2^21, 4 * Dd * Dt <= kCells and every Q1 product a non-negative int64 (aggBound64 over the batch), and that both key
+// fields are 1 byte wide.  Every stage or tile header's block lies inside the batch, so each of its rows has its cell and word budgets
+// and the 64-bit products of the fallback without a check in the kernel.
+// A frame is one TMA stage of kEncFrames tiles or one tile read with plain loads (the tail, or a batch without TMA); the cell words are
+// single-buffered: after the barrier that ends a frame each thread folds the cells it owns into 64-bit sums and zeroes them, and a
+// second barrier lets the next frame's atomics in.  Two stages in flight (50 KB of Q1 stages at TPC-H widths) and about 8 KB of static
+// shared memory leave three CTAs per SM, which hide the latency of each warp's dependent run (loads → compare → vote → atomics).
+constexpr int kFacStages = 2;
+__global__ void __launch_bounds__(kBlock, 3) scanQ1FactoredKernel(const __grid_constant__ GroupByParams p) {
+   using AL = Q1Aggs;
+   constexpr int N = AL::N, NV = 4, NK = 2;
+   constexpr int FC = NV + NK; // staged index of the filter's column
+   constexpr int GREG = 4;     // register groups (factored in the cells)
+   constexpr int LG = 16;      // CTA-local groups (registers + shared)
+   constexpr int kRun = 2;     // adjacent rows decoded together
+   constexpr int kOwned = kCells / kBlock;
+   __shared__ int32_t sKeys[LG][kMaxKeys];
+   __shared__ int32_t sSlot[LG];
+   __shared__ int32_t sCount, sLock;
+   __shared__ unsigned long long sAcc[LG][N][2];
+   __shared__ uint32_t sCell[kCellWords][kCells]; // {A, B, C} words per cell
+   __shared__ __align__(8) TileBarriers barsStorage;
+
+   unsigned long long* const selfTime = selfTimeStart(p.table);
+   for (int i = threadIdx.x; i < LG * N * 2; i += kBlock) (&sAcc[0][0][0])[i] = 0;
+   for (int i = threadIdx.x; i < kCellWords * kCells; i += kBlock) (&sCell[0][0])[i] = 0;
+   if (threadIdx.x == 0) sCount = sLock = 0;
+   __syncthreads();
+
+   const int64_t one = 100; // 10^scale of decimal(12,2); checked on the host
+   const uint32_t fDt = (uint32_t) p.encRange[kTax] + 1u, fDdDt = ((uint32_t) p.encRange[kDisc] + 1u) * fDt;
+   // 64-bit sums of the cells this thread owns (cell j * kBlock + threadIdx.x)
+   uint64_t cEp[kOwned], cCnt[kOwned], cQty[kOwned];
+#pragma unroll
+   for (int j = 0; j < kOwned; j++) cEp[j] = cCnt[j] = cQty[j] = 0;
+   auto foldCells = [&]() {
+#pragma unroll
+      for (int j = 0; j < kOwned; j++) {
+         const int cell = j * kBlock + threadIdx.x;
+         const uint32_t b = sCell[1][cell];
+         if (b != 0) { // B counts the cell's rows
+            cEp[j] += sCell[0][cell] + ((uint64_t) (b >> 12) << 20);
+            cCnt[j] += b & 0xfffu;
+            cQty[j] += sCell[2][cell];
+            sCell[0][cell] = sCell[1][cell] = sCell[2][cell] = 0;
          }
-         AL::warpFlush(sAcc[g], s, lane, typename AL::S{});
       }
-   } else {
+   };
+
+   // the frame's header bases and what follows from them: the offsets of its value fields from the batch minima (a value is
+   // encMin + off + field), the key bases, and the filter as a range of the raw field
+   uint32_t off[NV], cellOff = 0, kb0 = 0, kb1 = 0, flo = 0, fhi = 0;
+   bool finv = false;
+   // the register groups' keys as packed raw key fields of the frame (k0 - kb0 | (k1 - kb1) << 16); a group not registered yet, or whose
+   // keys lie outside the frame's 1-byte fields, holds ~0u, which no packed pair of 1-byte fields equals
+   uint32_t rk[GREG];
+   auto registerKeys = [&]() {
+      const int cnt = *((volatile int32_t*) &sCount);
 #pragma unroll
-      for (int g = 0; g < GREG; g++) AL::fold64(acc[g], acc64[g], typename AL::S{});
-      const int lane = threadIdx.x & 31;
+      for (int g = 0; g < GREG; g++) {
+         rk[g] = ~0u;
+         if (g < cnt) {
+            const uint32_t a = (uint32_t) ((volatile int32_t*) sKeys[g])[0] - kb0, b = (uint32_t) ((volatile int32_t*) sKeys[g])[1] - kb1;
+            if ((a | b) < 256u) rk[g] = a | b << 16;
+         }
+      }
+   };
+   auto setFrame = [&](const int64_t (&base)[NV], uint32_t k0, uint32_t k1, int32_t filterBase) {
 #pragma unroll
-      for (int g = 0; g < GREG; g++) AL::warpFlush(sAcc[g], acc[g], lane, typename AL::S{});
+      for (int c = 0; c < NV; c++) off[c] = (uint32_t) (base[c] - p.encMin[c]);
+      cellOff = off[kDisc] * fDt + off[kTax];
+      kb0 = k0;
+      kb1 = k1;
+      // `v cmp C` on the raw field x = v - base in [0, 2^32) is `flo <= x <= fhi`, negated for != (mask 5)
+      const FilterCol& f = p.src.filters.c[0];
+      const int64_t t = (int64_t) (int32_t) f.valA - (int64_t) filterBase;
+      finv = f.maskA == 5u;
+      const uint32_t m = finv ? 2u : f.maskA;
+      const int64_t l = (m & 1u) ? 0 : (m & 2u) ? t : t + 1, h = (m & 4u) ? 0xffffffffll : (m & 2u) ? t : t - 1;
+      const int64_t lc = l < 0 ? 0 : l, hc = h > 0xffffffffll ? 0xffffffffll : h;
+      flo = lc > hc ? 1u : (uint32_t) lc;
+      fhi = lc > hc ? 0u : (uint32_t) hc;
+      registerKeys();
+   };
+   // kRun rows of the frame (warp-collective): their raw key and filter fields, whether they exist, and a loader of their value fields
+   auto rows = [&](const uint32_t (&xk0)[kRun], const uint32_t (&xk1)[kRun], const uint32_t (&xf)[kRun], const bool (&valid)[kRun], const auto& values) {
+      bool pass[kRun], miss = false;
+      int id[kRun];
+#pragma unroll
+      for (int i = 0; i < kRun; i++) {
+         pass[i] = valid[i] & (((xf[i] >= flo) & (xf[i] <= fhi)) != finv);
+         const uint32_t pk = xk0[i] | xk1[i] << 16;
+         id[i] = -1;
+#pragma unroll
+         for (int g = 0; g < GREG; g++)
+            if (pk == rk[g]) id[i] = g;
+         miss |= pass[i] & (id[i] < 0);
+      }
+      if (__any_sync(0xffffffffu, miss)) { // a key outside the register groups: the CTA's shared list, then registration
+#pragma unroll
+         for (int i = 0; i < kRun; i++)
+            id[i] = ctaGroupLookup<LG>(p.table, sKeys, sSlot, &sCount, &sLock, (int32_t) (kb0 + xk0[i]), (int32_t) (kb1 + xk1[i]), pass[i] && id[i] < 0, id[i]);
+         registerKeys();
+      }
+      uint32_t xv[NV][kRun];
+      values(xv);
+#pragma unroll
+      for (int i = 0; i < kRun; i++) {
+         if (pass[i] && (uint32_t) id[i] < (uint32_t) GREG) {
+            const uint32_t cell = (uint32_t) id[i] * fDdDt + xv[kDisc][i] * fDt + xv[kTax][i] + cellOff;
+            const uint32_t ep = xv[kEp][i] + off[kEp];
+            atomicAdd(&sCell[0][cell], ep & 0xfffffu);
+            atomicAdd(&sCell[1][cell], (ep >> 20) << 12 | 1u);
+            atomicAdd(&sCell[2][cell], xv[kQty][i] + off[kQty]);
+         } else if (pass[i]) { // a group past the register set: its products in 64 bits (proven), shared sums or the HBM table
+            int64_t vals[NV], q[N];
+#pragma unroll
+            for (int c = 0; c < NV; c++) vals[c] = p.encMin[c] + (int64_t) (off[c] + xv[c][i]);
+            AL::eval64(q, vals, one, typename AL::S{});
+            i128 v[N];
+#pragma unroll
+            for (int a = 0; a < N; a++) v[a] = i128{(uint64_t) q[a], 0};
+            if (id[i] >= 0) {
+               AL::sharedAdd(sAcc[id[i]], v, typename AL::S{});
+            } else {
+               int32_t kk[2] = {(int32_t) (kb0 + xk0[i]), (int32_t) (kb1 + xk1[i])};
+               const int slot = groupLookupOrInsert(p.table, kk);
+               if (slot >= 0) AL::globalAdd(p.table, slot, v, typename AL::S{});
+            }
+         }
+      }
+   };
+
+   uint32_t frames = 0;
+   const StagedCols& sc = p.src.cols;
+   forEachTileUniform<kRowsPerThreadScan, kDecEncoded, kFacStages, kEncFrames>(sc, p.src.nRows, dynSmem, &barsStorage, [&](const auto& tile, int64_t, int nRows) {
+      if (frames++ > 0) { // every thread passed the barrier behind the previous frame's atomics
+         foldCells();
+         __syncthreads();
+      }
+      if constexpr (std::is_same_v<std::decay_t<decltype(tile)>, SmemTile<kDecEncoded>>) {
+         constexpr int R = kRowsPerThreadScan * kEncFrames; // rows of a thread
+         constexpr int kTileRows = kRowsPerThreadScan * kBlock;
+         constexpr int kFrameThreads = kBlock / kEncFrames; // threads per tile of the stage
+         // column c's tiles lie from stage + kEncFrames * smemOffset[c]; their headers are equal (kernels.h), tile 0's stands for all
+         auto col = [&](int c) { return tile.stage + (uint32_t) (kEncFrames * sc.smemOffset[c]); };
+         int64_t base[NV];
+#pragma unroll
+         for (int c = 0; c < NV; c++) base[c] = ldShared64(col(c));
+         setFrame(base, (uint32_t) ldShared32(col(NV)), (uint32_t) ldShared32(col(NV + 1)), ldShared32(col(FC)));
+         const uint32_t frame = threadIdx.x / kFrameThreads, ft = threadIdx.x % kFrameThreads;
+#pragma unroll 1
+         for (int run = 0; run < R / kRun; run++) {
+            // rows r0 .. r0 + kRun - 1 of tile `frame`: the lanes of a warp read consecutive kRun * W bytes, conflict-free at any W
+            const uint32_t r0 = (run * kFrameThreads + ft) * kRun;
+            auto fields = [&](int c, uint32_t (&x)[kRun]) {
+               const int sh = sc.encShift[c];
+               encodedFields2(col(c) + frame * (kEncodeTileHeader + ((uint32_t) kTileRows << sh)) + kEncodeTileHeader + (r0 << sh), sh, x);
+            };
+            uint32_t xk0[kRun], xk1[kRun], xf[kRun];
+            fields(NV, xk0);
+            fields(NV + 1, xk1);
+            fields(FC, xf);
+            const bool valid[kRun] = {true, true};
+            rows(xk0, xk1, xf, valid, [&](uint32_t (&xv)[NV][kRun]) {
+#pragma unroll
+               for (int c = 0; c < NV; c++) fields(c, xv[c]);
+            });
+         }
+      } else { // one tile through plain loads: thread t takes rows t and kBlock + t
+         int64_t base[NV];
+#pragma unroll
+         for (int c = 0; c < NV; c++) base[c] = (int64_t) tile.base(c);
+         setFrame(base, (uint32_t) tile.base(NV), (uint32_t) tile.base(NV + 1), (int32_t) tile.base(FC));
+         static_assert(kRowsPerThreadScan == kRun, "a tail tile is one run per thread");
+         int lr[kRun];
+         bool valid[kRun];
+         uint32_t xk0[kRun], xk1[kRun], xf[kRun];
+#pragma unroll
+         for (int i = 0; i < kRun; i++) {
+            lr[i] = i * kBlock + threadIdx.x;
+            valid[i] = lr[i] < nRows;
+            if (!valid[i]) lr[i] = 0;
+            xk0[i] = (uint32_t) tile.field(NV, lr[i]);
+            xk1[i] = (uint32_t) tile.field(NV + 1, lr[i]);
+            xf[i] = (uint32_t) tile.field(FC, lr[i]);
+         }
+         rows(xk0, xk1, xf, valid, [&](uint32_t (&xv)[NV][kRun]) {
+#pragma unroll
+            for (int c = 0; c < NV; c++)
+#pragma unroll
+               for (int i = 0; i < kRun; i++) xv[c][i] = (uint32_t) tile.field(c, lr[i]);
+         });
+      }
+   });
+   // ---- flush: the last frame's cells, then each owned cell's six aggregates, exact modulo 2^64 / 2^128 like the per-row sums; per
+   // register group this thread's owned cells of the group, summed over the warp, one shared atomic per warp and aggregate
+   __syncthreads();
+   if (frames > 0) foldCells();
+   const int lane = threadIdx.x & 31;
+#pragma unroll 1
+   for (int g = 0; g < GREG; g++) {
+      i128 s[N];
+#pragma unroll
+      for (int a = 0; a < N; a++) s[a] = i128{0, 0};
+#pragma unroll
+      for (int j = 0; j < kOwned; j++) {
+         const uint32_t cell = j * kBlock + threadIdx.x, dt = cell % fDdDt;
+         if (cCnt[j] == 0 || cell / fDdDt != (uint32_t) g) continue;
+         const int64_t d = p.encMin[kDisc] + (int64_t) (dt / fDt), t = p.encMin[kTax] + (int64_t) (dt % fDt);
+         const uint64_t n = cCnt[j];
+         const i128 ep = add128(i128{cEp[j], 0}, mul64x64(p.encMin[kEp], (int64_t) n));
+         const i128 epd = mul128x64(ep, one - d);
+         i128 v[N];
+         v[0] = i128{cQty[j] + (uint64_t) p.encMin[kQty] * n, 0};
+         v[1] = i128{ep.lo, 0};
+         v[2] = epd;
+         v[3] = mul128x64(epd, one + t);
+         v[4] = i128{(uint64_t) d * n, 0};
+         v[5] = i128{n, 0};
+         AL::accumulate(s, v, typename AL::S{});
+      }
+      AL::warpFlush(sAcc[g], s, lane, typename AL::S{});
    }
    __syncthreads();
-   const int cnt = sCount;
-   for (int i = threadIdx.x; i < cnt * N; i += kBlock) {
-      int g = i / N, a = i % N;
-      int slot = sSlot[g];
-      if (slot < 0) continue;
-      i128 s{sAcc[g][a][0], (int64_t) sAcc[g][a][1]};
-      if (s.lo | (uint64_t) s.hi) {
-         unsigned long long* dst = p.table.acc + ((size_t) slot * kMaxAggs + a) * 2;
-         atomicAdd128(dst, dst + 1, s); // 64-bit aggregates keep hi == 0 and are read back as i64
-      }
-   }
-   __syncthreads();
-   if (threadIdx.x == 0) {
-      unsigned long long t1;
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
-      atomicMax(selfTime + 1, t1);
-   }
+   flushCtaGroups<N>(p.table, sAcc, sSlot, sCount, selfTime);
 }
 
 // ---- signature registry
@@ -1294,18 +1453,11 @@ static bool hasInList(const FilterSet& f) { // "rare" filters: IN lists and LIKE
    return false;
 }
 template <int DB, bool IN, int FS, int NK, int NV, class... As>
-static void launchGBd(const GroupByParams& p, int smCount, cudaStream_t s, bool factored = false) {
+static void launchGBd(const GroupByParams& p, int smCount, cudaStream_t s) {
    size_t dyn;
    constexpr int tiles = encodedStages<DB, FS> ? kEncStages * kEncFrames : kStages; // tiles held in shared memory
-   if constexpr (encodedStages<DB, FS> && NK == 2 && NV == 4 && std::is_same_v<Aggs<As...>, Q1Aggs>) {
-      if (factored) {
-         int grid = persistentGrid(scanGroupByKernel<DB, IN, FS, true, NK, NV, As...>, p.src.cols, p.src.nRows, smCount, &dyn, kBlock, tiles);
-         scanGroupByKernel<DB, IN, FS, true, NK, NV, As...><<<grid, kBlock, dyn, s>>>(p);
-         return;
-      }
-   }
-   int grid = persistentGrid(scanGroupByKernel<DB, IN, FS, false, NK, NV, As...>, p.src.cols, p.src.nRows, smCount, &dyn, kBlock, tiles);
-   scanGroupByKernel<DB, IN, FS, false, NK, NV, As...><<<grid, kBlock, dyn, s>>>(p);
+   int grid = persistentGrid(scanGroupByKernel<DB, IN, FS, NK, NV, As...>, p.src.cols, p.src.nRows, smCount, &dyn, kBlock, tiles);
+   scanGroupByKernel<DB, IN, FS, NK, NV, As...><<<grid, kBlock, dyn, s>>>(p);
 }
 // The stage path reads fields of at most 4 bytes (an 8-byte field is a value column no product proof admits) and must fit its stages in
 // one CTA's shared memory; other encoded batches take the instance with the descriptor-driven filter.
@@ -1320,17 +1472,14 @@ static bool encodedStagesFit(K kernel, const StagedCols& sc) {
    cudaFuncGetAttributes(&fa, kernel);
    return (int64_t) kEncStages * kEncFrames * sc.stageBytes + (int64_t) fa.sharedSizeBytes <= optin;
 }
-// The factored stage path (Q1Aggs, kCells) runs when the batch's discount and tax domains give every register group its cells, and
-// the batch's own bounds (encMin, encRange) prove what each stage header would: ep - min_ep < 2^28 and qty - min_qty < 2^21 (the
-// word budgets) and the 64-bit product bound of the per-row stage path (aggBound64 on the batch range), so every stage factors and
-// only rows of groups past the register set take the instance's shared-atomic fallback.  The batch must also be short enough for the
-// 64-bit cell sums (2^36 rows of ep_off < 2^28), and its stages and cells must leave two CTAs per SM (one fewer resident CTA costs more
-// than the factoring saves).  Any other batch takes the per-row stage instance, which keeps its sums in registers.
-using Q1FactoredKernel = decltype(&scanGroupByKernel<kDecEncoded, false, FS_I32_ONE, true, 2, 4, C0, C1, Agg<LDB_EXPR_MUL_1MINUS, 1, 2>,
-                                                     Agg<LDB_EXPR_MUL_1MINUS_1PLUS, 1, 2, 3>, C2, ONE>);
+// The factored kernel (Q1Aggs, kCells) runs when the batch's discount and tax domains give every register group its cells, and the
+// batch's own bounds (encMin, encRange) prove what each stage header would: ep - min_ep < 2^28 and qty - min_qty < 2^21 (the word
+// budgets) and the 64-bit product bound of the per-row stage path (aggBound64 on the batch range), so every row of a register group
+// factors and only rows of groups past the register set take the fallback.  The batch must also be short enough for the 64-bit cell
+// sums (2^36 rows of ep_off < 2^28), its key fields 1 byte wide (the kernel compares both keys as one packed word), and its stages and
+// shared memory must leave three CTAs per SM (one fewer resident CTA costs more than the factoring saves).  Any other batch takes the
+// per-row stage instance, which keeps its sums in registers.
 static bool factoredFits(const GroupByParams& p) {
-   const Q1FactoredKernel kernel = scanGroupByKernel<kDecEncoded, false, FS_I32_ONE, true, 2, 4, C0, C1, Agg<LDB_EXPR_MUL_1MINUS, 1, 2>,
-                                                     Agg<LDB_EXPR_MUL_1MINUS_1PLUS, 1, 2, 3>, C2, ONE>;
    const uint64_t dd = p.encRange[kDisc], dt = p.encRange[kTax];
    if (dd >= kCells || dt >= kCells || 4 * (dd + 1) * (dt + 1) > (uint64_t) kCells || p.src.nRows >= (1ll << 36)) return false;
    if (p.encRange[kEp] >= (1ull << 28) || p.encRange[kQty] >= (1ull << 21)) return false;
@@ -1342,14 +1491,22 @@ static bool factoredFits(const GroupByParams& p) {
    if (p.encMin[kDisc] < -k31 || p.encMin[kDisc] > k31 || p.encMin[kTax] < -k31 || p.encMin[kTax] > k31) return false;
    if (epLo < 0 || epHi >= k31 || dLo < 0 || dHi >= k31 || tLo < 0 || tHi >= k31) return false;
    if ((unsigned __int128) epHi * (uint64_t) dHi * (uint64_t) tHi >= (unsigned __int128) ((1ull << 63) / (kRowsPerThreadScan * kEncFrames))) return false;
-   if (!encodedStagesFit(kernel, p.src.cols)) return false;
+   const StagedCols& sc = p.src.cols;
+   for (int c = 0; c < sc.n; c++)
+      if (sc.elemBytes[c] > 4) return false;
+   if (sc.elemBytes[4] != 1 || sc.elemBytes[5] != 1) return false; // the keys (signature order)
    int dev = 0, perSm = 0, reserved = 0;
    cudaFuncAttributes fa{};
    cudaGetDevice(&dev);
    cudaDeviceGetAttribute(&perSm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev);
    cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev);
-   cudaFuncGetAttributes(&fa, (const void*) kernel);
-   return 2 * ((int64_t) kEncStages * kEncFrames * p.src.cols.stageBytes + (int64_t) fa.sharedSizeBytes + reserved) <= perSm;
+   cudaFuncGetAttributes(&fa, (const void*) scanQ1FactoredKernel);
+   return 3 * ((int64_t) kFacStages * kEncFrames * sc.stageBytes + (int64_t) fa.sharedSizeBytes + reserved) <= perSm;
+}
+static void launchQ1Factored(const GroupByParams& p, int smCount, cudaStream_t s) {
+   size_t dyn;
+   int grid = persistentGrid(scanQ1FactoredKernel, p.src.cols, p.src.nRows, smCount, &dyn, kBlock, kFacStages * kEncFrames);
+   scanQ1FactoredKernel<<<grid, kBlock, dyn, s>>>(p);
 }
 // The encoded instance reads its columns' layout at constant indices: value column c is staged column c, key k is NV + k, and a
 // shaped filter's column is NV + NK.  Permutes the staged columns (and every index into them) into that order; returns the filter
@@ -1396,11 +1553,11 @@ static void launchGB(const GroupByParams& p, int smCount, cudaStream_t s) {
             if (fs == FS_I32_ONE) {
                if constexpr (NK == 2 && NV == 4 && std::is_same_v<Aggs<As...>, Q1Aggs>) {
                   if (factoredFits(q)) {
-                     launchGBd<kDecEncoded, false, FS_I32_ONE, NK, NV, As...>(q, smCount, s, true);
+                     launchQ1Factored(q, smCount, s);
                      return;
                   }
                }
-               if (encodedStagesFit(scanGroupByKernel<kDecEncoded, false, FS_I32_ONE, false, NK, NV, As...>, q.src.cols)) {
+               if (encodedStagesFit(scanGroupByKernel<kDecEncoded, false, FS_I32_ONE, NK, NV, As...>, q.src.cols)) {
                   launchGBd<kDecEncoded, false, FS_I32_ONE, NK, NV, As...>(q, smCount, s);
                   return;
                }
