@@ -860,6 +860,23 @@ __device__ __forceinline__ void encodedFields2(uint32_t a, int sh, uint32_t (&x)
       ldShared32x2(a, x[0], x[1]);
    }
 }
+// the same for 4 adjacent rows from shared address a (4W-byte aligned): a u32, u64 or u128 load
+__device__ __forceinline__ void encodedFields4(uint32_t a, int sh, uint32_t (&x)[4]) {
+   if (sh == 0) {
+      const uint32_t v = (uint32_t) ldShared32(a);
+#pragma unroll
+      for (int i = 0; i < 4; i++) x[i] = (v >> (8 * i)) & 0xffu;
+   } else if (sh == 1) {
+      uint32_t v0, v1;
+      ldShared32x2(a, v0, v1);
+      x[0] = v0 & 0xffffu;
+      x[1] = v0 >> 16;
+      x[2] = v1 & 0xffffu;
+      x[3] = v1 >> 16;
+   } else {
+      asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(x[0]), "=r"(x[1]), "=r"(x[2]), "=r"(x[3]) : "r"(a));
+   }
+}
 // CTA-local id of the keys of the lanes that `need` one (their register keys did not hold them; warp-collective: every lane calls it):
 // the CTA's shared key list first, then at the first sight of a key one elected lane registers it under the CTA lock (with its HBM
 // slot).  Keys are append-only, so ids never change.  A lane gets -1 when the CTA tracks LG groups already (its row goes straight to
@@ -1188,25 +1205,32 @@ __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_cons
 // qty - min_qty < 2^21, 4 * Dd * Dt <= kCells and every Q1 product a non-negative int64 (aggBound64 over the batch), and that both key
 // fields are 1 byte wide.  Every stage or tile header's block lies inside the batch, so each of its rows has its cell and word budgets
 // and the 64-bit products of the fallback without a check in the kernel.
-// A frame is one TMA stage of kEncFrames tiles or one tile read with plain loads (the tail, or a batch without TMA); the cell words are
-// single-buffered: after the barrier that ends a frame each thread folds the cells it owns into 64-bit sums and zeroes them, and a
-// second barrier lets the next frame's atomics in.  Two stages in flight (50 KB of Q1 stages at TPC-H widths) and about 8 KB of static
-// shared memory leave three CTAs per SM, which hide the latency of each warp's dependent run (loads → compare → vote → atomics).
-constexpr int kFacStages = 2;
+// A frame is one TMA stage of kFacTiles tiles or one tile read with plain loads (the tail, or a batch without TMA), and every frame ends
+// at a CTA barrier.  The cell words are single-buffered: at the start of the next frame each thread folds the cells it owns into 64-bit
+// sums and zeroes them, and a second barrier lets that frame's atomics in.  (Double-buffered words, without that barrier, measured 12 %
+// faster, but their 6 KB more static shared memory would cost batches of 16 bytes per row their third CTA per SM.)  The stage ring
+// holds kFacStages stages of kFacTiles tiles (50 KB at TPC-H widths; deeper rings of fewer tiles measured slower) and with about 8 KB of
+// static shared memory three CTAs fit an SM, which hide the latency of each warp's dependent run (loads → compare → vote → loads →
+// atomics).  A thread decodes its rows of a stage in runs of 4 adjacent rows, one shared load per column per run, so each chain
+// carries 4 independent rows.
+constexpr int kFacTiles = 4, kFacStages = 2;
 __global__ void __launch_bounds__(kBlock, 3) scanQ1FactoredKernel(const __grid_constant__ GroupByParams p) {
+   constexpr int F = kFacTiles, S = kFacStages;
    using AL = Q1Aggs;
    constexpr int N = AL::N, NV = 4, NK = 2;
    constexpr int FC = NV + NK; // staged index of the filter's column
    constexpr int GREG = 4;     // register groups (factored in the cells)
    constexpr int LG = 16;      // CTA-local groups (registers + shared)
-   constexpr int kRun = 2;     // adjacent rows decoded together
+   constexpr int RUN = 4;      // adjacent rows of a stage decoded together (encodedFields4)
    constexpr int kOwned = kCells / kBlock;
+   constexpr int kTileRows = kRowsPerThreadScan * kBlock;
+   static_assert(F * kTileRows <= 2048 && (2 * F) % RUN == 0 && 128 % F == 0, "a stage is one frame of whole runs in one block");
    __shared__ int32_t sKeys[LG][kMaxKeys];
    __shared__ int32_t sSlot[LG];
    __shared__ int32_t sCount, sLock;
    __shared__ unsigned long long sAcc[LG][N][2];
    __shared__ uint32_t sCell[kCellWords][kCells]; // {A, B, C} words per cell
-   __shared__ __align__(8) TileBarriers barsStorage;
+   __shared__ __align__(8) uint64_t sFull[S];        // stage s holds its tiles
 
    unsigned long long* const selfTime = selfTimeStart(p.table);
    for (int i = threadIdx.x; i < LG * N * 2; i += kBlock) (&sAcc[0][0][0])[i] = 0;
@@ -1232,6 +1256,12 @@ __global__ void __launch_bounds__(kBlock, 3) scanQ1FactoredKernel(const __grid_c
             sCell[0][cell] = sCell[1][cell] = sCell[2][cell] = 0;
          }
       }
+   };
+   // every thread passed the barrier behind the previous frame's atomics (or the set-up); folding cells nothing added to is a no-op, so
+   // the first frame needs no count
+   auto beginFrame = [&]() {
+      foldCells();
+      __syncthreads();
    };
 
    // the frame's header bases and what follows from them: the offsets of its value fields from the batch minima (a value is
@@ -1269,12 +1299,13 @@ __global__ void __launch_bounds__(kBlock, 3) scanQ1FactoredKernel(const __grid_c
       fhi = lc > hc ? 0u : (uint32_t) hc;
       registerKeys();
    };
-   // kRun rows of the frame (warp-collective): their raw key and filter fields, whether they exist, and a loader of their value fields
-   auto rows = [&](const uint32_t (&xk0)[kRun], const uint32_t (&xk1)[kRun], const uint32_t (&xf)[kRun], const bool (&valid)[kRun], const auto& values) {
-      bool pass[kRun], miss = false;
-      int id[kRun];
+   // K adjacent rows of the frame (warp-collective): their raw key and filter fields, whether they exist, and a loader of their value fields
+   auto rows = [&](const auto& xk0, const auto& xk1, const auto& xf, const auto& valid, const auto& values) {
+      constexpr int K = std::extent_v<std::remove_reference_t<decltype(xk0)>>;
+      bool pass[K], miss = false;
+      int id[K];
 #pragma unroll
-      for (int i = 0; i < kRun; i++) {
+      for (int i = 0; i < K; i++) {
          pass[i] = valid[i] & (((xf[i] >= flo) & (xf[i] <= fhi)) != finv);
          const uint32_t pk = xk0[i] | xk1[i] << 16;
          id[i] = -1;
@@ -1285,20 +1316,20 @@ __global__ void __launch_bounds__(kBlock, 3) scanQ1FactoredKernel(const __grid_c
       }
       if (__any_sync(0xffffffffu, miss)) { // a key outside the register groups: the CTA's shared list, then registration
 #pragma unroll
-         for (int i = 0; i < kRun; i++)
+         for (int i = 0; i < K; i++)
             id[i] = ctaGroupLookup<LG>(p.table, sKeys, sSlot, &sCount, &sLock, (int32_t) (kb0 + xk0[i]), (int32_t) (kb1 + xk1[i]), pass[i] && id[i] < 0, id[i]);
          registerKeys();
       }
-      uint32_t xv[NV][kRun];
+      uint32_t xv[NV][K];
       values(xv);
 #pragma unroll
-      for (int i = 0; i < kRun; i++) {
+      for (int i = 0; i < K; i++) {
          if (pass[i] && (uint32_t) id[i] < (uint32_t) GREG) {
-            const uint32_t cell = (uint32_t) id[i] * fDdDt + xv[kDisc][i] * fDt + xv[kTax][i] + cellOff;
+            const uint32_t c = (uint32_t) id[i] * fDdDt + xv[kDisc][i] * fDt + xv[kTax][i] + cellOff;
             const uint32_t ep = xv[kEp][i] + off[kEp];
-            atomicAdd(&sCell[0][cell], ep & 0xfffffu);
-            atomicAdd(&sCell[1][cell], (ep >> 20) << 12 | 1u);
-            atomicAdd(&sCell[2][cell], xv[kQty][i] + off[kQty]);
+            atomicAdd(&sCell[0][c], ep & 0xfffffu);
+            atomicAdd(&sCell[1][c], (ep >> 20) << 12 | 1u);
+            atomicAdd(&sCell[2][c], xv[kQty][i] + off[kQty]);
          } else if (pass[i]) { // a group past the register set: its products in 64 bits (proven), shared sums or the HBM table
             int64_t vals[NV], q[N];
 #pragma unroll
@@ -1317,73 +1348,112 @@ __global__ void __launch_bounds__(kBlock, 3) scanQ1FactoredKernel(const __grid_c
          }
       }
    };
-
-   uint32_t frames = 0;
    const StagedCols& sc = p.src.cols;
-   forEachTileUniform<kRowsPerThreadScan, kDecEncoded, kFacStages, kEncFrames>(sc, p.src.nRows, dynSmem, &barsStorage, [&](const auto& tile, int64_t, int nRows) {
-      if (frames++ > 0) { // every thread passed the barrier behind the previous frame's atomics
-         foldCells();
-         __syncthreads();
-      }
-      if constexpr (std::is_same_v<std::decay_t<decltype(tile)>, SmemTile<kDecEncoded>>) {
-         constexpr int R = kRowsPerThreadScan * kEncFrames; // rows of a thread
-         constexpr int kTileRows = kRowsPerThreadScan * kBlock;
-         constexpr int kFrameThreads = kBlock / kEncFrames; // threads per tile of the stage
-         // column c's tiles lie from stage + kEncFrames * smemOffset[c]; their headers are equal (kernels.h), tile 0's stands for all
-         auto col = [&](int c) { return tile.stage + (uint32_t) (kEncFrames * sc.smemOffset[c]); };
-         int64_t base[NV];
+   // one stage in shared memory: its F tiles of column c lie from stage + F * smemOffset[c] with equal headers (kernels.h), tile 0's
+   // stands for all; thread t takes 2F rows of tile t / (kBlock / F) in runs of RUN adjacent rows, the lanes of a warp reading
+   // consecutive RUN * W bytes per column, conflict-free at any W
+   auto stageFrame = [&](uint32_t stage) {
+      beginFrame();
+      auto col = [&](int c) { return stage + (uint32_t) (F * sc.smemOffset[c]); };
+      int64_t base[NV];
 #pragma unroll
-         for (int c = 0; c < NV; c++) base[c] = ldShared64(col(c));
-         setFrame(base, (uint32_t) ldShared32(col(NV)), (uint32_t) ldShared32(col(NV + 1)), ldShared32(col(FC)));
-         const uint32_t frame = threadIdx.x / kFrameThreads, ft = threadIdx.x % kFrameThreads;
+      for (int c = 0; c < NV; c++) base[c] = ldShared64(col(c));
+      setFrame(base, (uint32_t) ldShared32(col(NV)), (uint32_t) ldShared32(col(NV + 1)), ldShared32(col(FC)));
+      constexpr int kFrameThreads = kBlock / F; // threads per tile of the stage
+      const uint32_t frame = threadIdx.x / kFrameThreads, ft = threadIdx.x % kFrameThreads;
 #pragma unroll 1
-         for (int run = 0; run < R / kRun; run++) {
-            // rows r0 .. r0 + kRun - 1 of tile `frame`: the lanes of a warp read consecutive kRun * W bytes, conflict-free at any W
-            const uint32_t r0 = (run * kFrameThreads + ft) * kRun;
-            auto fields = [&](int c, uint32_t (&x)[kRun]) {
-               const int sh = sc.encShift[c];
-               encodedFields2(col(c) + frame * (kEncodeTileHeader + ((uint32_t) kTileRows << sh)) + kEncodeTileHeader + (r0 << sh), sh, x);
-            };
-            uint32_t xk0[kRun], xk1[kRun], xf[kRun];
-            fields(NV, xk0);
-            fields(NV + 1, xk1);
-            fields(FC, xf);
-            const bool valid[kRun] = {true, true};
-            rows(xk0, xk1, xf, valid, [&](uint32_t (&xv)[NV][kRun]) {
+      for (int run = 0; run < 2 * F / RUN; run++) {
+         const uint32_t r0 = (run * kFrameThreads + ft) * RUN;
+         auto fields = [&](int c, uint32_t (&x)[RUN]) {
+            const int sh = sc.encShift[c];
+            const uint32_t a = col(c) + frame * (kEncodeTileHeader + ((uint32_t) kTileRows << sh)) + kEncodeTileHeader + (r0 << sh);
+            encodedFields4(a, sh, x);
+         };
+         uint32_t xk0[RUN], xk1[RUN], xf[RUN];
+         fields(NV, xk0);
+         fields(NV + 1, xk1);
+         fields(FC, xf);
+         bool valid[RUN];
 #pragma unroll
-               for (int c = 0; c < NV; c++) fields(c, xv[c]);
-            });
-         }
-      } else { // one tile through plain loads: thread t takes rows t and kBlock + t
-         int64_t base[NV];
+         for (int i = 0; i < RUN; i++) valid[i] = true;
+         rows(xk0, xk1, xf, valid, [&](uint32_t (&xv)[NV][RUN]) {
 #pragma unroll
-         for (int c = 0; c < NV; c++) base[c] = (int64_t) tile.base(c);
-         setFrame(base, (uint32_t) tile.base(NV), (uint32_t) tile.base(NV + 1), (int32_t) tile.base(FC));
-         static_assert(kRowsPerThreadScan == kRun, "a tail tile is one run per thread");
-         int lr[kRun];
-         bool valid[kRun];
-         uint32_t xk0[kRun], xk1[kRun], xf[kRun];
-#pragma unroll
-         for (int i = 0; i < kRun; i++) {
-            lr[i] = i * kBlock + threadIdx.x;
-            valid[i] = lr[i] < nRows;
-            if (!valid[i]) lr[i] = 0;
-            xk0[i] = (uint32_t) tile.field(NV, lr[i]);
-            xk1[i] = (uint32_t) tile.field(NV + 1, lr[i]);
-            xf[i] = (uint32_t) tile.field(FC, lr[i]);
-         }
-         rows(xk0, xk1, xf, valid, [&](uint32_t (&xv)[NV][kRun]) {
-#pragma unroll
-            for (int c = 0; c < NV; c++)
-#pragma unroll
-               for (int i = 0; i < kRun; i++) xv[c][i] = (uint32_t) tile.field(c, lr[i]);
+            for (int c = 0; c < NV; c++) fields(c, xv[c]);
          });
       }
-   });
+   };
+   // one tile through plain loads: thread t takes rows t and kBlock + t
+   auto tileFrame = [&](int64_t t) {
+      beginFrame();
+      GlobalTile<kDecEncoded> tile{t * kTileRows, &sc};
+      const int nRows = (int) min(p.src.nRows - t * kTileRows, (int64_t) kTileRows);
+      int64_t base[NV];
+#pragma unroll
+      for (int c = 0; c < NV; c++) base[c] = (int64_t) tile.base(c);
+      setFrame(base, (uint32_t) tile.base(NV), (uint32_t) tile.base(NV + 1), (int32_t) tile.base(FC));
+      constexpr int K = kRowsPerThreadScan;
+      int lr[K];
+      bool valid[K];
+      uint32_t xk0[K], xk1[K], xf[K];
+#pragma unroll
+      for (int i = 0; i < K; i++) {
+         lr[i] = i * kBlock + threadIdx.x;
+         valid[i] = lr[i] < nRows;
+         if (!valid[i]) lr[i] = 0;
+         xk0[i] = (uint32_t) tile.field(NV, lr[i]);
+         xk1[i] = (uint32_t) tile.field(NV + 1, lr[i]);
+         xf[i] = (uint32_t) tile.field(FC, lr[i]);
+      }
+      rows(xk0, xk1, xf, valid, [&](uint32_t (&xv)[NV][K]) {
+#pragma unroll
+         for (int c = 0; c < NV; c++)
+#pragma unroll
+            for (int i = 0; i < K; i++) xv[c][i] = (uint32_t) tile.field(c, lr[i]);
+      });
+   };
+
+   // CTA b takes stages b, b + grid, ..; the full tiles after the last full stage and the partial tail tile go tile by tile through
+   // plain loads, continuing that round robin
+   const int64_t nFull = p.src.nRows / kTileRows;
+   int64_t done = nFull, turns = nFull; // tiles read by the loops below, and the round-robin turns they took
+   if (sc.useTma) {
+      const int64_t nStages = nFull / F;
+      done = nStages * F;
+      turns = nStages;
+      if (threadIdx.x == 0) {
+         for (int s = 0; s < S; s++) mbarInit(&sFull[s], 1);
+         mbarInitFence();
+      }
+      __syncthreads();
+      if (threadIdx.x == 0) {
+         for (int s = 0; s < S; s++) {
+            const int64_t t = (int64_t) blockIdx.x + (int64_t) s * gridDim.x;
+            if (t < nStages) issueTile<F>(sc, dynSmem, sFull, t, s);
+         }
+      }
+      for (int64_t t = blockIdx.x; t < nStages; t += gridDim.x) {
+         const uint32_t it = (uint32_t) (t - blockIdx.x) / gridDim.x; // this CTA's stage count (a batch has < 2^36 rows), not kept live
+         const int s = it % S;
+         mbarWait(&sFull[s], (uint32_t) (it / S) & 1u);
+         stageFrame(smemAddr(dynSmem) + (uint32_t) (s * F * sc.stageBytes));
+         __syncthreads(); // every thread is done with stage s → refill it
+         const int64_t nt = t + (int64_t) S * gridDim.x;
+         if (threadIdx.x == 0 && nt < nStages) issueTile<F>(sc, dynSmem, sFull, nt, s);
+      }
+   } else {
+      for (int64_t t = blockIdx.x; t < nFull; t += gridDim.x) {
+         tileFrame(t);
+         __syncthreads();
+      }
+   }
+   const int64_t nTiles = (p.src.nRows + kTileRows - 1) / kTileRows;
+   for (int64_t t = done + ((int64_t) blockIdx.x + gridDim.x - turns % gridDim.x) % gridDim.x; t < nTiles; t += gridDim.x) {
+      tileFrame(t);
+      __syncthreads();
+   }
    // ---- flush: the last frame's cells, then each owned cell's six aggregates, exact modulo 2^64 / 2^128 like the per-row sums; per
    // register group this thread's owned cells of the group, summed over the warp, one shared atomic per warp and aggregate
-   __syncthreads();
-   if (frames > 0) foldCells();
+   foldCells();
    const int lane = threadIdx.x & 31;
 #pragma unroll 1
    for (int g = 0; g < GREG; g++) {
@@ -1501,11 +1571,11 @@ static bool factoredFits(const GroupByParams& p) {
    cudaDeviceGetAttribute(&perSm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev);
    cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev);
    cudaFuncGetAttributes(&fa, (const void*) scanQ1FactoredKernel);
-   return 3 * ((int64_t) kFacStages * kEncFrames * sc.stageBytes + (int64_t) fa.sharedSizeBytes + reserved) <= perSm;
+   return 3 * ((int64_t) kFacStages * kFacTiles * sc.stageBytes + (int64_t) fa.sharedSizeBytes + reserved) <= perSm;
 }
 static void launchQ1Factored(const GroupByParams& p, int smCount, cudaStream_t s) {
    size_t dyn;
-   int grid = persistentGrid(scanQ1FactoredKernel, p.src.cols, p.src.nRows, smCount, &dyn, kBlock, kFacStages * kEncFrames);
+   int grid = persistentGrid(scanQ1FactoredKernel, p.src.cols, p.src.nRows, smCount, &dyn, kBlock, kFacStages * kFacTiles);
    scanQ1FactoredKernel<<<grid, kBlock, dyn, s>>>(p);
 }
 // The encoded instance reads its columns' layout at constant indices: value column c is staged column c, key k is NV + k, and a
