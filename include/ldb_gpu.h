@@ -576,6 +576,41 @@ int ldb_gpu_table_order_by_keys(LdbTable* t, int32_t n_keys, const char* const* 
  * more than bytes_cap bytes the call fails with LDB_ERR_CAPACITY, sets *bytes_needed and writes nothing else. */
 int ldb_gpu_table_gather_strings(LdbTable* t, const char* column, const int64_t* row_ids, int64_t n, int64_t* host_offsets /* n + 1 */, void* host_bytes,
                                  int64_t bytes_cap, int64_t* bytes_needed, uint8_t* host_valid, LdbError* err);
+/* Window functions: <func> OVER (PARTITION BY p… ORDER BY o… ROWS BETWEEN from AND to), the reference's relalg.window
+ * (WindowLowering, RelAlgToSubOp.cpp:2193-2553; csrc/window.cu cites each rule).
+ *   Partitions: rows equal on every partition key, NULL equal to NULL (IS NOT DISTINCT FROM), so NULL keys form one partition.  Within
+ *   a partition rows follow the order keys in the order of ldb_gpu_table_order_by_keys (a NULL greater than any value, DESC swaps);
+ *   rows that tie on every key keep their source row order.
+ *   Frame: ROWS [frame_from, frame_to] relative to the current row; INT64_MIN = UNBOUNDED PRECEDING, INT64_MAX = UNBOUNDED FOLLOWING,
+ *   0 = CURRENT ROW.  For the row at position j of a partition of length len a finite bound is min(len - 1, max(0, j + offset)), as in
+ *   the reference, so a frame is never empty (2 FOLLOWING .. 5 FOLLOWING on the last row is the last row).  UNBOUNDED FOLLOWING is the
+ *   partition end (the reference's i64 add wraps there; we keep the SQL meaning).  from > to, from = INT64_MAX or to = INT64_MIN:
+ *   LDB_ERR_INVALID.
+ *   Functions, over the frame [lo, hi] of row i (positions in window order): ROW_NUMBER = i - lo + 1 (the reference's RANK is this
+ *   function too), COUNT_STAR = hi - lo + 1, COUNT = the non-NULL values of `column`; SUM, MIN, MAX over the non-NULL values, NULL when
+ *   the frame has none.  SUM is exact modulo 2^128 (the wrapping of LDB_AGG_SUM).  AVG is SUM / COUNT, divided by the caller.
+ *   Result: *out = a new single-batch DEVICE table named `name` (NULL: "window") whose rows are in window order (partition keys
+ *   ascending, then the order keys, then source row).  It holds the carried columns (`columns`, NULL = every column of src; same names,
+ *   types and values, cells as ldb_gpu_table_exchange_varlen makes them, utf8 included), then one column per function, named by it:
+ *   ROW_NUMBER and the COUNTs int64 without NULLs; SUM decimal128(38, the argument's scale) in 16-byte cells; MIN and MAX the argument's
+ *   type and cell width; SUM, MIN and MAX with one validity byte per row.  Keys and arguments need not be carried.
+ *   Limits: a single-batch source (materialised results, exported groups, received or sorted tables, single-batch staged tables) of
+ *   fewer than 2^32 rows; 0..4 partition and 0..4 order keys of the types ldb_gpu_table_order_by_keys takes (int32, date32, char(1),
+ *   int64, decimal, utf8); 1..8 functions; 0..16 carried columns.  SUM takes int8..int64 and decimal (8- or 16-byte cells), MIN and MAX
+ *   those and date32 and char(1), COUNT any column.  A materialised column holding double bits is read as the decimal it is typed as.
+ *   Errors: LDB_ERR_UNSUPPORTED naming the column for a float or utf8 argument of SUM / MIN / MAX or a key of another type; also for a
+ *   multi-batch source, 2^32 rows or more, or a call inside a captured query (the sort reads string lengths on the host).
+ *   LDB_ERR_INVALID for null arguments, unknown columns or kinds, counts out of range or a bad frame.  Everything is checked before the
+ *   first launch. */
+enum LdbWindowKind { LDB_WIN_ROW_NUMBER = 1, LDB_WIN_COUNT_STAR = 2, LDB_WIN_COUNT = 3, LDB_WIN_SUM = 4, LDB_WIN_MIN = 5, LDB_WIN_MAX = 6 };
+typedef struct LdbWindowFunc {
+   int32_t kind;       /* LdbWindowKind */
+   const char* column; /* the argument; NULL for ROW_NUMBER and COUNT_STAR */
+   const char* name;   /* the output column */
+} LdbWindowFunc;
+int ldb_gpu_table_window(LdbTable* src, int32_t n_partition, const char* const* partition_columns, int32_t n_order, const char* const* order_columns,
+                         const int32_t* descending, int64_t frame_from, int64_t frame_to, int32_t n_funcs, const LdbWindowFunc* funcs, int32_t n_columns,
+                         const char* const* columns /* carried; NULL = all columns of src */, const char* name, LdbTable** out, LdbError* err);
 
 /* String dictionary (LDB_STATE_DICT): a device hash set of byte strings that gives each distinct string a dense int32 code, for
  * LDB_OP_STRCODE — group, join and sort keys over strings of any length.  Codes are 0..n-1 and stable for the dictionary's lifetime

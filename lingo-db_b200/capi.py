@@ -131,6 +131,14 @@ class HashAggRow(C.Structure):
     _fields_ = [("keys", C.c_int64 * 4), ("key_null_mask", C.c_uint32), ("agg_valid_mask", C.c_uint32), ("aggs", I128 * MAX_AGGS)]
 
 
+# LdbWindowKind; RANK is the reference's RankWindowFunc, which is ROW_NUMBER
+WIN = {"row_number": 1, "rank": 1, "count_star": 2, "count": 3, "sum": 4, "min": 5, "max": 6}
+
+
+class WindowFunc(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("column", C.c_char_p), ("name", C.c_char_p)]
+
+
 class Q5ShuffleStats(C.Structure):
     _fields_ = [(n, C.c_int64) for n in ("orders_tuples_sent", "orders_tuples_received", "lineitem_tuples_sent", "lineitem_tuples_received", "shuffle_bytes_out", "heap_bytes")]
 
@@ -205,6 +213,8 @@ SIGNATURES = {
     "ldb_gpu_table_gather": (C.c_int, [_P, C.c_char_p, C.POINTER(C.c_int64), C.c_int64, _P, _P, _E]),
     "ldb_gpu_table_order_by_keys": (C.c_int, [_P, C.c_int32, C.POINTER(C.c_char_p), C.POINTER(C.c_int32), C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int64), _E]),
     "ldb_gpu_table_gather_strings": (C.c_int, [_P, C.c_char_p, C.POINTER(C.c_int64), C.c_int64, C.POINTER(C.c_int64), _P, C.c_int64, C.POINTER(C.c_int64), _P, _E]),
+    "ldb_gpu_table_window": (C.c_int, [_P, C.c_int32, C.POINTER(C.c_char_p), C.c_int32, C.POINTER(C.c_char_p), C.POINTER(C.c_int32), C.c_int64, C.c_int64,
+                                       C.c_int32, C.POINTER(WindowFunc), C.c_int32, C.POINTER(C.c_char_p), C.c_char_p, C.POINTER(_P), _E]),
     "ldb_gpu_dict_create": (C.c_int, [_P, C.c_int64, C.c_int64, C.POINTER(_P), _E]),
     "ldb_gpu_dict_count": (C.c_int, [_P, C.POINTER(C.c_int64), _E]),
     "ldb_gpu_dict_to_table": (C.c_int, [_P, C.c_char_p, C.POINTER(_P), _E]),

@@ -305,6 +305,22 @@ LdbTable* addResultTable(LdbContext* ctx, std::string name, std::vector<LdbColum
 // row ids of the single-batch table `t` (n rows, n < 2^32) ordered by the keys (column index, descending), in `scratch`: ORDER BY,
 // dictionary ranks and the union of a unified dictionary (program_rt.cpp)
 uint32_t* sortRows(Scratch& scratch, LdbTable* t, const std::vector<std::pair<int, int>>& keys, int64_t n);
+// the cell width of a column of `type` in the single-batch tables the exchanges and the window operator make: a decimal in 16 bytes
+// whatever width it was staged at
+inline int32_t shipCellBytes(int type) {
+   switch (type) {
+      case LDB_INT8: return 1;
+      case LDB_INT16: return 2;
+      case LDB_INT64:
+      case LDB_FLOAT64: return 8;
+      case LDB_DECIMAL128: return 16;
+      default: return 4; // int32, date32, fsb4, float32
+   }
+}
+// rows ids[0..n) (null: 0..n-1) of columns `cols` of `t` (any number of batches, at most 16 columns) as a new single-batch LdbBatch whose
+// buffers are in `bufs`: fixed-width cells at outBytes[j] bytes (a narrowed decimal widened to 16), validity bytes, utf8 offsets and
+// bytes.  Synchronises.  The sort exchange and the window operator (peer.cu)
+LdbBatch permuteRows(LdbTable* t, const std::vector<int>& cols, const int32_t* outBytes, const uint32_t* ids, int64_t n, Scratch& bufs);
 } // namespace ldb
 // builds the missing encoded copies of columns cols[0..n) of a borrowed DEVICE batch (encode.cu) for tiles of `tileRows` rows;
 // true when every one of them has a copy.  Runs outside any capture and waits for its work on the host.

@@ -1144,16 +1144,6 @@ static void wantRegion(LdbComm* c, int64_t recv_offset, int64_t recv_bytes) {
    if (recv_offset < 0 || recv_bytes < 0 || recv_offset % 16 || recv_offset > (int64_t) c->userBytes || recv_bytes > (int64_t) c->userBytes - recv_offset)
       fail(LDB_ERR_INVALID, "receive region outside the comm's user heap or not 16-byte aligned");
 }
-static int32_t shipCellBytes(int type) {
-   switch (type) {
-      case LDB_INT8: return 1;
-      case LDB_INT16: return 2;
-      case LDB_INT64:
-      case LDB_FLOAT64: return 8;
-      case LDB_DECIMAL128: return 16;
-      default: return 4; // int32, date32, fsb4, float32
-   }
-}
 
 // One shipment of a table's rows, for arguments the caller checked.  The constructor takes what a rank needs before its first collective
 // (staging waits, temporaries, pinned scratch); ship() counts under an owner rule (the key hash, or the splitters of a sort) and runs the
@@ -1420,10 +1410,11 @@ int ldb_gpu_table_exchange_varlen(LdbTable* src, int32_t n_keys, const char* con
    return guarded(err, [&] { tableExchange(true, src, n_keys, key_columns, n_columns, columns, c, recv_offset, recv_bytes, name, out); });
 }
 
+} // extern "C"
 // Rows ids[0..n) (null: 0..n-1) of columns `cols` of `t` (any number of batches) into new single-batch buffers of `bufs`, cells at
 // outBytes: the permute kernels, with a host read of each utf8 column's byte total in between (it sizes the bytes array).  Returns the
 // batch (nRows, data, bytes, elemBytes, validBytes); synchronises.
-static LdbBatch permuteRows(LdbTable* t, const std::vector<int>& cols, const int32_t* outBytes, const uint32_t* ids, int64_t n, Scratch& bufs) {
+LdbBatch ldb::permuteRows(LdbTable* t, const std::vector<int>& cols, const int32_t* outBytes, const uint32_t* ids, int64_t n, Scratch& bufs) {
    LdbContext* ctx = t->ctx;
    Scratch tmp(ctx);
    PermuteParams q{};
@@ -1489,6 +1480,7 @@ static LdbBatch permuteRows(LdbTable* t, const std::vector<int>& cols, const int
    ctx->syncStream(ctx->compute); // the directory and the CTA sums go back to the pool
    return ob;
 }
+extern "C" {
 // the stable sort of a table of any number of batches by its key columns (index, descending): row ids global to the table, in `scratch`.
 // A single batch is sorted where it is; otherwise the keys are first permuted into one batch (16-byte decimal cells), whose order is the
 // same: sortRows composes a key's words from its canonical value (sortCell).

@@ -485,6 +485,26 @@ class RawTable:
         out = [raw[offs[i]:offs[i + 1]] if valid[i] else None for i in range(n)]
         return [s.decode() if decode and s is not None else s for s in out]
 
+    def window(self, partition_by=(), order_by=(), frame=None, funcs=(), columns=None, name="window") -> "RawTable":
+        """Window functions (ldb_gpu_table_window) as a new table in window order: the carried `columns` (None: every column), then one
+        column per function.  order_by: [(column, descending), …]; frame: (from, to) ROWS offsets relative to the current row, None for
+        an unbounded end (default: (None, 0) with ORDER BY, (None, None) without, as the SQL analyzer sets it); funcs: [(kind, column,
+        name), …] with kind one of capi.WIN ("row_number" / "rank", "count_star", "count", "sum", "min", "max"; column None for the
+        first two).  AVG is sum / count."""
+        if frame is None:
+            frame = (None, 0) if order_by else (None, None)
+        lo = -(1 << 63) if frame[0] is None else int(frame[0])
+        hi = (1 << 63) - 1 if frame[1] is None else int(frame[1])
+        enc = lambda xs: (C.c_char_p * max(1, len(xs)))(*[x.encode() for x in xs])
+        part, order = list(partition_by), list(order_by)
+        fs = (capi.WindowFunc * max(1, len(funcs)))(*[capi.WindowFunc(capi.WIN[k], c.encode() if c is not None else None, n.encode()) for k, c, n in funcs])
+        desc = (C.c_int32 * max(1, len(order)))(*[int(bool(d)) for _, d in order])
+        carried = None if columns is None else enc(list(columns))
+        t, e = C.c_void_p(), Error()
+        check(self.ctx.L.ldb_gpu_table_window(self.h, len(part), enc(part), len(order), enc([c for c, _ in order]), desc, lo, hi, len(funcs), fs,
+                                              0 if columns is None else len(columns), carried, name.encode(), C.byref(t), C.byref(e)), e)
+        return RawTable(self.ctx, t)
+
     def destroy(self):
         if self.h:
             self.ctx.L.ldb_gpu_table_destroy(self.h)
