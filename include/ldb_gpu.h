@@ -611,6 +611,40 @@ typedef struct LdbWindowFunc {
 int ldb_gpu_table_window(LdbTable* src, int32_t n_partition, const char* const* partition_columns, int32_t n_order, const char* const* order_columns,
                          const int32_t* descending, int64_t frame_from, int64_t frame_to, int32_t n_funcs, const LdbWindowFunc* funcs, int32_t n_columns,
                          const char* const* columns /* carried; NULL = all columns of src */, const char* name, LdbTable** out, LdbError* err);
+/* Set operations: SELECT DISTINCT, UNION [ALL], INTERSECT [ALL] and EXCEPT [ALL] over whole rows, the reference's relalg.projection
+ * distinct (ProjectionDistinctLowering, RelAlgToSubOp.cpp:337-394), relalg.union (UnionAllLowering :622-634, UnionDistinctLowering
+ * :636-727) and relalg.intersect / relalg.except (CountingSetOperationLowering :728-916); csrc/setop.cu cites each rule.
+ *   Rows: columns `left_columns` of left (NULL = every column) against `right_columns` of right (NULL = every column), by position;
+ *   n_columns is the length of the lists given (ignored when both are NULL), and both sides must come to the same number of columns.
+ *   Row equality is IS NOT DISTINCT FROM on every column (the reference's compareKeys, :142-153): NULL equals NULL and never a value,
+ *   and the bytes under a NULL cell are ignored; utf8 compares by bytes (a NULL string is not ''); a decimal by its value sign-extended
+ *   to 128 bits, so an 8-byte narrowed cell equals the same value in a 16-byte cell; a float by its bits after mapping -0.0 to +0.0 and
+ *   every NaN to one NaN.  The float rule is our definition: the reference compares floats with oeq but hashes their bits, so its
+ *   answer on zeros and NaN has no single meaning.
+ *   Multiplicities, for a row occurring cL times in left and cR times in right (:849-913): DISTINCT (right = NULL) and UNION emit it
+ *   once; UNION ALL emits the left rows, then the right rows, unchanged; INTERSECT once if cL > 0 and cR > 0; EXCEPT once if cL > 0 and
+ *   cR == 0; INTERSECT ALL min(cL, cR) times; EXCEPT ALL max(cL - cR, 0) times.
+ *   Order (the reference leaves it open; we fix it): each distinct row at the position of its first occurrence in the left rows
+ *   followed by the right rows, its ALL copies consecutive, its cells those of that first occurrence (which matters only for the sign
+ *   of a float zero).
+ *   Result: *out = a new single-batch DEVICE table named `name` (NULL: "setop") with left's column names, types and precisions (a
+ *   decimal's precision the larger of the two sides), cells as ldb_gpu_table_exchange_varlen makes them (decimals in 16 bytes, utf8
+ *   included) and validity bytes on every column.
+ *   Limits: sides of any number of batches (staged HOST tables, borrowed DEVICE batches, result tables), fewer than 2^32 rows together;
+ *   1..16 columns of int8, int16, int32, int64, date32, char(1), decimal, float32, float64 or utf8; left == right is allowed.
+ *   Errors, before the first launch: LDB_ERR_INVALID for a null argument, right given for DISTINCT or missing for another kind, an
+ *   unknown kind, unknown columns, 0 or more than 16 columns, column lists of different lengths or tables of different contexts;
+ *   LDB_ERR_UNSUPPORTED naming both columns for positional columns of different physical types, for decimals of different scales (the
+ *   caller casts, as the SQL analyzer does), for 2^32 rows or more and for a call inside a captured query (the output size is read on
+ *   the host).  After the set is built: LDB_ERR_UNSUPPORTED when a utf8 column of the result would hold more than 2^31 - 1 bytes (its
+ *   offsets are int32), and LDB_ERR_CAPACITY if a lookup ran past the device set's directory (not expected: it has two slots per
+ *   inserted row). */
+enum LdbSetOpKind { LDB_SET_DISTINCT = 1, LDB_SET_UNION_ALL = 2, LDB_SET_UNION = 3, LDB_SET_INTERSECT = 4,
+                    LDB_SET_INTERSECT_ALL = 5, LDB_SET_EXCEPT = 6, LDB_SET_EXCEPT_ALL = 7 };
+int ldb_gpu_table_setop(LdbTable* left, LdbTable* right /* NULL exactly for LDB_SET_DISTINCT */, int32_t kind, int32_t n_columns,
+                        const char* const* left_columns /* NULL = every column of left */,
+                        const char* const* right_columns /* NULL = every column of right; positional */,
+                        const char* name, LdbTable** out, LdbError* err);
 
 /* String dictionary (LDB_STATE_DICT): a device hash set of byte strings that gives each distinct string a dense int32 code, for
  * LDB_OP_STRCODE — group, join and sort keys over strings of any length.  Codes are 0..n-1 and stable for the dictionary's lifetime

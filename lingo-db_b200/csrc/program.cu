@@ -139,17 +139,6 @@ __device__ bool strLike(const ProgCol& c, int64_t row, const uint8_t* k, int kle
    return false;
 }
 // ---------------------------------------------------------------- string dictionary (DictDev, program.h)
-// placement hash of a byte string: 8-byte little-endian chunks (the last one zero padded) folded through mix64, seeded with the
-// length.  Internal: codes and results never depend on it.
-__device__ __forceinline__ uint64_t strHash(const uint8_t* s, int32_t n) {
-   uint64_t h = 0x9E3779B97F4A7C15ull ^ ((uint64_t) (uint32_t) n * 0xff51afd7ed558ccdull);
-   for (int32_t i = 0; i < n; i += 8) {
-      uint64_t w = 0;
-      for (int j = 0; j < 8 && i + j < n; j++) w |= (uint64_t) s[i + j] << (8 * j);
-      h = mix64(h ^ w) + 0x632BE59BD9B4E019ull;
-   }
-   return mix64(h);
-}
 // where a string with hash h lives in the directory: its tag (the high 32 bits of h, the upper half of its slot word), its first slot
 // and the linear probe sequence from there, at most dictProbeLimit slots long.  One definition for dictCode and the ranked build of a
 // unified dictionary, so that a lookup finds every string the build placed.

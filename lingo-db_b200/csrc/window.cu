@@ -30,19 +30,19 @@
 //   4. MIN / MAX: a segment tree over the sorted argument (NULL = the identity, plus an "any value" flag per node), built bottom-up
 //      one launch per level over a power-of-two leaf array, queried per row by the iterative O(log width) walk;
 //   5. winFramesKernel: per row its frame [lo, hi] by the clamping rule and every function's value.
-// The scans are tile scans of our own: per tile a reduction, one CTA's exclusive scan of the tile totals, then each tile rescanned
-// from its prefix.
+// The scans are the tile scans of tilescan.cuh: per tile a reduction, one CTA's exclusive scan of the tile totals, then each tile
+// rescanned from its prefix.
 #include "context.h"
 #include "progcol.cuh"
 #include "sortkey.cuh"
+#include "tilescan.cuh"
 
 #include <algorithm>
 #include <climits>
 
 namespace ldb {
 
-constexpr int kWinThreads = 256, kWinItems = 8;
-constexpr int64_t kWinTile = (int64_t) kWinThreads * kWinItems;
+constexpr int kWinThreads = 256;
 constexpr int kWinMaxFuncs = 8, kWinMaxCarried = 16;
 
 __device__ __forceinline__ int64_t winRow(const uint32_t* ids, int64_t i) { return ids ? (int64_t) ids[i] : i; }
@@ -77,13 +77,11 @@ __global__ void __launch_bounds__(kWinThreads) winHeadsKernel(const __grid_const
    }
 }
 
-// ---------------------------------------------------------------- tile scans
-// An Op has T, identity(), combine(a, b), load(k) (the value at scan position k) and store(k, inclusive scan at k).
+// ---------------------------------------------------------------- the scans' Ops (tilescan.cuh)
 struct WinSum {
    unsigned long long lo, hi, cnt; // i128 sum of the non-NULL values (wrapping), their count
 };
-__device__ __forceinline__ uint32_t winShflUp(uint32_t v, int o) { return __shfl_up_sync(0xffffffffu, v, o); }
-__device__ __forceinline__ WinSum winShflUp(const WinSum& v, int o) {
+__device__ __forceinline__ WinSum tileShflUp(const WinSum& v, int o) {
    return WinSum{__shfl_up_sync(0xffffffffu, v.lo, o), __shfl_up_sync(0xffffffffu, v.hi, o), __shfl_up_sync(0xffffffffu, v.cnt, o)};
 }
 // partition start of row k: the last head at or before k
@@ -138,75 +136,6 @@ struct WinSumOp {
       counts[k] = v.cnt;
    }
 };
-// the exclusive scan of one value per thread across the CTA; *total = the CTA's combined value
-template <class Op>
-__device__ __forceinline__ typename Op::T winBlockScan(const Op& op, typename Op::T v, typename Op::T* total) {
-   using T = typename Op::T;
-   __shared__ T warpTot[kWinThreads / 32];
-   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-   T x = v;
-   for (int o = 1; o < 32; o <<= 1) {
-      const T y = winShflUp(x, o);
-      if (lane >= o) x = op.combine(y, x);
-   }
-   T ex = winShflUp(x, 1);
-   if (lane == 0) ex = op.identity();
-   if (lane == 31) warpTot[warp] = x;
-   __syncthreads();
-   T pre = op.identity(), all = op.identity();
-   for (int w = 0; w < kWinThreads / 32; w++) {
-      if (w < warp) pre = op.combine(pre, warpTot[w]);
-      all = op.combine(all, warpTot[w]);
-   }
-   __syncthreads(); // warpTot is free for the next call
-   *total = all;
-   return op.combine(pre, ex);
-}
-template <class Op>
-__global__ void __launch_bounds__(kWinThreads) winScanReduceKernel(const __grid_constant__ Op op, int64_t n, typename Op::T* tileAgg) {
-   using T = typename Op::T;
-   const int64_t base = (int64_t) blockIdx.x * kWinTile + (int64_t) threadIdx.x * kWinItems;
-   T a = op.identity();
-#pragma unroll
-   for (int q = 0; q < kWinItems; q++)
-      if (base + q < n) a = op.combine(a, op.load(base + q));
-   T total;
-   winBlockScan(op, a, &total);
-   if (threadIdx.x == 0) tileAgg[blockIdx.x] = total;
-}
-// one CTA: the exclusive scan of the tile totals, in place
-template <class Op>
-__global__ void __launch_bounds__(kWinThreads) winScanTilesKernel(const __grid_constant__ Op op, int64_t nTiles, typename Op::T* tileAgg) {
-   using T = typename Op::T;
-   T carry = op.identity(); // the same in every thread
-   for (int64_t b = 0; b < nTiles; b += kWinThreads) {
-      const int64_t i = b + threadIdx.x;
-      T total;
-      const T ex = winBlockScan(op, i < nTiles ? tileAgg[i] : op.identity(), &total);
-      if (i < nTiles) tileAgg[i] = op.combine(carry, ex);
-      carry = op.combine(carry, total);
-   }
-}
-template <class Op>
-__global__ void __launch_bounds__(kWinThreads) winScanDownKernel(const __grid_constant__ Op op, int64_t n, const typename Op::T* tileAgg) {
-   using T = typename Op::T;
-   const int64_t base = (int64_t) blockIdx.x * kWinTile + (int64_t) threadIdx.x * kWinItems;
-   T item[kWinItems];
-   T a = op.identity();
-#pragma unroll
-   for (int q = 0; q < kWinItems; q++) {
-      item[q] = base + q < n ? op.load(base + q) : op.identity();
-      a = op.combine(a, item[q]);
-   }
-   T total;
-   T run = op.combine(tileAgg[blockIdx.x], winBlockScan(op, a, &total));
-#pragma unroll
-   for (int q = 0; q < kWinItems; q++) {
-      run = op.combine(run, item[q]);
-      if (base + q < n) op.store(base + q, run);
-   }
-}
-
 // ---------------------------------------------------------------- MIN / MAX segment tree
 // node k (1 <= k < 2 leaves) covers leaves [k << d, (k + 1) << d) of its level; leaf `leaves + i` is row i in window order.  A NULL
 // leaf (and the padding past n) holds the identity of the operation, and any[k] says whether the node covers a non-NULL value.
@@ -334,17 +263,6 @@ __global__ void __launch_bounds__(kWinThreads) winFramesKernel(const __grid_cons
 static unsigned winGrid(const LdbContext* ctx, uint64_t items) {
    return (unsigned) std::max<uint64_t>(1, std::min<uint64_t>((items + kWinThreads - 1) / kWinThreads, (uint64_t) ctx->smCount * 16));
 }
-template <class Op>
-static void winScan(LdbContext* ctx, Scratch& tmp, const Op& op, int64_t n) {
-   using T = typename Op::T;
-   const int64_t tiles = (n + kWinTile - 1) / kWinTile;
-   T* agg = tmp.alloc<T>((size_t) tiles * sizeof(T));
-   ctx->launch("window_scan", [&] {
-      winScanReduceKernel<Op><<<(unsigned) tiles, kWinThreads, 0, ctx->compute>>>(op, n, agg);
-      winScanTilesKernel<Op><<<1, kWinThreads, 0, ctx->compute>>>(op, tiles, agg);
-      winScanDownKernel<Op><<<(unsigned) tiles, kWinThreads, 0, ctx->compute>>>(op, n, agg);
-   });
-}
 template <class V>
 static void winTree(LdbContext* ctx, const ProgCol& arg, const uint32_t* ids, int64_t n, uint64_t leaves, int isMax, V* val, uint8_t* any) {
    ctx->launch("window_tree", [&] {
@@ -469,8 +387,8 @@ static void tableWindow(LdbTable* src, int32_t n_partition, const char* const* p
          wk.col[k].type = src->columns[keys[k].first].type;
       }
       ctx->launch("window_partition", [&] { winHeadsKernel<<<winGrid(ctx, (uint64_t) n), kWinThreads, 0, ctx->compute>>>(wk, ids, n, head); });
-      winScan(ctx, tmp, WinStartOp{head, start}, n);
-      winScan(ctx, tmp, WinEndOp{head, end, n}, n);
+      tileScan(ctx, tmp, WinStartOp{head, start}, n, "window_scan");
+      tileScan(ctx, tmp, WinEndOp{head, end, n}, n, "window_scan");
       fp.start = start;
       fp.end = end;
       // per function its scan or its tree
@@ -483,7 +401,7 @@ static void tableWindow(LdbTable* src, int32_t n_partition, const char* const* p
          if (f.kind == LDB_WIN_SUM || f.kind == LDB_WIN_COUNT) {
             unsigned long long* sums = f.kind == LDB_WIN_SUM ? tmp.alloc<unsigned long long>(rows * 16) : nullptr;
             unsigned long long* counts = tmp.alloc<unsigned long long>(rows * 8);
-            winScan(ctx, tmp, WinSumOp{arg, ids, sums, counts}, n);
+            tileScan(ctx, tmp, WinSumOp{arg, ids, sums, counts}, n, "window_scan");
             f.sums = sums;
             f.counts = counts;
          } else {

@@ -505,6 +505,24 @@ class RawTable:
                                               0 if columns is None else len(columns), carried, name.encode(), C.byref(t), C.byref(e)), e)
         return RawTable(self.ctx, t)
 
+    def setop(self, other, kind: str, columns=None, other_columns=None, name="setop") -> "RawTable":
+        """A set operation (ldb_gpu_table_setop) of this table's rows with `other`'s as a new table: kind one of capi.SETOP ("union_all",
+        "union", "intersect", "intersect_all", "except", "except_all"; "distinct" with other=None).  columns / other_columns: the
+        positional column lists (None: every column).  Each distinct row comes at its first occurrence in this table's rows followed by
+        other's, ALL copies consecutive.  `other` may be a RawTable, a runtime.Table or this table itself."""
+        enc = lambda xs: None if xs is None else (C.c_char_p * max(1, len(xs)))(*[x.encode() for x in xs])
+        cols = None if columns is None else list(columns)
+        ocols = None if other_columns is None else list(other_columns)
+        n = len(cols) if cols is not None else len(ocols) if ocols is not None else 0
+        t, e = C.c_void_p(), Error()
+        check(self.ctx.L.ldb_gpu_table_setop(self.h, None if other is None else other.h, capi.SETOP[kind], n, enc(cols), enc(ocols), name.encode(),
+                                             C.byref(t), C.byref(e)), e)
+        return RawTable(self.ctx, t)
+
+    def distinct(self, columns=None, name="distinct") -> "RawTable":
+        """SELECT DISTINCT over `columns` (None: every column), each distinct row at its first occurrence."""
+        return self.setop(None, "distinct", columns, None, name)
+
     def destroy(self):
         if self.h:
             self.ctx.L.ldb_gpu_table_destroy(self.h)
