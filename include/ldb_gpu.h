@@ -600,8 +600,9 @@ int ldb_gpu_table_gather_strings(LdbTable* t, const char* column, const int64_t*
  *   those and date32 and char(1), COUNT any column.  A materialised column holding double bits is read as the decimal it is typed as.
  *   Errors: LDB_ERR_UNSUPPORTED naming the column for a float or utf8 argument of SUM / MIN / MAX or a key of another type; also for a
  *   multi-batch source, 2^32 rows or more, or a call inside a captured query (the sort reads string lengths on the host).
- *   LDB_ERR_INVALID for null arguments, unknown columns or kinds, counts out of range or a bad frame.  Everything is checked before the
- *   first launch. */
+ *   LDB_ERR_INVALID for null arguments, unknown columns or kinds, counts out of range or a bad frame, and for two output columns of
+ *   one name (a function named like a carried column, carried columns of columns = NULL included; two functions of one name; a column
+ *   carried twice), naming the clash: later calls find result columns by name.  Everything is checked before the first launch. */
 enum LdbWindowKind { LDB_WIN_ROW_NUMBER = 1, LDB_WIN_COUNT_STAR = 2, LDB_WIN_COUNT = 3, LDB_WIN_SUM = 4, LDB_WIN_MIN = 5, LDB_WIN_MAX = 6 };
 typedef struct LdbWindowFunc {
    int32_t kind;       /* LdbWindowKind */

@@ -318,6 +318,18 @@ static void tableWindow(LdbTable* src, int32_t n_partition, const char* const* p
       for (int ci = 0; ci < (int) src->columns.size(); ci++) carried.push_back(ci);
       if (carried.size() > (size_t) kWinMaxCarried) fail(LDB_ERR_INVALID, "a window carries 0..16 columns: name them (the table has more)");
    }
+   // every column of the result is found by its name (the first match), so no two may share one: a function named like a carried
+   // column, two functions of one name or a column carried twice would leave a column that no later call can read
+   const size_t nCarried = carried.size();
+   for (size_t a = 0; a < nCarried + n_funcs; a++) {
+      const std::string na = a < nCarried ? src->columns[carried[a]].name : std::string(funcs[a - nCarried].name);
+      for (size_t b = 0; b < a; b++) {
+         const std::string nb = b < nCarried ? src->columns[carried[b]].name : std::string(funcs[b - nCarried].name);
+         if (na != nb) continue;
+         const char* what = a < nCarried ? "a column carried twice" : b < nCarried ? "a function named like a carried column" : "two functions of one name";
+         fail(LDB_ERR_INVALID, "window output column " + na + " is named twice (" + what + ")");
+      }
+   }
    if (src->batches.size() > 1) fail(LDB_ERR_UNSUPPORTED, "windows run over single-batch tables (materialised results, exported groups, received or sorted tables)");
    const int64_t n = src->numRows;
    if (n >= (int64_t) 1 << 32) fail(LDB_ERR_UNSUPPORTED, "a window handles up to 2^32 - 1 rows");
