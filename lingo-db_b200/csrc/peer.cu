@@ -19,6 +19,7 @@
 #include "progcol.cuh"
 #include "program.h"
 #include "sortkey.cuh"
+#include "tilescan.cuh"
 
 #include <algorithm>
 #include <cstring>
@@ -219,7 +220,7 @@ struct TableShipBatch {
    uint8_t* recv[kMaxPeers];    // every rank's receive region (peer-mapped)
    unsigned long long rows[kMaxPeers]; // the rows every rank receives (its N_d)
    unsigned long long base[kMaxPeers]; // the row of receiver d where this source's rows start
-   // utf8 columns (the string kernels only; the fixed-width kernels never read these)
+   // utf8 columns
    int32_t nStr;                       // shipped utf8 columns
    int8_t strCol[kShipMaxCols];        // utf8 column j: its index among the shipped columns
    int8_t strOf[kShipMaxCols];         // shipped column c: its utf8 index j, or -1
@@ -227,26 +228,13 @@ struct TableShipBatch {
    uint32_t byteBase[kMaxPeers][kShipMaxCols]; // the byte of receiver d's column j where this source's bytes start
 };
 static_assert(sizeof(TableShipBatch) <= 4096, "TableShipBatch is a __grid_constant__ kernel parameter (4 KiB at most)");
-// hist rows of the string count kernel: rows of destination d at row d, bytes of (destination d, utf8 column j) at row world + d nStr + j;
+// hist rows of the count kernel: rows of destination d at row d, bytes of (destination d, utf8 column j) at row world + d nStr + j;
 // the scan turns row r into totals[r], which the matrix all-gather carries (kShipBlockU64 u64 per rank at most)
 constexpr int kShipBlockU64 = kMaxPeers * (1 + kShipMaxCols);
-// byte offsets of the arrays of a receive region of n rows; returns its size
-__host__ __device__ inline uint64_t shipLayout(uint64_t n, const int32_t* outBytes, int nCols, uint64_t* colOff, uint64_t* validOff) {
-   uint64_t off = 0;
-   for (int c = 0; c < nCols; c++) {
-      colOff[c] = off;
-      off += (n * (uint64_t) outBytes[c] + 15) & ~uint64_t(15);
-   }
-   for (int c = 0; c < nCols; c++) {
-      validOff[c] = off;
-      off += (n + 15) & ~uint64_t(15);
-   }
-   return off;
-}
-// the same with utf8 columns: strOf[c] >= 0 marks a utf8 column (n + 1 int32 offsets) whose bytes, strBytes[strOf[c]], follow the cells
-// of every column; bytesOff[j] = where utf8 column j's bytes start.  Without utf8 columns this is shipLayout.
-__host__ __device__ inline uint64_t shipLayoutVar(uint64_t n, const int32_t* outBytes, int nCols, const int8_t* strOf, int nStr, const uint32_t* strBytes,
-                                                  uint64_t* colOff, uint64_t* validOff, uint64_t* bytesOff) {
+// byte offsets of the arrays of a receive region of n rows; returns its size.  strOf[c] >= 0 marks a utf8 column (n + 1 int32 offsets)
+// whose bytes, strBytes[strOf[c]], follow the cells of every column; bytesOff[j] = where utf8 column j's bytes start.
+__host__ __device__ inline uint64_t shipLayout(uint64_t n, const int32_t* outBytes, int nCols, const int8_t* strOf, int nStr, const uint32_t* strBytes,
+                                               uint64_t* colOff, uint64_t* validOff, uint64_t* bytesOff) {
    uint64_t off = 0;
    for (int c = 0; c < nCols; c++) {
       colOff[c] = off;
@@ -274,28 +262,6 @@ __device__ __forceinline__ int shipOwnerOf(const TableShipBatch& p, int64_t row)
    }
    return keyOwner(keyTupleHash(keys, p.nKeys, nulls), p.world);
 }
-// the count kernel's body for an owner rule ownerOf(row): tableShipCountKernel (key hash) and tableShipCountRangeKernel (sort splitters)
-template <class OwnerOf>
-__device__ __forceinline__ void shipCountRows(const TableShipBatch& p, const OwnerOf& ownerOf) {
-   __shared__ unsigned int cnt[kMaxPeers];
-   if (threadIdx.x < kMaxPeers) cnt[threadIdx.x] = 0;
-   __syncthreads();
-   const int lane = threadIdx.x & 31;
-   const int64_t begin = (int64_t) blockIdx.x * kShipTile, end = min(begin + kShipTile, p.nRows);
-   for (int64_t t = begin; t < end; t += kShipThreads) {
-      const int64_t i = t + threadIdx.x;
-      const bool valid = i < end;
-      const int d = valid ? ownerOf(i) : -1;
-      if (valid) p.owners[p.firstRow + i] = (uint8_t) d;
-      const unsigned same = __match_any_sync(0xffffffffu, d);
-      if (valid && lane == __ffs(same) - 1) atomicAdd(&cnt[d], (unsigned) __popc(same));
-   }
-   __syncthreads();
-   if (threadIdx.x < p.world) p.hist[(size_t) threadIdx.x * p.nCtas + p.ctaBase + blockIdx.x] = cnt[threadIdx.x];
-}
-__global__ void __launch_bounds__(kShipThreads) tableShipCountKernel(const __grid_constant__ TableShipBatch p) {
-   shipCountRows(p, [&](int64_t i) { return shipOwnerOf(p, i); });
-}
 // a utf8 cell's byte count: bytes[off[i] .. off[i+1]) as strCompare (program.cu) reads them; a NULL string ships none.  A warp's 32 cells
 // come from one batch, whose offsets are int32, so their sum fits 32 bits.
 __device__ __forceinline__ uint32_t shipStrLen(const ProgCol& c, int64_t row) {
@@ -303,10 +269,11 @@ __device__ __forceinline__ uint32_t shipStrLen(const ProgCol& c, int64_t row) {
    const int32_t* off = (const int32_t*) c.data + row;
    return (uint32_t) (off[1] - off[0]);
 }
-// tableShipCountKernel with utf8 columns: also the bytes per (destination, utf8 column, CTA), in hist row world + d nStr + j.  A broadcast
-// counts every row for destination 0 (the other destinations' rows stay 0) and writes no owners.
+// the count kernel's body for an owner rule ownerOf(row): tableShipCountKernel (key hash) and tableShipCountRangeKernel (sort splitters).
+// Per CTA the rows per destination, in hist row d, and with utf8 columns the bytes per (destination, utf8 column), in hist row
+// world + d nStr + j.  A broadcast counts every row for destination 0 (the other destinations' rows stay 0) and writes no owners.
 template <class OwnerOf>
-__device__ __forceinline__ void shipCountStrRows(const TableShipBatch& p, const OwnerOf& ownerOf) {
+__device__ __forceinline__ void shipCountRows(const TableShipBatch& p, const OwnerOf& ownerOf) {
    __shared__ unsigned int cnt[kMaxPeers];
    __shared__ unsigned long long bytes[kMaxPeers * kShipMaxCols];
    if (threadIdx.x < kMaxPeers) cnt[threadIdx.x] = 0;
@@ -332,43 +299,8 @@ __device__ __forceinline__ void shipCountStrRows(const TableShipBatch& p, const 
    if (threadIdx.x < p.world) p.hist[(size_t) threadIdx.x * p.nCtas + at] = cnt[threadIdx.x];
    for (int x = threadIdx.x; x < p.world * p.nStr; x += kShipThreads) p.hist[(size_t) (p.world + x) * p.nCtas + at] = bytes[x];
 }
-__global__ void __launch_bounds__(kShipThreads) tableShipCountStrKernel(const __grid_constant__ TableShipBatch p) {
-   shipCountStrRows(p, [&](int64_t i) { return shipOwnerOf(p, i); });
-}
-// CTA d: exclusive scan of destination d's per-CTA counts, in place; totals[d] = the rows this rank sends rank d
-__global__ void __launch_bounds__(1024) tableShipScanKernel(unsigned long long* hist, int64_t nCtas, unsigned long long* totals) {
-   __shared__ unsigned long long warpSums[32];
-   __shared__ unsigned long long carry;
-   unsigned long long* h = hist + (size_t) blockIdx.x * nCtas;
-   if (threadIdx.x == 0) carry = 0;
-   __syncthreads();
-   for (int64_t base = 0; base < nCtas; base += 1024) {
-      const int64_t i = base + threadIdx.x;
-      const unsigned long long v = i < nCtas ? h[i] : 0ull;
-      unsigned long long x = v;
-      for (int o = 1; o < 32; o <<= 1) {
-         const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o);
-         if ((threadIdx.x & 31) >= o) x += y;
-      }
-      if ((threadIdx.x & 31) == 31) warpSums[threadIdx.x >> 5] = x;
-      __syncthreads();
-      if (threadIdx.x < 32) {
-         const unsigned long long w = warpSums[threadIdx.x];
-         unsigned long long ws = w;
-         for (int o = 1; o < 32; o <<= 1) {
-            const unsigned long long y = __shfl_up_sync(0xffffffffu, ws, o);
-            if (threadIdx.x >= o) ws += y;
-         }
-         warpSums[threadIdx.x] = ws - w;
-      }
-      __syncthreads();
-      const unsigned long long excl = carry + warpSums[threadIdx.x >> 5] + (x - v);
-      if (i < nCtas) h[i] = excl;
-      __syncthreads();
-      if (threadIdx.x == 1023) carry = excl + v;
-      __syncthreads();
-   }
-   if (threadIdx.x == 0) totals[blockIdx.x] = carry;
+__global__ void __launch_bounds__(kShipThreads) tableShipCountKernel(const __grid_constant__ TableShipBatch p) {
+   shipCountRows(p, [&](int64_t i) { return shipOwnerOf(p, i); });
 }
 // one cell into the receive region: the low outBytes bytes of the source cell; a narrowed 8-byte decimal sign-extended to 16
 __device__ __forceinline__ void shipCell(const ProgCol& c, int w, int64_t row, uint8_t* dst) {
@@ -388,83 +320,39 @@ __device__ __forceinline__ void shipCell(const ProgCol& c, int w, int64_t row, u
       default: *dst = *s;
    }
 }
-__global__ void __launch_bounds__(kShipThreads) tableShipSendKernel(const __grid_constant__ TableShipBatch p) {
-   __shared__ uint64_t colOff[kMaxPeers][kShipMaxCols], validOff[kMaxPeers][kShipMaxCols];
-   __shared__ unsigned long long running[kMaxPeers];    // the next position of this CTA's rows in receiver d
-   __shared__ unsigned int warpCnt[kShipThreads / 32][kMaxPeers];
-   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-   const int64_t begin = (int64_t) blockIdx.x * kShipTile, end = min(begin + kShipTile, p.nRows);
-   if (threadIdx.x < p.world) {
-      const int d = threadIdx.x;
-      shipLayout(p.rows[d], p.outBytes, p.nCols, colOff[d], validOff[d]);
-      running[d] = p.base[d] + (p.broadcast ? (unsigned long long) (p.firstRow + begin) : p.hist[(size_t) d * p.nCtas + p.ctaBase + blockIdx.x]);
-   }
-   __syncthreads();
-   auto store = [&](int64_t i, int d, unsigned long long pos) {
-      uint8_t* r = p.recv[d];
-      for (int c = 0; c < p.nCols; c++) {
-         const bool null = colIsNull(p.cols[c], i);
-         shipCell(p.cols[c], p.outBytes[c], i, r + colOff[d][c] + pos * (uint64_t) p.outBytes[c]);
-         r[validOff[d][c] + pos] = null ? 0 : 1;
-      }
-   };
-   if (p.broadcast) { // row i of the batch is row base[d] + firstRow + i of every receiver
-      for (int64_t i = begin + threadIdx.x; i < end; i += kShipThreads)
-         for (int d = 0; d < p.world; d++) store(i, d, running[d] + (unsigned long long) (i - begin));
-      return;
-   }
-   for (int64_t t = begin; t < end; t += kShipThreads) {
-      if (threadIdx.x < kShipThreads / 32 * kMaxPeers) (&warpCnt[0][0])[threadIdx.x] = 0;
-      __syncthreads();
-      const int64_t i = t + threadIdx.x;
-      const bool valid = i < end;
-      const int d = valid ? p.owners[p.firstRow + i] : kMaxPeers;
-      const unsigned same = __match_any_sync(0xffffffffu, d);
-      const unsigned rankInWarp = __popc(same & ((1u << lane) - 1));
-      if (valid && rankInWarp == 0) warpCnt[warp][d] = __popc(same);
-      __syncthreads();
-      if (valid) {
-         unsigned before = 0;
-         for (int w = 0; w < warp; w++) before += warpCnt[w][d];
-         store(i, d, running[d] + before + rankInWarp);
-      }
-      __syncthreads();
-      if (threadIdx.x < p.world) {
-         unsigned tot = 0;
-         for (int w = 0; w < kShipThreads / 32; w++) tot += warpCnt[w][threadIdx.x];
-         running[threadIdx.x] += tot;
-      }
-      __syncthreads();
-   }
-}
-// tableShipSendKernel with utf8 columns.  Rows are ranked as there; a row's thread stores its fixed-width cells, its validity bytes and,
-// per utf8 column, the offset of its string in the receiver: this source's byte base + the CTA's scanned bytes + the bytes of earlier
-// passes, of earlier warps and of the earlier lanes of its warp with the same destination.  So the strings of one warp's rows for one
-// destination are adjacent in the receiver, and the whole warp copies that range: lanes take consecutive bytes, each walking the
-// warp's rows in (destination, lane) order.  A broadcast ranks every row for destination 0 and stores it into every rank.
+// The send kernel: a row's thread stores its fixed-width cells, its validity bytes and, per utf8 column, the offset of its string in the
+// receiver: this source's byte base + the CTA's scanned bytes + the bytes of earlier passes, of earlier warps and of the earlier lanes of
+// its warp with the same destination.  So the strings of one warp's rows for one destination are adjacent in the receiver, and the whole
+// warp copies that range: lanes take consecutive bytes, each walking the warp's rows in (destination, lane) order.  A broadcast ranks
+// every row for destination 0 and stores it into every rank; one without utf8 columns is not counted (hist is null), and its CTA's rows
+// start at firstRow + begin, where the scan would have put them.
+// kStrings = false, for shipments without utf8 columns, drops the string work and arrays (the string instance sent one int64 column 1.5x slower).
 constexpr int kShipWarps = kShipThreads / 32;
-__global__ void __launch_bounds__(kShipThreads) tableShipSendStrKernel(const __grid_constant__ TableShipBatch p) {
-   __shared__ uint64_t colOff[kMaxPeers][kShipMaxCols], validOff[kMaxPeers][kShipMaxCols], bytesOff[kMaxPeers][kShipMaxCols];
-   __shared__ unsigned long long running[kMaxPeers];                   // this CTA's rows for destination d before the pass (from base[d])
-   __shared__ unsigned long long byteRunning[kMaxPeers][kShipMaxCols]; // its bytes of utf8 column j for d before the pass (from byteBase)
+template <bool kStrings>
+__global__ void __launch_bounds__(kShipThreads) tableShipSendKernel(const __grid_constant__ TableShipBatch p) {
+   constexpr int kS = kStrings ? kShipMaxCols : 1, kSlots = kStrings ? 32 : 1; // the string arrays' extents
+   __shared__ uint64_t colOff[kMaxPeers][kShipMaxCols], validOff[kMaxPeers][kShipMaxCols], bytesOff[kMaxPeers][kS];
+   __shared__ unsigned long long running[kMaxPeers];        // this CTA's rows for destination d before the pass (from base[d])
+   __shared__ unsigned long long byteRunning[kMaxPeers][kS]; // its bytes of utf8 column j for d before the pass (from byteBase)
    __shared__ unsigned int warpCnt[kShipWarps][kMaxPeers];
-   __shared__ unsigned int warpBytes[kShipWarps][kMaxPeers][kShipMaxCols];
-   __shared__ uint32_t slotEnd[kShipWarps][33]; // the warp's lanes in (destination, lane) order: slot k's string is [slotEnd[k], slotEnd[k+1])
-   __shared__ int32_t slotSrc[kShipWarps][32];  // and starts at source byte slotSrc[k]
+   __shared__ unsigned int warpBytes[kShipWarps][kMaxPeers][kS];
+   __shared__ uint32_t slotEnd[kShipWarps][kSlots + 1]; // the warp's lanes in (destination, lane) order: slot k's string is [slotEnd[k], slotEnd[k+1])
+   __shared__ int32_t slotSrc[kShipWarps][kSlots];      // and starts at source byte slotSrc[k]
    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-   const int world = p.world, nStr = p.nStr;
+   const int world = p.world, nStr = kStrings ? p.nStr : 0;
    const int64_t begin = (int64_t) blockIdx.x * kShipTile, end = min(begin + kShipTile, p.nRows);
    const size_t at = (size_t) p.ctaBase + blockIdx.x;
    if (threadIdx.x < world) {
       const int d = threadIdx.x;
-      shipLayoutVar(p.rows[d], p.outBytes, p.nCols, p.strOf, nStr, p.strBytes[d], colOff[d], validOff[d], bytesOff[d]);
-      running[d] = p.hist[(size_t) d * p.nCtas + at];
+      shipLayout(p.rows[d], p.outBytes, p.nCols, p.strOf, nStr, p.strBytes[d], colOff[d], validOff[d], bytesOff[d]);
+      running[d] = p.hist ? p.hist[(size_t) d * p.nCtas + at] : (unsigned long long) (p.firstRow + begin);
    }
    for (int x = threadIdx.x; x < world * nStr; x += kShipThreads) byteRunning[x / nStr][x % nStr] = p.hist[(size_t) (world + x) * p.nCtas + at];
    __syncthreads();
    for (int64_t t = begin; t < end; t += kShipThreads) {
       for (int x = threadIdx.x; x < kShipWarps * kMaxPeers; x += kShipThreads) (&warpCnt[0][0])[x] = 0;
-      for (int x = threadIdx.x; x < kShipWarps * kMaxPeers * kShipMaxCols; x += kShipThreads) (&warpBytes[0][0][0])[x] = 0;
+      if constexpr (kStrings)
+         for (int x = threadIdx.x; x < kShipWarps * kMaxPeers * kShipMaxCols; x += kShipThreads) (&warpBytes[0][0][0])[x] = 0;
       __syncthreads();
       const int64_t i = t + threadIdx.x;
       const bool valid = i < end;
@@ -479,7 +367,7 @@ __global__ void __launch_bounds__(kShipThreads) tableShipSendStrKernel(const __g
       }
       __syncthreads();
       // the row's slot (invalid lanes take the last ones) and its position relative to the source's first row in a receiver
-      unsigned slot = __popc(__ballot_sync(0xffffffffu, valid)) + rankInWarp, first = 0;
+      unsigned slot = kStrings ? __popc(__ballot_sync(0xffffffffu, valid)) + rankInWarp : 0, first = 0;
       unsigned long long rel = 0;
       if (valid) {
          unsigned before = 0;
@@ -492,7 +380,7 @@ __global__ void __launch_bounds__(kShipThreads) tableShipSendStrKernel(const __g
             const unsigned long long pos = p.base[r] + rel;
             for (int c = 0; c < p.nCols; c++) {
                const bool null = colIsNull(p.cols[c], i);
-               if (p.strOf[c] < 0) shipCell(p.cols[c], p.outBytes[c], i, dst + colOff[r][c] + pos * (uint64_t) p.outBytes[c]);
+               if (!kStrings || p.strOf[c] < 0) shipCell(p.cols[c], p.outBytes[c], i, dst + colOff[r][c] + pos * (uint64_t) p.outBytes[c]);
                dst[validOff[r][c] + pos] = null ? 0 : 1;
             }
          }
@@ -616,9 +504,6 @@ __device__ __forceinline__ int sortRangeOwner(const TableShipBatch& p, const Sor
 __global__ void __launch_bounds__(kShipThreads) tableShipCountRangeKernel(const __grid_constant__ TableShipBatch p, const __grid_constant__ SortSplit s) {
    shipCountRows(p, [&](int64_t i) { return sortRangeOwner(p, s, i); });
 }
-__global__ void __launch_bounds__(kShipThreads) tableShipCountRangeStrKernel(const __grid_constant__ TableShipBatch p, const __grid_constant__ SortSplit s) {
-   shipCountStrRows(p, [&](int64_t i) { return sortRangeOwner(p, s, i); });
-}
 // sample j of a table of `total` rows is row mix64(j + c) mod total (a hash of the index, not a stride: a periodic input cannot alias
 // it); the launch over one batch writes the samples that fall into it, as tuples at out[j]
 __global__ void __launch_bounds__(256) sortSampleKernel(const __grid_constant__ TableShipBatch p, const __grid_constant__ SortSplit s, int64_t total, unsigned long long* out) {
@@ -634,7 +519,7 @@ __global__ void __launch_bounds__(256) sortSampleKernel(const __grid_constant__ 
 
 // Permute: rows ids[0..n) (ids null: rows 0..n-1) of a table of one or more batches into new single-batch columns: fixed-width cells at
 // outBytes (a narrowed decimal sign-extended, as the exchange ships it) and validity bytes by row id; a utf8 column's lengths by row id
-// (permuteCellsKernel, which also sums each CTA's bytes), the exclusive scan of the CTA sums (tableShipScanKernel), then its offsets and
+// (permuteCellsKernel, which also sums each CTA's bytes), the exclusive scan of the CTA sums (rowScanKernel), then its offsets and
 // bytes (permuteStringsKernel: each warp copies its 32 rows' strings, one contiguous range of the output, together).
 struct PermuteBatch {
    ProgCol cols[kShipMaxCols];
@@ -807,12 +692,10 @@ int ldb_gpu_comm_create(LdbContext* ctx, int32_t rank, int32_t world, int64_t us
       LDB_CUDA(cudaFuncGetAttributes(&fa, peerOrReduceKernel));
       LDB_CUDA(cudaFuncGetAttributes(&fa, peerPublishCountsKernel));
       LDB_CUDA(cudaFuncGetAttributes(&fa, tableShipCountKernel));
-      LDB_CUDA(cudaFuncGetAttributes(&fa, tableShipScanKernel));
-      LDB_CUDA(cudaFuncGetAttributes(&fa, tableShipSendKernel));
-      LDB_CUDA(cudaFuncGetAttributes(&fa, tableShipCountStrKernel));
-      LDB_CUDA(cudaFuncGetAttributes(&fa, tableShipSendStrKernel));
+      LDB_CUDA(cudaFuncGetAttributes(&fa, rowScanKernel<unsigned long long>));
+      LDB_CUDA(cudaFuncGetAttributes(&fa, tableShipSendKernel<false>));
+      LDB_CUDA(cudaFuncGetAttributes(&fa, tableShipSendKernel<true>));
       LDB_CUDA(cudaFuncGetAttributes(&fa, tableShipCountRangeKernel));
-      LDB_CUDA(cudaFuncGetAttributes(&fa, tableShipCountRangeStrKernel));
       LDB_CUDA(cudaFuncGetAttributes(&fa, sortSampleKernel));
       LDB_CUDA(cudaFuncGetAttributes(&fa, permuteCellsKernel));
       LDB_CUDA(cudaFuncGetAttributes(&fa, permuteStringsKernel));
@@ -894,16 +777,29 @@ static void wantConnected(LdbComm* c) {
    if (!c->connected && c->world > 1) fail(LDB_ERR_INVALID, "comm is not connected to its peers yet");
 }
 
+// the barrier on the compute stream (the current device is the comm's)
+static void commBarrier(LdbComm* c) {
+   if (c->world == 1) return;
+   LdbContext* ctx = c->ctx;
+   ctx->launch("peer_barrier", [&] {
+      peerBarrierKernel<<<c->world, 32, 0, ctx->compute>>>(c->view());
+      peerBumpKernel<<<1, 1, 0, ctx->compute>>>(c->view(), EPOCH_BARRIER, -1);
+   });
+}
+// waits for the compute stream and fails if a collective's wait timed out; the error word is read into pinned memory (a pageable copy
+// could stall a peer of the same process: see ldb_gpu_hashagg_exchange)
+static void checkPeers(LdbComm* c, int32_t* pinnedWord) {
+   LDB_CUDA(cudaMemcpyAsync(pinnedWord, c->error, 4, cudaMemcpyDeviceToHost, c->ctx->compute));
+   c->ctx->syncStream(c->ctx->compute);
+   if (*pinnedWord) fail(LDB_ERR_CUDA, "a peer did not arrive at a collective within the timeout (LDB_PEER_TIMEOUT_MS)");
+}
+
 int ldb_gpu_comm_barrier(LdbComm* c, LdbError* err) {
    return guarded(err, [&] {
       wantConnected(c);
       if (c->world == 1) return;
-      LdbContext* ctx = c->ctx;
-      LDB_CUDA(cudaSetDevice(ctx->device));
-      ctx->launch("peer_barrier", [&] {
-         peerBarrierKernel<<<c->world, 32, 0, ctx->compute>>>(c->view());
-         peerBumpKernel<<<1, 1, 0, ctx->compute>>>(c->view(), EPOCH_BARRIER, -1);
-      });
+      LDB_CUDA(cudaSetDevice(c->ctx->device));
+      commBarrier(c);
    });
 }
 
@@ -1086,24 +982,15 @@ int ldb_gpu_hashagg_exchange(LdbState* local, LdbState* owned, LdbComm* c, int64
       // while this rank's barrier waits for the peers, and a peer of the same process could then not launch its own barrier
       unsigned long long* counts = (unsigned long long*) ctx->scratch();
       int32_t* timedOut = (int32_t*) (counts + kMaxPeers);
-      auto barrier = [&] {
-         if (c->world == 1) return;
-         ctx->launch("peer_barrier", [&] {
-            peerBarrierKernel<<<c->world, 32, 0, ctx->compute>>>(c->view());
-            peerBumpKernel<<<1, 1, 0, ctx->compute>>>(c->view(), EPOCH_BARRIER, -1);
-         });
-      };
-      barrier();
+      commBarrier(c);
       ctx->launch("hashagg_send", [&] {
          LDB_CUDA(cudaMemsetAsync(x.cursors, 0, 8 * kMaxPeers, ctx->compute));
          launchHashAggSend(lt, x, ctx->smCount, ctx->compute);
          peerPublishCountsKernel<<<1, 32, 0, ctx->compute>>>(c->view(), kUserOff + cursorsOff, kUserOff + countsOff);
       });
-      barrier();
+      commBarrier(c);
       LDB_CUDA(cudaMemcpyAsync(counts, x.counts, 8 * (size_t) c->world, cudaMemcpyDeviceToHost, ctx->compute));
-      LDB_CUDA(cudaMemcpyAsync(timedOut, c->error, 4, cudaMemcpyDeviceToHost, ctx->compute));
-      ctx->syncStream(ctx->compute);
-      if (*timedOut) fail(LDB_ERR_CUDA, "a peer did not arrive at a collective within the timeout (LDB_PEER_TIMEOUT_MS)");
+      checkPeers(c, timedOut);
       const unsigned long long most = *std::max_element(counts, counts + c->world);
       if (most > (unsigned long long) capacity)
          fail(LDB_ERR_CAPACITY, "hash aggregation exchange: a source sent this rank " + std::to_string(most) + " groups, more than the receive capacity " +
@@ -1116,8 +1003,9 @@ int ldb_gpu_hashagg_exchange(LdbState* local, LdbState* owned, LdbComm* c, int64
 // the count matrix, capacity decision (identical on every rank) → barrier → send (per batch) → barrier → copy-out of the own region →
 // host wait.  While a rank's collectives wait for its peers nothing here blocks inside the driver: the temporaries and the pinned
 // scratch are taken before the first collective, the output buffers after the last, and host reads go to pinned memory.
-// With utf8 columns (ldb_gpu_table_exchange_varlen) the string kernels run instead, the matrix also carries every rank's bytes per
-// (destination, utf8 column), and the host decides the int32 limit of the receivers' offsets before the capacity.
+// With utf8 columns (ldb_gpu_table_exchange_varlen) the count and send kernels also count and ship the strings' bytes, the matrix also
+// carries every rank's bytes per (destination, utf8 column), and the host decides the int32 limit of the receivers' offsets before the
+// capacity.  A broadcast without utf8 columns skips the count: every rank receives every source's rows, which the host knows.
 // The sort exchange (ldb_gpu_table_sort_exchange) runs the same shipment with the range owner rule of its splitters; only the count
 // kernel differs, and what it does with the received region (sort and permute instead of copy-out).
 static_assert((size_t) kMaxPeers * kShipBlockU64 * 8 + 64 + 8 * kMaxPeers + 4 * kShipMaxCols <= LdbContext::kPinnedScratchBytes,
@@ -1179,7 +1067,7 @@ struct TableShipment {
       // before the first collective: staging waits, temporaries, pinned scratch
       for (auto& b : src->batches) ldb_gpu_wait_batch_internal(ctx, &b);
       for (auto& b : src->batches) nCtas += (b.nRows + kShipTile - 1) / kShipTile;
-      // the utf8 columns among the shipped ones: they select the string kernels, whose histograms have world (1 + nStr) rows
+      // the utf8 columns among the shipped ones: the histograms have world (1 + nStr) rows
       for (int j = 0; j < nCols; j++) {
          strOf[j] = -1;
          if (src->columns[ship[j]].type == LDB_UTF8) {
@@ -1233,18 +1121,6 @@ struct TableShipment {
          cta += (b.nRows + kShipTile - 1) / kShipTile;
       }
    }
-   void barrier() {
-      if (world == 1) return;
-      ctx->launch("peer_barrier", [&] {
-         peerBarrierKernel<<<world, 32, 0, ctx->compute>>>(c->view());
-         peerBumpKernel<<<1, 1, 0, ctx->compute>>>(c->view(), EPOCH_BARRIER, -1);
-      });
-   }
-   void checkPeers() {
-      LDB_CUDA(cudaMemcpyAsync(timedOut, c->error, 4, cudaMemcpyDeviceToHost, ctx->compute));
-      ctx->syncStream(ctx->compute);
-      if (*timedOut) fail(LDB_ERR_CUDA, "a peer did not arrive at a collective within the timeout (LDB_PEER_TIMEOUT_MS)");
-   }
    // range: the owner rule of the sort exchange's splitters (null: the key hash, or every rank without keys)
    void run(const SortSplit* range) {
       if (broadcast && !strings) {
@@ -1254,12 +1130,10 @@ struct TableShipment {
          ctx->launch("table_exchange_count", [&] {
             LDB_CUDA(cudaMemsetAsync(totals, 0, 8 * blockU64, ctx->compute));
             eachBatch([&](const TableShipBatch& q, int grid) {
-               if (range && strings) tableShipCountRangeStrKernel<<<grid, kShipThreads, 0, ctx->compute>>>(q, *range);
-               else if (range) tableShipCountRangeKernel<<<grid, kShipThreads, 0, ctx->compute>>>(q, *range);
-               else if (strings) tableShipCountStrKernel<<<grid, kShipThreads, 0, ctx->compute>>>(q);
+               if (range) tableShipCountRangeKernel<<<grid, kShipThreads, 0, ctx->compute>>>(q, *range);
                else tableShipCountKernel<<<grid, kShipThreads, 0, ctx->compute>>>(q);
             });
-            tableShipScanKernel<<<world * (1 + nStr), 1024, 0, ctx->compute>>>(hist, nCtas, totals);
+            rowScanKernel<<<world * (1 + nStr), 1024, 0, ctx->compute>>>(hist, nCtas, totals);
          });
       }
       // the count matrix on every rank
@@ -1269,7 +1143,7 @@ struct TableShipment {
          const uint8_t* gathered = allGatherSmall(c, totals, 8 * blockU64);
          LDB_CUDA(cudaMemcpy2DAsync(matrix, 8 * blockU64, gathered, kSlotBytes, 8 * blockU64, world, cudaMemcpyDeviceToHost, ctx->compute));
       }
-      checkPeers();
+      checkPeers(c, timedOut);
       // per receiver, from the same matrix on every rank: its rows and bytes, this source's bases in them, then the two decisions.  A
       // broadcast counted every row for destination 0, and every rank receives what destination 0 would.
       auto rowsOf = [&](int s, int d) { return matrix[s * blockU64 + (broadcast ? 0 : d)]; };
@@ -1297,14 +1171,14 @@ struct TableShipment {
       uint64_t need = 0;
       for (int d = 0; d < world; d++) {
          for (int j = 0; j < nStr; j++) p.strBytes[d][j] = (uint32_t) recvBytes[d][j];
-         need = std::max(need, shipLayoutVar(p.rows[d], outBytes, nCols, strOf, nStr, p.strBytes[d], colOff, validOff, bytesOff));
+         need = std::max(need, shipLayout(p.rows[d], outBytes, nCols, strOf, nStr, p.strBytes[d], colOff, validOff, bytesOff));
       }
       if (need > (uint64_t) regionBytes)
          fail(LDB_ERR_CAPACITY, "table exchange: a rank receives rows that need " + std::to_string(need) + " bytes of receive region, more than recv_bytes " +
                                    std::to_string(regionBytes) + "; retry with recv_bytes " + std::to_string(need));
       mine = p.rows[c->rank];
       for (int d = 0; d < world; d++) p.recv[d] = c->peerHeap[d] + kUserOff + recvOffset;
-      barrier(); // no peer still copies out of, or otherwise reads, the region it is about to receive into
+      commBarrier(c); // no peer still copies out of, or otherwise reads, the region it is about to receive into
       ctx->launch("table_exchange_send", [&] {
          eachBatch([&](const TableShipBatch& q, int grid) {
             TableShipBatch r = q;
@@ -1317,12 +1191,12 @@ struct TableShipment {
                   r.byteBase[d][j] = p.byteBase[d][j];
                }
             }
-            if (strings) tableShipSendStrKernel<<<grid, kShipThreads, 0, ctx->compute>>>(r);
-            else tableShipSendKernel<<<grid, kShipThreads, 0, ctx->compute>>>(r);
+            if (strings) tableShipSendKernel<true><<<grid, kShipThreads, 0, ctx->compute>>>(r);
+            else tableShipSendKernel<false><<<grid, kShipThreads, 0, ctx->compute>>>(r);
          });
       });
-      barrier(); // every peer's rows are in this rank's region
-      shipLayoutVar(mine, outBytes, nCols, strOf, nStr, p.strBytes[c->rank], colOff, validOff, bytesOff);
+      commBarrier(c); // every peer's rows are in this rank's region
+      shipLayout(mine, outBytes, nCols, strOf, nStr, p.strBytes[c->rank], colOff, validOff, bytesOff);
       region = c->heap + kUserOff + recvOffset;
       // a utf8 column's last offset is B_j, which the matrix gave: written into the region, its n + 1 offsets are one array
       for (int j = 0; j < nStr; j++) {
@@ -1345,7 +1219,7 @@ struct TableShipment {
          b.validBytes.push_back(region + validOff[j]);
       }
    }
-   void finish() { checkPeers(); } // the region is free for the next collective, the temporaries for the pool
+   void finish() { checkPeers(c, timedOut); } // the region is free for the next collective, the temporaries for the pool
 };
 
 static void tableExchange(bool varlen, LdbTable* src, int32_t n_keys, const char* const* key_columns, int32_t n_columns, const char* const* columns, LdbComm* c,
@@ -1459,7 +1333,7 @@ LdbBatch ldb::permuteRows(LdbTable* t, const std::vector<int>& cols, const int32
       ctx->launch("sort_exchange_permute", [&] {
          permuteCellsKernel<<<(unsigned) q.nCtas, kShipThreads, 0, ctx->compute>>>(q);
          if (q.nStr) {
-            tableShipScanKernel<<<q.nStr, 1024, 0, ctx->compute>>>(q.hist, q.nCtas, devTotals);
+            rowScanKernel<<<q.nStr, 1024, 0, ctx->compute>>>(q.hist, q.nCtas, devTotals);
             LDB_CUDA(cudaMemcpyAsync(totals, devTotals, 8 * (size_t) q.nStr, cudaMemcpyDeviceToHost, ctx->compute));
          }
       });
@@ -1588,7 +1462,7 @@ static void sortExchange(LdbTable* src, int32_t n_keys, const char* const* key_c
          const uint8_t* gathered = allGatherSmall(c, block, kSortBlockBytes);
          LDB_CUDA(cudaMemcpy2DAsync(pin, kSortBlockBytes, gathered, kSlotBytes, kSortBlockBytes, world, cudaMemcpyDeviceToHost, ctx->compute));
       }
-      s.checkPeers();
+      checkPeers(c, s.timedOut);
       // the splitters, the same on every rank: sample j of rank r stands for n_r / S_r rows; splitter d - 1 is the sample at which the
       // rows it and the smaller samples stand for first reach d N / world
       struct Sample {
@@ -1651,8 +1525,7 @@ int ldb_gpu_dict_unify(LdbState* local, LdbComm* c, int64_t recv_offset, int64_t
       if (local->kind != LDB_STATE_DICT) fail(LDB_ERR_INVALID, "not a string dictionary");
       if (local->ctx != c->ctx) fail(LDB_ERR_INVALID, "dictionary and comm belong to different contexts");
       wantConnected(c);
-      if (recv_offset < 0 || recv_bytes < 0 || recv_offset % 16 || recv_offset > (int64_t) c->userBytes || recv_bytes > (int64_t) c->userBytes - recv_offset)
-         fail(LDB_ERR_INVALID, "receive region outside the comm's user heap or not 16-byte aligned");
+      wantRegion(c, recv_offset, recv_bytes);
       LdbContext* ctx = c->ctx;
       if (ctx->capturing) fail(LDB_ERR_UNSUPPORTED, "dictionary unification reads the string counts on the host and cannot be captured");
       LDB_CUDA(cudaSetDevice(ctx->device));
@@ -1678,9 +1551,7 @@ int ldb_gpu_dict_unify(LdbState* local, LdbComm* c, int64_t recv_offset, int64_t
       ctx->launch("dict_export", [&] { launchDictExport(local->dict, n, offs, data, ctx->smCount, ctx->compute); });
       const uint8_t* gathered = allGatherSmall(c, block, 32);
       LDB_CUDA(cudaMemcpy2DAsync(blocks, 32, gathered, kSlotBytes, 32, world, cudaMemcpyDeviceToHost, ctx->compute));
-      LDB_CUDA(cudaMemcpyAsync(timedOut, c->error, 4, cudaMemcpyDeviceToHost, ctx->compute));
-      ctx->syncStream(ctx->compute);
-      if (*timedOut) fail(LDB_ERR_CUDA, "a peer did not arrive at a collective within the timeout (LDB_PEER_TIMEOUT_MS)");
+      checkPeers(c, timedOut);
       // every rank decides from the same gathered counts
       uint64_t blockOff[kMaxPeers + 1] = {}, byteBase[kMaxPeers + 1] = {}, rowBase[kMaxPeers + 1] = {};
       for (int s = 0; s < world; s++) {
@@ -1695,23 +1566,14 @@ int ldb_gpu_dict_unify(LdbState* local, LdbComm* c, int64_t recv_offset, int64_t
       if (blockOff[world] > (uint64_t) recv_bytes)
          fail(LDB_ERR_CAPACITY, "dictionary unification: the ranks' strings need " + std::to_string(blockOff[world]) + " bytes of receive region, more than recv_bytes " +
                                    std::to_string(recv_bytes) + "; retry with recv_bytes " + std::to_string(blockOff[world]));
-      auto barrier = [&] {
-         if (world == 1) return;
-         ctx->launch("peer_barrier", [&] {
-            peerBarrierKernel<<<world, 32, 0, ctx->compute>>>(c->view());
-            peerBumpKernel<<<1, 1, 0, ctx->compute>>>(c->view(), EPOCH_BARRIER, -1);
-         });
-      };
-      barrier(); // no peer still reads the region it is about to receive into
+      commBarrier(c); // no peer still reads the region it is about to receive into
       const size_t offVecs = align16((uint64_t) (n + 1) * 4) / 16, byteVecs = align16((uint64_t) bytes) / 16;
       ctx->launch("dict_unify_send", [&] {
          const dim3 grid((unsigned) std::min<size_t>(std::max<size_t>((offVecs + byteVecs + 255) / 256, 1), (size_t) ctx->smCount * 2), (unsigned) world);
          dictSendKernel<<<grid, 256, 0, ctx->compute>>>(c->view(), kUserOff + (size_t) recv_offset + blockOff[c->rank], (const int4*) offs, offVecs, (const int4*) data, byteVecs);
       });
-      barrier(); // every peer's block is in this rank's region
-      LDB_CUDA(cudaMemcpyAsync(timedOut, c->error, 4, cudaMemcpyDeviceToHost, ctx->compute));
-      ctx->syncStream(ctx->compute);
-      if (*timedOut) fail(LDB_ERR_CUDA, "a peer did not arrive at a collective within the timeout (LDB_PEER_TIMEOUT_MS)");
+      commBarrier(c); // every peer's block is in this rank's region
+      checkPeers(c, timedOut);
       // the received blocks as one utf8 column of N strings, in rank order
       const int64_t N = (int64_t) rowBase[world];
       Scratch col(ctx);

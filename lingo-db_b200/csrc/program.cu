@@ -5,6 +5,7 @@
 #include "progcol.cuh"
 #include "program.h"
 #include "sortkey.cuh"
+#include "tilescan.cuh"
 #include "../../include/ldb_gpu.h"
 
 #include <algorithm>
@@ -1096,37 +1097,6 @@ __global__ void __launch_bounds__(kSortThreads) sortHistKernel(const unsigned lo
    __syncthreads();
    hist[(size_t) threadIdx.x * gridDim.x + blockIdx.x] = h[threadIdx.x];
 }
-// exclusive scan over digit-major [256][nCtas] counts (single CTA; nCtas * 256 entries)
-__global__ void __launch_bounds__(1024) sortScanKernel(unsigned int* hist, int64_t total) {
-   __shared__ unsigned long long carry;
-   __shared__ unsigned int warpSums[32];
-   if (threadIdx.x == 0) carry = 0;
-   __syncthreads();
-   for (int64_t base = 0; base < total; base += 1024) {
-      const int64_t i = base + threadIdx.x;
-      unsigned int v = i < total ? hist[i] : 0u, x = v;
-      for (int o = 1; o < 32; o <<= 1) {
-         unsigned int y = __shfl_up_sync(0xffffffffu, x, o);
-         if ((threadIdx.x & 31) >= o) x += y;
-      }
-      if ((threadIdx.x & 31) == 31) warpSums[threadIdx.x >> 5] = x;
-      __syncthreads();
-      if (threadIdx.x < 32) {
-         unsigned int w = warpSums[threadIdx.x], ws = w;
-         for (int o = 1; o < 32; o <<= 1) {
-            unsigned int y = __shfl_up_sync(0xffffffffu, ws, o);
-            if (threadIdx.x >= o) ws += y;
-         }
-         warpSums[threadIdx.x] = ws - w; // exclusive
-      }
-      __syncthreads();
-      const unsigned long long excl = carry + warpSums[threadIdx.x >> 5] + (x - v);
-      if (i < total) hist[i] = (unsigned int) excl;
-      __syncthreads();
-      if (threadIdx.x == 1023) carry = excl + v;
-      __syncthreads();
-   }
-}
 __global__ void __launch_bounds__(kSortThreads) sortScatterKernel(const unsigned long long* keys, const uint32_t* vals, unsigned long long* keysOut, uint32_t* valsOut, int64_t n, int shift, const unsigned int* hist) {
    __shared__ unsigned int running[256];      // global base + items of this digit already placed by this CTA
    __shared__ unsigned int warpCnt[8][256];   // per-warp digit counts of the current tile
@@ -1172,7 +1142,7 @@ void launchRadixSortPairs(unsigned long long* keys, uint32_t* vals, unsigned lon
    uint32_t* vout = valsTmp;
    for (int pass = 0; pass < digits; pass++) {
       sortHistKernel<<<ctas, kSortThreads, 0, s>>>(kin, n, pass * 8, histScratch);
-      sortScanKernel<<<1, 1024, 0, s>>>(histScratch, (int64_t) ctas * 256);
+      rowScanKernel<<<1, 1024, 0, s>>>(histScratch, (int64_t) ctas * 256, nullptr); // digit-major [256][ctas]
       sortScatterKernel<<<ctas, kSortThreads, 0, s>>>(kin, vin, kout, vout, n, pass * 8, histScratch);
       std::swap(kin, kout);
       std::swap(vin, vout);
@@ -1250,7 +1220,7 @@ __global__ void dictCopyKernel(DictDev d, int64_t n, const uint32_t* offsets, ui
 void launchDictExport(const DictDev& d, int64_t n, uint32_t* offsets, uint8_t* bytes, int smCount, cudaStream_t s) {
    int grid = (int) std::min<int64_t>(std::max<int64_t>((n + 256) / 256, 1), (int64_t) smCount * 8);
    dictLengthsKernel<<<grid, 256, 0, s>>>(d.entryLen, n, offsets);
-   sortScanKernel<<<1, 1024, 0, s>>>(offsets, n + 1); // exclusive: offsets[n] = total bytes
+   rowScanKernel<<<1, 1024, 0, s>>>(offsets, n + 1, nullptr); // exclusive: offsets[n] = total bytes
    if (n) dictCopyKernel<<<(int) std::min<int64_t>((n + 7) / 8, (int64_t) smCount * 16), 256, 0, s>>>(d, n, offsets, bytes);
 }
 
@@ -1284,8 +1254,8 @@ __global__ void dictUnionFlagsKernel(const uint32_t* offsets, const uint8_t* byt
 void launchDictUnionRanks(const uint32_t* offsets, const uint8_t* bytes, const uint32_t* ids, int64_t n, uint32_t* codes, uint32_t* arenaOff, int smCount, cudaStream_t s) {
    int grid = (int) std::min<int64_t>(std::max<int64_t>((n + 256) / 256, 1), (int64_t) smCount * 8);
    dictUnionFlagsKernel<<<grid, 256, 0, s>>>(offsets, bytes, ids, n, codes, arenaOff);
-   sortScanKernel<<<1, 1024, 0, s>>>(codes, n + 1);
-   sortScanKernel<<<1, 1024, 0, s>>>(arenaOff, n + 1);
+   rowScanKernel<<<1, 1024, 0, s>>>(codes, n + 1, nullptr);
+   rowScanKernel<<<1, 1024, 0, s>>>(arenaOff, n + 1, nullptr);
 }
 // one thread per sorted position that starts a new string: its bytes into the arena at arenaOff[i], its entry at code codes[i], and a slot
 // on its probe sequence claimed and published with code + 1 in one CAS (nothing reads the dictionary during the build).  Which of two

@@ -1,5 +1,7 @@
 // tilescan.cuh — a device-wide inclusive scan over n positions for any associative Op: per tile a reduction, one CTA's exclusive scan
 // of the tile totals, then each tile rescanned from its prefix.  The window operator (window.cu) and the set operations (setop.cu).
+// And rowScanKernel, the one-launch exclusive sum of short rows: the radix sort's digit counts (program.cu), the table exchange's
+// histograms and the permute's byte sums (peer.cu).
 //
 // An Op has T, identity(), combine(a, b), load(k) (the value at scan position k) and store(k, inclusive scan at k).  T needs a
 // tileShflUp(T, offset) overload: uint32_t's is here, an Op's own struct brings its own (found by argument-dependent lookup).
@@ -91,6 +93,46 @@ static void tileScan(LdbContext* ctx, Scratch& tmp, const Op& op, int64_t n, con
       tileScanTilesKernel<Op><<<1, kTileScanThreads, 0, ctx->compute>>>(op, tiles, agg);
       tileScanDownKernel<Op><<<(unsigned) tiles, kTileScanThreads, 0, ctx->compute>>>(op, n, agg);
    });
+}
+
+// CTA r: the exclusive sum of row r (rows[r n .. r n + n)), in place, with a 64-bit carry across its 1024-element chunks; totals[r] =
+// the row's sum (totals null: none).  One launch, a CTA per row: for the few, short rows its callers scan, tileScan's three launches cost more.
+template <class T>
+__global__ void __launch_bounds__(1024) rowScanKernel(T* rows, int64_t n, unsigned long long* totals) {
+   __shared__ T warpSums[32];
+   __shared__ unsigned long long carry;
+   T* h = rows + (size_t) blockIdx.x * n;
+   if (threadIdx.x == 0) carry = 0;
+   __syncthreads();
+   T next = threadIdx.x < n ? h[threadIdx.x] : T(0);
+   for (int64_t base = 0; base < n; base += 1024) {
+      const int64_t i = base + threadIdx.x;
+      const T v = next;
+      next = i + 1024 < n ? h[i + 1024] : T(0); // the next chunk's load overlaps this chunk's scan: the loop is latency-bound
+      T x = v;
+      for (int o = 1; o < 32; o <<= 1) {
+         const T y = __shfl_up_sync(0xffffffffu, x, o);
+         if ((threadIdx.x & 31) >= o) x += y;
+      }
+      if ((threadIdx.x & 31) == 31) warpSums[threadIdx.x >> 5] = x;
+      __syncthreads();
+      if (threadIdx.x < 32) {
+         const T w = warpSums[threadIdx.x];
+         T ws = w;
+         for (int o = 1; o < 32; o <<= 1) {
+            const T y = __shfl_up_sync(0xffffffffu, ws, o);
+            if (threadIdx.x >= o) ws += y;
+         }
+         warpSums[threadIdx.x] = ws - w;
+      }
+      __syncthreads();
+      const unsigned long long excl = carry + warpSums[threadIdx.x >> 5] + (x - v);
+      if (i < n) h[i] = (T) excl;
+      __syncthreads();
+      if (threadIdx.x == 1023) carry = excl + v;
+      __syncthreads();
+   }
+   if (totals && threadIdx.x == 0) totals[blockIdx.x] = carry;
 }
 
 } // namespace ldb

@@ -277,17 +277,19 @@ def test_owner_depends_on_values_and_agrees_with_the_hash_aggregation_exchange(w
 # ---------------------------------------------------------------------------------------------------- 3. broadcast
 @pytest.mark.gpu
 def test_broadcast_gives_every_rank_the_same_concatenation():
-    world, n = 4, 900
-    v = R.gen_values(77, n, COLUMNS, null_rate=0.2, key_domain=1000)
-    bounds = [(0, 100), (100, 100), (100, 650), (650, 900)]
+    world = 4
     widths = {c: WIDTH[PHYS[c]] for c in FIXED}
-    with ranks(world) as (ctxs, comms):
-        tabs = [stage(c, f"s{r}", {k: x[lo:hi] for k, x in v.items()}, "host_sliced", r) if hi > lo else empty(c, f"s{r}") for r, (c, (lo, hi)) in enumerate(zip(ctxs, bounds))]
-        got = exchange(comms, tabs, [], columns=FIXED, name=None)
-        whole = rows_of(v, 0, n)
-        assert_received(got, [whole] * world, FIXED, widths, "broadcast")
-        for t in got:
-            t.destroy()
+    # one-tile shards; then shards of several 4 096-row tiles in ragged batches (staged with seeds 0..3) that end in partial tiles, a
+    # middle batch's included, so most tiles start at a source row that is not a multiple of the tile
+    for n, bounds in ((900, [(0, 100), (100, 100), (100, 650), (650, 900)]), (40000, [(0, 13000), (13000, 13000), (13000, 30000), (30000, 40000)])):
+        v = R.gen_values(77, n, COLUMNS, null_rate=0.2, key_domain=1000)
+        with ranks(world) as (ctxs, comms):
+            tabs = [stage(c, f"s{r}", {k: x[lo:hi] for k, x in v.items()}, "host_sliced", r) if hi > lo else empty(c, f"s{r}") for r, (c, (lo, hi)) in enumerate(zip(ctxs, bounds))]
+            got = exchange(comms, tabs, [], columns=FIXED, name=None)
+            whole = rows_of(v, 0, n)
+            assert_received(got, [whole] * world, FIXED, widths, f"broadcast of {n} rows")
+            for t in got:
+                t.destroy()
 
 
 # ---------------------------------------------------------------------------------------------------- 4. capacity
