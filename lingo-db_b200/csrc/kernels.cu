@@ -836,15 +836,17 @@ constexpr int kQty = 0, kEp = 1, kDisc = 2, kTax = 3;
 // hold modulo 2^64 and 2^128 too.  A row then costs three 32-bit shared atomics into its cell g*Dd*Dt + (d-min_d)*Dt + (t-min_t)
 // (64-bit shared atomics are CAS loops on sm_90a) and the products run once per cell and CTA at the end.  The summed columns enter
 // as offsets from their batch minimum (ep - min_ep, qty - min_qty; min * count is added back at the end, so negative values stay
-// exact), in three words that cannot overflow in one stage of 2 * kBlock * kEncFrames = 2048 rows when ep_off < 2^28 and
-// qty_off < 2^21 (the batch bounds, factoredFits):
-//   A = ep_off & 0xfffff  (< 2^20 per row),   B = (ep_off >> 20) << 12 | 1  (< 2^20 per row, the count in the low 12 bits),
-//   C = qty_off  (< 2^21 per row).
-// After each stage every thread folds the cells it owns (cell mod kBlock) into 64-bit sums in registers and zeroes them.  A batch has
-// fewer than 2^36 rows (factoredFits), so those sums stay below 2^64.
+// exact), in four 32-bit words per cell, with a split s of ep_off chosen per batch (factoredFold):
+//   L = ep_off & (2^s - 1),   H = ep_off >> s,   Q = qty_off,   N = 1  (the count).
+// A frame (a stage of 2 * kBlock * kEncFrames = 2048 rows, or one tile) adds at most 2048 rows to a cell, so K frames add at most
+// n = 2048 K, and the words cannot overflow while n (2^s - 1), n (range_ep >> s), n range_qty and n stay below 2^32.  The launcher
+// takes the s that allows the largest K (TPC-H: s = 12, K = 427; the worst batch factoredFits admits, ep_off < 2^28 and qty_off <
+// 2^21, still gets K = 1), and every K-th frame each thread folds the cells it owns (cell mod kBlock) into 64-bit sums in registers
+// and zeroes them.  A batch has fewer than 2^36 rows (factoredFits), so those sums stay below 2^64.
 constexpr int kCells = 512;
-constexpr int kCellWords = 3;
-static_assert(kEncFrames * kRowsPerThreadScan * kBlock <= 2048 && kCells % kBlock == 0, "factored cell words overflow");
+constexpr int kCellWords = 4;
+constexpr uint32_t kFacFrameRows = 2048;
+static_assert(kEncFrames * kRowsPerThreadScan * kBlock <= (int) kFacFrameRows && kCells % kBlock == 0, "factored cell words overflow");
 // the W-byte fields (W = 1 << sh <= 4) of 2 adjacent rows from shared address a (2W-byte aligned), zero-extended: one shared load
 __device__ __forceinline__ void encodedFields2(uint32_t a, int sh, uint32_t (&x)[2]) {
    if (sh == 0) {
@@ -1206,9 +1208,9 @@ __global__ void __launch_bounds__(kBlock, 2) scanGroupByKernel(const __grid_cons
 // fields are 1 byte wide.  Every stage or tile header's block lies inside the batch, so each of its rows has its cell and word budgets
 // and the 64-bit products of the fallback without a check in the kernel.
 // A frame is one TMA stage of kFacTiles tiles or one tile read with plain loads (the tail, or a batch without TMA), and every frame ends
-// at a CTA barrier.  The cell words are single-buffered: at the start of the next frame each thread folds the cells it owns into 64-bit
-// sums and zeroes them, and a second barrier lets that frame's atomics in.  (Double-buffered words, without that barrier, measured 12 %
-// faster, but their 6 KB more static shared memory would cost batches of 16 bytes per row their third CTA per SM.)  The stage ring
+// at a CTA barrier.  The cell words hold p.facFoldFrames frames (K, from the batch bounds): at the start of every K-th frame of a loop,
+// counted from the loop's index, and once before the tail tiles, each thread folds the cells it owns into 64-bit sums and zeroes them,
+// and a second barrier lets that frame's atomics in; the other frames pay neither.  The stage ring
 // holds kFacStages stages of kFacTiles tiles (50 KB at TPC-H widths; deeper rings of fewer tiles measured slower) and with about 8 KB of
 // static shared memory three CTAs fit an SM, which hide the latency of each warp's dependent run (loads → compare → vote → loads →
 // atomics).  A thread decodes its rows of a stage in runs of 4 adjacent rows, one shared load per column per run, so each chain
@@ -1229,7 +1231,7 @@ __global__ void __launch_bounds__(kBlock, 3) scanQ1FactoredKernel(const __grid_c
    __shared__ int32_t sSlot[LG];
    __shared__ int32_t sCount, sLock;
    __shared__ unsigned long long sAcc[LG][N][2];
-   __shared__ uint32_t sCell[kCellWords][kCells]; // {A, B, C} words per cell
+   __shared__ uint32_t sCell[kCellWords][kCells]; // {L, H, Q, N} words per cell
    __shared__ __align__(8) uint64_t sFull[S];        // stage s holds its tiles
 
    unsigned long long* const selfTime = selfTimeStart(p.table);
@@ -1248,20 +1250,21 @@ __global__ void __launch_bounds__(kBlock, 3) scanQ1FactoredKernel(const __grid_c
 #pragma unroll
       for (int j = 0; j < kOwned; j++) {
          const int cell = j * kBlock + threadIdx.x;
-         const uint32_t b = sCell[1][cell];
-         if (b != 0) { // B counts the cell's rows
-            cEp[j] += sCell[0][cell] + ((uint64_t) (b >> 12) << 20);
-            cCnt[j] += b & 0xfffu;
+         const uint32_t n = sCell[3][cell];
+         if (n != 0) {
+            cEp[j] += sCell[0][cell] + ((uint64_t) sCell[1][cell] << p.facShift);
+            cCnt[j] += n;
             cQty[j] += sCell[2][cell];
-            sCell[0][cell] = sCell[1][cell] = sCell[2][cell] = 0;
+            sCell[0][cell] = sCell[1][cell] = sCell[2][cell] = sCell[3][cell] = 0;
          }
       }
    };
-   // every thread passed the barrier behind the previous frame's atomics (or the set-up); folding cells nothing added to is a no-op, so
-   // the first frame needs no count
-   auto beginFrame = [&]() {
-      foldCells();
-      __syncthreads();
+   // every thread passed the barrier behind the previous frame's atomics (or the set-up); folding cells nothing added to is a no-op
+   auto beginFrame = [&](bool fold) {
+      if (fold) {
+         foldCells();
+         __syncthreads();
+      }
    };
 
    // the frame's header bases and what follows from them: the offsets of its value fields from the batch minima (a value is
@@ -1326,10 +1329,11 @@ __global__ void __launch_bounds__(kBlock, 3) scanQ1FactoredKernel(const __grid_c
       for (int i = 0; i < K; i++) {
          if (pass[i] && (uint32_t) id[i] < (uint32_t) GREG) {
             const uint32_t c = (uint32_t) id[i] * fDdDt + xv[kDisc][i] * fDt + xv[kTax][i] + cellOff;
-            const uint32_t ep = xv[kEp][i] + off[kEp];
-            atomicAdd(&sCell[0][c], ep & 0xfffffu);
-            atomicAdd(&sCell[1][c], (ep >> 20) << 12 | 1u);
+            const uint32_t ep = xv[kEp][i] + off[kEp], epHi = ep >> p.facShift;
+            atomicAdd(&sCell[0][c], ep - (epHi << p.facShift));
+            atomicAdd(&sCell[1][c], epHi);
             atomicAdd(&sCell[2][c], xv[kQty][i] + off[kQty]);
+            atomicAdd(&sCell[3][c], 1u);
          } else if (pass[i]) { // a group past the register set: its products in 64 bits (proven), shared sums or the HBM table
             int64_t vals[NV], q[N];
 #pragma unroll
@@ -1352,8 +1356,8 @@ __global__ void __launch_bounds__(kBlock, 3) scanQ1FactoredKernel(const __grid_c
    // one stage in shared memory: its F tiles of column c lie from stage + F * smemOffset[c] with equal headers (kernels.h), tile 0's
    // stands for all; thread t takes 2F rows of tile t / (kBlock / F) in runs of RUN adjacent rows, the lanes of a warp reading
    // consecutive RUN * W bytes per column, conflict-free at any W
-   auto stageFrame = [&](uint32_t stage) {
-      beginFrame();
+   auto stageFrame = [&](uint32_t stage, bool fold) {
+      beginFrame(fold);
       auto col = [&](int c) { return stage + (uint32_t) (F * sc.smemOffset[c]); };
       int64_t base[NV];
 #pragma unroll
@@ -1383,8 +1387,8 @@ __global__ void __launch_bounds__(kBlock, 3) scanQ1FactoredKernel(const __grid_c
       }
    };
    // one tile through plain loads: thread t takes rows t and kBlock + t
-   auto tileFrame = [&](int64_t t) {
-      beginFrame();
+   auto tileFrame = [&](int64_t t, bool fold) {
+      beginFrame(fold);
       GlobalTile<kDecEncoded> tile{t * kTileRows, &sc};
       const int nRows = (int) min(p.src.nRows - t * kTileRows, (int64_t) kTileRows);
       int64_t base[NV];
@@ -1413,7 +1417,9 @@ __global__ void __launch_bounds__(kBlock, 3) scanQ1FactoredKernel(const __grid_c
    };
 
    // CTA b takes stages b, b + grid, ..; the full tiles after the last full stage and the partial tail tile go tile by tile through
-   // plain loads, continuing that round robin
+   // plain loads, continuing that round robin.  Each loop folds the cell words at its frames 0, K, 2K, .. (frame 0 of the tail loop
+   // folds what the stages left)
+   const uint32_t K = p.facFoldFrames;
    const int64_t nFull = p.src.nRows / kTileRows;
    int64_t done = nFull, turns = nFull; // tiles read by the loops below, and the round-robin turns they took
    if (sc.useTma) {
@@ -1435,20 +1441,21 @@ __global__ void __launch_bounds__(kBlock, 3) scanQ1FactoredKernel(const __grid_c
          const uint32_t it = (uint32_t) (t - blockIdx.x) / gridDim.x; // this CTA's stage count (a batch has < 2^36 rows), not kept live
          const int s = it % S;
          mbarWait(&sFull[s], (uint32_t) (it / S) & 1u);
-         stageFrame(smemAddr(dynSmem) + (uint32_t) (s * F * sc.stageBytes));
+         stageFrame(smemAddr(dynSmem) + (uint32_t) (s * F * sc.stageBytes), it % K == 0);
          __syncthreads(); // every thread is done with stage s → refill it
          const int64_t nt = t + (int64_t) S * gridDim.x;
          if (threadIdx.x == 0 && nt < nStages) issueTile<F>(sc, dynSmem, sFull, nt, s);
       }
    } else {
       for (int64_t t = blockIdx.x; t < nFull; t += gridDim.x) {
-         tileFrame(t);
+         tileFrame(t, (uint32_t) (t - blockIdx.x) / gridDim.x % K == 0);
          __syncthreads();
       }
    }
    const int64_t nTiles = (p.src.nRows + kTileRows - 1) / kTileRows;
-   for (int64_t t = done + ((int64_t) blockIdx.x + gridDim.x - turns % gridDim.x) % gridDim.x; t < nTiles; t += gridDim.x) {
-      tileFrame(t);
+   const int64_t t0 = done + ((int64_t) blockIdx.x + gridDim.x - turns % gridDim.x) % gridDim.x;
+   for (int64_t t = t0; t < nTiles; t += gridDim.x) {
+      tileFrame(t, (uint32_t) (t - t0) / gridDim.x % K == 0);
       __syncthreads();
    }
    // ---- flush: the last frame's cells, then each owned cell's six aggregates, exact modulo 2^64 / 2^128 like the per-row sums; per
@@ -1573,7 +1580,25 @@ static bool factoredFits(const GroupByParams& p) {
    cudaFuncGetAttributes(&fa, (const void*) scanQ1FactoredKernel);
    return 3 * ((int64_t) kFacStages * kFacTiles * sc.stageBytes + (int64_t) fa.sharedSizeBytes + reserved) <= perSm;
 }
-static void launchQ1Factored(const GroupByParams& p, int smCount, cudaStream_t s) {
+// The factored kernel's cell-word split s and fold interval K (kernels.cu, Factored Q1): the s in [0, 28] that allows the largest K
+// with n = kFacFrameRows * K rows per cell between folds keeping n (2^s - 1), n (range_ep >> s), n range_qty and n below 2^32.  The
+// last bound caps K below 2^21.  Every batch factoredFits admits (range_ep < 2^28, range_qty < 2^21) gets K >= 1 at s = 20.
+static void factoredFold(GroupByParams& p) {
+   constexpr uint64_t kMaxN = 0xffffffffull;
+   const uint64_t rq = p.encRange[kQty];
+   p.facShift = 20;
+   p.facFoldFrames = 0;
+   for (uint32_t sh = 0; sh <= 28; sh++) {
+      const uint64_t top = std::max<uint64_t>(std::max<uint64_t>((1ull << sh) - 1, p.encRange[kEp] >> sh), std::max<uint64_t>(rq, 1));
+      const uint64_t k = kMaxN / (top * kFacFrameRows);
+      if (k > p.facFoldFrames) {
+         p.facShift = sh;
+         p.facFoldFrames = (uint32_t) k;
+      }
+   }
+}
+static void launchQ1Factored(GroupByParams p, int smCount, cudaStream_t s) {
+   factoredFold(p);
    size_t dyn;
    int grid = persistentGrid(scanQ1FactoredKernel, p.src.cols, p.src.nRows, smCount, &dyn, kBlock, kFacStages * kFacTiles);
    scanQ1FactoredKernel<<<grid, kBlock, dyn, s>>>(p);

@@ -163,6 +163,10 @@ struct GroupByParams {
    // block; the factored Q1 scan indexes its per-cell sums by them
    int64_t encMin[kMaxValueCols];
    uint64_t encRange[kMaxValueCols];
+   // the factored Q1 scan's cell words, chosen by the launcher from encRange (kernels.cu factoredFold): ep - min_ep splits into its low
+   // facShift bits and the rest, and the words are folded into 64-bit sums every facFoldFrames frames, before any of them can overflow
+   uint32_t facShift;
+   uint32_t facFoldFrames;
 };
 
 enum PayloadKind : int32_t { PAYLOAD_I32 = 0, PAYLOAD_YEAR_OF_DATE32 = 1, PAYLOAD_DEC_LO64 = 2 };
