@@ -634,7 +634,9 @@ int ldb_gpu_table_window(LdbTable* src, int32_t n_partition, const char* const* 
  *   Limits: sides of any number of batches (staged HOST tables, borrowed DEVICE batches, result tables), fewer than 2^32 rows together;
  *   1..16 columns of int8, int16, int32, int64, date32, char(1), decimal, float32, float64 or utf8; left == right is allowed.
  *   Errors, before the first launch: LDB_ERR_INVALID for a null argument, right given for DISTINCT or missing for another kind, an
- *   unknown kind, unknown columns, 0 or more than 16 columns, column lists of different lengths or tables of different contexts;
+ *   unknown kind, unknown columns, 0 or more than 16 columns, column lists of different lengths, tables of different contexts, or a
+ *   left column name that occurs twice among the left columns (named twice, or a NULL list over a table that repeats a name), naming
+ *   the clash: the result takes left's names and later calls find a column by its first match (right names are positional and may repeat);
  *   LDB_ERR_UNSUPPORTED naming both columns for positional columns of different physical types, for decimals of different scales (the
  *   caller casts, as the SQL analyzer does), for 2^32 rows or more and for a call inside a captured query (the output size is read on
  *   the host).  After the set is built: LDB_ERR_UNSUPPORTED when a utf8 column of the result would hold more than 2^31 - 1 bytes (its

@@ -1287,8 +1287,9 @@ int ldb_gpu_table_exchange_varlen(LdbTable* src, int32_t n_keys, const char* con
 } // extern "C"
 // Rows ids[0..n) (null: 0..n-1) of columns `cols` of `t` (any number of batches) into new single-batch buffers of `bufs`, cells at
 // outBytes: the permute kernels, with a host read of each utf8 column's byte total in between (it sizes the bytes array).  Returns the
-// batch (nRows, data, bytes, elemBytes, validBytes); synchronises.
-LdbBatch ldb::permuteRows(LdbTable* t, const std::vector<int>& cols, const int32_t* outBytes, const uint32_t* ids, int64_t n, Scratch& bufs) {
+// batch (nRows, data, bytes, elemBytes, validBytes); synchronises.  `what` names the caller's operation in the error for a utf8 column
+// of more than 2^31 - 1 bytes.
+LdbBatch ldb::permuteRows(LdbTable* t, const std::vector<int>& cols, const int32_t* outBytes, const uint32_t* ids, int64_t n, Scratch& bufs, const char* what) {
    LdbContext* ctx = t->ctx;
    Scratch tmp(ctx);
    PermuteParams q{};
@@ -1343,7 +1344,7 @@ LdbBatch ldb::permuteRows(LdbTable* t, const std::vector<int>& cols, const int32
       const int sj = q.strOf[j];
       const uint64_t nb = sj >= 0 && n > 0 ? totals[sj] : 0;
       if (nb > (uint64_t) INT32_MAX)
-         fail(LDB_ERR_UNSUPPORTED, "sort exchange: " + std::to_string(nb) + " bytes of utf8 column " + t->columns[cols[j]].name + " in one table, more than 2^31 - 1 (utf8 offsets are int32)");
+         fail(LDB_ERR_UNSUPPORTED, std::string(what) + ": " + std::to_string(nb) + " bytes of utf8 column " + t->columns[cols[j]].name + " in one table, more than 2^31 - 1 (utf8 offsets are int32)");
       q.chars[j] = sj >= 0 ? bufs.alloc<uint8_t>(std::max<size_t>(nb, 16)) : nullptr;
       ob.data.push_back(q.data[j]);
       ob.bytes.push_back(q.chars[j]);
@@ -1372,7 +1373,7 @@ static uint32_t* sortTableRows(Scratch& scratch, LdbTable* t, const std::vector<
       widths.push_back(shipCellBytes(t->columns[kc.first].type));
       k.columns.push_back(t->columns[kc.first]);
    }
-   k.batches.push_back(permuteRows(t, cols, widths.data(), nullptr, t->numRows, scratch));
+   k.batches.push_back(permuteRows(t, cols, widths.data(), nullptr, t->numRows, scratch, "sort exchange"));
    return sortRows(scratch, &k, at, t->numRows);
 }
 
@@ -1437,7 +1438,7 @@ static void sortExchange(LdbTable* src, int32_t n_keys, const char* const* key_c
       top.ctx = ctx;
       top.numRows = m;
       for (int ci : ship) top.columns.push_back(src->columns[ci]);
-      top.batches.push_back(permuteRows(src, ship, widths, ids, m, local));
+      top.batches.push_back(permuteRows(src, ship, widths, ids, m, local, "sort exchange"));
       from = &top;
       for (size_t j = 0; j < ship.size(); j++) fromCols[j] = (int) j;
       for (int k = 0; k < n_keys; k++) fromKeys[k] = keyAt[k];
@@ -1495,7 +1496,7 @@ static void sortExchange(LdbTable* src, int32_t n_keys, const char* const* key_c
    const uint32_t* ids = keep ? sortRows(sorted, &view, order, got) : nullptr;
    std::vector<int> outCols;
    for (int j = 0; j < nUser; j++) outCols.push_back(j);
-   LdbBatch ob = permuteRows(&view, outCols, s.outBytes, ids, keep, cols);
+   LdbBatch ob = permuteRows(&view, outCols, s.outBytes, ids, keep, cols, "sort exchange");
    s.finish();
    int64_t before = 0, all = 0;
    for (int d = 0; d < world; d++) {

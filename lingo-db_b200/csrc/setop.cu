@@ -65,19 +65,17 @@ __device__ __forceinline__ const SetBatch& setBatchOf(const SetParams& p, int64_
    }
    return p.dir[lo];
 }
-// a float's bits (float32 arrives widened to double) with -0.0 as +0.0 and every NaN as the one quiet NaN
-__device__ __forceinline__ uint64_t setF64Bits(double d) { return d == 0.0 ? 0ull : d != d ? 0x7ff8000000000000ull : (uint64_t) __double_as_longlong(d); }
 __device__ __forceinline__ bool setIsFloat(int type) { return type == LDB_FLOAT32 || type == LDB_FLOAT64; }
-// a cell's word for the row hash: equal cells (by the rule above) give equal words
+// a cell's word for the row hash (the value rules are keyhash.cuh's): equal cells (by the rule above) give equal words
 __device__ __forceinline__ uint64_t setCellWord(const ProgCol& c, int64_t r) {
-   if (colIsNull(c, r)) return 0x2545F4914F6CDD1Dull;
+   if (colIsNull(c, r)) return kSetNullWord;
    if (c.type == LDB_UTF8) {
       const int32_t* o = (const int32_t*) c.data;
       return strHash(c.bytes + o[r], o[r + 1] - o[r]);
    }
    const Val v = loadCol(c, r);
    if (setIsFloat(c.type)) return setF64Bits(asF64(v));
-   return (uint64_t) v.v ^ mix64((uint64_t) (v.v >> 64));
+   return setIntWord((uint64_t) v.v, (uint64_t) (v.v >> 64));
 }
 __device__ __forceinline__ bool setCellEq(const ProgCol& a, int64_t ra, const ProgCol& b, int64_t rb) {
    const bool na = colIsNull(a, ra), nb = colIsNull(b, rb);
@@ -97,9 +95,7 @@ __device__ __forceinline__ bool setCellEq(const ProgCol& a, int64_t ra, const Pr
 }
 // the whole-row hash: keyTupleHash's step over the cell words, in column order
 __device__ __forceinline__ uint64_t setRowHash(const SetParams& p, const SetBatch& b, int64_t r) {
-   uint64_t h = 0x9E3779B97F4A7C55ull;
-   for (int c = 0; c < p.nCols; c++) h = mix64(h ^ setCellWord(b.cols[c], r)) + 0x632BE59BD9B4E019ull * (c + 1);
-   return mix64(h);
+   return setRowFold(p.nCols, [&](int c) { return setCellWord(b.cols[c], r); });
 }
 __device__ __forceinline__ bool setRowsEqual(const SetParams& p, const SetBatch& b, int64_t r, int64_t other) {
    const SetBatch& o = setBatchOf(p, other);
@@ -259,6 +255,13 @@ static void tableSetop(LdbTable* left, LdbTable* right, int32_t kind, int32_t n_
    const std::vector<int> rc = right ? setColumns(right, n_columns, right_columns, "right") : lc;
    if (lc.size() != rc.size()) fail(LDB_ERR_INVALID, "the column lists of a set operation have different lengths (" + std::to_string(lc.size()) + " and " + std::to_string(rc.size()) + ")");
    if (lc.empty() || lc.size() > (size_t) kSetMaxCols) fail(LDB_ERR_INVALID, "a set operation takes 1..16 columns (it has " + std::to_string(lc.size()) + ")");
+   // the result takes left's names, and later calls find a column by its first match: a repeated left name would be unreadable (right
+   // names are positional and may repeat)
+   for (size_t j = 0; j < lc.size(); j++)
+      for (size_t k = 0; k < j; k++)
+         if (left->columns[lc[j]].name == left->columns[lc[k]].name)
+            fail(LDB_ERR_INVALID, "the set operation's result would have two columns named " + left->columns[lc[j]].name + " (left columns " +
+                                     std::to_string(k) + " and " + std::to_string(j) + ")");
    const LdbTable* rt = right ? right : left;
    std::vector<LdbColumn> outCols;
    std::vector<int32_t> widths;
@@ -351,7 +354,7 @@ static void tableSetop(LdbTable* left, LdbTable* right, int32_t kind, int32_t n_
          total = host[2];
       }
    }
-   LdbBatch ob = permuteRows(&view, all, widths.data(), ids, total, bufs);
+   LdbBatch ob = permuteRows(&view, all, widths.data(), ids, total, bufs, "set operation");
    *out = addResultTable(ctx, name ? name : "setop", std::move(outCols), std::move(ob), bufs);
 }
 

@@ -344,7 +344,7 @@ static void tableWindow(LdbTable* src, int32_t n_partition, const char* const* p
    for (int ci : carried) widths.push_back(shipCellBytes(src->columns[ci].type));
    LdbBatch ob;
    if (!carried.empty()) {
-      ob = permuteRows(src, carried, widths.data(), ids, n, cols);
+      ob = permuteRows(src, carried, widths.data(), ids, n, cols, "window");
    } else {
       ob.nRows = n;
    }

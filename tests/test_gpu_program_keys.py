@@ -11,6 +11,8 @@ from collections import Counter
 import numpy as np
 import pytest
 
+import _keyhash as K
+
 from lingodb_b200 import capi, datagen, parallel, program as P, runtime
 
 pytestmark = pytest.mark.gpu
@@ -69,22 +71,9 @@ def _read(ctx, out_h, n_cols):
     return rows
 
 
-def _mix64(x):
-    x ^= x >> np.uint64(33)
-    x *= np.uint64(0xFF51AFD7ED558CCD)
-    x ^= x >> np.uint64(33)
-    x *= np.uint64(0xC4CEB9FE1A85EC53)
-    x ^= x >> np.uint64(33)
-    return x
-
-
 def _tuple_hash(cols):
-    """the table's placement hash (csrc/program.cu keyTupleHash, seed 0) over int64 key columns, vectorised"""
-    with np.errstate(over="ignore"):
-        h = np.full(len(cols[0]), 0x9E3779B97F4A7C55, dtype=np.uint64)
-        for k, c in enumerate(cols):
-            h = _mix64(h ^ c.astype(np.uint64)) + np.uint64((0x632BE59BD9B4E019 * (k + 1)) & M64)
-    return h
+    """the table's placement hash (csrc/keyhash.cuh keyTupleHash, seed 0) over int64 key columns, vectorised"""
+    return K.key_tuple_hash_np([np.asarray(c).astype(np.int64) for c in cols])
 
 
 def _tag_twins(prefix, rng):

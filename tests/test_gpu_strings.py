@@ -11,6 +11,8 @@ from collections import Counter
 import numpy as np
 import pytest
 
+import _keyhash as K
+
 from lingodb_b200 import capi, dbgen, program as P, runtime
 from lingodb_b200.datagen import ColumnSpec
 
@@ -131,22 +133,8 @@ def test_round_trip(gpu_ctx, layout):
 
 def test_tag_collision_compares_the_whole_string(gpu_ctx):
     """Two strings that share their first 8 bytes and, in a 16-slot directory, their home slot and their 32-bit tag (found with the
-    hash below, a copy of strHash in csrc/program.cu): the dictionary must still tell them apart."""
-    M = (1 << 64) - 1
-
-    def mix(x):
-        x ^= x >> 33
-        x = x * 0xff51afd7ed558ccd & M
-        x ^= x >> 33
-        x = x * 0xc4ceb9fe1a85ec53 & M
-        return x ^ (x >> 33)
-
-    def h(b):
-        v = 0x9E3779B97F4A7C15 ^ (len(b) * 0xff51afd7ed558ccd & M)
-        for i in range(0, len(b), 8):
-            v = (mix(v ^ int.from_bytes(b[i:i + 8].ljust(8, b"\0"), "little")) + 0x632BE59BD9B4E019) & M
-        return mix(v)
-
+    hash of tests/_keyhash.py, pinned to strHash in csrc/keyhash.cuh): the dictionary must still tell them apart."""
+    h = K.str_hash
     a, b = b"COLLIDE#imldaaaa", b"COLLIDE#hzlbiaaa"
     assert h(a) >> 32 == h(b) >> 32 and h(a) & 15 == h(b) & 15  # still a collision for the current hash
     for vals in ([a, b] * 200, [b, a], [a] * 100 + [b] * 100):

@@ -18,7 +18,9 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 import pytest
 
+import _keyhash as K
 import _progref as R
+from _keyhash import mix64
 from lingodb_b200 import capi, datagen
 
 M64 = (1 << 64) - 1
@@ -34,21 +36,9 @@ SUBSET = ["f8", "i8", "dw", "k"]
 
 
 # ---------------------------------------------------------------------------------------------------- the model
-def mix64(x: int) -> int:
-    x ^= x >> 33
-    x = (x * 0xFF51AFD7ED558CCD) & M64
-    x ^= x >> 33
-    x = (x * 0xC4CEB9FE1A85EC53) & M64
-    return x ^ (x >> 33)
-
-
 def key_tuple_hash(keys: list) -> int:
     """keyTupleHash over key values (None = NULL: hashes as 0, sets bit k of the seed); a value is taken as int64 (its low 64 bits)"""
-    seed = sum(1 << k for k, v in enumerate(keys) if v is None)
-    h = 0x9E3779B97F4A7C55 ^ seed
-    for k, v in enumerate(keys):
-        h = (mix64(h ^ (0 if v is None else v & M64)) + 0x632BE59BD9B4E019 * (k + 1)) & M64
-    return h
+    return K.key_tuple_hash([0 if v is None else v for v in keys], sum(1 << k for k, v in enumerate(keys) if v is None))
 
 
 def owner(keys: list, world: int) -> int:
@@ -417,19 +407,10 @@ TILE_ROWS = 4096  # rows per CTA of the count and send kernels (kShipTile)
 
 def owners_np(keys: list, world: int) -> np.ndarray:
     """the owner of every row: keys = [(int64 values, valid mask)] per key column, the same fold as key_tuple_hash, in numpy"""
-    def mix(x):
-        x = x ^ (x >> np.uint64(33))
-        x = x * np.uint64(0xFF51AFD7ED558CCD)
-        x = x ^ (x >> np.uint64(33))
-        x = x * np.uint64(0xC4CEB9FE1A85EC53)
-        return x ^ (x >> np.uint64(33))
-    n = len(keys[0][0])
-    seed = np.zeros(n, np.uint64)
+    seed = np.zeros(len(keys[0][0]), np.uint64)
     for k, (_, valid) in enumerate(keys):
         seed |= (~valid).astype(np.uint64) << np.uint64(k)
-    h = np.uint64(0x9E3779B97F4A7C55) ^ seed
-    for k, (vals, valid) in enumerate(keys):
-        h = mix(h ^ np.where(valid, vals.astype(np.int64).view(np.uint64), np.uint64(0))) + np.uint64((0x632BE59BD9B4E019 * (k + 1)) & M64)
+    h = K.key_tuple_hash_np([np.where(valid, vals.astype(np.int64), 0) for vals, valid in keys], seed)
     return (((h >> np.uint64(32)) * np.uint64(world)) >> np.uint64(32)).astype(np.int64)
 
 
