@@ -648,6 +648,59 @@ int ldb_gpu_table_setop(LdbTable* left, LdbTable* right /* NULL exactly for LDB_
                         const char* const* left_columns /* NULL = every column of left */,
                         const char* const* right_columns /* NULL = every column of right; positional */,
                         const char* name, LdbTable** out, LdbError* err);
+/* Nested-loop joins: joins whose predicate has no equality to hash on, and cross products, the reference's translateNLJ
+ * (RelAlgToSubOp.cpp:948) for inner, semi, anti, mark and outer joins, translateNLJWithMarker (:1217) for the joins that keep the
+ * build side (right and full outer) and CrossProductLowering (:1306); csrc/nljoin.cu cites each rule.
+ *   Predicate: the conjunction of conds[0..n_conds), 0..8 conditions of which at most 4 compare a column of left with a column of right
+ *   (left.col OP right.col); the others compare one column with a constant (left NULL: value OP right.col; right NULL: left.col OP
+ *   value).  A pair matches when every condition is TRUE; a NULL operand makes its condition UNKNOWN, which is not TRUE.  Floats compare
+ *   as the reference's ordered predicates (OEQ, ONE, OLT …, LowerToStd.cpp:876-894): a NaN operand is never TRUE, not even for <>, and
+ *   -0.0 = +0.0.  A condition on one side only is part of ON, not a filter before the join: under an outer, anti, mark or count join a
+ *   left row failing it is unmatched, not dropped.  n_conds = 0 is a cross product.  Any other predicate (x.b < t1.b * 10, OR) is the
+ *   caller's to compose: a program materialises the derived column first, and the join compares it.
+ *   Operand types: int8 .. int64 compare by value across widths; date32 only with date32; char(1) only with char(1); decimals by value
+ *   at equal scales, 8- or 16-byte cells alike; float32 and float64 with each other as doubles.  A constant is `value` (integers, days,
+ *   char(1) codes, unscaled decimals at the column's scale) or, for a float column, `fvalue`; the other field is 0 or the same number,
+ *   else LDB_ERR_INVALID (so a non-integral fvalue is never read as an integer `value`).  utf8 operands and every other mix:
+ *   LDB_ERR_UNSUPPORTED, naming both columns.
+ *   Kinds and their rows, in this fixed order:
+ *     INNER        the matching pairs, in left row order, then right row order within a left row;
+ *     LEFT_OUTER   as INNER, plus each left row without a match, its right cells NULL, at its own position;
+ *     RIGHT_OUTER  as INNER, then the right rows without a match, in right row order, their left cells NULL;
+ *     FULL_OUTER   as LEFT_OUTER, then the unmatched right rows as RIGHT_OUTER appends them;
+ *     SEMI / ANTI  the left rows with / without a match, in order (left columns only);
+ *     MARK         every left row, plus `value_name` int32 1 when some pair matched, else 0, never NULL (translateNLJWithMarker and
+ *                  LDB_OP_EXISTS; the reference gives = ANY no NULL result either);
+ *     COUNT        every left row, plus `value_name` int64, the number of right rows it matches: a correlated
+ *                  (SELECT count(*) … WHERE x.b < t1.b) at O(n + m) output instead of n x m pairs grouped afterwards.
+ *   Result: *out = a new single-batch DEVICE table named `name` (NULL: "nljoin"): the carried left columns (left_columns, NULL = every
+ *   column), then the carried right columns (right_columns, NULL = every column; not for SEMI, ANTI, MARK or COUNT, which carry none),
+ *   named right_names[j] (NULL: their own names), then the value column; cells as ldb_gpu_table_exchange_varlen makes them (decimals in
+ *   16 bytes, utf8 carried) with validity bytes on every column.  It may feed programs, ORDER BY, the window and set operators and the
+ *   next join.
+ *   Limits: sides of any number of batches (staged HOST tables, borrowed DEVICE batches at bit offsets, result tables), each of fewer
+ *   than 2^32 - 1 rows; left == right is allowed (a self join); 0..16 carried columns per side.  The result's row count is computed
+ *   before anything is written.
+ *   Errors, before the first launch: LDB_ERR_INVALID for null arguments, an unknown kind, column or op, a condition with both columns
+ *   NULL, more than 8 conditions or 4 column-to-column ones, more than 16 carried columns, tables of different contexts, right columns
+ *   given to SEMI / ANTI / MARK / COUNT, a missing value_name for MARK / COUNT, and two output columns of one name (a self join
+ *   without right_names), naming the clash; LDB_ERR_UNSUPPORTED for the type mixes above, a side of 2^32 - 1 rows or more and a call
+ *   inside a captured query (the output size is read on the host).  After counting: LDB_ERR_CAPACITY naming the row count when the
+ *   result does not fit device memory, and LDB_ERR_UNSUPPORTED when a utf8 column of the result would hold more than 2^31 - 1 bytes. */
+enum LdbNlJoinKind { LDB_NLJ_INNER = 1, LDB_NLJ_LEFT_OUTER = 2, LDB_NLJ_RIGHT_OUTER = 3, LDB_NLJ_FULL_OUTER = 4,
+                     LDB_NLJ_SEMI = 5, LDB_NLJ_ANTI = 6, LDB_NLJ_MARK = 7, LDB_NLJ_COUNT = 8 };
+typedef struct LdbJoinCond {
+   const char* left;  /* a column of left, or NULL: compare the constant with `right` */
+   int32_t op;        /* LDB_EQ .. LDB_GTE, read as  left OP right */
+   const char* right; /* a column of right, or NULL: compare `left` with the constant */
+   LdbI128 value;     /* integer / date / char(1) / unscaled decimal constant */
+   double fvalue;     /* float constant */
+} LdbJoinCond;
+int ldb_gpu_table_nl_join(LdbTable* left, LdbTable* right, int32_t kind, int32_t n_conds, const LdbJoinCond* conds,
+                          int32_t n_left_columns, const char* const* left_columns /* carried; NULL = all */,
+                          int32_t n_right_columns, const char* const* right_columns /* carried; NULL = all */,
+                          const char* const* right_names /* output names of the carried right columns; NULL = their own */,
+                          const char* value_name /* the MARK / COUNT column */, const char* name, LdbTable** out, LdbError* err);
 
 /* String dictionary (LDB_STATE_DICT): a device hash set of byte strings that gives each distinct string a dense int32 code, for
  * LDB_OP_STRCODE — group, join and sort keys over strings of any length.  Codes are 0..n-1 and stable for the dictionary's lifetime

@@ -142,6 +142,13 @@ class WindowFunc(C.Structure):
 # LdbSetOpKind
 SETOP = {"distinct": 1, "union_all": 2, "union": 3, "intersect": 4, "intersect_all": 5, "except": 6, "except_all": 7}
 
+# LdbNlJoinKind
+NLJOIN = {"inner": 1, "left": 2, "right": 3, "full": 4, "semi": 5, "anti": 6, "mark": 7, "count": 8}
+
+
+class JoinCond(C.Structure):
+    _fields_ = [("left", C.c_char_p), ("op", C.c_int32), ("right", C.c_char_p), ("value", I128), ("fvalue", C.c_double)]
+
 
 class Q5ShuffleStats(C.Structure):
     _fields_ = [(n, C.c_int64) for n in ("orders_tuples_sent", "orders_tuples_received", "lineitem_tuples_sent", "lineitem_tuples_received", "shuffle_bytes_out", "heap_bytes")]
@@ -220,6 +227,8 @@ SIGNATURES = {
     "ldb_gpu_table_window": (C.c_int, [_P, C.c_int32, C.POINTER(C.c_char_p), C.c_int32, C.POINTER(C.c_char_p), C.POINTER(C.c_int32), C.c_int64, C.c_int64,
                                        C.c_int32, C.POINTER(WindowFunc), C.c_int32, C.POINTER(C.c_char_p), C.c_char_p, C.POINTER(_P), _E]),
     "ldb_gpu_table_setop": (C.c_int, [_P, _P, C.c_int32, C.c_int32, C.POINTER(C.c_char_p), C.POINTER(C.c_char_p), C.c_char_p, C.POINTER(_P), _E]),
+    "ldb_gpu_table_nl_join": (C.c_int, [_P, _P, C.c_int32, C.c_int32, C.POINTER(JoinCond), C.c_int32, C.POINTER(C.c_char_p), C.c_int32, C.POINTER(C.c_char_p),
+                                        C.POINTER(C.c_char_p), C.c_char_p, C.c_char_p, C.POINTER(_P), _E]),
     "ldb_gpu_dict_create": (C.c_int, [_P, C.c_int64, C.c_int64, C.POINTER(_P), _E]),
     "ldb_gpu_dict_count": (C.c_int, [_P, C.POINTER(C.c_int64), _E]),
     "ldb_gpu_dict_to_table": (C.c_int, [_P, C.c_char_p, C.POINTER(_P), _E]),

@@ -319,7 +319,8 @@ inline int32_t shipCellBytes(int type) {
 }
 // rows ids[0..n) (null: 0..n-1) of columns `cols` of `t` (any number of batches, at most 16 columns) as a new single-batch LdbBatch whose
 // buffers are in `bufs`: fixed-width cells at outBytes[j] bytes (a narrowed decimal widened to 16), validity bytes, utf8 offsets and
-// bytes.  Synchronises.  The sort exchange and the window operator (peer.cu)
+// bytes.  An id of 0xffffffff makes a row of NULL cells (zero bytes, validity 0, empty strings).  Synchronises.  The sort exchange, the
+// window, set and nested-loop join operators (peer.cu)
 LdbBatch permuteRows(LdbTable* t, const std::vector<int>& cols, const int32_t* outBytes, const uint32_t* ids, int64_t n, Scratch& bufs, const char* what);
 } // namespace ldb
 // builds the missing encoded copies of columns cols[0..n) of a borrowed DEVICE batch (encode.cu) for tiles of `tileRows` rows;

@@ -521,6 +521,7 @@ __global__ void __launch_bounds__(256) sortSampleKernel(const __grid_constant__ 
 // outBytes (a narrowed decimal sign-extended, as the exchange ships it) and validity bytes by row id; a utf8 column's lengths by row id
 // (permuteCellsKernel, which also sums each CTA's bytes), the exclusive scan of the CTA sums (rowScanKernel), then its offsets and
 // bytes (permuteStringsKernel: each warp copies its 32 rows' strings, one contiguous range of the output, together).
+constexpr uint32_t kPermuteNone = 0xffffffffu; // the id of a row of NULL cells (no caller has 2^32 - 1 rows)
 struct PermuteBatch {
    ProgCol cols[kShipMaxCols];
    int64_t firstRow, nRows;
@@ -555,13 +556,22 @@ __global__ void __launch_bounds__(kShipThreads) permuteCellsKernel(const __grid_
    for (int64_t t = begin; t < end; t += kShipThreads) {
       const int64_t i = t + threadIdx.x;
       const bool ok = i < end;
-      const int64_t row = !ok ? 0 : q.ids ? (int64_t) q.ids[i] : i;
+      const uint32_t id = ok && q.ids ? q.ids[i] : 0u;
+      const bool none = id == kPermuteNone; // a NULL row: NULL cells (the nested-loop join's unmatched side)
+      const int64_t row = !ok || none ? 0 : q.ids ? (int64_t) id : i;
       const PermuteBatch& b = permuteBatchOf(q, row);
-      const int64_t r = row - b.firstRow;
+      const int64_t r = none ? 0 : row - b.firstRow;
       for (int c = 0; c < q.nCols; c++) {
          const ProgCol& col = b.cols[c];
          uint32_t len = 0;
-         if (ok) {
+         if (ok && none) {
+            q.valid[c][i] = 0;
+            if (q.strOf[c] < 0) {
+               for (int x = 0; x < q.outBytes[c]; x++) q.data[c][(size_t) i * q.outBytes[c] + x] = 0;
+            } else {
+               ((uint32_t*) q.data[c])[i] = 0;
+            }
+         } else if (ok) {
             const bool null = colIsNull(col, r);
             q.valid[c][i] = null ? 0 : 1;
             if (q.strOf[c] < 0) {
@@ -1326,6 +1336,7 @@ LdbBatch ldb::permuteRows(LdbTable* t, const std::vector<int>& cols, const int32
    }
    unsigned long long* totals = (unsigned long long*) ((uint8_t*) ctx->scratch() + LdbContext::kPinnedScratchBytes) - kShipMaxCols;
    if (n > 0) {
+      if (dir.empty()) dir.push_back(PermuteBatch{}); // a table without rows: every id is kPermuteNone, the entry is never read for a row
       PermuteBatch* dd = tmp.alloc<PermuteBatch>(dir.size() * sizeof(PermuteBatch));
       LDB_CUDA(cudaMemcpyAsync(dd, dir.data(), dir.size() * sizeof(PermuteBatch), cudaMemcpyHostToDevice, ctx->compute));
       q.dir = dd;

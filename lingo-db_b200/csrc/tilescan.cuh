@@ -14,6 +14,7 @@ constexpr int kTileScanThreads = 256, kTileScanItems = 8;
 constexpr int64_t kTileScanTile = (int64_t) kTileScanThreads * kTileScanItems;
 
 __device__ __forceinline__ uint32_t tileShflUp(uint32_t v, int o) { return __shfl_up_sync(0xffffffffu, v, o); }
+__device__ __forceinline__ unsigned long long tileShflUp(unsigned long long v, int o) { return __shfl_up_sync(0xffffffffu, v, o); }
 // the exclusive scan of one value per thread across the CTA; *total = the CTA's combined value
 template <class Op>
 __device__ __forceinline__ typename Op::T tileBlockScan(const Op& op, typename Op::T v, typename Op::T* total) {

@@ -519,6 +519,33 @@ class RawTable:
                                              C.byref(t), C.byref(e)), e)
         return RawTable(self.ctx, t)
 
+    def nl_join(self, other, kind: str, conds=(), columns=None, other_columns=None, other_names=None, value_name=None, name="nljoin") -> "RawTable":
+        """A nested-loop join (ldb_gpu_table_nl_join) of this table (left) with `other` (right) as a new table: kind one of capi.NLJOIN
+        ("inner", "left", "right", "full", "semi", "anti", "mark", "count").  conds: the conjunction of (left column, op, right column)
+        triples, op one of "=", "!=", "<", "<=", ">", ">=", with None for one column to compare the other with a constant: (column, op,
+        None, value) or (None, op, column, value), value an int (integers, days, char(1) codes, unscaled decimals; float columns
+        too) or a float (float columns; against any other column only an integral one).  No conds: a cross product.  columns /
+        other_columns: the carried columns (None: every column; other's only for the pair kinds), other_names: their output names; value_name: the MARK (int32 0 / 1) or COUNT (int64) column.  Rows come in left
+        row order, then right row order; unmatched right rows of right / full joins last.  `other` may be a RawTable, a runtime.Table
+        or this table itself."""
+        cs = []
+        for c in conds:
+            lcol, op, rcol = c[0], c[1], c[2]
+            v = c[3] if len(c) > 3 else 0
+            # a float column reads fvalue, any other column value: an int sets both, a float its integral value too, so a non-integral
+            # float constant against a non-float column is refused (LDB_ERR_INVALID) instead of being read as 0
+            fv = float(v)
+            iv = int(v) if isinstance(v, int) or float(v).is_integer() else 0
+            cs.append(capi.JoinCond(None if lcol is None else lcol.encode(), capi.OPS[op], None if rcol is None else rcol.encode(),
+                                    capi.I128(iv & ((1 << 64) - 1), iv >> 64), fv))
+        arr = (capi.JoinCond * max(1, len(cs)))(*cs)
+        enc = lambda xs: None if xs is None else (C.c_char_p * max(1, len(xs)))(*[x.encode() for x in xs])
+        t, e = C.c_void_p(), Error()
+        check(self.ctx.L.ldb_gpu_table_nl_join(self.h, other.h, capi.NLJOIN[kind], len(cs), arr, 0 if columns is None else len(columns), enc(columns),
+                                               0 if other_columns is None else len(other_columns), enc(other_columns), enc(other_names),
+                                               None if value_name is None else value_name.encode(), name.encode(), C.byref(t), C.byref(e)), e)
+        return RawTable(self.ctx, t)
+
     def distinct(self, columns=None, name="distinct") -> "RawTable":
         """SELECT DISTINCT over `columns` (None: every column), each distinct row at its first occurrence."""
         return self.setop(None, "distinct", columns, None, name)
