@@ -603,7 +603,10 @@ int ldb_gpu_table_gather_strings(LdbTable* t, const char* column, const int64_t*
  *   LDB_ERR_INVALID for null arguments, unknown columns or kinds, counts out of range or a bad frame, and for two output columns of
  *   one name (a function named like a carried column, carried columns of columns = NULL included; two functions of one name; a column
  *   carried twice), naming the clash: later calls find result columns by name.  Everything is checked before the first launch. */
-enum LdbWindowKind { LDB_WIN_ROW_NUMBER = 1, LDB_WIN_COUNT_STAR = 2, LDB_WIN_COUNT = 3, LDB_WIN_SUM = 4, LDB_WIN_MIN = 5, LDB_WIN_MAX = 6 };
+enum LdbWindowKind { LDB_WIN_ROW_NUMBER = 1, LDB_WIN_COUNT_STAR = 2, LDB_WIN_COUNT = 3, LDB_WIN_SUM = 4, LDB_WIN_MIN = 5, LDB_WIN_MAX = 6,
+                     /* ldb_gpu_table_window_ex only */
+                     LDB_WIN_RANK = 7, LDB_WIN_DENSE_RANK = 8, LDB_WIN_PERCENT_RANK = 9, LDB_WIN_CUME_DIST = 10, LDB_WIN_NTILE = 11,
+                     LDB_WIN_LAG = 12, LDB_WIN_LEAD = 13, LDB_WIN_FIRST_VALUE = 14, LDB_WIN_LAST_VALUE = 15, LDB_WIN_NTH_VALUE = 16 };
 typedef struct LdbWindowFunc {
    int32_t kind;       /* LdbWindowKind */
    const char* column; /* the argument; NULL for ROW_NUMBER and COUNT_STAR */
@@ -612,6 +615,51 @@ typedef struct LdbWindowFunc {
 int ldb_gpu_table_window(LdbTable* src, int32_t n_partition, const char* const* partition_columns, int32_t n_order, const char* const* order_columns,
                          const int32_t* descending, int64_t frame_from, int64_t frame_to, int32_t n_funcs, const LdbWindowFunc* funcs, int32_t n_columns,
                          const char* const* columns /* carried; NULL = all columns of src */, const char* name, LdbTable** out, LdbError* err);
+/* Window functions with RANGE frames and the ranking, offset and value functions: everything ldb_gpu_table_window does, plus the kinds
+ * 7..16 below and frame->mode.  ldb_gpu_table_window is this call with a ROWS frame and kinds 1..6 (it refuses the others).  The new
+ * functions follow standard SQL as PostgreSQL implements it (the reference has ROWS frames, ROW_NUMBER and the aggregates only).
+ *   Peers: two rows of a partition are peers when they are equal on every order key, NULL equal to NULL; without order keys every row
+ *   of a partition is a peer of every other.
+ *   ROWS frames: exactly ldb_gpu_table_window's (the reference's clamping; never empty; ROW_NUMBER = i - lo + 1).
+ *   RANGE frames: each bound is UNBOUNDED (INT64_MIN / INT64_MAX: the partition start / end), 0 (CURRENT ROW: the first / last peer)
+ *   or a signed offset (negative = PRECEDING): the frame holds the rows whose key lies in [key - |from|, key + to] in the order's
+ *   direction, so under DESC 3 PRECEDING means keys up to key + 3.  An offset bound needs exactly one order key of type int32, int64,
+ *   date32 or decimal (8- or 16-byte cells; offsets unscaled at the key's scale, days for date32); key +- offset never wraps (an int64
+ *   key at INT64_MAX with 5 FOLLOWING ends at the partition's last non-NULL key).  A row whose key is NULL takes its NULL peers for
+ *   every offset bound, and a row with a non-NULL key never has a NULL-key row in its offset range (PostgreSQL's rule).  A RANGE frame
+ *   may be empty: COUNT_STAR and COUNT are 0, SUM, MIN, MAX, FIRST_VALUE, LAST_VALUE and NTH_VALUE NULL.
+ *   Functions over the frame: COUNT_STAR, COUNT, SUM, MIN, MAX as above; FIRST_VALUE / LAST_VALUE / NTH_VALUE(n) the value at that
+ *   position of the frame, NULL included (RESPECT NULLS), NTH_VALUE NULL when the frame has fewer than n rows.
+ *   Functions that ignore the frame, for the row at position j of a partition of len rows: ROW_NUMBER under RANGE = j + 1; RANK = 1 +
+ *   the rows before its first peer; DENSE_RANK = the 1-based index of its peer group; PERCENT_RANK = (RANK - 1) / (len - 1), 0 when
+ *   len = 1; CUME_DIST = (position of its last peer + 1) / len; NTILE(n) = its bucket when the partition is split into n buckets, the
+ *   first len % n holding one row more (1..len when n > len); LAG(n) / LEAD(n) = the value n rows before / after within the partition,
+ *   else the default (has_default) or NULL; a NULL value inside the partition stays NULL.
+ *   Result columns: RANK, DENSE_RANK, NTILE int64 and PERCENT_RANK, CUME_DIST float64, without NULLs; LAG, LEAD, FIRST_VALUE,
+ *   LAST_VALUE and NTH_VALUE the argument's type, precision and scale in the carried columns' cells (utf8 included, float bits
+ *   unchanged), with validity bytes.
+ *   Errors, before the first launch, besides ldb_gpu_table_window's: LDB_ERR_INVALID for a null frame, an unknown mode, n < 0 for LAG /
+ *   LEAD, n < 1 for NTILE / NTH_VALUE, a default on another kind, a default whose value and fvalue differ (as LdbJoinCond's constant) or
+ *   which does not fit the argument's type (integer range, |value| < 10^precision for decimals, float32 range); LDB_ERR_UNSUPPORTED for
+ *   a RANGE offset bound without exactly one order key or over a key of another type, and a default for a utf8 argument. */
+enum LdbWindowFrameMode { LDB_FRAME_ROWS = 0, LDB_FRAME_RANGE = 1 };
+typedef struct LdbWindowFrame {
+   int32_t mode;     /* LdbWindowFrameMode */
+   int32_t pad;
+   int64_t from, to; /* INT64_MIN / INT64_MAX = UNBOUNDED, 0 = CURRENT ROW, else a signed offset (negative = PRECEDING) */
+} LdbWindowFrame;
+typedef struct LdbWindowFuncEx {
+   int32_t kind;        /* LdbWindowKind */
+   int32_t has_default; /* LAG / LEAD: value / fvalue where the offset row is outside the partition */
+   const char* column;  /* the argument; NULL for ROW_NUMBER, COUNT_STAR and the ranking functions */
+   const char* name;    /* the output column */
+   int64_t n;           /* LAG / LEAD offset (>= 0), NTILE buckets (>= 1), NTH_VALUE position (>= 1) */
+   LdbI128 value;       /* the default: integer, days, char(1) code or unscaled decimal */
+   double fvalue;       /* the default of a float argument */
+} LdbWindowFuncEx;
+int ldb_gpu_table_window_ex(LdbTable* src, int32_t n_partition, const char* const* partition_columns, int32_t n_order, const char* const* order_columns,
+                            const int32_t* descending, const LdbWindowFrame* frame, int32_t n_funcs, const LdbWindowFuncEx* funcs, int32_t n_columns,
+                            const char* const* columns /* carried; NULL = all columns of src */, const char* name, LdbTable** out, LdbError* err);
 /* Set operations: SELECT DISTINCT, UNION [ALL], INTERSECT [ALL] and EXCEPT [ALL] over whole rows, the reference's relalg.projection
  * distinct (ProjectionDistinctLowering, RelAlgToSubOp.cpp:337-394), relalg.union (UnionAllLowering :622-634, UnionDistinctLowering
  * :636-727) and relalg.intersect / relalg.except (CountingSetOperationLowering :728-916); csrc/setop.cu cites each rule.

@@ -131,12 +131,25 @@ class HashAggRow(C.Structure):
     _fields_ = [("keys", C.c_int64 * 4), ("key_null_mask", C.c_uint32), ("agg_valid_mask", C.c_uint32), ("aggs", I128 * MAX_AGGS)]
 
 
-# LdbWindowKind; RANK is the reference's RankWindowFunc, which is ROW_NUMBER
-WIN = {"row_number": 1, "rank": 1, "count_star": 2, "count": 3, "sum": 4, "min": 5, "max": 6}
+# LdbWindowKind; "rank" is the reference's RankWindowFunc, which is ROW_NUMBER; "sql_rank" is SQL's RANK (ties share a rank).  Kinds
+# from "sql_rank" on are ldb_gpu_table_window_ex's only
+WIN = {"row_number": 1, "rank": 1, "count_star": 2, "count": 3, "sum": 4, "min": 5, "max": 6, "sql_rank": 7, "dense_rank": 8, "percent_rank": 9,
+       "cume_dist": 10, "ntile": 11, "lag": 12, "lead": 13, "first_value": 14, "last_value": 15, "nth_value": 16}
+# LdbWindowFrameMode
+FRAME = {"rows": 0, "range": 1}
 
 
 class WindowFunc(C.Structure):
     _fields_ = [("kind", C.c_int32), ("column", C.c_char_p), ("name", C.c_char_p)]
+
+
+class WindowFrame(C.Structure):
+    _fields_ = [("mode", C.c_int32), ("pad", C.c_int32), ("from_", C.c_int64), ("to", C.c_int64)]
+
+
+class WindowFuncEx(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("has_default", C.c_int32), ("column", C.c_char_p), ("name", C.c_char_p), ("n", C.c_int64), ("value", I128),
+                ("fvalue", C.c_double)]
 
 
 # LdbSetOpKind
@@ -226,6 +239,8 @@ SIGNATURES = {
     "ldb_gpu_table_gather_strings": (C.c_int, [_P, C.c_char_p, C.POINTER(C.c_int64), C.c_int64, C.POINTER(C.c_int64), _P, C.c_int64, C.POINTER(C.c_int64), _P, _E]),
     "ldb_gpu_table_window": (C.c_int, [_P, C.c_int32, C.POINTER(C.c_char_p), C.c_int32, C.POINTER(C.c_char_p), C.POINTER(C.c_int32), C.c_int64, C.c_int64,
                                        C.c_int32, C.POINTER(WindowFunc), C.c_int32, C.POINTER(C.c_char_p), C.c_char_p, C.POINTER(_P), _E]),
+    "ldb_gpu_table_window_ex": (C.c_int, [_P, C.c_int32, C.POINTER(C.c_char_p), C.c_int32, C.POINTER(C.c_char_p), C.POINTER(C.c_int32), C.POINTER(WindowFrame),
+                                          C.c_int32, C.POINTER(WindowFuncEx), C.c_int32, C.POINTER(C.c_char_p), C.c_char_p, C.POINTER(_P), _E]),
     "ldb_gpu_table_setop": (C.c_int, [_P, _P, C.c_int32, C.c_int32, C.POINTER(C.c_char_p), C.POINTER(C.c_char_p), C.c_char_p, C.POINTER(_P), _E]),
     "ldb_gpu_table_nl_join": (C.c_int, [_P, _P, C.c_int32, C.c_int32, C.POINTER(JoinCond), C.c_int32, C.POINTER(C.c_char_p), C.c_int32, C.POINTER(C.c_char_p),
                                         C.POINTER(C.c_char_p), C.c_char_p, C.c_char_p, C.POINTER(_P), _E]),

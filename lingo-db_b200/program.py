@@ -485,24 +485,46 @@ class RawTable:
         out = [raw[offs[i]:offs[i + 1]] if valid[i] else None for i in range(n)]
         return [s.decode() if decode and s is not None else s for s in out]
 
-    def window(self, partition_by=(), order_by=(), frame=None, funcs=(), columns=None, name="window") -> "RawTable":
-        """Window functions (ldb_gpu_table_window) as a new table in window order: the carried `columns` (None: every column), then one
-        column per function.  order_by: [(column, descending), …]; frame: (from, to) ROWS offsets relative to the current row, None for
-        an unbounded end (default: (None, 0) with ORDER BY, (None, None) without, as the SQL analyzer sets it); funcs: [(kind, column,
-        name), …] with kind one of capi.WIN ("row_number" / "rank", "count_star", "count", "sum", "min", "max"; column None for the
-        first two).  AVG is sum / count."""
+    def window(self, partition_by=(), order_by=(), frame=None, funcs=(), columns=None, name="window", mode="rows") -> "RawTable":
+        """Window functions (ldb_gpu_table_window / _ex) as a new table in window order: the carried `columns` (None: every column), then
+        one column per function.  order_by: [(column, descending), …]; frame: (from, to) offsets relative to the current row, None for an
+        unbounded end, 0 for CURRENT ROW (default: (None, 0) with ORDER BY, (None, None) without, as the SQL analyzer sets it); mode:
+        "rows" or "range" (RANGE offsets are key distances, and (None, 0) is SQL's default frame there); funcs: [(kind, column, name[, n[,
+        default]]), …] with kind one of capi.WIN ("row_number", "rank" (the reference's: ROW_NUMBER), "count_star", "count", "sum", "min",
+        "max", "sql_rank", "dense_rank", "percent_rank", "cume_dist", "ntile", "lag", "lead", "first_value", "last_value",
+        "nth_value"; column None for those without an argument), n the LAG / LEAD offset (default 1), NTILE's buckets or NTH_VALUE's
+        position, and default LAG / LEAD's value outside the partition, an int or a float as in nl_join.  AVG is sum / count."""
         if frame is None:
             frame = (None, 0) if order_by else (None, None)
         lo = -(1 << 63) if frame[0] is None else int(frame[0])
         hi = (1 << 63) - 1 if frame[1] is None else int(frame[1])
         enc = lambda xs: (C.c_char_p * max(1, len(xs)))(*[x.encode() for x in xs])
         part, order = list(partition_by), list(order_by)
-        fs = (capi.WindowFunc * max(1, len(funcs)))(*[capi.WindowFunc(capi.WIN[k], c.encode() if c is not None else None, n.encode()) for k, c, n in funcs])
         desc = (C.c_int32 * max(1, len(order)))(*[int(bool(d)) for _, d in order])
         carried = None if columns is None else enc(list(columns))
         t, e = C.c_void_p(), Error()
-        check(self.ctx.L.ldb_gpu_table_window(self.h, len(part), enc(part), len(order), enc([c for c, _ in order]), desc, lo, hi, len(funcs), fs,
-                                              0 if columns is None else len(columns), carried, name.encode(), C.byref(t), C.byref(e)), e)
+        funcs = [tuple(f) for f in funcs]
+        if mode == "rows" and all(len(f) == 3 and capi.WIN[f[0]] <= capi.WIN["max"] for f in funcs):
+            fs = (capi.WindowFunc * max(1, len(funcs)))(*[capi.WindowFunc(capi.WIN[k], c.encode() if c is not None else None, n.encode()) for k, c, n in funcs])
+            check(self.ctx.L.ldb_gpu_table_window(self.h, len(part), enc(part), len(order), enc([c for c, _ in order]), desc, lo, hi, len(funcs), fs,
+                                                  0 if columns is None else len(columns), carried, name.encode(), C.byref(t), C.byref(e)), e)
+            return RawTable(self.ctx, t)
+        fx = []
+        for f in funcs:
+            kind, col, nm = f[0], f[1], f[2]
+            n = int(f[3]) if len(f) > 3 and f[3] is not None else (1 if kind in ("lag", "lead") else 0)
+            w = capi.WindowFuncEx(capi.WIN[kind], 0, None if col is None else col.encode(), nm.encode(), n)
+            if len(f) > 4 and f[4] is not None:
+                # a float argument reads fvalue, any other value: an int sets both, a float its integral value too (as nl_join)
+                v = f[4]
+                iv = int(v) if isinstance(v, int) or float(v).is_integer() else 0
+                iv = iv if -(1 << 127) <= iv < (1 << 127) else 0  # a float beyond i128 (1e300): fvalue only
+                w.has_default, w.value, w.fvalue = 1, capi.I128(iv & ((1 << 64) - 1), iv >> 64), float(v)
+            fx.append(w)
+        fs = (capi.WindowFuncEx * max(1, len(fx)))(*fx)
+        fr = capi.WindowFrame(capi.FRAME[mode], 0, lo, hi)
+        check(self.ctx.L.ldb_gpu_table_window_ex(self.h, len(part), enc(part), len(order), enc([c for c, _ in order]), desc, C.byref(fr), len(fx), fs,
+                                                 0 if columns is None else len(columns), carried, name.encode(), C.byref(t), C.byref(e)), e)
         return RawTable(self.ctx, t)
 
     def setop(self, other, kind: str, columns=None, other_columns=None, name="setop") -> "RawTable":
