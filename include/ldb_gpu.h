@@ -734,7 +734,13 @@ int ldb_gpu_table_setop(LdbTable* left, LdbTable* right /* NULL exactly for LDB_
  *   given to SEMI / ANTI / MARK / COUNT, a missing value_name for MARK / COUNT, and two output columns of one name (a self join
  *   without right_names), naming the clash; LDB_ERR_UNSUPPORTED for the type mixes above, a side of 2^32 - 1 rows or more and a call
  *   inside a captured query (the output size is read on the host).  After counting: LDB_ERR_CAPACITY naming the row count when the
- *   result does not fit device memory, and LDB_ERR_UNSUPPORTED when a utf8 column of the result would hold more than 2^31 - 1 bytes. */
+ *   result does not fit device memory, and LDB_ERR_UNSUPPORTED when a utf8 column of the result would hold more than 2^31 - 1 bytes.
+ *   How the call runs (the rows, order and errors above are the same either way; csrc/nljoin_sorted.cu, DESIGN §7 "Sorted ranges"):
+ *   when some column-to-column condition is an equality or a range (<, <=, >, >=), the sides hold n m >= 2^24 pairs and the scratch
+ *   fits, one side is sorted by its equality operands and the column it bounds most, and every row of the other side binary-searches
+ *   its contiguous range of sorted rows, in O((n + m) log + candidates); COUNT, SEMI, ANTI and MARK need no pairs at all.  <> and
+ *   range conditions on a second sorted column are checked per candidate.  Otherwise, and when the candidates exceed n m / 256, the
+ *   loop compares every pair, at about 1.6e12 pair checks/s on an H100. */
 enum LdbNlJoinKind { LDB_NLJ_INNER = 1, LDB_NLJ_LEFT_OUTER = 2, LDB_NLJ_RIGHT_OUTER = 3, LDB_NLJ_FULL_OUTER = 4,
                      LDB_NLJ_SEMI = 5, LDB_NLJ_ANTI = 6, LDB_NLJ_MARK = 7, LDB_NLJ_COUNT = 8 };
 typedef struct LdbJoinCond {

@@ -31,7 +31,10 @@
 //      a scan of the unmarked right rows their places after the pairs, the host reads the totals and allocates the result, the write
 //      pass and nljFillKernel (the NULL-extended rows) write the id pairs, and permuteRows (peer.cu) gathers each side's cells, an id
 //      of 0xffffffff giving NULL cells.  COUNT, MARK, SEMI and ANTI need no pairs: their rows are left rows.
-#include "context.h"
+//   Step 2's passes give way to the sorted ranges (nljoin_sorted.cu) when an equality or range condition can key a sort and the
+//   sides hold at least kNljSortMinPairs pairs: they produce the same per-left-row counts and right markers (as one chunk), and step 3
+//   runs on them unchanged.
+#include "nljoin.cuh"
 #include "progcol.cuh"
 #include "tilescan.cuh"
 
@@ -44,8 +47,6 @@ constexpr int kNljThreads = 256, kNljRows = 4; // a thread's left rows
 constexpr int64_t kNljLeftTile = (int64_t) kNljThreads * kNljRows;
 constexpr int kNljRightTile = 512;                          // right rows per shared-memory tile
 constexpr int64_t kNljMinChunk = 2 * kNljRightTile;          // right rows of a chunk at least
-constexpr int kNljMaxConds = 8, kNljMaxPairs = 4, kNljMaxCols = 16;
-constexpr uint32_t kNljNone = 0xffffffffu; // permuteRows' id of a row of NULL cells
 
 // ---------------------------------------------------------------- 1. words
 struct NljSideBatch {
@@ -323,9 +324,6 @@ __global__ void __launch_bounds__(256) nljFillKernel(const uint8_t* unmatched, c
 }
 
 // ---------------------------------------------------------------- host side
-static unsigned nljGrid(const LdbContext* ctx, uint64_t items) {
-   return (unsigned) std::max<uint64_t>(1, std::min<uint64_t>((items + 255) / 256, (uint64_t) ctx->smCount * 16));
-}
 // the comparable families: 1 integers, 2 date32, 3 char(1), 4 decimal, 5 float; 0 none (utf8 and anything else)
 static int nljFamily(int type) {
    switch (type) {
@@ -533,6 +531,10 @@ static void tableNlJoin(LdbTable* left, LdbTable* right, int32_t kind, int32_t n
          if (outCols[j].name == outCols[k].name)
             fail(LDB_ERR_INVALID, "the nested-loop join's result would have two columns named " + outCols[j].name + " (output columns " + std::to_string(k) +
                                      " and " + std::to_string(j) + "; name the right columns with right_names)");
+   std::vector<int32_t> lw, rw;
+   size_t rowBytes = !leftOnly ? 8 : 0;
+   for (int ci : lc) lw.push_back(shipCellBytes(left->columns[ci].type)), rowBytes += lw.back() + 1;
+   for (int ci : rc) rw.push_back(shipCellBytes(right->columns[ci].type)), rowBytes += rw.back() + 1;
    const int64_t nL = left->numRows, nR = right->numRows;
    if (nL >= (int64_t) kNljNone || nR >= (int64_t) kNljNone) fail(LDB_ERR_UNSUPPORTED, "a nested-loop join takes sides of fewer than 2^32 - 1 rows");
    LdbContext* ctx = left->ctx;
@@ -573,12 +575,14 @@ static void tableNlJoin(LdbTable* left, LdbTable* right, int32_t kind, int32_t n
    p.nChunks = (int32_t) nChunks;
    p.exists = kind == LDB_NLJ_SEMI || kind == LDB_NLJ_ANTI || kind == LDB_NLJ_MARK;
    for (int c = 0; c < nc; c++) p.mask[c] = masks[c];
-   const int64_t nPos = nL * nChunks;
+   int64_t nPos = nL * nChunks;
    uint32_t* keep = nullptr;
    uint8_t* unmatched = nullptr;
    unsigned long long* offs = nullptr;
    uint32_t* rightAt = nullptr;
    uint32_t* ids = nullptr; // semi / anti: the kept left rows
+   NljSortedRun sr(ctx);
+   bool sorted = false;
    if (nL > 0 && nR > 0) {
       int64_t *lLo, *lHi, *rLo, *rHi;
       uint8_t *lOk, *rOk;
@@ -590,13 +594,41 @@ static void tableNlJoin(LdbTable* left, LdbTable* right, int32_t kind, int32_t n
       p.rHi = rHi;
       p.lOk = lOk;
       p.rOk = rOk;
-      p.counts = tmp.alloc<uint32_t>((size_t) nPos * 4);
-      if (markRight) {
-         p.rightMark = tmp.alloc<uint8_t>((size_t) nR);
-         LDB_CUDA(cudaMemsetAsync(p.rightMark, 0, (size_t) nR, ctx->compute));
+      // the sorted ranges when some condition keys a sort, the pairs are many and its scratch fits where the loop's does
+      if (nljSortedPlan(nc, masks.data(), ls.pairCols.data(), rs.pairCols.data(), nL, nR, &sr.plan) && (double) nL * (double) nR >= kNljSortMinPairs) {
+         const int64_t nS = sr.plan.sLeft ? nL : nR, nP = sr.plan.sLeft ? nR : nL;
+         const double sortBytes = (double) nS * (24 + 16 * (wide ? 2 : 1) * (sr.plan.nEq + 1)) + (double) nP * 20 + (double) nL * 4;
+         const double loopBytes = (double) nPos * 12;
+         size_t freeB = 0, totalB = 0;
+         LDB_CUDA(cudaMemGetInfo(&freeB, &totalB));
+         if (sortBytes <= (double) freeB || loopBytes > (double) freeB) {
+            sr.left = NljWordsRef{lLo, lHi, lOk, nL};
+            sr.right = NljWordsRef{rLo, rHi, rOk, nR};
+            sr.wide = wide;
+            sr.kind = kind;
+            sr.resultRowBytes = (double) rowBytes;
+            sorted = nljSortedCount(ctx, tmp, sr);
+            if (!sorted) { // the loop's scratch comes next: the sorted path's goes back to the device first
+               sr.keep.toDevice();
+               sr.sortOnly.toDevice();
+            }
+         }
       }
-      const dim3 grid((unsigned) leftTiles, (unsigned) nChunks);
-      ctx->launch("nljoin_count", [&] { nljLoop(ctx, nc, wide, false, grid, p); });
+      if (sorted) {
+         nChunks = 1;
+         nPos = nL;
+         p.nChunks = 1;
+         p.counts = sr.counts;
+         p.rightMark = sr.rightMark;
+      } else {
+         p.counts = tmp.alloc<uint32_t>((size_t) nPos * 4);
+         if (markRight) {
+            p.rightMark = tmp.alloc<uint8_t>((size_t) nR);
+            LDB_CUDA(cudaMemsetAsync(p.rightMark, 0, (size_t) nR, ctx->compute));
+         }
+         const dim3 grid((unsigned) leftTiles, (unsigned) nChunks);
+         ctx->launch("nljoin_count", [&] { nljLoop(ctx, nc, wide, false, grid, p); });
+      }
    } else if (nL > 0) {
       p.counts = tmp.alloc<uint32_t>((size_t) nPos * 4); // no right rows: no matches
       LDB_CUDA(cudaMemsetAsync(p.counts, 0, (size_t) nPos * 4, ctx->compute));
@@ -629,12 +661,12 @@ static void tableNlJoin(LdbTable* left, LdbTable* right, int32_t kind, int32_t n
 
    // the result's rows
    const int64_t total = pairs ? (int64_t) (nPairs + nRightOnly) : kind == LDB_NLJ_SEMI || kind == LDB_NLJ_ANTI ? (int64_t) nKept : nL;
-   std::vector<int32_t> lw, rw;
-   size_t rowBytes = pairs ? 8 : 0;
-   for (int ci : lc) lw.push_back(shipCellBytes(left->columns[ci].type)), rowBytes += lw.back() + 1;
-   for (int ci : rc) rw.push_back(shipCellBytes(right->columns[ci].type)), rowBytes += rw.back() + 1;
    size_t freeB = 0, totalB = 0;
    LDB_CUDA(cudaMemGetInfo(&freeB, &totalB));
+   if ((double) total * (double) rowBytes > (double) freeB && !sr.sortOnly.empty()) { // the sort's buffers are done with: give them back
+      sr.sortOnly.toDevice();
+      LDB_CUDA(cudaMemGetInfo(&freeB, &totalB));
+   }
    if ((double) total * (double) rowBytes > (double) freeB)
       fail(LDB_ERR_CAPACITY, "the nested-loop join's result has " + std::to_string(total) + " rows, which need " + std::to_string((double) total * rowBytes / 1e9) +
                                 " GB of device memory; " + std::to_string(freeB / 1e9) + " GB are free");
@@ -642,7 +674,9 @@ static void tableNlJoin(LdbTable* left, LdbTable* right, int32_t kind, int32_t n
    if (pairs && total > 0) {
       outL = tmp.alloc<uint32_t>((size_t) total * 4);
       outR = tmp.alloc<uint32_t>((size_t) total * 4);
-      if (nPairs > 0 && nR > 0) {
+      if (sorted) {
+         nljSortedWrite(ctx, tmp, sr, offs, outL, outR);
+      } else if (nPairs > 0 && nR > 0) {
          p.offs = offs;
          p.outL = outL;
          p.outR = outR;
@@ -657,6 +691,7 @@ static void tableNlJoin(LdbTable* left, LdbTable* right, int32_t kind, int32_t n
             nljFillKernel<<<nljGrid(ctx, (uint64_t) std::max(nL, nR)), 256, 0, ctx->compute>>>(unmatched, offs, unmatched ? nL : 0, p.nChunks, markRight ? p.rightMark : nullptr,
                                                                                                 rightAt, ctr, markRight ? nR : 0, outL, outR);
          });
+      if (sorted) nljSortedOrder(ctx, tmp, sr, (int64_t) nPairs, outL, outR);
    }
 
    // the cells

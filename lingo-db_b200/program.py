@@ -549,7 +549,8 @@ class RawTable:
         too) or a float (float columns; against any other column only an integral one).  No conds: a cross product.  columns /
         other_columns: the carried columns (None: every column; other's only for the pair kinds), other_names: their output names; value_name: the MARK (int32 0 / 1) or COUNT (int64) column.  Rows come in left
         row order, then right row order; unmatched right rows of right / full joins last.  `other` may be a RawTable, a runtime.Table
-        or this table itself."""
+        or this table itself.  Joins with an equality or a range condition over at least 2^24 pairs sort one side and binary-search each
+        row's range of matches instead of comparing every pair (DESIGN §7, "Sorted ranges")."""
         cs = []
         for c in conds:
             lcol, op, rcol = c[0], c[1], c[2]
